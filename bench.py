@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py - Msamples/s of the Mode S receive hot path (IQ demod + preamble detect + slice + CRC).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--log2n 28]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--log2n 28] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workload (BASELINE.json configs[1]): synthetic 1090 MHz IQ at 4 Msps, 2^28 complex samples (2 GiB) per GPU,
@@ -42,7 +42,7 @@ def measured_peak_gbs():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, copy kernel)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3; not reached)"
 
 
 class ClockSampler:
@@ -180,8 +180,30 @@ def parity_check(rx, q, iq, rate, threads):
             "detections": d, "oracle": kind, "seconds": round(time.perf_counter() - t0, 1)}
 
 
-def run_config(key, n, args, rank, local_rank, world, device, fan=None, steps=None):
-    """Device-resident timing + full-size parity of one BASELINE config. Returns (result dict, iq, rx, q)."""
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, frames):
+    """Write the frames a step returned (rx_path.drain(): one amb_frame per detection, stream order) as one .npy per
+    field, float64 for the 64-bit and 32-bit integer fields and the timestamp, float32 for the rest. Past 64 MB in all a
+    fixed, seeded sample of the frames is written; `row` holds the index of every written frame in the full list."""
+    from gr_air_modes_b200._lib import Frame
+    wide = ("sample_index", "secs", "frac", "crc")
+    rec = np.ctypeslib.as_array((Frame * len(frames))(*frames)) if frames else np.zeros(0, np.ctypeslib.as_array((Frame * 1)()).dtype)
+    cols = {k: rec[k].astype(np.float64 if k in wide else np.float32) for k in rec.dtype.names if k != "pad_"}
+    cols["row"] = np.arange(len(rec), dtype=np.float64)
+    per_frame = sum(a[:1].nbytes for a in cols.values())
+    if len(rec) * per_frame > DUMP_LIMIT_BYTES:
+        keep = np.sort(np.random.default_rng(0).choice(len(rec), DUMP_LIMIT_BYTES // per_frame, replace=False))
+        cols = {k: a[keep] for k, a in cols.items()}
+    os.makedirs(out_dir, exist_ok=True)
+    for k, a in cols.items():
+        np.save(os.path.join(out_dir, k + ".npy"), a)
+
+
+def run_config(key, n, args, rank, local_rank, world, device, fan=None, steps=None, dump_dir=None):
+    """Device-resident timing + full-size parity of one BASELINE config. Returns (result dict, iq, rx, q).
+    dump_dir: where to write the frames of the last timed step (dump_outputs)."""
     import torch
     import torch.distributed as dist
     import gr_air_modes_b200 as am
@@ -224,7 +246,10 @@ def run_config(key, n, args, rank, local_rank, world, device, fan=None, steps=No
     scan_ms = rx._ctx.scan_times_ms(min(steps, 64))
     st = rx.stats()
     launches = st.kernel_launches - launches0
-    rx.drain(); q.flush()
+    rx.drain()                     # reset() at the start of every step: these are the last timed step's frames
+    if dump_dir:
+        dump_outputs(dump_dir, rx.frames)
+    q.flush()
     ms_max = shard.max_over_ranks(ms, world, device)
     scan_avg = shard.max_over_ranks(float(np.mean(scan_ms)), world, device)
     peak, peak_src = measured_peak_gbs()
@@ -605,6 +630,8 @@ def main():
     ap.add_argument("--dense", action="store_true", help="shorthand for --config c4")
     ap.add_argument("--extra-configs", default=None, help="comma list of further configs measured into configs[] "
                     "(default: the other three on one GPU, c1 on several; 'none' to skip)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the frames of the headline config's last timed step to DIR/<field>.npy")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--no-e2e-extras", action="store_true")
@@ -661,7 +688,10 @@ def main():
     if rank == 0:
         sampler.start()
     all_cpus = os.sched_getaffinity(0)
-    head, iq, rx, q = run_config(key, n, args, rank, local_rank, world, device)
+    dump_dir = None
+    if args.dump_outputs:
+        dump_dir = args.dump_outputs if world == 1 else os.path.join(args.dump_outputs, "rank%d" % rank)
+    head, iq, rx, q = run_config(key, n, args, rank, local_rank, world, device, dump_dir=dump_dir)
     e2e, e2e_extras = (None, {}) if args.no_e2e else e2e_legs(rx, q, iq, n, args, local_rank, world, device)
     clocks = sampler.stop() if rank == 0 else None     # sampled across the headline's timed regions (device + end to end)
     os.sched_setaffinity(0, all_cpus)                  # the CPU legs below get every host thread back
@@ -695,7 +725,7 @@ def main():
                        "e2e_steps": args.e2e_steps, "msgs_per_step": head["msgs_per_step"],
                        "candidates_per_step": head["candidates"], "detections_per_step": head["detections"]},
             "roofline": {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                         "traffic": None, "kernel": scan_name, "peak_source": peak_src,
+                         "traffic": None, "traffic_note": "no DRAM-counter capture", "kernel": scan_name, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": 8 * n, "scan_ms": head["scan_ms"],
                          "whole_step_frac": head["step_frac"]},
             "e2e": e2e,
@@ -708,32 +738,12 @@ def main():
             line["parity"] = head["parity"]
         line.update(e2e_extras)
         line["configs"] = others
-        line["roofline"].update(scan_traffic(key, args.log2n))
         if not args.no_cpu_baseline and world == 1:
             line["cpu_baseline"] = cpu_baseline_leg(key, args.log2n)
         print(json.dumps(line))
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
-
-
-def scan_traffic(key, log2n):
-    """dram bytes per scan launch from the committed ncu capture - only if that capture was taken of the kernel
-    source that is built now (profiles/scan_traffic.json records the sha256 of csrc/amb_kernels.cu)."""
-    import hashlib
-    tr = os.path.join(ROOT, "profiles", "scan_traffic.json")
-    try:
-        rec = json.load(open(tr))
-        src = os.path.join(ROOT, "gr_air_modes_b200", "csrc", "amb_kernels.cu")
-        sha = hashlib.sha256(open(src, "rb").read()).hexdigest()
-        ent = rec.get("%s_2p%d" % (key, log2n))
-        if not ent:
-            return {"traffic": None, "traffic_note": "no ncu capture of this config committed"}
-        if ent.get("kernels_sha256") != sha:
-            return {"traffic": None, "traffic_note": "committed ncu capture is of another revision of amb_kernels.cu"}
-        return {"traffic": ent["dram_bytes_per_launch"], "traffic_source": ent.get("source")}
-    except Exception as e:      # noqa: BLE001
-        return {"traffic": None, "traffic_note": "profiles/scan_traffic.json unreadable (%s)" % type(e).__name__}
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""gr-air-modes_b200: the Mode S / ADS-B receive hot path of gr-air-modes as sm_100a CUDA.
+"""gr-air-modes_b200: the Mode S / ADS-B receive hot path of gr-air-modes as sm_90a CUDA.
 
 Python identifiers cannot contain '-', so the package directory is gr_air_modes_b200. It exports the
 reference's names for the path (python/__init__.py:34,44 exports the swig blocks and rx_path):

@@ -1,6 +1,6 @@
 """ctypes binding of libairmodes_b200.so (include/airmodes_b200.h).
 
-There is no CPU implementation behind this module: if the CUDA library cannot be loaded, or no sm_100
+There is no CPU implementation behind this module: if the CUDA library cannot be loaded, or no sm_90
 device is present, the constructors raise RuntimeError. That is deliberate (BASELINE north_star: no CPU
 fallback); nothing here imports or calls oracle/.
 """

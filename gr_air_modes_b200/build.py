@@ -1,4 +1,4 @@
-"""In-tree build of libairmodes_b200.so (nvcc, sm_100a only). Cross-compiles without a GPU."""
+"""In-tree build of libairmodes_b200.so (nvcc, sm_90a only). Cross-compiles without a GPU."""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,7 @@ SOURCES = ["amb_kernels.cu", "amb_api.cu", "amb_decode.cu"]
 HEADERS = ["amb_internal.h", "amb_launch.h", "amb_params.h", "amb_decode_core.h", "amb_decode_kernels.cuh", "amb_decode_v3.cuh", "amb_order_kernels.cuh", os.path.join("..", "..", "include", "airmodes_b200.h")]
 # amb_decode.cu follows cpr.py operation by operation in IEEE double: no fused multiply-add contraction there
 EXTRA_FLAGS = {"amb_decode.cu": ["-fmad=false"]}
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "--compiler-options", "-fPIC,-fvisibility=hidden", "-Xcompiler", "-Wall"]
 
 

@@ -17,7 +17,7 @@
 #include <thread>
 #include <vector>
 
-#define AMB_VERSION "gr-air-modes_b200 0.1 (sm_100a)"
+#define AMB_VERSION "gr-air-modes_b200 0.1 (sm_90a)"
 
 typedef CUresult (*amb_encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -239,7 +239,7 @@ const char* amb_strerror(int code)
     switch (code) {
         case AMB_OK: return "ok";
         case AMB_ERR_INVALID: return "invalid argument";
-        case AMB_ERR_NO_DEVICE: return "no usable sm_100 CUDA device (there is no CPU path)";
+        case AMB_ERR_NO_DEVICE: return "no usable sm_90 CUDA device (there is no CPU path)";
         case AMB_ERR_CUDA: return "CUDA runtime error";
         case AMB_ERR_RATE: return "unsupported sample rate";
         case AMB_ERR_OVERFLOW: return "internal buffer overflow";
@@ -260,7 +260,7 @@ int amb_create(int device, float rate, float threshold_db, int use_pmf, int use_
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) return AMB_ERR_NO_DEVICE;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return AMB_ERR_NO_DEVICE;
-    if (prop.major != 10) return AMB_ERR_NO_DEVICE;  // sm_100a cubin only
+    if (prop.major != 9 || prop.minor != 0) return AMB_ERR_NO_DEVICE;  // sm_90a cubin only
     amb_ctx* ctx = new amb_ctx();
     ctx->device = device; ctx->sm_count = prop.multiProcessorCount;
     ctx->rate_arg = rate; ctx->thr_db = threshold_db; ctx->use_pmf = use_pmf ? 1 : 0;
@@ -608,8 +608,8 @@ static int process_core(amb_ctx* ctx, const float* iq, size_t n_complex, int mem
         if (n_main) { int rc2 = make_tmap(ctx, &a.tm_main, src, (size_t)n_main); if (rc2) return rc2; }
         else a.tm_main = ctx->tm_tail[set];
 
-        // ---- stream A: stage the tail + reset the group counts (2 us, in front of the scan: a hop over to stream C and
-        // back cost ~14 us of idle scan stream per call), then stream over the IQ. Stream C's carry kernel reads the tail.
+        // ---- stream A: stage the tail + reset the group counts (in front of the scan: a hop over to stream C and
+        // back would leave the scan stream idle), then stream over the IQ. Stream C's carry kernel reads the tail.
         CK(amb_launch_prologue(ctx->tail[set], ctx->tail_cap, src + n_main, n_tv, a.group_count, 128, sa));
         CK(cudaEventRecord(ctx->e_in, sa));
         CK(cudaStreamWaitEvent(sc, ctx->e_in, 0));
@@ -1536,7 +1536,7 @@ int amb_preamble_process(amb_ctx* ctx, const float* in0, const float* in1, size_
         if (e == cudaSuccess) e = cudaMemsetAsync(ctx->span_count[0], 0, (size_t)(ctx->spans_cap + 128) * sizeof(uint32_t), s);
         if (e == cudaSuccess) e = cudaMemsetAsync(ctx->ctr, 0, sizeof(AmbCounters), s);
         if (e == cudaSuccess && first) e = cudaMemsetAsync(ctx->st, 0, sizeof(AmbWalkState), s);
-        if (e == cudaSuccess) e = amb_launch_stream_candidates(a, d0, d1, (long long)m, s);
+        if (e == cudaSuccess) e = amb_launch_stream_candidates(a, d0, d1, (long long)m, ctx->sm_count, s);
         if (e == cudaSuccess) e = amb_launch_compact(a, ctx->cand_j, ctx->cand_cap, ctx->ctr, ctx->walk_scratch, (long long)m + P.H + 4096, s);
         AmbExactArgs ea{};
         ea.P = P; ea.cand_j = ctx->cand_j; ea.cand_info = ctx->cand_info; ea.cand_avg = ctx->cand_avg; ea.ctr = ctx->ctr;

@@ -158,7 +158,7 @@ int amb_decoder_create(int device, int have_location, double lat, double lon, am
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) return AMB_ERR_NO_DEVICE;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return AMB_ERR_NO_DEVICE;
-    if (prop.major != 10) return AMB_ERR_NO_DEVICE;      // sm_100a cubin only; there is no CPU path
+    if (prop.major != 9 || prop.minor != 0) return AMB_ERR_NO_DEVICE;   // sm_90a cubin only; there is no CPU path
     amb_decoder* d = new (std::nothrow) amb_decoder();
     if (!d) return AMB_ERR_INVALID;
     d->device = device; d->sm_count = prop.multiProcessorCount;

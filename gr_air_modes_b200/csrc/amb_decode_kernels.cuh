@@ -75,7 +75,7 @@ amb_pair_kernel(const AmbPosRec* __restrict__ pos, int n, AmbCprSlot* table, Amb
 
 #ifdef AMB_PAIR_V2
 // EXPERIMENT (tools/variants.py "pair_v2"; NOT in the product build, not yet run on a GPU). The first pairing kernel is
-// L2-bandwidth-bound: each of its warps reads the whole 24-byte report list (profiles/r1_decode_summary.txt). Here
+// L2-bandwidth-bound: each of its warps reads the whole 24-byte report list. Here
 // the ownership test reads a 4-byte key array, eight independent steps' keys are in flight per iteration, and only
 // the lanes that own a report load the rest of it. The per-step logic is the first kernel's, unchanged.
 #define AMB_PAIR_V2_U 8

@@ -1,8 +1,8 @@
 // Pairing stage of the batch decoder with O(n) memory traffic - the product path since round 2 (AMB_PAIR_V3 is the
-// default in amb_decode.cu; profiles/r2_decode_summary.txt, r2_decode_kernels_ncu.txt: 0.29 ms for 2^20 frames).
+// default in amb_decode.cu).
 //
 // Round 1's pairing kernel (still selectable with -DAMB_PAIR_V1) lets every warp walk the whole report list and pick out
-// its own aircraft (profiles/r1_decode_summary.txt: 100 GB of L2 reads for 2^20 frames). Here the reports are first PARTITIONED by
+// its own aircraft (n warps x n reports of L2 reads). Here the reports are first PARTITIONED by
 // owner: a stable counting sort of the frame indices into AMB_V3_B buckets (bucket = hash of the aircraft key), so
 // that each bucket's list keeps stream order; then one warp per bucket walks only its own list with the same
 // per-step logic (match/ballot inside a step, the direct-mapped HBM table across steps and batches).

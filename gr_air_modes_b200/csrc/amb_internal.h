@@ -127,7 +127,8 @@ cudaError_t amb_launch_walk_par(const AmbWalkArgs& a, void* scratch, unsigned in
 size_t amb_walk_scratch_bytes(unsigned int cand_cap, long long n_samples);
 cudaError_t amb_launch_slice(const AmbSliceArgs& a, int sm_count, cudaStream_t s);
 cudaError_t amb_launch_carry(const AmbSegs& S, float2* dst, int kc, cudaStream_t s);
-cudaError_t amb_launch_stream_candidates(const AmbScanArgs& a, const float* in0, const float* in1, long long n, cudaStream_t s);
+cudaError_t amb_launch_stream_candidates(const AmbScanArgs& a, const float* in0, const float* in1, long long n, int sm_count,
+                                         cudaStream_t s);
 cudaError_t amb_launch_slice_chips(const float* chips, int ndet, amb_frame* frames, cudaStream_t s);
 cudaError_t amb_launch_crc(const uint8_t* data, int n, int length, uint32_t* out, cudaStream_t s);
 cudaError_t amb_upload_tables(const int* chip_off);

@@ -1,4 +1,4 @@
-// sm_100a kernels of the Mode S receive hot path. Citations are file:line under gr-air-modes.
+// sm_90a kernels of the Mode S receive hot path. Citations are file:line under gr-air-modes.
 //
 // Pipeline per amb_process() call (all on one CUDA stream, nothing round-trips to the host):
 //   scan     amb_scan_kernel      streaming pass over IQ (8 B/sample, the HBM-bound kernel): |x|^2, pulse
@@ -29,14 +29,13 @@
 #ifndef AMB_SCAN_REGS
 #define AMB_SCAN_REGS 112
 #endif
-// ... applied where it costs nothing (spc <= 2: no spills, same speed); the long filters keep all 128 registers
-// (capped at 112 the 20 Msps kernel runs 13 % slower - profiles/r2_scan_register_caps.txt).
+// ... applied where it costs no spills (spc <= 2); the long filters keep all 128 registers.
 #ifndef AMB_SCAN_REGS_HI
 #define AMB_SCAN_REGS_HI 120
 #endif
-// spc 3..5: 120 registers leave 4 K registers (and 25 KiB of shared memory) for the sparse kernels: the 10 Msps step
-// drops from 0.40 to 0.36 ms although the scan alone is 1 % slower. spc >= 6: the prefix ring leaves too little shared
-// memory for anything to be resident beside the scan, so it keeps every register (profiles/r2_scan_register_caps.txt).
+// spc 3..5: 120 registers leave 4 K registers (and 25 KiB of shared memory) for the sparse kernels, so that they overlap
+// the scan. spc >= 6: the prefix ring leaves too little shared memory for anything to be resident beside the scan, so it
+// keeps every register. (The SM's 64 K registers and 228 KiB of shared memory are the same on sm_90 and sm_100.)
 #define AMB_SCAN_REGS_FOR(SPC) ((SPC) <= 2 ? AMB_SCAN_REGS : (SPC) <= 5 ? AMB_SCAN_REGS_HI : 128)
 
 __constant__ unsigned int c_crc_rem[96]; // x^(t+24) mod 0xFFF409, t = distance of a message bit from the parity field
@@ -618,8 +617,8 @@ __device__ __forceinline__ float stream_at(const float* in, long long n, int H, 
 //             ascending sum of bb[c-L+1 .. c] = LITERALLY the canonical noise-floor window of the start c, then the
 //             pulse tests, the late gate and the quiet zones from the row. Rows have an odd stride, so 32 lanes
 //             walking 32 rows in step never collide on a bank. No shuffles, no votes: 32 candidates advance per warp
-//             instruction (the round-1 kernel spent a whole warp, ~560 instructions and five barriers on ONE
-//             candidate and was instruction-bound in dense traffic - profiles/r2_dense_sparse_before.txt).
+//             instruction (the warp-per-candidate kernel spends a whole warp and five barriers on ONE candidate,
+//             which makes it instruction-bound in dense traffic).
 // After a late shift the window of c+i is acc - head + tail when every addend's exponent lies within 19 of the
 // others (then every partial sum of <= 1024 such floats is exact in fp64, 24+19+10 = 53 bits, so any association
 // gives the canonical bits); otherwise that window is summed again, literally ascending.
@@ -798,7 +797,7 @@ __global__ void __launch_bounds__(64) amb_exact_kernel(const AmbExactArgs a, con
 // ---- exact stage, sparse traffic: one WARP per candidate (round-1 kernel) -----------------------------------------
 // With a few thousand candidates per call what counts is the latency of ONE candidate, not throughput: here the 32
 // lanes share a candidate's window sums (order-independent when every addend's exponent lies within 19 of the others,
-// else the literal ascending loop), so a candidate is decided in one memory round trip and ~10 us. It needs ~560 warp
+// else the literal ascending loop), so a candidate is decided in one memory round trip. It needs hundreds of warp
 // instructions per candidate, though, which is what made dense traffic instruction-bound: beyond dense_threshold
 // candidates per call amb_exact_kernel (rows + one lane per candidate) takes over. Both kernels are launched; the one
 // whose regime it is not returns at once. Writes info = late | real<<8 | valid<<9 and avg at the shifted index.
@@ -1187,8 +1186,8 @@ struct AmbParScratch {
 };
 
 // Pass 1 keeps everything that would be a same-address atomic per packet or per cluster in registers and folds it
-// once per warp at the end (with 236 k packets and 224 k clusters per call in dense traffic those atomics WERE the
-// kernel: 0.3 ms at 9 % issue utilisation); the slicer's work list is built by pass 2 from the verdict bits.
+// once per warp at the end (with 236 k packets and 224 k clusters per call in dense traffic those atomics would be the
+// kernel's whole cost); the slicer's work list is built by pass 2 from the verdict bits.
 __global__ void __launch_bounds__(64) amb_walk_par1_kernel(const AmbWalkArgs a, AmbParScratch* sc, long long* first_fin,
                                                             unsigned long long* buckets, long long zone)
 {
@@ -1386,7 +1385,8 @@ __global__ void amb_walk_reset_kernel(const AmbWalkArgs a, unsigned long long* s
 cudaError_t amb_launch_walk_reset(const AmbWalkArgs& a, void* scratch, long long n_samples, cudaStream_t s)
 {
     const int n64 = scratch ? (int)(32 + (n_samples >> AMB_BUCKET_SHIFT) + 8) : 0;   // as the compaction kernel clears it
-    AMB_LAUNCH((amb_walk_reset_kernel), 148, 256, 0, s, a, reinterpret_cast<unsigned long long*>(scratch), n64);
+    AMB_LAUNCH((amb_walk_reset_kernel), a.sm_count > 0 ? a.sm_count : 8, 256, 0, s, a,
+               reinterpret_cast<unsigned long long*>(scratch), n64);
     return cudaGetLastError();
 }
 
@@ -1408,7 +1408,7 @@ cudaError_t amb_launch_walk_summary(const AmbWalkArgs& a, cudaStream_t s)
 {
     cudaError_t e = cudaMemsetAsync(&a.st->first_real, 0xff, 2 * sizeof(unsigned long long), s);
     if (e != cudaSuccess) return e;
-    AMB_LAUNCH((amb_walk_summary_kernel), 148, 256, 0, s, a);
+    AMB_LAUNCH((amb_walk_summary_kernel), a.sm_count > 0 ? a.sm_count : 8, 256, 0, s, a);
     return cudaGetLastError();
 }
 
@@ -1840,9 +1840,10 @@ __global__ void __launch_bounds__(256) amb_stream_cand_kernel(const __grid_const
         }
     }
 }
-cudaError_t amb_launch_stream_candidates(const AmbScanArgs& a, const float* in0, const float* in1, long long n, cudaStream_t s)
+cudaError_t amb_launch_stream_candidates(const AmbScanArgs& a, const float* in0, const float* in1, long long n, int sm_count,
+                                         cudaStream_t s)
 {
-    AMB_LAUNCH((amb_stream_cand_kernel), 592, 256, 0, s, a, in0, in1, n);
+    AMB_LAUNCH((amb_stream_cand_kernel), 4 * sm_count, 256, 0, s, a, in0, in1, n);
     return cudaGetLastError();
 }
 

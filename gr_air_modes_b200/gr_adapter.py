@@ -1,4 +1,4 @@
-"""GNU Radio adapters: the B200 receive path as drop-ins for the reference's blocks inside a flowgraph.
+"""GNU Radio adapters: the H100 receive path as drop-ins for the reference's blocks inside a flowgraph.
 
     air_modes.rx_path(rate, threshold, queue, use_pmf, use_dcblock)   python/rx_path.py:27      -> rx_path (sink of gr_complex)
     air_modes.preamble(channel_rate, threshold_db)                    preamble.h:36-45          -> preamble (2 x float in, float out)

@@ -238,8 +238,8 @@ def dist_all_gather6(world: int, device):
 
 # ---- the speculative pass with nothing waiting on the host -----------------------------------------------------------
 # process_time_sharded_speculative reads each span's summary back (a device synchronisation), all-gathers Python
-# integers and composes the entries on the host: ~0.2 ms per pass of host-driven latency next to a scan share of
-# 0.16 ms on 8 GPUs. Here a pass is a fixed sequence of enqueues: summary kernel -> all-gather of 6 int64 per span on the
+# integers and composes the entries on the host: host-driven latency per pass that, on many GPUs, exceeds a span's
+# scan share. Here a pass is a fixed sequence of enqueues: summary kernel -> all-gather of 6 int64 per span on the
 # device -> compose kernel (every rank, all spans) -> the last span resolves with the entry that kernel wrote. The host
 # looks at the verdict (out[0]) only after the passes it wants have been enqueued; a pass whose speculation failed
 # (out[0] < len(plan) - 1: rare, a packet straddling a cut in an unlucky way) is redone with the functions above.

@@ -1,12 +1,12 @@
 /* airmodes_b200.h - C ABI of libairmodes_b200.so: the Mode S / ADS-B receive hot path of
  * gr-air-modes (|x|^2 -> pulse matched filter -> noise floor -> preamble detect -> PPM slice with
- * confidence -> 24-bit CRC) as hand-written sm_100a CUDA.
+ * confidence -> 24-bit CRC) as hand-written sm_90a CUDA.
  *
  * This is the drop-in boundary for that path. The reference exposes it as GNU Radio C++ blocks
  * behind SWIG (swig/air_modes_swig.i:15-16); each entry point below names the reference interface
  * it replaces (file:line relative to the gr-air-modes tree). Plain pointers and sizes only.
  * There is NO CPU fallback: every compute entry point fails with AMB_ERR_NO_DEVICE / a CUDA error
- * when no sm_100 device is usable.
+ * when no sm_90 device is usable.
  *
  * Conventions
  *   IQ input    : interleaved float32 I,Q = gr_complex (python/rx_path.py:29), host or device memory.
@@ -32,7 +32,7 @@ extern "C" {
 
 #define AMB_OK 0
 #define AMB_ERR_INVALID (-1)      /* bad argument */
-#define AMB_ERR_NO_DEVICE (-2)    /* no CUDA device / not sm_100: there is no CPU path */
+#define AMB_ERR_NO_DEVICE (-2)    /* no CUDA device / not sm_90: there is no CPU path */
 #define AMB_ERR_CUDA (-3)         /* CUDA runtime error, see amb_last_error() */
 #define AMB_ERR_RATE (-4)         /* rate < 2 Msps or samples/chip > 10 (unsupported geometry) */
 #define AMB_ERR_OVERFLOW (-5)     /* internal candidate/frame buffers exhausted even after growth */
@@ -337,7 +337,7 @@ AMB_API int amb_decoder_reset(amb_decoder* d);                      /* forget ev
 /* Decode n frames (host or device array, stream order = non-decreasing time). out: n records in host memory.
  * Frames with passed == 0 get AMB_FS_NOT_QUEUED and do not touch the CPR state. */
 AMB_API int amb_decode_frames(amb_decoder* d, const amb_frame* frames, int n, int mem_kind, amb_fields* out);
-/* The same with frames AND records in device memory: no host copies (2^20 frames: 0.6 ms of kernels on a B200). */
+/* The same with frames AND records in device memory: no host copies. */
 AMB_API int amb_decode_frames_device(amb_decoder* d, const amb_frame* frames_dev, int n, amb_fields* out_dev);
 /* Kernels launched so far / device time in ms of the last amb_decode_frames call (H2D, kernels, D2H). */
 AMB_API int amb_decoder_stats(amb_decoder* d, uint64_t* kernel_launches, float* ms_last);

@@ -3,7 +3,7 @@
     python tests/golden/make_decode_golden.py
 
 Every message of tests/decode_cases.CASES is pushed through the UNMODIFIED reference modules python/parse.py,
-python/altitude.py and python/cpr.py (imported where they lie under /root/reference behind a stub `air_modes`
+python/altitude.py and python/cpr.py (imported where they lie in the gr-air-modes tree, $AMB_REFERENCE_TREE, behind a stub `air_modes`
 package; nothing is copied), calling exactly what the reference's own consumer python/msprint.py calls per DF
 (handle0/4/5/11/17, printTCAS). The only patch: cpr.py stamps reports with time.time() (cpr.py:219-221); here
 time.time returns the message's own timestamp secs + frac, which is the clock a batch decoder has.
@@ -20,7 +20,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-REF = "/root/reference/python"
+REF = os.path.join(os.environ.get("AMB_REFERENCE_TREE", "/root/reference"), "python")
 
 
 def _load(name, path):

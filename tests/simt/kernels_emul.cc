@@ -49,7 +49,7 @@ extern "C" int emul_preamble(const float* in0, const float* in1, int n, float ra
     a.coarse = coarse.data(); a.fine = fine.data(); a.span_count = span_count.data();
     a.group_count = span_count.data() + spans_cap;
     cudaStream_t s = nullptr;
-    if (amb_launch_stream_candidates(a, d0.data(), d1.data(), (long long)m, s) != cudaSuccess) return -1;
+    if (amb_launch_stream_candidates(a, d0.data(), d1.data(), (long long)m, sm_count, s) != cudaSuccess) return -1;
     const bool par = resolver != 1;
     if (amb_launch_compact(a, cand_j.data(), cand_cap, &ctr, par ? walk_scratch.data() : nullptr, n_samples, s) != cudaSuccess) return -2;
     AmbExactArgs ea{};
@@ -149,7 +149,7 @@ extern "C" int emul_process_iq(const float* iq, int n, const float* bb, const fl
         std::vector<float> s0((size_t)n + shift + 1, 0.f), s1((size_t)n + shift + 1, 0.f);
         std::copy(bb, bb + n, s0.begin() + shift);
         std::copy(avg, avg + n, s1.begin() + shift);
-        if (amb_launch_stream_candidates(a, s0.data(), s1.data(), (long long)n + shift, s) != cudaSuccess) return -2;
+        if (amb_launch_stream_candidates(a, s0.data(), s1.data(), (long long)n + shift, sm_count, s) != cudaSuccess) return -2;
     }
     const bool par = resolver != 1;
     if (amb_launch_compact(a, cand_j.data(), cand_cap, &ctr, par ? walk_scratch.data() : nullptr, n_samples, s) != cudaSuccess) return -3;

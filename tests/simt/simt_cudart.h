@@ -2,12 +2,12 @@
 // uses, so that amb_api.cu and amb_decode.cu can be compiled into a test-only emulated library (tests/simt/
 // library_emul.cc). "Device" memory is host memory; streams and events are inert because an emulated kernel launch
 // runs to completion inside AMB_LAUNCH (program order is one valid execution of the stream/event graph the real code
-// builds). One emulated device: compute capability 10.0 with two SMs (grids are sized from the SM count).
+// builds). One emulated device: compute capability 9.0 with two SMs (grids are sized from the SM count).
 #pragma once
 #include <stdlib.h>
 #include <string.h>
 
-struct cudaDeviceProp { int major = 10, minor = 0, multiProcessorCount = 2; };
+struct cudaDeviceProp { int major = 9, minor = 0, multiProcessorCount = 2; };
 typedef void* cudaEvent_t;
 enum { cudaStreamNonBlocking = 1, cudaEventDisableTiming = 2, cudaEnableDefault = 0 };
 enum cudaMemcpyKind { cudaMemcpyHostToHost, cudaMemcpyHostToDevice, cudaMemcpyDeviceToHost, cudaMemcpyDeviceToDevice };

@@ -7,7 +7,7 @@ and the 60 M-sample configs[0] scene (hours of emulation), tests that start othe
 library (CLI, C example, stress tool), and the threaded speculative-resolution test (one emulated device, not
 thread-safe; tests/test_library_simt.py has its sequential form).
 
-This is the CPU tier's rehearsal of the GPU tier, not a substitute: the driver still runs `pytest -m gpu` on a B200.
+This is the CPU tier's rehearsal of the GPU tier, not a substitute: `pytest -m gpu` still has to run on an H100.
 """
 import os
 import subprocess

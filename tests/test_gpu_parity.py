@@ -1,4 +1,4 @@
-"""Parity tests proper: the CUDA path through the C ABI vs the CPU oracle / reference goldens. Need a B200."""
+"""Parity tests proper: the CUDA path through the C ABI vs the CPU oracle / reference goldens. Need an H100."""
 import ctypes as C
 import hashlib
 import os

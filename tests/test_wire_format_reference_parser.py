@@ -1,18 +1,16 @@
 """SURVEY.md 8 row f2: the message strings we emit are consumed by the reference's UNMODIFIED parser
-(python/parse.py make_parser, :422-436). Runs only where /root/reference exists (this container); the reference
-files are imported in place behind a stub `air_modes` package, never copied."""
+(python/parse.py make_parser, :422-436). What the parser made of each message is recorded in
+tests/golden/ref_python.json.gz (the `ref_py` fixture, tests/ref_golden.py); while recording, the reference files are
+imported in place behind a stub `air_modes` package, never copied."""
 import importlib.util
 import math
 import os
 import sys
 import types
 
-import pytest
-
 from helpers import load_golden
 
-REF = "/root/reference/python"
-pytestmark = pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not present")
+REF = os.path.join(os.environ.get("AMB_REFERENCE_TREE", "/root/reference"), "python")
 
 
 def _load(name, path):
@@ -23,8 +21,8 @@ def _load(name, path):
     return mod
 
 
-@pytest.fixture()
-def ref_parser():
+def _parse_with_reference(msgs):
+    """-> per message None (no handler) or what the reference's make_parser published for it."""
     saved = {k: v for k, v in sys.modules.items() if k == "air_modes" or k.startswith("air_modes.")}
     pkg = types.ModuleType("air_modes")
     pkg.__path__ = []
@@ -34,32 +32,42 @@ def ref_parser():
         _load("air_modes.altitude", os.path.join(REF, "altitude.py"))
         mt = _load("air_modes.modes_types", os.path.join(REF, "modes_types.py"))
         pkg.modes_report, pkg.stamp = mt.modes_report, mt.stamp
-        yield _load("air_modes.parse", os.path.join(REF, "parse.py"))
+        parser = _load("air_modes.parse", os.path.join(REF, "parse.py"))
+        out = []
+        for m in msgs:
+            pub = {}
+            parser.make_parser(pub)(m)
+            if "modes_dl" not in pub:       # the parser drops types it has no handler for (ADSBError)
+                out.append(None)
+                continue
+            rep = pub["modes_dl"]
+            df = rep.data.get_type()
+            out.append({"ecc": rep.ecc, "rssi": rep.rssi, "secs": rep.timestamp.secs, "frac_secs": rep.timestamp.frac_secs,
+                        "df": df, "typed": ("type%i_dl" % df) in pub,
+                        "aa": rep.data["aa"] if df in (11, 17) else None})
+        return out
     finally:
         for k in [k for k in sys.modules if k == "air_modes" or k.startswith("air_modes.")]:
             del sys.modules[k]
         sys.modules.update(saved)
 
 
-def test_reference_parser_accepts_our_messages(ref_parser):
+def test_reference_parser_accepts_our_messages(ref_py):
     meta, scenes = load_golden()
     seen = 0
     for s, _ in scenes:
-        pub = {}
-        publish = ref_parser.make_parser(pub)
-        for m in s["msgs"]:
-            pub.clear()
-            publish(m)
+        parsed = ref_py.get("make_parser/" + s["name"], s["msgs"], lambda: _parse_with_reference(s["msgs"]))
+        assert len(parsed) == len(s["msgs"])
+        for m, rep in zip(s["msgs"], parsed):
             data, ecc, ref, secs, frac = m.split()
-            if "modes_dl" not in pub:       # the parser drops types it has no handler for (ADSBError)
+            if rep is None:
                 continue
-            rep = pub["modes_dl"]
-            assert rep.ecc == int(ecc, 16)
-            assert abs(rep.rssi - 10.0 * math.log10(max(1e-8, float(ref)))) < 1e-12
-            assert rep.timestamp.secs == int(secs) and rep.timestamp.frac_secs == float(frac)
+            assert rep["ecc"] == int(ecc, 16)
+            assert abs(rep["rssi"] - 10.0 * math.log10(max(1e-8, float(ref)))) < 1e-12
+            assert rep["secs"] == int(secs) and rep["frac_secs"] == float(frac)
             df = int(data[:2], 16) >> 3
-            assert rep.data.get_type() == df and ("type%i_dl" % df) in pub
+            assert rep["df"] == df and rep["typed"]
             if df in (11, 17) and data in s["sent"]:
-                assert rep.data["aa"] == int(data[2:8], 16)      # ICAO address straight from our payload
+                assert rep["aa"] == int(data[2:8], 16)      # ICAO address straight from our payload
                 seen += 1
     assert seen >= 20

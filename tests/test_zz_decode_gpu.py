@@ -51,7 +51,7 @@ def test_decode_matches_reference_golden(dec_mod):
             n += 1
     print("decode golden: %d messages, %d positions, %d bit-identical lat/lon" % (n, npos, exact))
     assert n > 5000 and npos > 2000
-    assert exact == npos            # measured on a B200: every latitude/longitude bit-identical to the reference's
+    assert exact == npos            # every latitude/longitude bit-identical to the reference's
 
 
 def test_decode_equals_oracle_record_for_record(dec_mod):

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""modes_rx-style front end for the B200 receive chain (SURVEY.md 8 row f1).
+"""modes_rx-style front end for the H100 receive chain (SURVEY.md 8 row f1).
 
 The receiver half of apps/modes_rx + python/radio.py: the same "Receiver setup options" where they make sense
 without a radio (radio.py:89-121), the same two offline sources (radio.py:221-232: a cfile or a UDP stream of
