@@ -152,6 +152,27 @@ def test_slicer_and_crc_kernels_under_the_emulator(emul, port):
         assert [int(x) for x in out] == [port.crc24(bytes(r)) for r in data]
 
 
+def test_slicer_kernel_at_its_limits_under_the_emulator(emul, port):
+    """The packets of tests/test_decision_edges_gpu.py's slicer test: chips exactly on highlimit / lowlimit and their
+    float neighbours, around lowlimit*0.5, equal chips, +-0, NaN, +-Inf, at ordinary, negative, zero, denormal, huge,
+    overflowing and NaN reference levels, and headers / low-confidence counts deciding DF and the packet rules.
+    Checks slice_packet_warp's warp logic on the host; nvcc's code generation only the GPU test can."""
+    from gr_air_modes_b200 import _lib
+    from helpers import slicer_edge_packets
+    chips, _ = slicer_edge_packets()
+    n = chips.shape[0]
+    want = port.run_slicer(chips, np.zeros(n, np.uint64), np.zeros(n)).frames
+    frames = (_lib.Frame * n)()
+    assert emul.emul_slicer(chips.ctypes.data, n, C.cast(frames, C.c_void_p)) == 0
+    for k in range(n):
+        f, g = frames[k], want[k]
+        assert bytes(f.data) == bytes(g.data) and f.crc == g.crc and f.nbits == g.nbits, k
+        assert f.numlowconf == g.numlowconf and bytes(f.lowconfbits) == bytes(g.lowconfbits), k
+        assert f.passed == g.passed, k
+        assert np.float32(f.ref_level).tobytes() == np.float32(g.ref_level).tobytes() or (np.isnan(f.ref_level) and np.isnan(g.ref_level)), k
+    assert {g.passed for g in want} == {0, 1}
+
+
 def test_scan_kernel_under_the_emulator_on_pathological_inputs(emul, port):
     """The scan kernel is a conservative fp32 FILTER (FMA |x|^2, prefix-sum windows, lowered thresholds); whatever it
     is fed - 1e-17 / 1e-21 / 3e14 amplitude scales, NaN/Inf samples, silence, a DC offset, dense garble - the chain's

@@ -7,7 +7,7 @@ import pytest
 from gr_air_modes_b200 import synth
 from oracle import cpu_oracle as co
 
-from helpers import load_golden, parse_msg
+from helpers import EDGE_MATRIX, constructed_tie_cases, edge_scene, knife_edges, load_golden, parse_msg, slicer_edge_packets
 from ref_golden import chips_sha256, same_chips
 
 KNOWN = [("8D4840D6202CC371C32CE0576098", 0x576098), ("8D40621D58C382D690C8AC2863A7", 0x2863A7)]
@@ -29,7 +29,9 @@ def test_crc_port_equals_reference(port, ref):
     assert ref.crc24(bytes([0, 0, 1])) == 0xFFF409  # crc_table[1] == POLY (modes_crc.cc:57)
 
 
-@pytest.mark.parametrize("rate,thr", [(2e6, 7.0), (4e6, 7.0), (10e6, 3.5), (20e6, 7.0), (3e6, 7.0), (5e6, 9.0), (2.4e6, 7.0)])
+@pytest.mark.parametrize("rate,thr", [(2e6, 7.0), (4e6, 7.0), (10e6, 3.5), (20e6, 7.0), (3e6, 7.0), (5e6, 9.0), (2.4e6, 7.0),
+                                      (6e6, 7.0), (7e6, 7.0), (8e6, 7.0), (9e6, 7.0), (11e6, 7.0), (12e6, 7.0), (12.5e6, 7.0),
+                                      (14e6, 7.0), (15e6, 7.0), (16e6, 7.0), (17e6, 7.0), (18e6, 7.0), (19e6, 7.0)])
 def test_params_match_reference(port, ref, rate, thr):
     p = port.params(rate, thr)
     r, t, h = ref.preamble_params(rate, thr)
@@ -181,6 +183,49 @@ def test_port_matches_reference_random_sweep(port, ref):
         assert r.msgs == p.msgs and r.calls == p.calls, where
         total += len(r.index)
     assert total > 300
+
+
+@pytest.mark.parametrize("rate,pmf", EDGE_MATRIX)
+def test_port_matches_reference_at_threshold_knife_edges(port, ref, rate, pmf):
+    """The scenes and threshold pairs at which tests/test_decision_edges_gpu.py holds the chain to the oracle: two
+    adjacent float32 thresholds around each change of the output, on every rate class (fractional samples per chip up
+    to 9.5 included). The oracle must answer as the reference on both sides."""
+    sc = edge_scene(rate, pmf)
+    bb, avg = port.frontend(sc.iq, rate, pmf, co.MA_CANONICAL)
+    edges, _ = knife_edges(port, bb, avg, rate)
+    assert edges
+    for lo, hi, kind in edges:
+        outs = []
+        for t in (lo, hi):
+            r = ref.run_streams(bb, avg, rate, t)
+            p = port.run_streams(bb, avg, rate, t)
+            where = (rate, pmf, t, kind)
+            assert np.array_equal(r.index, p.index) and r.msgs == p.msgs and r.calls == p.calls, where
+            assert same_chips(r.chips, p.chips), where
+            outs.append(([int(x) for x in r.index], r.msgs))
+        assert outs[0] != outs[1]                          # the reference, too, changes its answer between them
+
+
+def test_port_matches_reference_at_constructed_ties(port, ref):
+    """The exact ties of tests/test_decision_edges_gpu.py (peak test, late gate, quiet zone)."""
+    cases, _ = constructed_tie_cases(port)
+    for case in cases:
+        bb, avg = port.frontend(case.iq, case.rate, case.pmf, co.MA_CANONICAL)
+        r = ref.run_streams(bb, avg, case.rate, case.threshold_db)
+        p = port.run_streams(bb, avg, case.rate, case.threshold_db)
+        assert np.array_equal(r.index, p.index) and r.msgs == p.msgs and same_chips(r.chips, p.chips), case.name
+
+
+def test_slicer_matches_reference_at_its_limits(port, ref):
+    """The packets of the slicer knife-edge tests: chips on llslicer's limits (slicer_impl.cc:67-100) and packets on
+    the rules of :162-182."""
+    chips, _ = slicer_edge_packets()
+    n = chips.shape[0]
+    secs = np.arange(n, dtype=np.uint64)
+    frac = np.linspace(0.0, 0.999, n)
+    r = ref.run_slicer(chips, secs, frac)
+    p = port.run_slicer(chips, secs, frac)
+    assert r.msgs == p.msgs and len(r.msgs) > 0
 
 
 def test_port_matches_reference_on_pathological_inputs(port, ref):
