@@ -14,14 +14,31 @@ LIB_PATH = os.path.join(HERE, "libairmodes_b200.so")
 
 OK = 0
 MEM_HOST, MEM_DEVICE, MEM_HOST_SC16, MEM_DEVICE_SC16 = 0, 1, 2, 3
+# amb_frame.ec (include/airmodes_b200.h AMB_EC_*)
+EC_NOT_TRIED, EC_FIXED, EC_TOO_MANY, EC_NO_SOLUTION, EC_AMBIGUOUS = 0, 1, 2, 3, 4
+EC_MAX = 23
 
 
 class Frame(C.Structure):
-    """struct amb_frame (80 bytes) = modes_packet (types.h:29-41) + preamble tag."""
+    """struct amb_frame (80 bytes) = modes_packet (types.h:29-41) + preamble tag.
+
+    The header's `ec` / `ec_flips` are the first two of the six tail bytes, which stay one `pad_` field here: the
+    record layout that numpy views and per-field dumps of frames see (np.dtype(Frame)) is the one the frame had before
+    error correction existed. They are read through the properties below."""
     _fields_ = [("sample_index", C.c_uint64), ("secs", C.c_uint64), ("frac", C.c_double),
                 ("ref_level", C.c_float), ("crc", C.c_uint32), ("nbits", C.c_uint8), ("df", C.c_uint8),
                 ("numlowconf", C.c_uint8), ("passed", C.c_uint8), ("lowconfbits", C.c_uint8 * 24),
                 ("data", C.c_uint8 * 14), ("pad_", C.c_uint8 * 6)]
+
+    @property
+    def ec(self) -> int:
+        """amb_frame.ec: error-correction outcome, EC_* (0 unless option "ec" tried this frame)."""
+        return self.pad_[0]
+
+    @property
+    def ec_flips(self) -> int:
+        """amb_frame.ec_flips: bits the correction flipped (EC_FIXED), else 0."""
+        return self.pad_[1]
 
     def payload(self) -> bytes:
         return bytes(self.data[: self.nbits // 8])
@@ -31,7 +48,7 @@ class Stats(C.Structure):
     _fields_ = [("samples_in", C.c_uint64), ("candidates", C.c_uint64), ("candidates_real", C.c_uint64),
                 ("detections", C.c_uint64), ("frames_passed", C.c_uint64), ("kernel_launches", C.c_uint64),
                 ("ms_scan", C.c_float), ("ms_total", C.c_float), ("resolver_fallback", C.c_int),
-                ("reserved_", C.c_int)]
+                ("ec_fixed", C.c_int)]
 
 
 class Geometry(C.Structure):

@@ -155,6 +155,7 @@ class _Context:
                                    int(bool(use_dcblock)), C.byref(h)))
         self._h = h
         self.device = int(device)
+        self.ec = 0                 # option "ec" as last set (the library keeps it; there is no getter in the C ABI)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -219,12 +220,25 @@ def format_message(frame: Frame, first: bool) -> str:
 
 
 class slicer:
-    """air_modes.slicer(queue): turns 240-chip packets into queue messages (slicer_impl.cc:102-198)."""
+    """air_modes.slicer(queue): turns 240-chip packets into queue messages (slicer_impl.cc:102-198).
 
-    def __init__(self, queue, device: int = 0, _ctx: _Context | None = None):
+    ec=K (1..23, extension; default 0 = off, the reference's behaviour): DF11/DF17 packets that fail only their CRC
+    are corrected over at most K low-confidence bits when exactly one set of flips fits (see amb_frame.ec)."""
+
+    def __init__(self, queue, device: int = 0, _ctx: _Context | None = None, ec: int = 0):
         self._queue = queue
         self._ctx = _ctx or _Context(4e6, 7.0, False, False, device)
         self._first = True          # d_payload precision: 6 until the first message (slicer_impl.cc:192)
+        if ec:
+            self.set_ec(ec)
+
+    def set_ec(self, k: int):
+        """Error correction over at most k low-confidence bits (0 = off); takes effect at the next call."""
+        self._ctx.call("amb_set_option", b"ec", int(k))
+        self._ctx.ec = int(k)
+
+    def get_ec(self) -> int:
+        return self._ctx.ec
 
     def emit(self, frames, n: int | None = None) -> int:
         """Queue one message per frame that passed the slicer rules (slicer_impl.cc:186-194). Returns how many.
@@ -303,16 +317,20 @@ class rx_path:
 
     A sink of gr_complex: feed it with process(iq) (numpy complex64 / interleaved float32 on the host, or a
     torch CUDA tensor that is read in place). Decoded frames are pushed to `queue` as the reference's
-    ASCII messages."""
+    ASCII messages.
 
-    def __init__(self, rate, threshold, queue, use_pmf=False, use_dcblock=False, device: int = 0):
+    ec=K (extension, default 0 = off): error correction over at most K (1..23) low-confidence bits of the DF11/DF17
+    frames the reference drops for their CRC (slicer_impl.cc:182); a frame with exactly one fitting set of flips becomes
+    an ordinary message with crc token 000000. Frames record the outcome in .ec / .ec_flips."""
+
+    def __init__(self, rate, threshold, queue, use_pmf=False, use_dcblock=False, device: int = 0, ec: int = 0):
         self._rate = int(rate)                      # rx_path.py:32
         self._threshold = threshold
         self._queue = queue
         self._spc = int(rate / 2e6)                 # rx_path.py:35
         self._use_pmf = bool(use_pmf)
         self._ctx = _Context(rate, threshold, use_pmf, use_dcblock, device)
-        self._slicer = slicer(queue, device, _ctx=self._ctx)
+        self._slicer = slicer(queue, device, _ctx=self._ctx, ec=ec)
         self.frames = []                            # every detection of the last process() call
         self._keep = []                             # device inputs still being read
 
@@ -338,6 +356,13 @@ class rx_path:
 
     def get_threshold(self):
         return float(self._ctx._lib.amb_get_threshold(self._ctx._h))
+
+    # -- extension: error correction (see the class docstring); persists across reset() and set_rate()
+    def set_ec(self, k: int):
+        self._slicer.set_ec(k)
+
+    def get_ec(self) -> int:
+        return self._slicer.get_ec()
 
     # -- data path
     def process(self, iq, flush: bool = False, collect: bool = True) -> int:
@@ -409,7 +434,9 @@ class rx_path:
 
     def set_option(self, name: str, value: int):
         """Library options: "coalesce", "ingest_chunk", "copy_threads", "resolver", "overlap", "keep_chips", "exact_dense",
-        "scan_ctas", "order_tile"."""
+        "scan_ctas", "order_tile", "ec"."""
+        if name == "ec":
+            return self.set_ec(value)
         self._ctx.call("amb_set_option", name.encode(), int(value))
 
     def reset(self):

@@ -102,6 +102,7 @@ struct amb_ctx {
     cudaEvent_t ring_done[64] = {};      // ... and the end of the same calls' sparse stages (stream B)
     unsigned ring_n = 0;
     int resolver = 0;
+    int ec = 0;                          // option "ec": error correction over up to K low-confidence bits (0 = off)
     // time-sharded operation (amb_seek / amb_resolve): a call whose walk + slice stages are still to run
     int defer = 0;                       // option "defer_resolve"
     int def_kind = 0;                    // 0 nothing pending, 1 full (walk + slice), 2 sequential walk only, 3 state only
@@ -403,6 +404,7 @@ int amb_set_option(amb_ctx* ctx, const char* name, int value)
 {
     if (!ctx || !name) return AMB_ERR_INVALID;
     if (!strcmp(name, "resolver")) { ctx->resolver = value; return AMB_OK; }
+    if (!strcmp(name, "ec")) { if (value < 0 || value > 23) return AMB_ERR_INVALID; ctx->ec = value; return AMB_OK; }
     if (!strcmp(name, "keep_chips")) { ctx->keep_chips = value != 0; return AMB_OK; }
     if (!strcmp(name, "overlap")) { ctx->overlap = value != 0; return AMB_OK; }
     if (!strcmp(name, "coalesce")) {                       // samples of small host calls gathered before a dispatch
@@ -503,6 +505,28 @@ static int ensure_call_buffers(amb_ctx* ctx, size_t rows_need, int n_spans, unsi
     }
     if (ctx->keep_chips && !ctx->chips) CK(cudaMalloc(&ctx->chips, (size_t)ctx->frame_cap * 240 * sizeof(float)));
     return AMB_OK;
+}
+
+// The slicer stage of every path: slice, then - with option "ec" on - correct the frames it dropped for their CRC, in
+// place. Everything that reads frames or the call's counters (polls, drain, walk summaries, completion events) is
+// enqueued after this on the same stream.
+static cudaError_t launch_ec_if_on(amb_ctx* ctx, amb_frame* frames, unsigned frame_cap, AmbCounters* ctr, int n, cudaStream_t s)
+{
+    if (!ctx->ec) return cudaSuccess;
+    ctx->stats.kernel_launches += 1;
+    return amb_launch_ec(frames, frame_cap, ctr, n, ctx->ec, ctx->sm_count, s);
+}
+static cudaError_t slice_and_correct(amb_ctx* ctx, const AmbSliceArgs& sl, cudaStream_t s)
+{
+    cudaError_t e = amb_launch_slice(sl, ctx->sm_count, s);
+    if (e == cudaSuccess) e = launch_ec_if_on(ctx, sl.frames, sl.frame_cap, sl.ctr, 0, s);
+    return e;
+}
+static cudaError_t slice_chips_and_correct(amb_ctx* ctx, const float* chips, int ndet, amb_frame* frames, cudaStream_t s)
+{
+    cudaError_t e = amb_launch_slice_chips(chips, ndet, frames, s);
+    if (e == cudaSuccess) e = launch_ec_if_on(ctx, frames, (unsigned)ndet, nullptr, ndet, s);
+    return e;
 }
 
 // One call of the chain over n_complex samples that are in DEVICE memory (or, mem_kind == AMB_MEM_HOST, in host
@@ -643,7 +667,7 @@ static int process_core(amb_ctx* ctx, const float* iq, size_t n_complex, int mem
         } else {
             if (!par) { CK(amb_launch_walk_seq(wa, sb)); ctx->stats.kernel_launches += 1; }
             else { CK(amb_launch_walk_par(wa, ctx->walk_scratch, ctx->cand_cap, (long long)S.n_carry + S.n_main + S.n_tail, sb)); ctx->stats.kernel_launches += 3; }
-            CK(amb_launch_slice(sl, ctx->sm_count, sb));
+            CK(slice_and_correct(ctx, sl, sb));
             ctx->stats.kernel_launches += 5;
         }
         ctx->ev_valid = ctx->timing;
@@ -974,7 +998,7 @@ int amb_resolve(amb_ctx* ctx, const amb_walk_state* entry)
     if (ctx->def_kind == 1) {
         if (!ctx->def_par) { CK(amb_launch_walk_seq(ctx->def_wa, sb)); ctx->stats.kernel_launches += 1; }
         else { CK(amb_launch_walk_par(ctx->def_wa, ctx->walk_scratch, ctx->cand_cap, ctx->def_nsamp, sb)); ctx->stats.kernel_launches += 3; }
-        CK(amb_launch_slice(ctx->def_sl, ctx->sm_count, sb));
+        CK(slice_and_correct(ctx, ctx->def_sl, sb));
         ctx->stats.kernel_launches += 1;
     } else if (ctx->def_kind == 2) {
         CK(amb_launch_walk_seq(ctx->def_wa, sb));
@@ -1067,7 +1091,7 @@ int amb_resolve_device(amb_ctx* ctx, const int64_t* entry_dev, void* after_strea
     if (ctx->def_kind == 1) {
         if (!ctx->def_par) { CK(amb_launch_walk_seq(ctx->def_wa, sb)); ctx->stats.kernel_launches += 1; }
         else { CK(amb_launch_walk_par(ctx->def_wa, ctx->walk_scratch, ctx->cand_cap, ctx->def_nsamp, sb)); ctx->stats.kernel_launches += 3; }
-        CK(amb_launch_slice(ctx->def_sl, ctx->sm_count, sb));
+        CK(slice_and_correct(ctx, ctx->def_sl, sb));
         ctx->stats.kernel_launches += 1;
     } else if (ctx->def_kind == 2) {
         CK(amb_launch_walk_seq(ctx->def_wa, sb));
@@ -1140,6 +1164,7 @@ static int collect_sync(amb_ctx* ctx, AmbCounters* h)
     ctx->stats.candidates_real = h->nreal_call;
     ctx->stats.detections = h->ndet_call;
     ctx->stats.frames_passed = h->npassed_call;
+    ctx->stats.ec_fixed = (int)h->nec_fixed;
     if (h->overflow) return fail(ctx, AMB_ERR_OVERFLOW, "candidate buffer overflow");
     if (h->frame_overflow) return fail(ctx, AMB_ERR_OVERFLOW, "frame buffer overflow");
     return AMB_OK;
@@ -1282,6 +1307,7 @@ int amb_get_stats(amb_ctx* ctx, amb_stats* out)
     ctx->stats.candidates_real = h.nreal_call;
     ctx->stats.detections = h.ndet_call;
     ctx->stats.frames_passed = h.npassed_call;
+    ctx->stats.ec_fixed = (int)h.nec_fixed;
     ctx->stats.resolver_fallback = st.fallback;
     if (ctx->timing) {
         float ms = 0.f;
@@ -1471,7 +1497,7 @@ int amb_slicer_process(amb_ctx* ctx, const float* chips, int ndet, const uint64_
     CK(cudaMalloc(&f, (size_t)ndet * sizeof(amb_frame)));
     cudaError_t e = cudaMemsetAsync(f, 0, (size_t)ndet * sizeof(amb_frame), ctx->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d, chips, (size_t)ndet * 240 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = amb_launch_slice_chips(d, ndet, f, ctx->stream);
+    if (e == cudaSuccess) e = slice_chips_and_correct(ctx, d, ndet, f, ctx->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(out, f, (size_t)ndet * sizeof(amb_frame), cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
     cudaFree(d); cudaFree(f);
@@ -1552,7 +1578,7 @@ int amb_preamble_process(amb_ctx* ctx, const float* in0, const float* in1, size_
         sl.det_list = ctx->det_list;
         sl.frames = ctx->frames; sl.frame_cap = ctx->frame_cap; sl.chips_out = ctx->chips; sl.org = b0;
         sl.in0 = d0; sl.in1 = d1; sl.n_streams = (long long)m;
-        if (e == cudaSuccess) e = amb_launch_slice(sl, ctx->sm_count, s);
+        if (e == cudaSuccess) e = slice_and_correct(ctx, sl, s);
         if (e == cudaSuccess) e = cudaStreamSynchronize(s);
         ctx->stats.kernel_launches += 8;
         if (e != cudaSuccess) { rc = fail(ctx, AMB_ERR_CUDA, "amb_preamble_process", e); break; }

@@ -64,6 +64,7 @@ struct AmbCounters {
     unsigned int nreal_call;
     unsigned int ndet_list;    // entries of the detection list of this call (indices into the candidate arrays)
     unsigned int frame_base;   // frames queued before this call's (set by the resolver; slot = frame_base + list position)
+    unsigned int nec_fixed;    // frames of this call the error correction fixed (also counted in npassed_call)
 };
 
 struct AmbScanArgs {
@@ -130,6 +131,10 @@ cudaError_t amb_launch_carry(const AmbSegs& S, float2* dst, int kc, cudaStream_t
 cudaError_t amb_launch_stream_candidates(const AmbScanArgs& a, const float* in0, const float* in1, long long n, int sm_count,
                                          cudaStream_t s);
 cudaError_t amb_launch_slice_chips(const float* chips, int ndet, amb_frame* frames, cudaStream_t s);
+// error correction of the frames a slice kernel just wrote: ctr != nullptr: the call's slots [frame_base, frame_base +
+// ndet_list) below frame_cap, counted into ctr; ctr == nullptr: frames [0, n)
+cudaError_t amb_launch_ec(amb_frame* frames, unsigned int frame_cap, AmbCounters* ctr, int n, int k_max, int sm_count,
+                          cudaStream_t s);
 cudaError_t amb_launch_crc(const uint8_t* data, int n, int length, uint32_t* out, cudaStream_t s);
 cudaError_t amb_upload_tables(const int* chip_off);
 cudaError_t amb_prefer_max_shared();

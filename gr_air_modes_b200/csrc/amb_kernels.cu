@@ -519,7 +519,9 @@ __global__ void __launch_bounds__(128) amb_compact_kernel(const __grid_constant_
 {
     // per-call resets of what the later kernels of this call accumulate into
     for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < n_scratch64; k += gridDim.x * blockDim.x) scratch64[k] = 0ull;
-    if (blockIdx.x == 0 && threadIdx.x == 0) { ctr->ndet_call = 0; ctr->npassed_call = 0; ctr->nreal_call = 0; ctr->ndet_list = 0; }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        ctr->ndet_call = 0; ctr->npassed_call = 0; ctr->nreal_call = 0; ctr->ndet_list = 0; ctr->nec_fixed = 0;
+    }
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int span = blockIdx.x * 4 + warp;
     if (span >= a.n_spans) return;
@@ -1378,6 +1380,7 @@ __global__ void amb_walk_reset_kernel(const AmbWalkArgs a, unsigned long long* s
     for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < n64; k += gridDim.x * blockDim.x) scratch64[k] = 0ull;
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         a.ctr->ndet_call = 0; a.ctr->npassed_call = 0; a.ctr->nreal_call = 0; a.ctr->ndet_list = 0; a.ctr->nframes = 0;
+        a.ctr->nec_fixed = 0;
         a.st->done = 0; a.st->fallback = 0;
     }
 }
@@ -1561,7 +1564,9 @@ __device__ __forceinline__ bool slice_packet_warp(float p0, float p2, float p7, 
             before += __popc(lw[k]);
         }
     }
-    if (lane >= 24 && lane < 30) f->pad_[lane - 24] = 0;
+    if (lane == 24) f->ec = 0;                                                // the error correction fills these (amb_ec_kernel)
+    if (lane == 25) f->ec_flips = 0;
+    if (lane >= 26 && lane < 30) f->pad_[lane - 26] = 0;
     if (lane == 31) {
         f->ref_level = ref;
         f->crc = syn;
@@ -1723,6 +1728,91 @@ cudaError_t amb_launch_slice_chips(const float* chips, int ndet, amb_frame* fram
     if (ndet <= 0) return cudaSuccess;
     int blocks = (ndet + 3) / 4; if (blocks > 2048) blocks = 2048;
     AMB_LAUNCH((amb_slice_chips_kernel), blocks, 128, 0, s, chips, ndet, frames);
+    return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------------
+// error correction (option "ec" = K, off by default): the frames slicer_impl.cc:182 drops - passed == 0 with crc != 0,
+// i.e. DF11 / DF17 with a non-zero syndrome - are searched for the subsets S of their low-confidence bits L
+// (lowconfbits minus the DF field, bits 0-4) whose flips zero the syndrome. The syndrome is linear over GF(2): flipping
+// message bit j XORs crc_rem[nbits-25-j] into it, flipping parity bit j XORs 1 << (nbits-1-j). So instead of trying
+// 2^|L| subsets, a 24-step elimination spread over the warp decides the system: lane i holds the syndrome vector of
+// L[i] and the subset (a mask of lanes) it currently stands for, pivots travel by shuffle. The syndrome outside the span
+// of L: no solution; inside it with rank < |L|: several solutions; otherwise exactly one, which is applied.
+// A warp reads 32 frame headers, ballots the candidates and solves them one after the other (O(24 |L|) each).
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(64) amb_ec_kernel(amb_frame* __restrict__ frames, unsigned int frame_cap, AmbCounters* ctr,
+                                                    int n_host, int k_max)
+{
+    __shared__ unsigned int s_crc[96];
+    for (int i = threadIdx.x; i < 96; i += blockDim.x) s_crc[i] = c_crc_rem[i];
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    unsigned int base = 0, n = (unsigned)n_host;
+    if (ctr) {                                                 // this call's slots; those past the capacity were never written
+        base = ctr->frame_base;
+        n = base < frame_cap ? min(ctr->ndet_list, frame_cap - base) : 0u;
+    }
+    unsigned int nfixed = 0;
+    const unsigned int nwarps = gridDim.x * (blockDim.x >> 5);
+    for (unsigned int w0 = (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * 32u; w0 < n; w0 += nwarps * 32u) {
+        bool cand = false;
+        if (w0 + lane < n) { const amb_frame* f = frames + base + w0 + lane; cand = !f->passed && f->crc != 0u; }
+        unsigned int todo = __ballot_sync(FULL, cand);
+        while (todo) {                                         // warp-uniform from here on
+            amb_frame* f = frames + base + w0 + (__ffs(todo) - 1);
+            todo &= todo - 1u;
+            const unsigned nlow = f->numlowconf;
+            if (nlow > (unsigned)k_max) { if (lane == 0) f->ec = AMB_EC_TOO_MANY; continue; }
+            const int nbits = f->nbits;
+            const int pos = lane < (int)nlow ? (int)f->lowconfbits[lane] : 0;
+            const bool in_l = pos >= 5;                        // the DF field is never flipped
+            uint32_t v = 0u, m = in_l ? 1u << lane : 0u;
+            if (in_l) v = pos < nbits - 24 ? s_crc[nbits - 25 - pos] : 1u << (nbits - 1 - pos);
+            const int size_l = __popc(__ballot_sync(FULL, in_l));
+            uint32_t syn = f->crc, sol = 0u;
+            bool pivot = false;
+            int rank = 0;
+            for (int b = 23; b >= 0; b--) {
+                const unsigned int rows = __ballot_sync(FULL, !pivot && ((v >> b) & 1u));
+                if (!rows) continue;
+                const int p = __ffs(rows) - 1;
+                const uint32_t pv = __shfl_sync(FULL, v, p), pm = __shfl_sync(FULL, m, p);
+                if (lane == p) pivot = true;
+                else if ((v >> b) & 1u) { v ^= pv; m ^= pm; }
+                if ((syn >> b) & 1u) { syn ^= pv; sol ^= pm; }
+                rank++;
+            }
+            const unsigned status = syn ? AMB_EC_NO_SOLUTION : rank < size_l ? AMB_EC_AMBIGUOUS : AMB_EC_FIXED;
+            if (status != AMB_EC_FIXED) { if (lane == 0) f->ec = (uint8_t)status; continue; }
+            // flips as four MSB-first words of the packet (bit 31 of word k = bit 32k), OR-reduced over the lanes
+            const uint32_t bit = ((sol >> lane) & 1u) ? 1u << (31 - (pos & 31)) : 0u;
+            uint32_t x0 = (pos >> 5) == 0 ? bit : 0u, x1 = (pos >> 5) == 1 ? bit : 0u;
+            uint32_t x2 = (pos >> 5) == 2 ? bit : 0u, x3 = (pos >> 5) == 3 ? bit : 0u;
+#pragma unroll
+            for (int d = 16; d > 0; d >>= 1) {
+                x0 |= __shfl_xor_sync(FULL, x0, d); x1 |= __shfl_xor_sync(FULL, x1, d);
+                x2 |= __shfl_xor_sync(FULL, x2, d); x3 |= __shfl_xor_sync(FULL, x3, d);
+            }
+            if (lane < 14) {
+                const uint32_t w = lane < 4 ? x0 : lane < 8 ? x1 : lane < 12 ? x2 : x3;
+                f->data[lane] ^= (uint8_t)(w >> (24 - 8 * (lane & 3)));
+            }
+            if (lane == 31) {
+                f->crc = 0u; f->passed = 1;
+                f->ec = AMB_EC_FIXED; f->ec_flips = (uint8_t)__popc(sol);
+            }
+            nfixed++;
+        }
+    }
+    if (ctr && lane == 0 && nfixed) { atomicAdd(&ctr->npassed_call, nfixed); atomicAdd(&ctr->nec_fixed, nfixed); }
+}
+
+cudaError_t amb_launch_ec(amb_frame* frames, unsigned int frame_cap, AmbCounters* ctr, int n, int k_max, int sm_count,
+                          cudaStream_t s)
+{
+    if (!ctr && n <= 0) return cudaSuccess;
+    AMB_LAUNCH((amb_ec_kernel), sm_count > 0 ? sm_count : 8, 64, 0, s, frames, frame_cap, ctr, n, k_max);
     return cudaGetLastError();
 }
 
@@ -2074,6 +2164,7 @@ cudaError_t amb_prefer_max_shared()
     if (e == cudaSuccess) e = prefer_shared(amb_set_state_dev_kernel);
     if (e == cudaSuccess) e = prefer_shared(amb_slice_kernel<true, 0, false>);
     if (e == cudaSuccess) e = prefer_shared(amb_slice_chips_kernel);
+    if (e == cudaSuccess) e = prefer_shared(amb_ec_kernel);
     if (e == cudaSuccess) e = prefer_shared(amb_carry_kernel);
     if (e == cudaSuccess) e = prefer_shared(amb_prologue_kernel);
     if (e == cudaSuccess) e = prefer_shared(amb_widen_sc16_kernel);

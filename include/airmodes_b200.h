@@ -63,8 +63,20 @@ typedef struct amb_frame {
     uint8_t passed;
     uint8_t lowconfbits[24];
     uint8_t data[14];
-    uint8_t pad_[6];
+    uint8_t ec;              /* error correction outcome, AMB_EC_* (option "ec"); 0 unless it was attempted */
+    uint8_t ec_flips;        /* bits flipped by a correction (AMB_EC_FIXED), else 0 */
+    uint8_t pad_[4];
 } amb_frame;                 /* 80 bytes */
+
+/* amb_frame.ec: what the opt-in error correction (amb_set_option(ctx, "ec", K), K in 1..23) made of a DF11/DF17 frame
+ * that the reference drops for a non-zero CRC syndrome (slicer_impl.cc:182). It searches the frame's low-confidence
+ * bits (lowconfbits, minus the DF field 0-4) for the subsets whose flips zero the syndrome. Names after
+ * bruteResultTypeDef (include/gr_air_modes/types.h:27). */
+#define AMB_EC_NOT_TRIED 0       /* not a candidate, or the option is off */
+#define AMB_EC_FIXED 1           /* Solution_Found: exactly one subset; data corrected, crc = 0, passed = 1 */
+#define AMB_EC_TOO_MANY 2        /* Too_Many_LCBs: numlowconf > K (a saturated count of 24 always) */
+#define AMB_EC_NO_SOLUTION 3     /* No_Solution: no subset zeroes the syndrome */
+#define AMB_EC_AMBIGUOUS 4       /* Multiple_Solutions: more than one does; the frame stays dropped */
 
 typedef struct amb_stats {
     uint64_t samples_in;     /* complex samples accepted so far on this stream */
@@ -76,7 +88,7 @@ typedef struct amb_stats {
     float ms_scan;           /* device time of the streaming scan kernel, last call (timing on) */
     float ms_total;          /* device time of the whole call incl. copies on the ctx stream */
     int resolver_fallback;   /* 1 if the exact sequential resolver had to replace the parallel one */
-    int reserved_;
+    int ec_fixed;            /* frames the error correction fixed (last call; counted in frames_passed too) */
 } amb_stats;
 
 /* ---- lifetime -------------------------------------------------------------------------------
@@ -214,7 +226,9 @@ AMB_API int amb_wait_stream(amb_ctx* ctx, void* cuda_stream);
  * exact-stage verdict: bits 0-7 late shift, bit 8 passes preamble_impl.cc:174-179, bit 9 valid preamble
  * (:205-209), bit 10 visited-and-accepted. Returns count. */
 AMB_API int amb_debug_candidates(amb_ctx* ctx, uint64_t* index, uint32_t* info, int max);
-AMB_API int amb_set_option(amb_ctx* ctx, const char* name, int value); /* "resolver": 0 auto, 1 sequential, 2 parallel */
+/* "resolver": 0 auto, 1 sequential, 2 parallel. "ec": K = 0 (default, off) .. 23, error correction over the
+ * low-confidence bits of frames dropped for their CRC (see AMB_EC_*); persists across amb_reset / amb_set_rate. */
+AMB_API int amb_set_option(amb_ctx* ctx, const char* name, int value);
 /* Parity dump of the GNU Radio front end wired in rx_path.py:38-54, for a short HOST buffer taken as a whole stream
  * (zeros before sample 0): stage M2 = complex_to_mag_squared (:38), BB = the preamble block's in0 (PMF output, :48-51,
  * or m2 when the PMF is off), AVG = its in1 (:54). n_complex floats are written to `out` (2*n_complex for DC). The hot path never

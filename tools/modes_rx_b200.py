@@ -157,6 +157,8 @@ def main(argv=None):
     ap.add_argument("--chunk", type=int, default=1 << 24, help="complex samples per amb_process call")
     ap.add_argument("--udp-idle", type=float, default=2.0, help="end a UDP stream after this many idle seconds")
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--ec", type=int, default=0, metavar="K",
+                    help="correct DF11/DF17 frames over at most K (1..23) low-confidence bits; 0 = off, as the reference")
     args = ap.parse_args(argv)
 
     if args.source in ("uhd", "osmocom"):
@@ -190,7 +192,8 @@ def main(argv=None):
         from gr_air_modes_b200.zmq_pub import zmq_queue
         pub = zmq_queue(["tcp://*:%i" % args.tcp])
         sinks.append(pub)
-    rx = air_modes.rx_path(rx_rate, args.threshold, tee_queue(sinks), args.pmf, args.dcblock, device=args.device)   # radio.py:55-56
+    rx = air_modes.rx_path(rx_rate, args.threshold, tee_queue(sinks), args.pmf, args.dcblock, device=args.device,
+                           ec=args.ec)   # radio.py:55-56
 
     if ":" in args.source and not os.path.exists(args.source):
         m = re.search(r"(.*)\:(\d{1,5})$", args.source)                                                           # radio.py:223-226
