@@ -17,14 +17,15 @@ MEM_HOST, MEM_DEVICE, MEM_HOST_SC16, MEM_DEVICE_SC16 = 0, 1, 2, 3
 # amb_frame.ec (include/airmodes_b200.h AMB_EC_*)
 EC_NOT_TRIED, EC_FIXED, EC_TOO_MANY, EC_NO_SOLUTION, EC_AMBIGUOUS = 0, 1, 2, 3, 4
 EC_MAX = 23
+EC_ANY_MAX = 2              # option "ec_any": at most 2 flipped bits
 
 
 class Frame(C.Structure):
     """struct amb_frame (80 bytes) = modes_packet (types.h:29-41) + preamble tag.
 
-    The header's `ec` / `ec_flips` are the first two of the six tail bytes, which stay one `pad_` field here: the
-    record layout that numpy views and per-field dumps of frames see (np.dtype(Frame)) is the one the frame had before
-    error correction existed. They are read through the properties below."""
+    The header's `ec`, `ec_flips` and the first three bytes of its `pad_[4]` (AMB_FRAME_EC_ANY / AMB_FRAME_EC_ANY_BIT)
+    are the first five of the six tail bytes, which stay one `pad_` field here: the record layout that numpy views and per-field dumps of frames see (np.dtype(Frame)) is
+    the one the frame had before error correction existed. They are read through the properties below."""
     _fields_ = [("sample_index", C.c_uint64), ("secs", C.c_uint64), ("frac", C.c_double),
                 ("ref_level", C.c_float), ("crc", C.c_uint32), ("nbits", C.c_uint8), ("df", C.c_uint8),
                 ("numlowconf", C.c_uint8), ("passed", C.c_uint8), ("lowconfbits", C.c_uint8 * 24),
@@ -39,6 +40,16 @@ class Frame(C.Structure):
     def ec_flips(self) -> int:
         """amb_frame.ec_flips: bits the correction flipped (EC_FIXED), else 0."""
         return self.pad_[1]
+
+    @property
+    def ec_any(self) -> int:
+        """AMB_FRAME_EC_ANY (byte 76): outcome of the second pass (option "ec_any"): EC_NOT_TRIED, EC_FIXED or EC_NO_SOLUTION."""
+        return self.pad_[2]
+
+    @property
+    def ec_any_bits(self) -> tuple:
+        """AMB_FRAME_EC_ANY_BIT(f, 0..1) (bytes 77-78): the two positions that pass flipped, ascending; 0 = unused slot."""
+        return (self.pad_[3], self.pad_[4])
 
     def payload(self) -> bytes:
         return bytes(self.data[: self.nbits // 8])

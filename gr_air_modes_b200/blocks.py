@@ -156,6 +156,7 @@ class _Context:
         self._h = h
         self.device = int(device)
         self.ec = 0                 # option "ec" as last set (the library keeps it; there is no getter in the C ABI)
+        self.ec_any = 0             # option "ec_any", likewise
 
     def close(self):
         if getattr(self, "_h", None):
@@ -223,14 +224,18 @@ class slicer:
     """air_modes.slicer(queue): turns 240-chip packets into queue messages (slicer_impl.cc:102-198).
 
     ec=K (1..23, extension; default 0 = off, the reference's behaviour): DF11/DF17 packets that fail only their CRC
-    are corrected over at most K low-confidence bits when exactly one set of flips fits (see amb_frame.ec)."""
+    are corrected over at most K low-confidence bits when exactly one set of flips fits (see amb_frame.ec).
+    ec_any=M (1 or 2, extension; default 0 = off): DF17 packets still dropped for their CRC after that are corrected
+    by at most M flipped bits anywhere in 5..111, whatever their confidence (see AMB_FRAME_EC_ANY)."""
 
-    def __init__(self, queue, device: int = 0, _ctx: _Context | None = None, ec: int = 0):
+    def __init__(self, queue, device: int = 0, _ctx: _Context | None = None, ec: int = 0, ec_any: int = 0):
         self._queue = queue
         self._ctx = _ctx or _Context(4e6, 7.0, False, False, device)
         self._first = True          # d_payload precision: 6 until the first message (slicer_impl.cc:192)
         if ec:
             self.set_ec(ec)
+        if ec_any:
+            self.set_ec_any(ec_any)
 
     def set_ec(self, k: int):
         """Error correction over at most k low-confidence bits (0 = off); takes effect at the next call."""
@@ -239,6 +244,14 @@ class slicer:
 
     def get_ec(self) -> int:
         return self._ctx.ec
+
+    def set_ec_any(self, m: int):
+        """DF17 correction by at most m (1, 2) bits anywhere in 5..111 (0 = off); takes effect at the next call."""
+        self._ctx.call("amb_set_option", b"ec_any", int(m))
+        self._ctx.ec_any = int(m)
+
+    def get_ec_any(self) -> int:
+        return self._ctx.ec_any
 
     def emit(self, frames, n: int | None = None) -> int:
         """Queue one message per frame that passed the slicer rules (slicer_impl.cc:186-194). Returns how many.
@@ -321,16 +334,21 @@ class rx_path:
 
     ec=K (extension, default 0 = off): error correction over at most K (1..23) low-confidence bits of the DF11/DF17
     frames the reference drops for their CRC (slicer_impl.cc:182); a frame with exactly one fitting set of flips becomes
-    an ordinary message with crc token 000000. Frames record the outcome in .ec / .ec_flips."""
+    an ordinary message with crc token 000000. Frames record the outcome in .ec / .ec_flips.
 
-    def __init__(self, rate, threshold, queue, use_pmf=False, use_dcblock=False, device: int = 0, ec: int = 0):
+    ec_any=M (extension, default 0 = off): DF17 frames still dropped for their CRC after that are corrected by at most
+    M (1, 2) flipped bits anywhere in 5..111, whatever their confidence; the one- and two-bit fits are unique there.
+    Frames record the outcome in .ec_any / .ec_any_bits."""
+
+    def __init__(self, rate, threshold, queue, use_pmf=False, use_dcblock=False, device: int = 0, ec: int = 0,
+                 ec_any: int = 0):
         self._rate = int(rate)                      # rx_path.py:32
         self._threshold = threshold
         self._queue = queue
         self._spc = int(rate / 2e6)                 # rx_path.py:35
         self._use_pmf = bool(use_pmf)
         self._ctx = _Context(rate, threshold, use_pmf, use_dcblock, device)
-        self._slicer = slicer(queue, device, _ctx=self._ctx, ec=ec)
+        self._slicer = slicer(queue, device, _ctx=self._ctx, ec=ec, ec_any=ec_any)
         self.frames = []                            # every detection of the last process() call
         self._keep = []                             # device inputs still being read
 
@@ -363,6 +381,12 @@ class rx_path:
 
     def get_ec(self) -> int:
         return self._slicer.get_ec()
+
+    def set_ec_any(self, m: int):
+        self._slicer.set_ec_any(m)
+
+    def get_ec_any(self) -> int:
+        return self._slicer.get_ec_any()
 
     # -- data path
     def process(self, iq, flush: bool = False, collect: bool = True) -> int:
@@ -434,9 +458,11 @@ class rx_path:
 
     def set_option(self, name: str, value: int):
         """Library options: "coalesce", "ingest_chunk", "copy_threads", "resolver", "overlap", "keep_chips", "exact_dense",
-        "scan_ctas", "order_tile", "ec"."""
+        "scan_ctas", "order_tile", "ec", "ec_any"."""
         if name == "ec":
             return self.set_ec(value)
+        if name == "ec_any":
+            return self.set_ec_any(value)
         self._ctx.call("amb_set_option", name.encode(), int(value))
 
     def reset(self):

@@ -103,6 +103,7 @@ struct amb_ctx {
     unsigned ring_n = 0;
     int resolver = 0;
     int ec = 0;                          // option "ec": error correction over up to K low-confidence bits (0 = off)
+    int ec_any = 0;                      // option "ec_any": DF17 correction over up to M (1, 2) bits anywhere (0 = off)
     // time-sharded operation (amb_seek / amb_resolve): a call whose walk + slice stages are still to run
     int defer = 0;                       // option "defer_resolve"
     int def_kind = 0;                    // 0 nothing pending, 1 full (walk + slice), 2 sequential walk only, 3 state only
@@ -405,6 +406,7 @@ int amb_set_option(amb_ctx* ctx, const char* name, int value)
     if (!ctx || !name) return AMB_ERR_INVALID;
     if (!strcmp(name, "resolver")) { ctx->resolver = value; return AMB_OK; }
     if (!strcmp(name, "ec")) { if (value < 0 || value > 23) return AMB_ERR_INVALID; ctx->ec = value; return AMB_OK; }
+    if (!strcmp(name, "ec_any")) { if (value < 0 || value > 2) return AMB_ERR_INVALID; ctx->ec_any = value; return AMB_OK; }
     if (!strcmp(name, "keep_chips")) { ctx->keep_chips = value != 0; return AMB_OK; }
     if (!strcmp(name, "overlap")) { ctx->overlap = value != 0; return AMB_OK; }
     if (!strcmp(name, "coalesce")) {                       // samples of small host calls gathered before a dispatch
@@ -507,14 +509,14 @@ static int ensure_call_buffers(amb_ctx* ctx, size_t rows_need, int n_spans, unsi
     return AMB_OK;
 }
 
-// The slicer stage of every path: slice, then - with option "ec" on - correct the frames it dropped for their CRC, in
-// place. Everything that reads frames or the call's counters (polls, drain, walk summaries, completion events) is
+// The slicer stage of every path: slice, then - with option "ec" or "ec_any" on - correct the frames it dropped for
+// their CRC, in place (one launch for both passes). Everything that reads frames or the call's counters (polls, drain, walk summaries, completion events) is
 // enqueued after this on the same stream.
 static cudaError_t launch_ec_if_on(amb_ctx* ctx, amb_frame* frames, unsigned frame_cap, AmbCounters* ctr, int n, cudaStream_t s)
 {
-    if (!ctx->ec) return cudaSuccess;
+    if (!ctx->ec && !ctx->ec_any) return cudaSuccess;
     ctx->stats.kernel_launches += 1;
-    return amb_launch_ec(frames, frame_cap, ctr, n, ctx->ec, ctx->sm_count, s);
+    return amb_launch_ec(frames, frame_cap, ctr, n, ctx->ec, ctx->ec_any, ctx->sm_count, s);
 }
 static cudaError_t slice_and_correct(amb_ctx* ctx, const AmbSliceArgs& sl, cudaStream_t s)
 {

@@ -132,9 +132,10 @@ cudaError_t amb_launch_stream_candidates(const AmbScanArgs& a, const float* in0,
                                          cudaStream_t s);
 cudaError_t amb_launch_slice_chips(const float* chips, int ndet, amb_frame* frames, cudaStream_t s);
 // error correction of the frames a slice kernel just wrote: ctr != nullptr: the call's slots [frame_base, frame_base +
-// ndet_list) below frame_cap, counted into ctr; ctr == nullptr: frames [0, n)
-cudaError_t amb_launch_ec(amb_frame* frames, unsigned int frame_cap, AmbCounters* ctr, int n, int k_max, int sm_count,
-                          cudaStream_t s);
+// ndet_list) below frame_cap, counted into ctr; ctr == nullptr: frames [0, n). k_max: option "ec", m_any: option
+// "ec_any" (0 skips that pass)
+cudaError_t amb_launch_ec(amb_frame* frames, unsigned int frame_cap, AmbCounters* ctr, int n, int k_max, int m_any,
+                          int sm_count, cudaStream_t s);
 cudaError_t amb_launch_crc(const uint8_t* data, int n, int length, uint32_t* out, cudaStream_t s);
 cudaError_t amb_upload_tables(const int* chip_off);
 cudaError_t amb_prefer_max_shared();

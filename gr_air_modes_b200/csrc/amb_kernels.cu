@@ -1740,12 +1740,57 @@ cudaError_t amb_launch_slice_chips(const float* chips, int ndet, amb_frame* fram
 // L[i] and the subset (a mask of lanes) it currently stands for, pivots travel by shuffle. The syndrome outside the span
 // of L: no solution; inside it with rank < |L|: several solutions; otherwise exactly one, which is applied.
 // A warp reads 32 frame headers, ballots the candidates and solves them one after the other (O(24 |L|) each).
+//
+// Second phase (option "ec_any" = M in {1, 2}, off by default): a DF17 frame still dropped after the first phase is
+// searched for the patterns of at most M bits anywhere in 5..111 whose flips zero the syndrome, whatever their
+// confidence. The 107 one-bit syndromes s_i and the 5,671 two-bit syndromes s_i ^ s_j are non-zero and pairwise
+// distinct over these positions, so a fit is unique when it exists. Lane l owns positions 5+l, 37+l, 69+l, 101+l: it
+// tests syn == s_i, and looks syn ^ s_i up in a CTA-wide hash of (s_j -> j) for a partner j > i. DF11 is left alone:
+// its parity carries the interrogator code (II/SI) on top of the CRC, so a small syndrome is often not an error.
 // ------------------------------------------------------------------------------------------------
+constexpr int EC_HASH = 512;                                   // slots of the (s_j -> j) table: 107 keys, load 0.21
+__device__ __forceinline__ unsigned ec_hash(uint32_t s) { return (s * 0x9E3779B1u) >> 23; }
+__device__ __forceinline__ uint32_t ec_bit_syndrome(const unsigned int* s_crc, int i)   // a 112-bit frame's bit i
+{
+    return i < 88 ? s_crc[87 - i] : 1u << (111 - i);
+}
+
+// XOR the flips into f->data: each lane contributes the bits of its four MSB-first words of the packet (bit 31 of word
+// k = bit 32k); they are OR-reduced over the warp.
+__device__ __forceinline__ void ec_apply_flips(amb_frame* f, int lane, uint32_t x0, uint32_t x1, uint32_t x2, uint32_t x3)
+{
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        x0 |= __shfl_xor_sync(FULL, x0, d); x1 |= __shfl_xor_sync(FULL, x1, d);
+        x2 |= __shfl_xor_sync(FULL, x2, d); x3 |= __shfl_xor_sync(FULL, x3, d);
+    }
+    if (lane < 14) {
+        const uint32_t w = lane < 4 ? x0 : lane < 8 ? x1 : lane < 12 ? x2 : x3;
+        f->data[lane] ^= (uint8_t)(w >> (24 - 8 * (lane & 3)));
+    }
+}
+__device__ __forceinline__ void ec_word_bit(int pos, uint32_t& x0, uint32_t& x1, uint32_t& x2, uint32_t& x3)
+{
+    const uint32_t bit = 1u << (31 - (pos & 31));
+    if ((pos >> 5) == 0) x0 |= bit; else if ((pos >> 5) == 1) x1 |= bit; else if ((pos >> 5) == 2) x2 |= bit; else x3 |= bit;
+}
+
 __global__ void __launch_bounds__(64) amb_ec_kernel(amb_frame* __restrict__ frames, unsigned int frame_cap, AmbCounters* ctr,
-                                                    int n_host, int k_max)
+                                                    int n_host, int k_max, int m_any)
 {
     __shared__ unsigned int s_crc[96];
+    __shared__ unsigned int s_hash[EC_HASH];                   // (s_j << 8) | j, 0 = empty (no s_j is 0); m_any == 2 only
     for (int i = threadIdx.x; i < 96; i += blockDim.x) s_crc[i] = c_crc_rem[i];
+    if (m_any > 1) for (int i = threadIdx.x; i < EC_HASH; i += blockDim.x) s_hash[i] = 0u;
+    __syncthreads();
+    if (m_any > 1 && threadIdx.x == 0) {                       // linear probing, once per CTA
+        for (int j = 5; j < 112; j++) {
+            const uint32_t s = ec_bit_syndrome(s_crc, j);
+            unsigned h = ec_hash(s);
+            while (s_hash[h]) h = (h + 1) & (EC_HASH - 1);
+            s_hash[h] = (s << 8) | (unsigned)j;
+        }
+    }
     __syncthreads();
     const int lane = threadIdx.x & 31;
     unsigned int base = 0, n = (unsigned)n_host;
@@ -1762,45 +1807,79 @@ __global__ void __launch_bounds__(64) amb_ec_kernel(amb_frame* __restrict__ fram
         while (todo) {                                         // warp-uniform from here on
             amb_frame* f = frames + base + w0 + (__ffs(todo) - 1);
             todo &= todo - 1u;
-            const unsigned nlow = f->numlowconf;
-            if (nlow > (unsigned)k_max) { if (lane == 0) f->ec = AMB_EC_TOO_MANY; continue; }
-            const int nbits = f->nbits;
-            const int pos = lane < (int)nlow ? (int)f->lowconfbits[lane] : 0;
-            const bool in_l = pos >= 5;                        // the DF field is never flipped
-            uint32_t v = 0u, m = in_l ? 1u << lane : 0u;
-            if (in_l) v = pos < nbits - 24 ? s_crc[nbits - 25 - pos] : 1u << (nbits - 1 - pos);
-            const int size_l = __popc(__ballot_sync(FULL, in_l));
-            uint32_t syn = f->crc, sol = 0u;
-            bool pivot = false;
-            int rank = 0;
-            for (int b = 23; b >= 0; b--) {
-                const unsigned int rows = __ballot_sync(FULL, !pivot && ((v >> b) & 1u));
-                if (!rows) continue;
-                const int p = __ffs(rows) - 1;
-                const uint32_t pv = __shfl_sync(FULL, v, p), pm = __shfl_sync(FULL, m, p);
-                if (lane == p) pivot = true;
-                else if ((v >> b) & 1u) { v ^= pv; m ^= pm; }
-                if ((syn >> b) & 1u) { syn ^= pv; sol ^= pm; }
-                rank++;
+            const uint32_t syn0 = f->crc;
+            if (k_max > 0) {                                   // first phase: the low-confidence bits
+                const unsigned nlow = f->numlowconf;
+                unsigned status = AMB_EC_TOO_MANY;
+                if (nlow <= (unsigned)k_max) {
+                    const int nbits = f->nbits;
+                    const int pos = lane < (int)nlow ? (int)f->lowconfbits[lane] : 0;
+                    const bool in_l = pos >= 5;                // the DF field is never flipped
+                    uint32_t v = 0u, m = in_l ? 1u << lane : 0u;
+                    if (in_l) v = pos < nbits - 24 ? s_crc[nbits - 25 - pos] : 1u << (nbits - 1 - pos);
+                    const int size_l = __popc(__ballot_sync(FULL, in_l));
+                    uint32_t syn = syn0, sol = 0u;
+                    bool pivot = false;
+                    int rank = 0;
+                    for (int b = 23; b >= 0; b--) {
+                        const unsigned int rows = __ballot_sync(FULL, !pivot && ((v >> b) & 1u));
+                        if (!rows) continue;
+                        const int p = __ffs(rows) - 1;
+                        const uint32_t pv = __shfl_sync(FULL, v, p), pm = __shfl_sync(FULL, m, p);
+                        if (lane == p) pivot = true;
+                        else if ((v >> b) & 1u) { v ^= pv; m ^= pm; }
+                        if ((syn >> b) & 1u) { syn ^= pv; sol ^= pm; }
+                        rank++;
+                    }
+                    status = syn ? AMB_EC_NO_SOLUTION : rank < size_l ? AMB_EC_AMBIGUOUS : AMB_EC_FIXED;
+                    if (status == AMB_EC_FIXED) {
+                        uint32_t x0 = 0u, x1 = 0u, x2 = 0u, x3 = 0u;
+                        if ((sol >> lane) & 1u) ec_word_bit(pos, x0, x1, x2, x3);
+                        ec_apply_flips(f, lane, x0, x1, x2, x3);
+                        if (lane == 31) {
+                            f->crc = 0u; f->passed = 1;
+                            f->ec = AMB_EC_FIXED; f->ec_flips = (uint8_t)__popc(sol);
+                        }
+                        nfixed++;
+                        continue;                              // a frame the first phase fixed is not tried again
+                    }
+                }
+                if (lane == 0) f->ec = (uint8_t)status;
             }
-            const unsigned status = syn ? AMB_EC_NO_SOLUTION : rank < size_l ? AMB_EC_AMBIGUOUS : AMB_EC_FIXED;
-            if (status != AMB_EC_FIXED) { if (lane == 0) f->ec = (uint8_t)status; continue; }
-            // flips as four MSB-first words of the packet (bit 31 of word k = bit 32k), OR-reduced over the lanes
-            const uint32_t bit = ((sol >> lane) & 1u) ? 1u << (31 - (pos & 31)) : 0u;
-            uint32_t x0 = (pos >> 5) == 0 ? bit : 0u, x1 = (pos >> 5) == 1 ? bit : 0u;
-            uint32_t x2 = (pos >> 5) == 2 ? bit : 0u, x3 = (pos >> 5) == 3 ? bit : 0u;
+            if (m_any <= 0 || f->df != 17) continue;
+            // second phase: every pattern of at most m_any bits in 5..111
+            int i1 = 0, j1 = 0;                                // this lane's fit: position(s), 0 = none
+            int nfit = 0;
 #pragma unroll
-            for (int d = 16; d > 0; d >>= 1) {
-                x0 |= __shfl_xor_sync(FULL, x0, d); x1 |= __shfl_xor_sync(FULL, x1, d);
-                x2 |= __shfl_xor_sync(FULL, x2, d); x3 |= __shfl_xor_sync(FULL, x3, d);
+            for (int q = 0; q < 4; q++) {
+                const int i = 5 + lane + 32 * q;
+                if (i >= 112) break;
+                const uint32_t si = ec_bit_syndrome(s_crc, i);
+                if (si == syn0) { i1 = i; j1 = 0; nfit++; }
+                if (m_any > 1) {
+                    const uint32_t want = syn0 ^ si;
+                    for (unsigned h = ec_hash(want);; h = (h + 1) & (EC_HASH - 1)) {
+                        const uint32_t e = s_hash[h];
+                        if (!e) break;
+                        if ((e >> 8) == want) {
+                            if ((int)(e & 0xFFu) > i) { i1 = i; j1 = (int)(e & 0xFFu); nfit++; }
+                            break;
+                        }
+                    }
+                }
             }
-            if (lane < 14) {
-                const uint32_t w = lane < 4 ? x0 : lane < 8 ? x1 : lane < 12 ? x2 : x3;
-                f->data[lane] ^= (uint8_t)(w >> (24 - 8 * (lane & 3)));
+            const unsigned fit_lanes = __ballot_sync(FULL, nfit > 0);
+            if (__popc(fit_lanes) != 1 || __any_sync(FULL, nfit > 1)) {          // none, or (never seen) not unique
+                if (lane == 0) AMB_FRAME_EC_ANY(f) = AMB_EC_NO_SOLUTION;
+                continue;
             }
-            if (lane == 31) {
+            uint32_t x0 = 0u, x1 = 0u, x2 = 0u, x3 = 0u;
+            if (nfit) { ec_word_bit(i1, x0, x1, x2, x3); if (j1) ec_word_bit(j1, x0, x1, x2, x3); }
+            ec_apply_flips(f, lane, x0, x1, x2, x3);
+            if (lane == __ffs(fit_lanes) - 1) {
                 f->crc = 0u; f->passed = 1;
-                f->ec = AMB_EC_FIXED; f->ec_flips = (uint8_t)__popc(sol);
+                AMB_FRAME_EC_ANY(f) = AMB_EC_FIXED;
+                AMB_FRAME_EC_ANY_BIT(f, 0) = (uint8_t)i1; AMB_FRAME_EC_ANY_BIT(f, 1) = (uint8_t)j1;
             }
             nfixed++;
         }
@@ -1808,11 +1887,11 @@ __global__ void __launch_bounds__(64) amb_ec_kernel(amb_frame* __restrict__ fram
     if (ctr && lane == 0 && nfixed) { atomicAdd(&ctr->npassed_call, nfixed); atomicAdd(&ctr->nec_fixed, nfixed); }
 }
 
-cudaError_t amb_launch_ec(amb_frame* frames, unsigned int frame_cap, AmbCounters* ctr, int n, int k_max, int sm_count,
-                          cudaStream_t s)
+cudaError_t amb_launch_ec(amb_frame* frames, unsigned int frame_cap, AmbCounters* ctr, int n, int k_max, int m_any,
+                          int sm_count, cudaStream_t s)
 {
     if (!ctr && n <= 0) return cudaSuccess;
-    AMB_LAUNCH((amb_ec_kernel), sm_count > 0 ? sm_count : 8, 64, 0, s, frames, frame_cap, ctr, n, k_max);
+    AMB_LAUNCH((amb_ec_kernel), sm_count > 0 ? sm_count : 8, 64, 0, s, frames, frame_cap, ctr, n, k_max, m_any);
     return cudaGetLastError();
 }
 

@@ -4,7 +4,8 @@
     air_modes.preamble(channel_rate, threshold_db)                    preamble.h:36-45          -> preamble (2 x float in, float out)
     air_modes.slicer(queue)                                           slicer.h:37-42            -> slicer (sink of float)
 
-rx_path and slicer also take ec=K (default 0 = off): error correction over low-confidence bits (blocks.rx_path).
+rx_path and slicer also take ec=K (default 0 = off): error correction over low-confidence bits, and ec_any=M (default
+0 = off): DF17 correction by at most M bits anywhere (blocks.rx_path).
 
 Importable only where gnuradio (and its pmt) is installed; radio.py:55-56,73-76 keep working:
 `self.connect(source, rx_path(rate, threshold, queue, pmf, dcblock))`, and so does the reference's own wiring of the
@@ -24,10 +25,12 @@ from . import blocks
 
 
 class rx_path(gr.sync_block):
-    def __init__(self, rate, threshold, queue, use_pmf=False, use_dcblock=False, device=0, ec=0):
+    def __init__(self, rate, threshold, queue, use_pmf=False, use_dcblock=False, device=0, ec=0, ec_any=0):
         gr.sync_block.__init__(self, "modes_rx_path_b200", in_sig=[np.complex64], out_sig=None)
-        self._impl = blocks.rx_path(rate, threshold, queue, use_pmf, use_dcblock, device=device, ec=ec)
-        for name in ("set_rate", "set_threshold", "set_pmf", "get_pmf", "get_threshold", "set_ec", "get_ec"):
+        self._impl = blocks.rx_path(rate, threshold, queue, use_pmf, use_dcblock, device=device, ec=ec,
+                                    ec_any=ec_any)
+        for name in ("set_rate", "set_threshold", "set_pmf", "get_pmf", "get_threshold", "set_ec", "get_ec",
+                     "set_ec_any", "get_ec_any"):
             setattr(self, name, getattr(self._impl, name))
         self._open = False
 
@@ -109,10 +112,11 @@ class preamble(gr.basic_block):
 class slicer(gr.sync_block):
     """Sink of the preamble block's stream: 240 chips per `preamble_found` tag -> queue messages (slicer_impl.cc:102-198)."""
 
-    def __init__(self, queue, device=0, ec=0):
+    def __init__(self, queue, device=0, ec=0, ec_any=0):
         gr.sync_block.__init__(self, "modes_slicer_b200", in_sig=[np.float32], out_sig=None)
-        self._impl = blocks.slicer(queue, device=device, ec=ec)
+        self._impl = blocks.slicer(queue, device=device, ec=ec, ec_any=ec_any)
         self.set_ec, self.get_ec = self._impl.set_ec, self._impl.get_ec
+        self.set_ec_any, self.get_ec_any = self._impl.set_ec_any, self._impl.get_ec_any
         self.set_output_multiple(240)
 
     def work(self, input_items, output_items):

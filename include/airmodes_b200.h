@@ -65,7 +65,7 @@ typedef struct amb_frame {
     uint8_t data[14];
     uint8_t ec;              /* error correction outcome, AMB_EC_* (option "ec"); 0 unless it was attempted */
     uint8_t ec_flips;        /* bits flipped by a correction (AMB_EC_FIXED), else 0 */
-    uint8_t pad_[4];
+    uint8_t pad_[4];         /* [0] ec_any, [1..2] ec_any_bits (option "ec_any", read through AMB_FRAME_EC_ANY*), [3] 0 */
 } amb_frame;                 /* 80 bytes */
 
 /* amb_frame.ec: what the opt-in error correction (amb_set_option(ctx, "ec", K), K in 1..23) made of a DF11/DF17 frame
@@ -77,6 +77,16 @@ typedef struct amb_frame {
 #define AMB_EC_TOO_MANY 2        /* Too_Many_LCBs: numlowconf > K (a saturated count of 24 always) */
 #define AMB_EC_NO_SOLUTION 3     /* No_Solution: no subset zeroes the syndrome */
 #define AMB_EC_AMBIGUOUS 4       /* Multiple_Solutions: more than one does; the frame stays dropped */
+
+/* ec_any: what the opt-in second pass (amb_set_option(ctx, "ec_any", M), M in 1..2) made of a DF17 frame still
+ * dropped for its CRC after the "ec" pass (when that is on too). It searches every pattern of at most M bits in
+ * positions 5..111, whatever their confidence. The one- and two-bit syndromes there are non-zero and pairwise
+ * distinct, so a fit is unique: AMB_EC_FIXED (data corrected, crc = 0, passed = 1, bits recorded) or
+ * AMB_EC_NO_SOLUTION; AMB_EC_NOT_TRIED otherwise. DF11 is never tried: its parity may carry the interrogator's II/SI
+ * code. The outcome and the flipped positions live in the first three bytes of amb_frame.pad_ (bytes 76-78 of the
+ * frame), so the declared layout of amb_frame is the one it had before this pass existed: */
+#define AMB_FRAME_EC_ANY(f) ((f)->pad_[0])                  /* AMB_EC_NOT_TRIED, AMB_EC_FIXED or AMB_EC_NO_SOLUTION */
+#define AMB_FRAME_EC_ANY_BIT(f, i) ((f)->pad_[1 + (i)])     /* i = 0, 1: flipped positions, ascending; 0 = unused */
 
 typedef struct amb_stats {
     uint64_t samples_in;     /* complex samples accepted so far on this stream */
@@ -227,7 +237,9 @@ AMB_API int amb_wait_stream(amb_ctx* ctx, void* cuda_stream);
  * (:205-209), bit 10 visited-and-accepted. Returns count. */
 AMB_API int amb_debug_candidates(amb_ctx* ctx, uint64_t* index, uint32_t* info, int max);
 /* "resolver": 0 auto, 1 sequential, 2 parallel. "ec": K = 0 (default, off) .. 23, error correction over the
- * low-confidence bits of frames dropped for their CRC (see AMB_EC_*); persists across amb_reset / amb_set_rate. */
+ * low-confidence bits of frames dropped for their CRC (see AMB_EC_*); persists across amb_reset / amb_set_rate.
+ * "ec_any": M = 0 (default, off), 1 or 2, correction of DF17 frames by at most M flipped bits anywhere in 5..111, after
+ * "ec" (see amb_frame.ec_any); persists likewise. Both apply from the next call. */
 AMB_API int amb_set_option(amb_ctx* ctx, const char* name, int value);
 /* Parity dump of the GNU Radio front end wired in rx_path.py:38-54, for a short HOST buffer taken as a whole stream
  * (zeros before sample 0): stage M2 = complex_to_mag_squared (:38), BB = the preamble block's in0 (PMF output, :48-51,

@@ -1,17 +1,20 @@
-"""What the opt-in error correction (option "ec") adds on synthetic scenes, and what it costs.
+"""What the opt-in error correction (options "ec" and "ec_any") adds on synthetic scenes, and what it costs.
 
 For each scene (2^28 samples at 4 Msps: the configs[1] and configs[4] workloads of bench.py, and a low-SNR scene) and
-each K in {4, 8, 12} next to K = 0 (off), one pass of the chain over the device-resident recording reports:
+each setting - "ec" = K for K in --ks alone, "ec_any" = M for M in --ec-any alone, and "ec" = 8 with "ec_any" = 2 -
+next to both off, one pass of the chain over the device-resident recording reports:
   messages     frames queued (passed), corrections included
-  fixed        frames the correction fixed (amb_frame.ec == AMB_EC_FIXED)
-  true / false fixed frames whose corrected payload is / is not one of the frames the scene sent
+  fixed        frames a correction fixed, split by pass: fixed_ec (amb_frame.ec == AMB_EC_FIXED) and fixed_any
+               (AMB_FRAME_EC_ANY == AMB_EC_FIXED)
+  true / false fixed frames whose corrected payload is / is not one of the frames the scene generated, before or
+               after garbling
   ms_step      device time of one pass (CUDA events on the caller's stream, process -> join), median over the
-               steps; passes with the option off and on alternate in the same process
-The synthetic scenes garble bits BEFORE modulation, so those errors are high-confidence: the correction, which only
-flips low-confidence bits, is not expected to recover them. The card name and its power limit are printed with the
-numbers. Needs an H100.
+               steps; passes with the options off and on alternate in the same process
+The synthetic scenes garble bits BEFORE modulation, so those errors are high-confidence: "ec", which only flips
+low-confidence bits, is not expected to recover them; "ec_any" is. The card name and its power limit are printed with
+the numbers. Needs an H100.
 
-    python tools/ec_yield.py [--steps 5] [--log2n 28] [--json out.json]
+    python tools/ec_yield.py [--steps 5] [--log2n 28] [--ks 4,8,12] [--ec-any 1,2] [--json out.json]
 """
 from __future__ import annotations
 
@@ -25,6 +28,8 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+
+import numpy as np
 
 FIXED = 1   # AMB_EC_FIXED
 
@@ -44,6 +49,20 @@ def card():
     except Exception:
         out = "unknown"
     return name, out or "unknown"
+
+
+def clean_frames(rate, n, nb, seed, garbled, nbytes):
+    """The frames synth.make_scene_device generated before garbling them: its random draws replayed up to
+    make_frames, with garble_frac 0. Checked against the garbled frames (equal, or at most 5 bits apart)."""
+    from gr_air_modes_b200 import synth
+    rng = np.random.Generator(np.random.PCG64(seed))
+    span = 240 * rate / 2e6 + 8
+    rng.uniform(span, n - 2 * span, nb)
+    dfs = np.asarray((11, 17))[rng.integers(0, 2, nb)]
+    clean, nb2 = synth.make_frames(dfs, rng, 0.0)
+    diff = np.unpackbits(clean ^ garbled, axis=1).sum(axis=1)
+    assert np.array_equal(nb2, nbytes) and diff.max() <= 5, "replay of make_scene_device out of step"
+    return {clean[k, :nbytes[k]].tobytes() for k in range(nb)}
 
 
 def one_pass(rx, dev, torch):
@@ -67,6 +86,7 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--log2n", type=int, default=28)
     ap.add_argument("--ks", default="4,8,12")
+    ap.add_argument("--ec-any", default="1,2")
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     rate, n = 4e6, 1 << args.log2n
@@ -78,19 +98,21 @@ def main():
         nb = cfg["n_bursts"] or int(cfg["bursts_per_s"] * n / rate)
         iq, _, (fr, nbytes) = synth.make_scene_device(rate, n, nb, cfg["seed"], dev0, noise_sigma=0.01, snr_db=cfg["snr_db"],
                                                       garble_frac=cfg["garble_frac"], fruit=nb // 4 if cfg["fruit"] else 0)
-        sent = {fr[k, :nbytes[k]].tobytes() for k in range(nb)}
+        sent = {fr[k, :nbytes[k]].tobytes() for k in range(nb)} | clean_frames(rate, n, nb, cfg["seed"], fr, nbytes)
         stream = torch.cuda.current_stream(dev0).cuda_stream
         off = am.rx_path(rate, 7.0, am.msg_queue(), use_pmf=True)
         off.use_stream(stream)
         one_pass(off, iq, torch)                                  # warm-up
         base = off.drain()
-        for k in [int(x) for x in args.ks.split(",")]:
-            on = am.rx_path(rate, 7.0, am.msg_queue(), use_pmf=True, ec=k)
+        settings = [(int(k), 0) for k in args.ks.split(",") if k] + [(0, int(m)) for m in args.ec_any.split(",") if m]
+        settings.append((8, 2))
+        for k, m in settings:
+            on = am.rx_path(rate, 7.0, am.msg_queue(), use_pmf=True, ec=k, ec_any=m)
             on.use_stream(stream)
             one_pass(on, iq, torch)
             msgs = on.drain()
             frames = on.frames
-            fixed = [f for f in frames if f.ec == FIXED]
+            fixed = [f for f in frames if f.ec == FIXED or f.ec_any == FIXED]
             true = sum(f.payload() in sent for f in fixed)
             t_off, t_on = [], []
             for _ in range(args.steps):                           # off and on alternate
@@ -98,7 +120,8 @@ def main():
                 t_on.append(one_pass(on, iq, torch))
             off.drain()
             on.drain()
-            row = dict(scene=scene, samples=n, bursts=nb, k=k, messages_off=base, messages=msgs, fixed=len(fixed),
+            row = dict(scene=scene, samples=n, bursts=nb, k=k, m=m, messages_off=base, messages=msgs, fixed=len(fixed),
+                       fixed_ec=sum(f.ec == FIXED for f in fixed), fixed_any=sum(f.ec_any == FIXED for f in fixed),
                        true_fixes=true, false_fixes=len(fixed) - true, ms_step_off=round(statistics.median(t_off), 3),
                        ms_step_on=round(statistics.median(t_on), 3), card=name, power_limit=power)
             rows.append(row)
@@ -107,11 +130,12 @@ def main():
         off.close()
         del iq
         torch.cuda.empty_cache()
-    print("\n%-11s %3s %9s %9s %7s %6s %6s %9s %9s" % ("scene", "K", "msgs_off", "msgs_on", "fixed", "true", "false",
-                                                     "ms_off", "ms_on"))
+    print("\n%-11s %3s %2s %9s %9s %7s %7s %6s %6s %9s %9s" % ("scene", "K", "M", "msgs_off", "msgs_on", "fix_ec",
+                                                              "fix_any", "true", "false", "ms_off", "ms_on"))
     for r in rows:
-        print("%-11s %3d %9d %9d %7d %6d %6d %9.3f %9.3f" % (r["scene"], r["k"], r["messages_off"], r["messages"], r["fixed"],
-                                                          r["true_fixes"], r["false_fixes"], r["ms_step_off"], r["ms_step_on"]))
+        print("%-11s %3d %2d %9d %9d %7d %7d %6d %6d %9.3f %9.3f" % (
+            r["scene"], r["k"], r["m"], r["messages_off"], r["messages"], r["fixed_ec"], r["fixed_any"], r["true_fixes"],
+            r["false_fixes"], r["ms_step_off"], r["ms_step_on"]))
     if args.json:
         with open(args.json, "w") as f:
             json.dump(rows, f, indent=1)

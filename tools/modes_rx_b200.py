@@ -159,6 +159,8 @@ def main(argv=None):
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--ec", type=int, default=0, metavar="K",
                     help="correct DF11/DF17 frames over at most K (1..23) low-confidence bits; 0 = off, as the reference")
+    ap.add_argument("--ec-any", type=int, default=0, metavar="M",
+                    help="correct DF17 frames by at most M (1, 2) flipped bits anywhere, after --ec; 0 = off, as the reference")
     args = ap.parse_args(argv)
 
     if args.source in ("uhd", "osmocom"):
@@ -193,7 +195,7 @@ def main(argv=None):
         pub = zmq_queue(["tcp://*:%i" % args.tcp])
         sinks.append(pub)
     rx = air_modes.rx_path(rx_rate, args.threshold, tee_queue(sinks), args.pmf, args.dcblock, device=args.device,
-                           ec=args.ec)   # radio.py:55-56
+                           ec=args.ec, ec_any=args.ec_any)   # radio.py:55-56
 
     if ":" in args.source and not os.path.exists(args.source):
         m = re.search(r"(.*)\:(\d{1,5})$", args.source)                                                           # radio.py:223-226
