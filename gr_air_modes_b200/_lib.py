@@ -18,13 +18,16 @@ MEM_HOST, MEM_DEVICE, MEM_HOST_SC16, MEM_DEVICE_SC16 = 0, 1, 2, 3
 EC_NOT_TRIED, EC_FIXED, EC_TOO_MANY, EC_NO_SOLUTION, EC_AMBIGUOUS = 0, 1, 2, 3, 4
 EC_MAX = 23
 EC_ANY_MAX = 2              # option "ec_any": at most 2 flipped bits
+# AMB_FRAME_AP (include/airmodes_b200.h AMB_AP_*), option "ap_filter" = S seconds (0 = off)
+AP_NOT_CHECKED, AP_KNOWN, AP_UNKNOWN = 0, 1, 2
+AP_FILTER_MAX = 3600
 
 
 class Frame(C.Structure):
     """struct amb_frame (80 bytes) = modes_packet (types.h:29-41) + preamble tag.
 
-    The header's `ec`, `ec_flips` and the first three bytes of its `pad_[4]` (AMB_FRAME_EC_ANY / AMB_FRAME_EC_ANY_BIT)
-    are the first five of the six tail bytes, which stay one `pad_` field here: the record layout that numpy views and per-field dumps of frames see (np.dtype(Frame)) is
+    The header's `ec`, `ec_flips` and the four bytes of its `pad_[4]` (AMB_FRAME_EC_ANY / AMB_FRAME_EC_ANY_BIT /
+    AMB_FRAME_AP) are the six tail bytes, which stay one `pad_` field here: the record layout that numpy views and per-field dumps of frames see (np.dtype(Frame)) is
     the one the frame had before error correction existed. They are read through the properties below."""
     _fields_ = [("sample_index", C.c_uint64), ("secs", C.c_uint64), ("frac", C.c_double),
                 ("ref_level", C.c_float), ("crc", C.c_uint32), ("nbits", C.c_uint8), ("df", C.c_uint8),
@@ -50,6 +53,11 @@ class Frame(C.Structure):
     def ec_any_bits(self) -> tuple:
         """AMB_FRAME_EC_ANY_BIT(f, 0..1) (bytes 77-78): the two positions that pass flipped, ascending; 0 = unused slot."""
         return (self.pad_[3], self.pad_[4])
+
+    @property
+    def ap(self) -> int:
+        """AMB_FRAME_AP (byte 79): address/parity check (option "ap_filter"): AP_NOT_CHECKED, AP_KNOWN or AP_UNKNOWN."""
+        return self.pad_[5]
 
     def payload(self) -> bytes:
         return bytes(self.data[: self.nbits // 8])

@@ -157,6 +157,7 @@ class _Context:
         self.device = int(device)
         self.ec = 0                 # option "ec" as last set (the library keeps it; there is no getter in the C ABI)
         self.ec_any = 0             # option "ec_any", likewise
+        self.ap_filter = 0          # option "ap_filter", likewise
 
     def close(self):
         if getattr(self, "_h", None):
@@ -338,10 +339,17 @@ class rx_path:
 
     ec_any=M (extension, default 0 = off): DF17 frames still dropped for their CRC after that are corrected by at most
     M (1, 2) flipped bits anywhere in 5..111, whatever their confidence; the one- and two-bit fits are unique there.
-    Frames record the outcome in .ec_any / .ec_any_bits."""
+    Frames record the outcome in .ec_any / .ec_any_bits.
+
+    ap_filter=S (extension, default 0 = off): address/parity check. Replies whose parity carries the address (DF0/4/5/
+    16/20/21 and any other DF but 11/17) are dropped unless a CRC-clean DF11/DF17 frame of that address arrived in the
+    last S seconds of the stream (counted in samples, S * int(rate)); DF11 replies whose parity carries a non-zero
+    interrogator code (syndrome 1..0x7F) are accepted when their address is known that way. Frames record the outcome in
+    .ap. reset() / set_rate() forget the confirmed addresses and keep the option. Not available with seek() /
+    defer_resolve()."""
 
     def __init__(self, rate, threshold, queue, use_pmf=False, use_dcblock=False, device: int = 0, ec: int = 0,
-                 ec_any: int = 0):
+                 ec_any: int = 0, ap_filter: int = 0):
         self._rate = int(rate)                      # rx_path.py:32
         self._threshold = threshold
         self._queue = queue
@@ -349,6 +357,8 @@ class rx_path:
         self._use_pmf = bool(use_pmf)
         self._ctx = _Context(rate, threshold, use_pmf, use_dcblock, device)
         self._slicer = slicer(queue, device, _ctx=self._ctx, ec=ec, ec_any=ec_any)
+        if ap_filter:
+            self.set_ap_filter(ap_filter)
         self.frames = []                            # every detection of the last process() call
         self._keep = []                             # device inputs still being read
 
@@ -387,6 +397,15 @@ class rx_path:
 
     def get_ec_any(self) -> int:
         return self._slicer.get_ec_any()
+
+    def set_ap_filter(self, seconds: int):
+        """Address/parity check against the aircraft confirmed in the last `seconds` (0 = off, up to 3600); takes effect
+        at the next call. Not available together with seek() / defer_resolve()."""
+        self._ctx.call("amb_set_option", b"ap_filter", int(seconds))
+        self._ctx.ap_filter = int(seconds)
+
+    def get_ap_filter(self) -> int:
+        return self._ctx.ap_filter
 
     # -- data path
     def process(self, iq, flush: bool = False, collect: bool = True) -> int:
@@ -458,11 +477,13 @@ class rx_path:
 
     def set_option(self, name: str, value: int):
         """Library options: "coalesce", "ingest_chunk", "copy_threads", "resolver", "overlap", "keep_chips", "exact_dense",
-        "scan_ctas", "order_tile", "ec", "ec_any"."""
+        "scan_ctas", "order_tile", "ec", "ec_any", "ap_filter"."""
         if name == "ec":
             return self.set_ec(value)
         if name == "ec_any":
             return self.set_ec_any(value)
+        if name == "ap_filter":
+            return self.set_ap_filter(value)
         self._ctx.call("amb_set_option", name.encode(), int(value))
 
     def reset(self):

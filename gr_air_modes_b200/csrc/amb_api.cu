@@ -104,6 +104,9 @@ struct amb_ctx {
     int resolver = 0;
     int ec = 0;                          // option "ec": error correction over up to K low-confidence bits (0 = off)
     int ec_any = 0;                      // option "ec_any": DF17 correction over up to M (1, 2) bits anywhere (0 = off)
+    int ap_filter = 0;                   // option "ap_filter": address/parity check against the last S seconds (0 = off)
+    AmbApState ap{};                     // its device state (allocated at the first call with the option on)
+    bool seeked = false;                 // positioned by amb_seek since the last reset (no "ap_filter" there)
     // time-sharded operation (amb_seek / amb_resolve): a call whose walk + slice stages are still to run
     int defer = 0;                       // option "defer_resolve"
     int def_kind = 0;                    // 0 nothing pending, 1 full (walk + slice), 2 sequential walk only, 3 state only
@@ -229,6 +232,11 @@ static int reset_stream(amb_ctx* ctx)
     ctx->pend_n = 0;                                   // samples gathered but not dispatched belong to the old stream
     ctx->snap_tail = ctx->snap_head; ctx->polled = 0;
     ctx->time_tags.clear();
+    ctx->seeked = false;
+    if (ctx->ap.last) {                // confirmed addresses belong to the stream; the option itself stays
+        CK(cudaMemsetAsync(ctx->ap.last, 0, sizeof(unsigned long long) << 24, ctx->stream_b));
+        CK(cudaMemsetAsync(ctx->ap.count, 0, AMB_AP_BUCKETS * sizeof(unsigned), ctx->stream_b));
+    }
     return AMB_OK;
 }
 
@@ -313,6 +321,7 @@ void amb_destroy(amb_ctx* ctx)
     free_dev(ctx);
     ingest_free(ctx);
     cudaFree(ctx->ord_key); cudaFree(ctx->ord_val); cudaFree(ctx->tags_dev);
+    cudaFree(ctx->ap.last); cudaFree(ctx->ap.count); cudaFree(ctx->ap.off); cudaFree(ctx->ap.cursor); cudaFree(ctx->ap.ent);
     if (ctx->stream_h) cudaStreamDestroy(ctx->stream_h);
     if (ctx->ctr_snap) cudaFreeHost(ctx->ctr_snap);
     for (int k = 0; k < AMB_SNAPS; k++) if (ctx->snap_ev[k]) cudaEventDestroy(ctx->snap_ev[k]);
@@ -407,6 +416,12 @@ int amb_set_option(amb_ctx* ctx, const char* name, int value)
     if (!strcmp(name, "resolver")) { ctx->resolver = value; return AMB_OK; }
     if (!strcmp(name, "ec")) { if (value < 0 || value > 23) return AMB_ERR_INVALID; ctx->ec = value; return AMB_OK; }
     if (!strcmp(name, "ec_any")) { if (value < 0 || value > 2) return AMB_ERR_INVALID; ctx->ec_any = value; return AMB_OK; }
+    if (!strcmp(name, "ap_filter")) {
+        if (value < 0 || value > 3600) return AMB_ERR_INVALID;
+        if (value && (ctx->defer || ctx->seeked))
+            return fail(ctx, AMB_ERR_STATE, "ap_filter needs the whole stream: not available in time-sharded operation");
+        ctx->ap_filter = value; return AMB_OK;
+    }
     if (!strcmp(name, "keep_chips")) { ctx->keep_chips = value != 0; return AMB_OK; }
     if (!strcmp(name, "overlap")) { ctx->overlap = value != 0; return AMB_OK; }
     if (!strcmp(name, "coalesce")) {                       // samples of small host calls gathered before a dispatch
@@ -433,6 +448,7 @@ int amb_set_option(amb_ctx* ctx, const char* name, int value)
     }
     if (!strcmp(name, "defer_resolve")) {
         if (ctx->def_kind && !ctx->def_resolved) return fail(ctx, AMB_ERR_STATE, "amb_resolve pending");
+        if (value && ctx->ap_filter) return fail(ctx, AMB_ERR_STATE, "defer_resolve is not available with ap_filter on");
         ctx->def_kind = 0; ctx->def_resolved = false;
         ctx->defer = value != 0; return AMB_OK;
     }
@@ -510,18 +526,50 @@ static int ensure_call_buffers(amb_ctx* ctx, size_t rows_need, int n_spans, unsi
 }
 
 // The slicer stage of every path: slice, then - with option "ec" or "ec_any" on - correct the frames it dropped for
-// their CRC, in place (one launch for both passes). Everything that reads frames or the call's counters (polls, drain, walk summaries, completion events) is
-// enqueued after this on the same stream.
+// their CRC, in place (one launch for both passes), then - with "ap_filter" on, fused paths only - check the address/parity
+// replies against the confirmed addresses (four launches). Everything that reads frames or the call's counters (polls,
+// drain, walk summaries, completion events) is enqueued after this on the same stream.
 static cudaError_t launch_ec_if_on(amb_ctx* ctx, amb_frame* frames, unsigned frame_cap, AmbCounters* ctr, int n, cudaStream_t s)
 {
     if (!ctx->ec && !ctx->ec_any) return cudaSuccess;
     ctx->stats.kernel_launches += 1;
     return amb_launch_ec(frames, frame_cap, ctr, n, ctx->ec, ctx->ec_any, ctx->sm_count, s);
 }
+static cudaError_t launch_ap_if_on(amb_ctx* ctx, amb_frame* frames, unsigned frame_cap, AmbCounters* ctr, cudaStream_t s)
+{
+    if (!ctx->ap_filter) return cudaSuccess;
+    AmbApState& ap = ctx->ap;
+    cudaError_t e = cudaSuccess;
+    if (!ap.last) {                    // first call with the option on: 128 MiB table of 2^24 addresses, zeroed in order
+        unsigned long long* last = nullptr;
+        e = cudaMalloc(&last, sizeof(unsigned long long) << 24);
+        if (e == cudaSuccess) e = cudaMalloc(&ap.count, AMB_AP_BUCKETS * sizeof(unsigned));
+        if (e == cudaSuccess) e = cudaMalloc(&ap.off, AMB_AP_BUCKETS * sizeof(unsigned));
+        if (e == cudaSuccess) e = cudaMalloc(&ap.cursor, AMB_AP_BUCKETS * sizeof(unsigned));
+        if (e == cudaSuccess) e = cudaMemsetAsync(last, 0, sizeof(unsigned long long) << 24, s);
+        if (e == cudaSuccess) e = cudaMemsetAsync(ap.count, 0, AMB_AP_BUCKETS * sizeof(unsigned), s);
+        if (e != cudaSuccess) {        // all or nothing: the next call tries again
+            cudaFree(last); cudaFree(ap.count); cudaFree(ap.off); cudaFree(ap.cursor);
+            ap.count = ap.off = ap.cursor = nullptr;
+            return e;
+        }
+        ap.last = last;
+    }
+    if (ap.ent_cap < frame_cap) {      // grows with the frame buffer (which synchronised when it grew)
+        if ((e = cudaStreamSynchronize(s)) != cudaSuccess) return e;
+        cudaFree(ap.ent); ap.ent = nullptr; ap.ent_cap = 0;
+        if ((e = cudaMalloc(&ap.ent, (size_t)frame_cap * sizeof(AmbApEntry))) != cudaSuccess) return e;
+        ap.ent_cap = frame_cap;
+    }
+    const unsigned long long window = (unsigned long long)ctx->ap_filter * (unsigned long long)ctx->P.rate_int;
+    ctx->stats.kernel_launches += amb_launch_ap(frames, frame_cap, ctr, ap, window, ctx->sm_count, s, &e);
+    return e;
+}
 static cudaError_t slice_and_correct(amb_ctx* ctx, const AmbSliceArgs& sl, cudaStream_t s)
 {
     cudaError_t e = amb_launch_slice(sl, ctx->sm_count, s);
     if (e == cudaSuccess) e = launch_ec_if_on(ctx, sl.frames, sl.frame_cap, sl.ctr, 0, s);
+    if (e == cudaSuccess) e = launch_ap_if_on(ctx, sl.frames, sl.frame_cap, sl.ctr, s);
     return e;
 }
 static cudaError_t slice_chips_and_correct(amb_ctx* ctx, const float* chips, int ndet, amb_frame* frames, cudaStream_t s)
@@ -975,6 +1023,7 @@ int amb_seek(amb_ctx* ctx, uint64_t first_sample, uint64_t first_decision, const
             return fail(ctx, AMB_ERR_INVALID, "first_decision must be at least first_sample + shard_back");
     }
     if (first_sample > (1ull << 62) || first_decision > (1ull << 62)) return fail(ctx, AMB_ERR_INVALID, "index out of range");
+    if (ctx->ap_filter) return fail(ctx, AMB_ERR_STATE, "amb_seek is not available with ap_filter on (it needs the whole stream)");
     int rc = reset_stream(ctx);
     if (rc != AMB_OK) return rc;
     ctx->n_in = first_sample;
@@ -982,6 +1031,7 @@ int amb_seek(amb_ctx* ctx, uint64_t first_sample, uint64_t first_decision, const
     const long long pos = entry ? (long long)entry->pos : (long long)first_decision;
     const long long p = entry ? (long long)entry->p : (long long)first_decision;
     CK(amb_launch_set_state(ctx->st, pos, p, ctx->stream_b));          // after reset_stream's memset on stream B
+    ctx->seeked = true;
     return AMB_OK;
 }
 

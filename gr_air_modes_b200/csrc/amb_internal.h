@@ -136,6 +136,19 @@ cudaError_t amb_launch_slice_chips(const float* chips, int ndet, amb_frame* fram
 // "ec_any" (0 skips that pass)
 cudaError_t amb_launch_ec(amb_frame* frames, unsigned int frame_cap, AmbCounters* ctr, int n, int k_max, int m_any,
                           int sm_count, cudaStream_t s);
+// address/parity check (option "ap_filter") of the call's slots [frame_base, frame_base + ndet_list), after the error
+// correction. Device state: last[2^24] = 1 + sample index of the latest confirmer of each address in earlier calls
+// (0 = none); count / off / cursor: AMB_AP_BUCKETS words each (count all zero between calls); ent: frame_cap entries.
+#define AMB_AP_BUCKET_BITS 11
+#define AMB_AP_BUCKETS (1 << AMB_AP_BUCKET_BITS)
+#define AMB_AP_TILE 256         // entries of a bucket sorted and resolved in shared memory (4 KiB); larger ones in place
+struct AmbApEntry { unsigned long long si; unsigned key; unsigned slot; };   // key = address | kind << 24
+struct AmbApState {
+    unsigned long long* last; unsigned* count; unsigned* off; unsigned* cursor; AmbApEntry* ent; unsigned ent_cap;
+};
+// window = S * rate_int samples. Returns the number of kernels launched (fixed).
+int amb_launch_ap(amb_frame* frames, unsigned int frame_cap, AmbCounters* ctr, const AmbApState& ap,
+                  unsigned long long window, int sm_count, cudaStream_t s, cudaError_t* err);
 cudaError_t amb_launch_crc(const uint8_t* data, int n, int length, uint32_t* out, cudaStream_t s);
 cudaError_t amb_upload_tables(const int* chip_off);
 cudaError_t amb_prefer_max_shared();

@@ -1895,6 +1895,210 @@ cudaError_t amb_launch_ec(amb_frame* frames, unsigned int frame_cap, AmbCounters
     return cudaGetLastError();
 }
 
+// ------------------------------------------------------------------------------------------------
+// Address/parity check (option "ap_filter" = S seconds, off by default), after the error correction. The semantics are
+// in include/airmodes_b200.h (AMB_FRAME_AP). Four launches per call, all on the slicer's stream:
+//   amb_ap_count_kernel    classify the call's slots; count confirmers and subjects per bucket (a hash of the address)
+//   amb_ap_scan_kernel     bucket offsets; re-zeroes the counts for the next call
+//   amb_ap_scatter_kernel  classify again, append (sample index, address | kind, slot) to the bucket
+//   amb_ap_resolve_kernel  per bucket: sort by (address, sample index) - in shared memory up to AMB_AP_TILE entries,
+//                          in place in global memory beyond - then a max-scan over the confirmer positions gives each
+//                          subject the latest earlier confirmer of its address in this call (same address = the same
+//                          sorted run), else the table's latest confirmer of an earlier call. The last entry of each
+//                          address run writes the table: one writer per address, no atomics.
+// Every frame of a later call lies after every frame of an earlier one (DESIGN.md section 4), so "latest confirmer
+// before this call" is all the table has to hold. Sample indices are unique per stream, so the sort key is a total order
+// and the result does not depend on the order the scatter's atomics produced.
+// ------------------------------------------------------------------------------------------------
+constexpr unsigned AP_NONE = 0, AP_CONF = 1, AP_SUBJECT = 2, AP_IISI = 3;
+
+__device__ __forceinline__ unsigned ap_classify(const amb_frame* f, unsigned& addr)
+{
+    const unsigned df = f->df;
+    const unsigned crc = f->crc;
+    const unsigned aa = ((unsigned)f->data[1] << 16) | ((unsigned)f->data[2] << 8) | f->data[3];
+    if (f->passed) {
+        if (df != 11 && df != 17) { addr = crc & 0xFFFFFFu; return AP_SUBJECT; }
+        if (crc == 0u && f->ec != AMB_EC_FIXED && AMB_FRAME_EC_ANY(f) != AMB_EC_FIXED) { addr = aa; return AP_CONF; }
+        return AP_NONE;
+    }
+    if (df == 11 && crc != 0u && crc < 0x80u) { addr = aa; return AP_IISI; }
+    return AP_NONE;
+}
+__device__ __forceinline__ unsigned ap_bucket(unsigned addr) { return (addr * 0x9E3779B1u) >> (32 - AMB_AP_BUCKET_BITS); }
+__device__ __forceinline__ void ap_call_slots(const AmbCounters* ctr, unsigned frame_cap, unsigned& base, unsigned& n)
+{
+    base = ctr->frame_base;                                    // slots past the capacity were never written
+    n = base < frame_cap ? min(ctr->ndet_list, frame_cap - base) : 0u;
+}
+
+__global__ void __launch_bounds__(128) amb_ap_count_kernel(const amb_frame* __restrict__ frames, unsigned int frame_cap,
+                                                          const AmbCounters* ctr, unsigned* __restrict__ count)
+{
+    unsigned base, n;
+    ap_call_slots(ctr, frame_cap, base, n);
+    for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        unsigned addr = 0;
+        if (ap_classify(frames + base + i, addr) != AP_NONE) atomicAdd(&count[ap_bucket(addr)], 1u);
+    }
+}
+
+__global__ void __launch_bounds__(128) amb_ap_scan_kernel(unsigned* __restrict__ count, unsigned* __restrict__ off,
+                                                         unsigned* __restrict__ cursor)
+{
+    constexpr unsigned PER = AMB_AP_BUCKETS / 128;
+    __shared__ unsigned s_sum[128];
+    const unsigned t = threadIdx.x;
+    unsigned sum = 0;
+    for (unsigned k = 0; k < PER; k++) sum += count[t * PER + k];
+    s_sum[t] = sum;
+    __syncthreads();
+    for (unsigned d = 1; d < 128; d <<= 1) {                   // inclusive scan over the threads' sums
+        const unsigned v = t >= d ? s_sum[t - d] : 0u;
+        __syncthreads();
+        s_sum[t] += v;
+        __syncthreads();
+    }
+    unsigned run = s_sum[t] - sum;
+    for (unsigned k = 0; k < PER; k++) {
+        const unsigned c = count[t * PER + k];
+        off[t * PER + k] = run; cursor[t * PER + k] = run; count[t * PER + k] = 0u;
+        run += c;
+    }
+}
+
+__global__ void __launch_bounds__(128) amb_ap_scatter_kernel(const amb_frame* __restrict__ frames, unsigned int frame_cap,
+                                                            const AmbCounters* ctr, unsigned* __restrict__ cursor,
+                                                            AmbApEntry* __restrict__ ent)
+{
+    unsigned base, n;
+    ap_call_slots(ctr, frame_cap, base, n);
+    for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const amb_frame* f = frames + base + i;
+        unsigned addr = 0;
+        const unsigned kind = ap_classify(f, addr);
+        if (kind == AP_NONE) continue;
+        const unsigned pos = atomicAdd(&cursor[ap_bucket(addr)], 1u);
+        AmbApEntry e; e.si = f->sample_index; e.key = addr | (kind << 24); e.slot = base + i;
+        ent[pos] = e;
+    }
+}
+
+__device__ __forceinline__ bool ap_less(const AmbApEntry& a, const AmbApEntry& b)
+{
+    const unsigned ka = a.key & 0xFFFFFFu, kb = b.key & 0xFFFFFFu;
+    return ka != kb ? ka < kb : a.si < b.si;
+}
+// CTA-wide sort of e[0, n) by (address, sample index): a bitonic network in the form whose every compare-exchange puts
+// the smaller element at the lower index (a flip stage, then half-cleaners), so the missing elements up to the next
+// power of two act as +infinity at the end and their pairs are simply skipped. e may be shared or global memory.
+__device__ void ap_sort(AmbApEntry* e, unsigned n)
+{
+    unsigned npad = 1;
+    while (npad < n) npad <<= 1;
+    for (unsigned k = 2; k <= npad; k <<= 1) {
+        for (unsigned p = threadIdx.x; p < (npad >> 1); p += blockDim.x) {
+            const unsigned h = k >> 1, b0 = (p / h) * k, o = p % h;
+            const unsigned i = b0 + o, l = b0 + k - 1 - o;
+            if (l < n && ap_less(e[l], e[i])) { const AmbApEntry x = e[i]; e[i] = e[l]; e[l] = x; }
+        }
+        __syncthreads();
+        for (unsigned j = k >> 2; j > 0; j >>= 1) {
+            for (unsigned p = threadIdx.x; p < (npad >> 1); p += blockDim.x) {
+                const unsigned i = ((p & ~(j - 1)) << 1) | (p & (j - 1)), l = i + j;
+                if (l < n && ap_less(e[l], e[i])) { const AmbApEntry x = e[i]; e[i] = e[l]; e[l] = x; }
+            }
+            __syncthreads();
+        }
+    }
+}
+
+__global__ void __launch_bounds__(128, 16) amb_ap_resolve_kernel(amb_frame* __restrict__ frames, AmbCounters* ctr,
+                                                                 const unsigned* __restrict__ off,
+                                                                 const unsigned* __restrict__ cursor, AmbApEntry* ent,
+                                                                 unsigned long long* __restrict__ last,
+                                                                 unsigned long long window)
+{
+    __shared__ AmbApEntry s_ent[AMB_AP_TILE];
+    __shared__ int s_wmax[4];
+    __shared__ unsigned s_delta;
+    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) s_delta = 0u;
+    __syncthreads();
+    int delta = 0;                                           // change of the call's passed count
+    for (unsigned b = blockIdx.x; b < AMB_AP_BUCKETS; b += gridDim.x) {
+        const unsigned lo = off[b], n = cursor[b] - lo;
+        if (n == 0u) continue;
+        AmbApEntry* e = ent + lo;
+        if (n <= AMB_AP_TILE) {
+            for (unsigned t = threadIdx.x; t < n; t += blockDim.x) s_ent[t] = e[t];
+            e = s_ent;
+        }
+        __syncthreads();
+        ap_sort(e, n);
+        int carry = -1;                                        // position of the latest confirmer before this chunk
+        for (unsigned c0 = 0; c0 < n; c0 += AMB_AP_TILE) {
+            const unsigned m = min(n - c0, (unsigned)AMB_AP_TILE);
+            const unsigned q0 = 2 * threadIdx.x;               // this thread's two positions of the chunk
+            const int v0 = q0 < m && (e[c0 + q0].key >> 24) == AP_CONF ? (int)(c0 + q0) : -1;
+            const int v1 = max(v0, q0 + 1 < m && (e[c0 + q0 + 1].key >> 24) == AP_CONF ? (int)(c0 + q0 + 1) : -1);
+            int x = v1;                                        // inclusive max-scan over the warp
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) { const int y = __shfl_up_sync(FULL, x, d); if ((int)lane >= d) x = max(x, y); }
+            const int xprev = __shfl_up_sync(FULL, x, 1);
+            if (lane == 31) s_wmax[warp] = x;
+            __syncthreads();
+            int pre = carry;
+            for (unsigned w = 0; w < warp; w++) pre = max(pre, s_wmax[w]);
+            if (lane > 0) pre = max(pre, xprev);
+            const int incl[2] = {max(pre, v0), max(pre, v1)};  // latest confirmer at or before each position
+#pragma unroll
+            for (int r = 0; r < 2; r++) {                      // subjects decide (before any table write of this chunk)
+                const unsigned q = q0 + r;
+                if (q >= m) break;
+                const AmbApEntry en = e[c0 + q];
+                const unsigned kind = en.key >> 24, addr = en.key & 0xFFFFFFu;
+                if (kind == AP_CONF) continue;
+                const int p = incl[r];
+                const unsigned long long g1 = p >= 0 && (e[p].key & 0xFFFFFFu) == addr ? e[p].si + 1ull : last[addr];
+                const bool known = g1 != 0ull && en.si + 1ull - g1 <= window;
+                amb_frame* f = frames + en.slot;
+                AMB_FRAME_AP(f) = known ? AMB_AP_KNOWN : AMB_AP_UNKNOWN;
+                if (kind == AP_SUBJECT && !known) { f->passed = 0; delta--; }
+                if (kind == AP_IISI && known) { f->passed = 1; delta++; }
+            }
+            __syncthreads();
+#pragma unroll
+            for (int r = 0; r < 2; r++) {                      // the last entry of each address run writes the table
+                const unsigned q = q0 + r;
+                if (q >= m) break;
+                const unsigned addr = e[c0 + q].key & 0xFFFFFFu;
+                const bool run_end = c0 + q + 1 == n || (e[c0 + q + 1].key & 0xFFFFFFu) != addr;
+                const int p = incl[r];
+                if (run_end && p >= 0 && (e[p].key & 0xFFFFFFu) == addr) last[addr] = e[p].si + 1ull;
+            }
+            for (unsigned w = 0; w < 4; w++) carry = max(carry, s_wmax[w]);
+            __syncthreads();
+        }
+    }
+    if (delta) atomicAdd(&s_delta, (unsigned)delta);
+    __syncthreads();
+    if (threadIdx.x == 0 && s_delta) atomicAdd(&ctr->npassed_call, s_delta);
+}
+
+int amb_launch_ap(amb_frame* frames, unsigned int frame_cap, AmbCounters* ctr, const AmbApState& ap,
+                  unsigned long long window, int sm_count, cudaStream_t s, cudaError_t* err)
+{
+    const int g = sm_count > 0 ? sm_count : 8;
+    AMB_LAUNCH((amb_ap_count_kernel), g, 128, 0, s, frames, frame_cap, ctr, ap.count);
+    AMB_LAUNCH((amb_ap_scan_kernel), 1, 128, 0, s, ap.count, ap.off, ap.cursor);
+    AMB_LAUNCH((amb_ap_scatter_kernel), g, 128, 0, s, frames, frame_cap, ctr, ap.cursor, ap.ent);
+    AMB_LAUNCH((amb_ap_resolve_kernel), min(AMB_AP_BUCKETS, 4 * g), 128, 0, s, frames, ctr, ap.off, ap.cursor, ap.ent,
+               ap.last, window);
+    *err = cudaGetLastError();
+    return 4;
+}
+
 // device CRC parity hook: same XOR fold as the slicer
 __global__ void amb_crc_kernel(const uint8_t* __restrict__ data, int n, int length, uint32_t* out)
 {

@@ -5,7 +5,8 @@
     air_modes.slicer(queue)                                           slicer.h:37-42            -> slicer (sink of float)
 
 rx_path and slicer also take ec=K (default 0 = off): error correction over low-confidence bits, and ec_any=M (default
-0 = off): DF17 correction by at most M bits anywhere (blocks.rx_path).
+0 = off): DF17 correction by at most M bits anywhere (blocks.rx_path). rx_path also takes ap_filter=S (default 0 = off):
+the address/parity check against the aircraft confirmed in the last S seconds.
 
 Importable only where gnuradio (and its pmt) is installed; radio.py:55-56,73-76 keep working:
 `self.connect(source, rx_path(rate, threshold, queue, pmf, dcblock))`, and so does the reference's own wiring of the
@@ -25,12 +26,13 @@ from . import blocks
 
 
 class rx_path(gr.sync_block):
-    def __init__(self, rate, threshold, queue, use_pmf=False, use_dcblock=False, device=0, ec=0, ec_any=0):
+    def __init__(self, rate, threshold, queue, use_pmf=False, use_dcblock=False, device=0, ec=0, ec_any=0,
+                 ap_filter=0):
         gr.sync_block.__init__(self, "modes_rx_path_b200", in_sig=[np.complex64], out_sig=None)
         self._impl = blocks.rx_path(rate, threshold, queue, use_pmf, use_dcblock, device=device, ec=ec,
-                                    ec_any=ec_any)
+                                    ec_any=ec_any, ap_filter=ap_filter)
         for name in ("set_rate", "set_threshold", "set_pmf", "get_pmf", "get_threshold", "set_ec", "get_ec",
-                     "set_ec_any", "get_ec_any"):
+                     "set_ec_any", "get_ec_any", "set_ap_filter", "get_ap_filter"):
             setattr(self, name, getattr(self._impl, name))
         self._open = False
 

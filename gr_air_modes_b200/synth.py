@@ -261,3 +261,165 @@ def make_scene_device(rate: float, n: int, n_bursts: int, seed: int, device, *, 
         iq2.index_add_(0, idx[ok], vals[ok])
     hexs = [frames[k, :nbytes[k]].tobytes().hex() for k in range(n_bursts)] if n_bursts <= 4096 else None
     return iq, hexs, (frames, nbytes)
+
+
+# ---------------------------------------------------------------------------------------------------------
+# Fleet scenes: a fixed set of aircraft whose replies carry their addresses the way Mode S does, for the address/parity
+# check (rx_path(..., ap_filter=S)). The generators above stay as they are; these are separate functions.
+#   DF17      squitter, AA in bytes 1..3, parity = CRC
+#   DF11      all-call reply, AA in bytes 1..3, parity = CRC xor II (II = 0, or an interrogator code 1..0x7F)
+#   AP        DF0/4/5/16/20/21 reply, parity = CRC xor address (address/parity)
+# ---------------------------------------------------------------------------------------------------------
+FLEET_AP_DFS = (0, 4, 5, 16, 20, 21)
+FLEET_MIX = (0.40, 0.15, 0.10, 0.35)      # DF17, DF11 with II = 0, DF11 with an II code, AP replies
+
+
+def make_fleet_frames(dfs: np.ndarray, addrs: np.ndarray, codes: np.ndarray, rng: np.random.Generator,
+                      garble_frac: float = 0.0):
+    """(frames uint8[nb,14], nbytes int[nb]): per burst a frame of format dfs[k] from the aircraft addrs[k]. DF11/DF17
+    carry the address in bytes 1..3 and CRC xor codes[k] as parity (codes[k] = 0 for DF17); every other format carries
+    random fields and CRC xor address as parity. Short frames are zero beyond byte 7; garble flips 1..5 random bits."""
+    nb = dfs.size
+    fr, nbytes = make_frames(dfs, rng)                  # random bodies, CRC parity (II = 0)
+    sq = (dfs == 11) | (dfs == 17)
+    for k in range(3):
+        fr[sq, 1 + k] = (addrs[sq] >> (16 - 8 * k)) & 0xFF
+    long_ = nbytes == 14
+    T = _crc_table()
+    crc_s = np.zeros(nb, np.uint32)
+    crc_l = np.zeros(nb, np.uint32)
+    for i in range(11):                                 # the CRC again over the bodies with their addresses
+        crc_l = T[((crc_l >> 16) ^ fr[:, i]) & 0xFF] ^ ((crc_l << 8) & 0xFFFFFF)
+        if i == 3:
+            crc_s = crc_l.copy()
+    par = np.where(long_, crc_l, crc_s) ^ np.where(sq, codes, addrs).astype(np.uint32)
+    col = np.where(long_, 11, 4)
+    rows = np.arange(nb)
+    for k in range(3):
+        fr[rows, col + k] = (par >> (16 - 8 * k)) & 0xFF
+    if garble_frac > 0:
+        g = np.nonzero(rng.random(nb) < garble_frac)[0]
+        nflip = rng.integers(1, 6, g.size)
+        for k in range(5):
+            sel = g[nflip > k]
+            bit = (rng.random(sel.size) * (nbytes[sel] * 8)).astype(np.int64)
+            fr[sel, bit // 8] ^= (0x80 >> (bit % 8)).astype(np.uint8)
+    return fr, nbytes
+
+
+def fleet_plan(n_aircraft: int, n_bursts: int, rng: np.random.Generator, mix=FLEET_MIX):
+    """(dfs, addrs, codes, who) of n_bursts replies from n_aircraft aircraft with distinct random addresses; who[k] is
+    the aircraft of burst k (uniform), the formats follow `mix` (see FLEET_MIX)."""
+    fleet = rng.choice(np.arange(1, 1 << 24), n_aircraft, replace=False).astype(np.uint32)
+    who = rng.integers(0, n_aircraft, n_bursts)
+    kind = rng.choice(4, n_bursts, p=np.asarray(mix, np.float64) / np.sum(mix))
+    dfs = np.where(kind == 0, 17, np.where(kind == 3, np.asarray(FLEET_AP_DFS)[rng.integers(0, 6, n_bursts)], 11))
+    codes = np.where(kind == 2, rng.integers(1, 0x80, n_bursts), 0).astype(np.uint32)
+    return dfs, fleet[who], codes, who
+
+
+def make_fleet_scene(rate: float, n: int, n_aircraft: int, n_bursts: int, seed: int, *, noise_sigma: float = 0.01,
+                     snr_db=(8.0, 30.0), mix=FLEET_MIX, garble_frac: float = 0.0, fruit: int = 0,
+                     min_gap: float | None = 16.0, quantize_bits: int | None = None) -> Scene:
+    """make_scene's waveform model (per burst, on the CPU) for a fleet: n_bursts replies of n_aircraft aircraft
+    (fleet_plan, make_fleet_frames), non-overlapping on a jittered grid with min_gap samples between bursts (None:
+    uniform starts, overlaps allowed). Each Burst's frame is the frame sent."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    spc = rate / 2e6
+    iq = (rng.standard_normal((n, 2), dtype=np.float32) * np.float32(noise_sigma))
+    c = iq.view(np.complex64).reshape(n)
+    span = 240 * spc + 8
+    if min_gap is not None:
+        slots = int((n - 2 * span) // (span + min_gap))
+        pick = np.sort(rng.choice(slots, size=min(n_bursts, slots), replace=False))
+        starts = span / 2 + pick * (span + min_gap) + rng.uniform(0, min_gap, pick.size)
+    else:
+        starts = np.sort(rng.uniform(span, n - 2 * span, n_bursts))
+    dfs, addrs, codes, _ = fleet_plan(n_aircraft, starts.size, rng, mix)
+    frames, nbytes = make_fleet_frames(dfs, addrs, codes, rng, garble_frac)
+    bursts = []
+    for k, s in enumerate(starts):
+        amp = float(np.sqrt(2.0 * noise_sigma ** 2 * 10 ** (rng.uniform(*snr_db) / 10)))
+        b = Burst(float(s), frames[k, :nbytes[k]].tobytes(), amp, float(rng.uniform(0, 2 * np.pi)))
+        n0, w = burst_waveform(b, spc)
+        lo, hi = max(n0, 0), min(n0 + w.size, n)
+        if hi > lo:
+            c[lo:hi] += w[lo - n0:hi - n0]
+        bursts.append(b)
+    for _ in range(fruit):
+        s = rng.uniform(0, n - 64 * spc)
+        amp = float(np.sqrt(2.0 * max(noise_sigma, 1e-3) ** 2 * 10 ** (rng.uniform(10, 30) / 10)))
+        ph = rng.uniform(0, 2 * np.pi)
+        for off in (0.0, rng.integers(1, 14) * 1.45 * 2 * spc):
+            a0 = int(s + off)
+            a1 = min(a0 + max(int(round(0.9 * spc)), 1), n)
+            c[a0:a1] += np.complex64(amp * np.exp(1j * ph))
+    if quantize_bits is not None:
+        q = float(1 << (quantize_bits - 1))
+        np.clip(np.rint(iq * q), -q, q - 1, out=iq)
+        iq /= np.float32(q)
+    return Scene(rate, n, iq.reshape(2 * n), bursts)
+
+
+def make_fleet_scene_device(rate: float, n: int, n_aircraft: int, n_bursts: int, seed: int, device, *,
+                            noise_sigma: float = 0.01, snr_db=(6.0, 30.0), mix=FLEET_MIX, garble_frac: float = 0.0,
+                            fruit: int = 0, out=None):
+    """The fleet on the device, for long scenes: make_scene_device's renderer (uniform starts, overlaps allowed) over
+    the frames of fleet_plan / make_fleet_frames. Returns (iq float32 CUDA tensor[2n], (frames, nbytes, starts, who))."""
+    import torch
+    rng = np.random.Generator(np.random.PCG64(seed))
+    spc = rate / 2e6
+    g = torch.Generator(device=device)
+    g.manual_seed(2000 + seed)
+    iq = out if out is not None else torch.empty(2 * n, device=device, dtype=torch.float32)
+    step = 1 << 26
+    for a in range(0, 2 * n, step):
+        m = min(step, 2 * n - a)
+        torch.randn(m, device=device, generator=g, out=iq[a:a + m])
+        iq[a:a + m] *= noise_sigma
+    iq2 = iq.view(n, 2)
+    span = 240 * spc + 8
+    starts = np.sort(rng.uniform(span, n - 2 * span, n_bursts))
+    dfs, addrs, codes, who = fleet_plan(n_aircraft, n_bursts, rng, mix)
+    frames, nbytes = make_fleet_frames(dfs, addrs, codes, rng, garble_frac)
+    snr = rng.uniform(snr_db[0], snr_db[1], n_bursts)
+    amp = np.sqrt(2.0 * noise_sigma ** 2 * 10 ** (snr / 10))
+    phase = rng.uniform(0, 2 * np.pi, n_bursts)
+    bits = np.unpackbits(frames, axis=1)
+    valid = np.arange(112)[None, :] < (nbytes * 8)[:, None]
+    chips = np.zeros((n_bursts, 240), np.float32)
+    chips[:, [0, 2, 7, 9]] = 1.0
+    chips[:, 16:240:2] = bits * valid
+    chips[:, 17:240:2] = (1 - bits) * valid
+    M = int(np.ceil(240 * spc)) + 2
+    mgrid = torch.arange(M + 1, device=device, dtype=torch.float64)
+    B = max(1, (1 << 24) // (M + 1))
+    for a in range(0, n_bursts, B):
+        b = min(a + B, n_bursts)
+        s = torch.from_numpy(starts[a:b]).to(device)
+        n0 = torch.floor(s)
+        ch = torch.from_numpy(chips[a:b]).to(device).to(torch.float64)
+        cum = torch.cumsum(ch, 1) - ch
+        t = (((n0 - s)[:, None] + mgrid[None, :]) / spc).clamp_(0.0, 240.0)
+        k = t.floor().clamp_(max=239.0)
+        ki = k.to(torch.int64)
+        integ = (torch.gather(cum, 1, ki) + torch.gather(ch, 1, ki) * (t - k)) * spc
+        w = torch.from_numpy(amp[a:b]).to(device)[:, None] * (integ[:, 1:] - integ[:, :-1])
+        ph = torch.from_numpy(phase[a:b]).to(device)[:, None]
+        vals = torch.stack((w * torch.cos(ph), w * torch.sin(ph)), 2).to(torch.float32).reshape(-1, 2)
+        idx = (n0.to(torch.int64)[:, None] + torch.arange(M, device=device)[None, :]).reshape(-1)
+        ok = (idx >= 0) & (idx < n)
+        iq2.index_add_(0, idx[ok], vals[ok])
+    if fruit:
+        s = rng.uniform(0, n - 64 * spc, fruit)
+        fa = np.sqrt(2.0 * max(noise_sigma, 1e-3) ** 2 * 10 ** (rng.uniform(10, 30, fruit) / 10))
+        ph = rng.uniform(0, 2 * np.pi, fruit)
+        off2 = rng.integers(1, 14, fruit) * 1.45 * 2 * spc
+        wlen = max(int(round(0.9 * spc)), 1)
+        a0 = np.concatenate([s.astype(np.int64), (s + off2).astype(np.int64)])
+        idx = torch.from_numpy((a0[:, None] + np.arange(wlen)[None, :]).reshape(-1)).to(device)
+        v = np.stack([fa * np.cos(ph), fa * np.sin(ph)], 1).astype(np.float32)
+        vals = torch.from_numpy(np.repeat(np.concatenate([v, v]), wlen, axis=0)).to(device)
+        ok = (idx >= 0) & (idx < n)
+        iq2.index_add_(0, idx[ok], vals[ok])
+    return iq, (frames, nbytes, starts, who)

@@ -65,7 +65,7 @@ typedef struct amb_frame {
     uint8_t data[14];
     uint8_t ec;              /* error correction outcome, AMB_EC_* (option "ec"); 0 unless it was attempted */
     uint8_t ec_flips;        /* bits flipped by a correction (AMB_EC_FIXED), else 0 */
-    uint8_t pad_[4];         /* [0] ec_any, [1..2] ec_any_bits (option "ec_any", read through AMB_FRAME_EC_ANY*), [3] 0 */
+    uint8_t pad_[4];         /* [0] ec_any, [1..2] ec_any_bits (AMB_FRAME_EC_ANY*), [3] ap_filter outcome (AMB_FRAME_AP) */
 } amb_frame;                 /* 80 bytes */
 
 /* amb_frame.ec: what the opt-in error correction (amb_set_option(ctx, "ec", K), K in 1..23) made of a DF11/DF17 frame
@@ -87,6 +87,22 @@ typedef struct amb_frame {
  * frame), so the declared layout of amb_frame is the one it had before this pass existed: */
 #define AMB_FRAME_EC_ANY(f) ((f)->pad_[0])                  /* AMB_EC_NOT_TRIED, AMB_EC_FIXED or AMB_EC_NO_SOLUTION */
 #define AMB_FRAME_EC_ANY_BIT(f, i) ((f)->pad_[1 + (i)])     /* i = 0, 1: flipped positions, ascending; 0 = unused */
+
+/* Address/parity check (amb_set_option(ctx, "ap_filter", S), S in 1..3600 seconds), after both correction passes.
+ * A confirmer is a DF11/DF17 frame that passed with crc == 0 and that neither correction pass fixed; its address is
+ * AA (data[1..3]). Subjects are never confirmers:
+ *   AP subject     passed and df not in {11, 17}; its address is the syndrome in crc (AP xor parity)
+ *   II/SI subject  df == 11, not passed, 0 < crc < 0x80 (an interrogator code in the parity); its address is AA
+ * A subject is KNOWN when a confirmer g of the same address lies in this stream (since amb_reset / amb_set_rate, in a
+ * call made with the option on) with g.sample_index < f.sample_index <= g.sample_index + S * (int)rate. A known AP
+ * subject is unchanged and an unknown one gets passed = 0; a known II/SI subject gets passed = 1 (its message shows the
+ * code as the crc token) and an unknown one stays dropped. data and crc are never changed. frames_passed counts the
+ * result. The outcome lives in the last byte of amb_frame.pad_ (byte 79 of the frame), which the slicer zeroes.
+ * The split-form amb_slicer_process carries no stream position and leaves it at AMB_AP_NOT_CHECKED. */
+#define AMB_FRAME_AP(f) ((f)->pad_[3])
+#define AMB_AP_NOT_CHECKED 0     /* not a subject, or the option was off */
+#define AMB_AP_KNOWN 1           /* a confirmer of its address lies in the window */
+#define AMB_AP_UNKNOWN 2         /* none does: an AP reply is dropped, an II/SI reply stays dropped */
 
 typedef struct amb_stats {
     uint64_t samples_in;     /* complex samples accepted so far on this stream */
@@ -239,7 +255,12 @@ AMB_API int amb_debug_candidates(amb_ctx* ctx, uint64_t* index, uint32_t* info, 
 /* "resolver": 0 auto, 1 sequential, 2 parallel. "ec": K = 0 (default, off) .. 23, error correction over the
  * low-confidence bits of frames dropped for their CRC (see AMB_EC_*); persists across amb_reset / amb_set_rate.
  * "ec_any": M = 0 (default, off), 1 or 2, correction of DF17 frames by at most M flipped bits anywhere in 5..111, after
- * "ec" (see amb_frame.ec_any); persists likewise. Both apply from the next call. */
+ * "ec" (see amb_frame.ec_any); persists likewise. Both apply from the next call.
+ * "ap_filter": S = 0 (default, off) .. 3600 seconds, the address/parity check against the aircraft confirmed within
+ * the last S seconds (see AMB_FRAME_AP); persists likewise and applies from the next call, while the table of confirmed
+ * addresses (128 MiB of device memory, allocated at the first call with the option on) is cleared by amb_reset /
+ * amb_set_rate. Not available in time-sharded operation: with S > 0, amb_seek and "defer_resolve" = 1 return
+ * AMB_ERR_STATE, and so does setting S > 0 while "defer_resolve" is on or after an amb_seek (until amb_reset). */
 AMB_API int amb_set_option(amb_ctx* ctx, const char* name, int value);
 /* Parity dump of the GNU Radio front end wired in rx_path.py:38-54, for a short HOST buffer taken as a whole stream
  * (zeros before sample 0): stage M2 = complex_to_mag_squared (:38), BB = the preamble block's in0 (PMF output, :48-51,

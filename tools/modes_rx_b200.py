@@ -161,6 +161,9 @@ def main(argv=None):
                     help="correct DF11/DF17 frames over at most K (1..23) low-confidence bits; 0 = off, as the reference")
     ap.add_argument("--ec-any", type=int, default=0, metavar="M",
                     help="correct DF17 frames by at most M (1, 2) flipped bits anywhere, after --ec; 0 = off, as the reference")
+    ap.add_argument("--ap-filter", type=int, default=0, metavar="S",
+                    help="drop address/parity replies from aircraft not confirmed by a clean DF11/DF17 in the last S "
+                         "seconds, and accept DF11 replies with an II/SI code from confirmed ones; 0 = off, as the reference")
     args = ap.parse_args(argv)
 
     if args.source in ("uhd", "osmocom"):
@@ -195,7 +198,7 @@ def main(argv=None):
         pub = zmq_queue(["tcp://*:%i" % args.tcp])
         sinks.append(pub)
     rx = air_modes.rx_path(rx_rate, args.threshold, tee_queue(sinks), args.pmf, args.dcblock, device=args.device,
-                           ec=args.ec, ec_any=args.ec_any)   # radio.py:55-56
+                           ec=args.ec, ec_any=args.ec_any, ap_filter=args.ap_filter)   # radio.py:55-56
 
     if ":" in args.source and not os.path.exists(args.source):
         m = re.search(r"(.*)\:(\d{1,5})$", args.source)                                                           # radio.py:223-226
