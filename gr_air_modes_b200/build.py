@@ -30,9 +30,8 @@ def needs_build() -> bool:
     return any(os.path.getmtime(os.path.join(CSRC, f)) > t for f in SOURCES + HEADERS)
 
 
-def build_native(force: bool = False, verbose: bool = False, defines=(), out_path: str | None = None) -> str:
-    """defines/out: experiment builds (tools/variants.py); the product build uses neither."""
-    if out_path is None and not force and not needs_build():
+def build_native(force: bool = False, verbose: bool = False) -> str:
+    if not force and not needs_build():
         return LIB
     nvcc = _nvcc()
     env = dict(os.environ)
@@ -40,8 +39,8 @@ def build_native(force: bool = False, verbose: bool = False, defines=(), out_pat
     objs = []
     procs = []
     for src in SOURCES:
-        obj = os.path.join(CSRC, src.replace(".cu", ".o" if out_path is None else "." + os.path.basename(out_path) + ".o"))
-        cmd = [nvcc, "-ccbin", host, *NVCC_FLAGS, *EXTRA_FLAGS.get(src, []), *["-D" + d for d in defines], "-c", os.path.join(CSRC, src), "-o", obj]
+        obj = os.path.join(CSRC, src.replace(".cu", ".o"))
+        cmd = [nvcc, "-ccbin", host, *NVCC_FLAGS, *EXTRA_FLAGS.get(src, []), "-c", os.path.join(CSRC, src), "-o", obj]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
         procs.append((cmd, subprocess.Popen(cmd, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)))
@@ -52,10 +51,9 @@ def build_native(force: bool = False, verbose: bool = False, defines=(), out_pat
             raise RuntimeError("nvcc failed: %s\n%s" % (" ".join(cmd), out.decode()))
         if verbose:
             print(out.decode())
-    target = LIB if out_path is None else out_path
-    cmd = [nvcc, "-ccbin", host, "-shared", "-Wno-deprecated-gpu-targets", "-o", target, *objs, "-cudart", "shared"]
+    cmd = [nvcc, "-ccbin", host, "-shared", "-Wno-deprecated-gpu-targets", "-o", LIB, *objs, "-cudart", "shared"]
     subprocess.run(cmd, check=True, env=env)
-    return target
+    return LIB
 
 
 if __name__ == "__main__":

@@ -1,23 +1,15 @@
 // Batch field decode (SURVEY.md 8 row f4): kernels + C ABI of amb_decoder (include/airmodes_b200.h).
-// The per-message arithmetic is in amb_decode_core.h, the three kernels in amb_decode_kernels.cuh (a launch-free
-// header, so that tests/simt can run the same kernel source under a host emulator); this file holds the per-aircraft
-// report table and the host orchestration. Compiled with -fmad=false: latitude/longitude follow cpr.py operation by
-// operation in IEEE double, nothing may be contracted. Citations are file:line under gr-air-modes/python.
+// The per-message arithmetic is in amb_decode_core.h, the kernels in amb_decode_kernels.cuh and amb_decode_v3.cuh
+// (launch-free headers, so that tests/simt can run the same kernel source under a host emulator); this file holds the
+// per-aircraft report table and the host orchestration. Compiled with -fmad=false: latitude/longitude follow cpr.py
+// operation by operation in IEEE double, nothing may be contracted. Citations are file:line under gr-air-modes/python.
 //
+// Seven launches per decode, in stream order:
 //   amb_fields_kernel   one thread per frame: bit fields, altitude, squawk, ident, velocity; emits the CPR report
-//   amb_pair_kernel     cpr_decoder's bookkeeping (cpr.py:206-229): for every position message, the latest even and
-//                       odd report of its aircraft as of that message. The reference does this one message at a time
-//                       against four dicts; here aircraft are dealt out to warps by a hash of their key, every warp
-//                       walks the batch in stream order 32 frames per step, resolves same-aircraft reports inside a
-//                       step with match/ballot and everything older through a direct-mapped table in HBM
-//                       (2^26 x 16 B: one slot per (ICAO, surface, even/odd), so no probing, no collisions, no locks -
-//                       a slot has exactly one owner warp).
+//   amb_v3_*            five kernels, cpr_decoder's bookkeeping (cpr.py:206-229): for every position message, the latest
+//                       even and odd report of its aircraft as of that message, from the reports partitioned by owner
+//                       bucket and a direct-mapped table in HBM (2^26 x 16 B) that carries them from batch to batch
 //   amb_resolve_kernel  one thread per frame: global CPR decode, range/bearing.
-// The pairing stage is the bucket-partition version (amb_decode_v3.cuh: O(n) traffic, one warp per owner bucket);
-// -DAMB_PAIR_V1 / -DAMB_PAIR_V2 select the two earlier experiments (every warp walks the whole report list).
-#if !defined(AMB_PAIR_V1) && !defined(AMB_PAIR_V2) && !defined(AMB_PAIR_V3)
-#define AMB_PAIR_V3 1
-#endif
 #include "amb_launch.h"
 #include "amb_decode_core.h"
 #include "amb_decode_kernels.cuh"
@@ -29,7 +21,7 @@
 #include <string>
 
 struct amb_decoder {
-    int device = 0, sm_count = 0;
+    int device = 0;
     cudaStream_t stream = nullptr;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     int have_loc = 0; double lat = 0.0, lon = 0.0;
@@ -40,12 +32,7 @@ struct amb_decoder {
     // host <-> device staging: pageable caller arrays go through two pinned bounce buffers per direction so that the
     // copies run at PCIe speed and overlap the memcpy of the next piece
     void* pin[2] = {nullptr, nullptr}; cudaEvent_t pin_ev[2] = {nullptr, nullptr}; size_t pin_bytes = 0;
-#ifdef AMB_PAIR_V2
-    uint32_t* d_keys = nullptr;
-#endif
-#ifdef AMB_PAIR_V3
-    AmbV3Bufs v3;
-#endif
+    AmbV3Bufs v3;                        // scratch of the pairing stage
     uint64_t launches = 0; float ms_last = 0.f;
     std::string err;
 };
@@ -122,10 +109,6 @@ static void free_bufs(amb_decoder* d)
     if (d->d_fields) cudaFree(d->d_fields);
     if (d->d_pos) cudaFree(d->d_pos);
     if (d->d_pair) cudaFree(d->d_pair);
-#ifdef AMB_PAIR_V2
-    if (d->d_keys) cudaFree(d->d_keys);
-    d->d_keys = nullptr;
-#endif
     d->d_frames = nullptr; d->d_fields = nullptr; d->d_pos = nullptr; d->d_pair = nullptr; d->cap = 0;
 }
 
@@ -139,9 +122,6 @@ static int ensure_cap(amb_decoder* d, int n)
     DCK(cudaMalloc(&d->d_fields, (size_t)cap * sizeof(amb_fields)));
     DCK(cudaMalloc(&d->d_pos, (size_t)cap * sizeof(AmbPosRec)));
     DCK(cudaMalloc(&d->d_pair, (size_t)cap * sizeof(AmbPair)));
-#ifdef AMB_PAIR_V2
-    DCK(cudaMalloc(&d->d_keys, (size_t)cap * sizeof(uint32_t)));
-#endif
     d->cap = cap;
     return AMB_OK;
 }
@@ -161,7 +141,7 @@ int amb_decoder_create(int device, int have_location, double lat, double lon, am
     if (prop.major != 9 || prop.minor != 0) return AMB_ERR_NO_DEVICE;   // sm_90a cubin only; there is no CPU path
     amb_decoder* d = new (std::nothrow) amb_decoder();
     if (!d) return AMB_ERR_INVALID;
-    d->device = device; d->sm_count = prop.multiProcessorCount;
+    d->device = device;
     d->have_loc = have_location ? 1 : 0; d->lat = lat; d->lon = lon;
     int rc = AMB_OK;
     do {
@@ -189,9 +169,7 @@ void amb_decoder_destroy(amb_decoder* d)
     cudaSetDevice(d->device);
     if (d->stream) cudaStreamSynchronize(d->stream);
     free_bufs(d);
-#ifdef AMB_PAIR_V3
     amb_v3_free(&d->v3);
-#endif
     for (int k = 0; k < 2; k++) { if (d->pin[k]) cudaFreeHost(d->pin[k]); if (d->pin_ev[k]) cudaEventDestroy(d->pin_ev[k]); }
     if (d->table) cudaFree(d->table);
     if (d->nl_T) cudaFree(d->nl_T);
@@ -251,40 +229,12 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
     const int nb = (n + 127) / 128;
     AMB_LAUNCH((amb_fields_kernel), nb, 128, 0, s, src, n, fields, d->d_pos, d->d_pair);
     DCK(cudaGetLastError());
-    // one warp per ~256 frames, at most 8 CTAs per SM: every warp reads the whole key list (L2-resident) but only
-    // touches the table for its own aircraft
-    int warps = n / 256;
-    const int max_warps = d->sm_count * 8 * AMB_PAIR_WARPS_PER_CTA;
-    if (warps > max_warps) warps = max_warps;
-    if (warps < AMB_PAIR_WARPS_PER_CTA) warps = AMB_PAIR_WARPS_PER_CTA;
-    const int pair_ctas = (warps + AMB_PAIR_WARPS_PER_CTA - 1) / AMB_PAIR_WARPS_PER_CTA;
-#if defined(AMB_PAIR_V3)
-    {
-        cudaError_t e3 = cudaSuccess;
-        const int k3 = amb_v3_launch(&d->v3, d->d_pos, n, d->table, d->d_pair, s, &e3);
-        if (k3 < 0) return dfail(d, AMB_ERR_CUDA, "pairing v3", e3);
-        (void)pair_ctas;
-        d->launches += (uint64_t)(k3 - 1);
-    }
-#elif defined(AMB_PAIR_V2)
-    {
-        int w2 = n / 1024;
-        if (w2 > max_warps) w2 = max_warps;
-        if (w2 < AMB_PAIR_WARPS_PER_CTA) w2 = AMB_PAIR_WARPS_PER_CTA;
-        AMB_LAUNCH((amb_keys_kernel), nb, 128, 0, s, d->d_pos, n, d->d_keys);
-        DCK(cudaGetLastError());
-        AMB_LAUNCH((amb_pair_kernel_v2), (w2 + AMB_PAIR_WARPS_PER_CTA - 1) / AMB_PAIR_WARPS_PER_CTA, 32 * AMB_PAIR_WARPS_PER_CTA, 0, s,
-                   d->d_keys, d->d_pos, n, d->table, d->d_pair);
-        (void)pair_ctas;
-        d->launches += 1;
-    }
-#else
-    AMB_LAUNCH((amb_pair_kernel), pair_ctas, 32 * AMB_PAIR_WARPS_PER_CTA, 0, s, d->d_pos, n, d->table, d->d_pair);
-#endif
-    DCK(cudaGetLastError());
+    cudaError_t e = cudaSuccess;
+    const int k = amb_v3_launch(&d->v3, d->d_pos, n, d->table, d->d_pair, s, &e);
+    if (k < 0) return dfail(d, AMB_ERR_CUDA, "pairing", e);
     AMB_LAUNCH((amb_resolve_kernel), nb, 128, 0, s, fields, d->d_pos, d->d_pair, n, d->have_loc, d->lat, d->lon, d->nl_T);
     DCK(cudaGetLastError());
-    d->launches += 3;
+    d->launches += 2 + (uint64_t)k;
     if (!out_on_device) {
         rc = staged_d2h(d, out, d->d_fields, (size_t)n * sizeof(amb_fields), s);
         if (rc != AMB_OK) return rc;

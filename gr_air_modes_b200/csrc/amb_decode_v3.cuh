@@ -1,11 +1,10 @@
-// Pairing stage of the batch decoder with O(n) memory traffic - the product path since round 2 (AMB_PAIR_V3 is the
-// default in amb_decode.cu).
-//
-// Round 1's pairing kernel (still selectable with -DAMB_PAIR_V1) lets every warp walk the whole report list and pick out
-// its own aircraft (n warps x n reports of L2 reads). Here the reports are first PARTITIONED by
-// owner: a stable counting sort of the frame indices into AMB_V3_B buckets (bucket = hash of the aircraft key), so
-// that each bucket's list keeps stream order; then one warp per bucket walks only its own list with the same
-// per-step logic (match/ballot inside a step, the direct-mapped HBM table across steps and batches).
+// Pairing stage of the batch decoder: cpr_decoder's bookkeeping (cpr.py:206-229). For every position message it finds
+// the latest even and odd report of its aircraft as of that message; the reference does this one message at a time
+// against four dicts. Here the reports are first PARTITIONED by owner: a stable counting sort of the frame indices into
+// AMB_V3_B buckets (bucket = hash of the aircraft key), so that each bucket's list keeps stream order. Then one warp per
+// bucket walks only its own list, 32 reports per step: same-aircraft reports inside a step are resolved with
+// match/ballot, everything older through a direct-mapped table in HBM (AMB_TABLE_SLOTS x 16 B: one slot per (ICAO,
+// surface, even/odd), so no probing, no collisions, no locks - a slot has exactly one owner bucket). O(n) memory traffic.
 //
 //   amb_v3_count    per tile of 8192 frames: histogram of the buckets (shared-memory atomics) -> cnt[bucket][tile]
 //   amb_v3_rowscan  one warp per bucket: exclusive scan along the tiles -> off[bucket][tile], tot[bucket]
@@ -137,10 +136,12 @@ __global__ void __launch_bounds__(128) amb_v3_pair(const AmbPosRec* __restrict__
         const int k = mine ? (int)order[i] : 0;
         AmbPosRec me; me.key = AMB_NO_KEY; me.lat = me.lon = 0; me.fmt = 0; me.t = 0.0;
         if (mine) me = pos[k];
-        // from here on: the product kernel's step (amb_pair_kernel), lane order = stream order inside the bucket
+        // same aircraft inside this step (lane order = stream order inside the bucket); lanes past the end of the bucket
+        // get a private value
         const unsigned peers = __match_any_sync(0xffffffffu, mine ? me.key : (0x80000000u | lane));
         const unsigned evens = __ballot_sync(0xffffffffu, mine && me.fmt == 0);
         const unsigned odds = __ballot_sync(0xffffffffu, mine && me.fmt != 0);
+        // the latest report of the OTHER format at or before this message: an earlier lane of this step, else the table
         const unsigned other_here = peers & (me.fmt ? evens : odds) & lt;
         const int src = other_here ? (31 - __clz(other_here)) : (int)lane;
         uint32_t o_lat = __shfl_sync(0xffffffffu, me.lat, src);
@@ -150,18 +151,19 @@ __global__ void __launch_bounds__(128) amb_v3_pair(const AmbPosRec* __restrict__
         const size_t slot_other = ((size_t)me.key << 1) | (me.fmt ? 0u : 1u);
         const size_t slot_mine = ((size_t)me.key << 1) | (me.fmt ? 1u : 0u);
         if (mine && !o_have) {
-            const uint4 v = __ldcg(reinterpret_cast<const uint4*>(&table[slot_other]));
+            const uint4 v = __ldcg(reinterpret_cast<const uint4*>(&table[slot_other]));     // L2, never a stale L1 line
             if (v.x != 0xFFFFFFFFu) { o_lat = v.x; o_lon = v.y; o_t = __hiloint2double((int)v.w, (int)v.z); o_have = true; }
         }
         if (mine) pair[k] = amb_make_pair(me, o_have ? 1 : 0, o_lat, o_lon, o_t);
-        __syncwarp();
+        __syncwarp();                                                       // every table read of this step is done
+        // cpr.py:214-221: the message's own report replaces the stored one; the last lane per (aircraft, format) wins
         const unsigned same = peers & (me.fmt ? odds : evens);
         if (mine && (int)lane == 31 - __clz(same)) {
             const uint4 v = make_uint4(me.lat, me.lon, (unsigned)__double2loint(me.t), (unsigned)__double2hiint(me.t));
             __stcg(reinterpret_cast<uint4*>(&table[slot_mine]), v);
             __threadfence_block();
         }
-        __syncwarp();
+        __syncwarp();                                                       // ... and visible to the next step's reads
     }
 }
 

@@ -14,29 +14,6 @@
 #include "amb_internal.h"
 
 #define FULL 0xffffffffu
-#ifndef AMB_EXACT_DENSE
-#define AMB_EXACT_DENSE 65536u     // candidates per call beyond which the row-based exact kernel takes over
-#endif
-#ifndef AMB_NST
-#define AMB_NST 2
-#endif
-#ifndef AMB_PROXY_FENCE
-#define AMB_PROXY_FENCE 0
-#endif
-// Register cap of the scan kernel. Four of its CTAs are resident per SM for the whole pass (one wave); at 112 registers
-// they leave 8 K registers (and ~60 KiB of shared memory) per SM free, which is what lets the sparse kernels of the
-// previous call (<= 128 threads x 64 registers, or 64 x 128) run UNDER the scan instead of after it.
-#ifndef AMB_SCAN_REGS
-#define AMB_SCAN_REGS 112
-#endif
-// ... applied where it costs no spills (spc <= 2); the long filters keep all 128 registers.
-#ifndef AMB_SCAN_REGS_HI
-#define AMB_SCAN_REGS_HI 120
-#endif
-// spc 3..5: 120 registers leave 4 K registers (and 25 KiB of shared memory) for the sparse kernels, so that they overlap
-// the scan. spc >= 6: the prefix ring leaves too little shared memory for anything to be resident beside the scan, so it
-// keeps every register. (The SM's 64 K registers and 228 KiB of shared memory are the same on sm_90 and sm_100.)
-#define AMB_SCAN_REGS_FOR(SPC) ((SPC) <= 2 ? AMB_SCAN_REGS : (SPC) <= 5 ? AMB_SCAN_REGS_HI : 128)
 
 __constant__ unsigned int c_crc_rem[96]; // x^(t+24) mod 0xFFF409, t = distance of a message bit from the parity field
 
@@ -47,7 +24,7 @@ __constant__ unsigned int c_crc_rem[96]; // x^(t+24) mod 0xFFF409, t = distance 
 // shared table: two contexts with different rates can coexist on one device)
 __device__ __forceinline__ int chip_off(int j, float spc_f) { return __float2int_rz(__fmul_rn((float)j, spc_f)); }
 
-#ifndef AMB_SIMT_EMUL   // PTX (mbarrier / TMA): tests/simt supplies host stand-ins for these seven helpers
+#ifndef AMB_SIMT_EMUL   // PTX (mbarrier / TMA): tests/simt supplies host stand-ins for these six helpers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
@@ -73,7 +50,6 @@ __device__ __forceinline__ bool elect_one() {   // one lane of the (converged) w
     asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
     return pred != 0;
 }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
 #endif
@@ -118,7 +94,7 @@ template <int SPC, bool PMF, int PREF> struct ScanCfg {
     static constexpr int RB = L / AMB_ROW;
     static constexpr int LMOD = L % AMB_ROW;
     static constexpr int PRR = RB + 2;             // prefix ring rows: k, ..., k-RB-1
-    static constexpr int NST = AMB_NST;            // TMA tile ring depth per warp (tile = 2 rows = 4 KiB)
+    static constexpr int NST = 2;                  // TMA tile ring depth per warp (tile = 2 rows = 4 KiB)
     static constexpr int WARM = (RB + 2 + 1) & ~1;
     static constexpr int IQ_BYTES = NST * 4096;                    // per warp, 1 KiB aligned
     static constexpr int BB_FLOATS = (PREF == 2) ? 0 : 512;               // look-ahead ring only when pulse offsets are run-time values
@@ -286,11 +262,7 @@ struct ScanWarp {
         cur.t[6] = (cAg - d1.z) + p[6]; cur.t[7] = (cAg - d1.w) + p[7];
         // ---- evaluate row k-1 (its look-ahead reaches into row k, now in registers / the ring)
         const int ke = k - 1;
-#ifdef AMB_DBG_NOEVAL
-        if (ke >= ra && cur.t[0] + cur.t[3] + cur.t[7] == 12345.678f) {
-#else
         if (ke >= ra) {
-#endif
             // A candidate needs all four preamble pulses above the (lowered) threshold of its start sample
             // (:174, :177-179). With integer samples/chip the pulse offsets are the compile-time 2,7,9*SPC and
             // the look-ahead comes from registers + one shuffle each; otherwise only the first pulse is
@@ -388,8 +360,15 @@ struct ScanWarp {
     }
 };
 
+// Register cap of the scan kernel. Four of its CTAs are resident per SM for the whole pass (one wave); at 112 registers
+// they leave 8 K registers (and ~60 KiB of shared memory) per SM free, which is what lets the sparse kernels of the
+// previous call (<= 128 threads x 64 registers, or 64 x 128) run UNDER the scan instead of after it. 112 is applied
+// where it costs no spills (spc <= 2). spc 3..5: 120 registers leave 4 K registers (and 25 KiB of shared memory) for the
+// sparse kernels, so that they overlap the scan. spc >= 6: the prefix ring leaves too little shared memory for anything
+// to be resident beside the scan, so it keeps every register. (The SM's 64 K registers and 228 KiB of shared memory are
+// the same on sm_90 and sm_100.)
 template <int SPC, bool PMF, int PREF>
-__global__ void __maxnreg__(AMB_SCAN_REGS_FOR(SPC)) amb_scan_kernel(const __grid_constant__ AmbScanArgs a)
+__global__ void __maxnreg__((SPC) <= 2 ? 112 : (SPC) <= 5 ? 120 : 128) amb_scan_kernel(const __grid_constant__ AmbScanArgs a)
 {
     using C = ScanCfg<SPC, PMF, PREF>;
     AMB_DYN_SMEM(unsigned char, smem, 1024);
@@ -445,22 +424,11 @@ __global__ void __maxnreg__(AMB_SCAN_REGS_FOR(SPC)) amb_scan_kernel(const __grid
         while (!mbar_try_wait(w.bar0 + 8 * slot, par)) {}
         const unsigned char* st = w.iq + slot * 4096;
         const int k = (t0 + tl) << 1;
-#ifdef AMB_DBG_LOADONLY
-        {
-            const float4 v0 = *reinterpret_cast<const float4*>(st + w.off[0]);
-            const float4 v1 = *reinterpret_cast<const float4*>(st + 2048 + w.off[3]);
-            if (v0.x + v1.w == 12345.678f) w.cnt++;
-        }
-#else
         w.step(k, st, ra_, rb_);
         if (k + 1 <= w.rb) w.step(k + 1, st + 2048, rb_, ra_);
-#endif
         __syncwarp();
         if (tl + C::NST < ntiles) {                         // refill this slot with tile tl+NST (warp-uniform condition)
-            if (elect_one()) {
-                if (AMB_PROXY_FENCE) fence_proxy_async();
-                w.issue(t0 + tl + C::NST, slot);
-            }
+            if (elect_one()) w.issue(t0 + tl + C::NST, slot);
         }
         if (++slot == C::NST) { slot = 0; par ^= 1u; }
     }

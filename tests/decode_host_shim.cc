@@ -1,6 +1,6 @@
 // TEST HARNESS, not a product path: compiles the product's per-message decode functions
 // (gr_air_modes_b200/csrc/amb_decode_core.h - the __host__ __device__ code the CUDA kernels call) for the host, so
-// that tests/test_decode_cpu.py can check that arithmetic against the reference's golden without a GPU. The three
+// that tests/test_decode_cpu.py can check that arithmetic against the reference's golden without a GPU. The
 // kernels of amb_decode.cu are replayed one message at a time; the report table is a std::unordered_map here
 // (direct-mapped HBM table + warp bookkeeping on the device - that part is only exercised by the GPU tests).
 // Built by the test into a temporary directory with plain g++; never shipped, never loaded by the package.
@@ -22,7 +22,7 @@ extern "C" int shim_decode(const amb_frame* frames, int n, int have_loc, double 
         if (me.key == AMB_NO_KEY) continue;
         const uint64_t slot_other = ((uint64_t)me.key << 1) | (me.fmt ? 0u : 1u);
         const uint64_t slot_mine = ((uint64_t)me.key << 1) | (me.fmt ? 1u : 0u);
-        auto it = table.find(slot_other);                           // amb_pair_kernel, one lane at a time
+        auto it = table.find(slot_other);                           // amb_v3_pair, one lane at a time
         const bool have = it != table.end();
         const AmbPair pr = amb_make_pair(me, have, have ? it->second.lat : 0, have ? it->second.lon : 0, have ? it->second.t : 0.0);
         table[slot_mine] = Slot{me.lat, me.lon, me.t};

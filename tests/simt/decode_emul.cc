@@ -1,11 +1,10 @@
-// TEST HARNESS (not a product path): runs the decoder's kernel source - gr_air_modes_b200/csrc/amb_decode_kernels.cuh,
-// including the experimental pairing variants behind AMB_PAIR_V2 / AMB_PAIR_V3 - on the host under tests/simt/simt_emul.h,
-// with the launch sequence of amb_decode_frames (amb_decode.cu) replayed kernel by kernel. tests/test_decode_simt.py
-// compares the result with the sequential host shim and the oracle. Built by the test with plain g++.
+// TEST HARNESS (not a product path): runs the decoder's kernel source - gr_air_modes_b200/csrc/amb_decode_kernels.cuh
+// and amb_decode_v3.cuh - on the host under tests/simt/simt_emul.h, in the launch sequence of amb_decode_frames
+// (amb_decode.cu): the fields kernel, the pairing stage through its own launcher amb_v3_launch, the resolve kernel.
+// tests/test_decode_simt.py compares the result with the sequential host shim and the oracle. Built by the test with
+// plain g++.
 #include "simt_emul.h"
 
-#define AMB_PAIR_V2 1
-#define AMB_PAIR_V3 1
 #include "../../gr_air_modes_b200/csrc/amb_decode_kernels.cuh"
 
 #include <vector>
@@ -13,6 +12,7 @@
 struct Emul {
     std::vector<AmbCprSlot> table;
     double T[AMB_NL_MAX];
+    AmbV3Bufs v3;                                       // kept across calls, like the decoder's
 };
 
 extern "C" void* emul_new(int log2_slots)
@@ -23,11 +23,14 @@ extern "C" void* emul_new(int log2_slots)
     amb_build_nl_table(e->T);
     return e;
 }
-extern "C" void emul_free(void* h) { delete static_cast<Emul*>(h); }
+extern "C" void emul_free(void* h)
+{
+    Emul* e = static_cast<Emul*>(h);
+    amb_v3_free(&e->v3);
+    delete e;
+}
 
-// variant 1 = the product's pairing kernel, 2 / 3 = the experiments. `warps` = pairing warps of variants 1 and 2.
-extern "C" int emul_decode(void* h, const amb_frame* frames, int n, int variant, int warps, int have_loc, double lat,
-                           double lon, amb_fields* out)
+extern "C" int emul_decode(void* h, const amb_frame* frames, int n, int have_loc, double lat, double lon, amb_fields* out)
 {
     Emul* e = static_cast<Emul*>(h);
     if (n <= 0) return 0;
@@ -37,23 +40,8 @@ extern "C" int emul_decode(void* h, const amb_frame* frames, int n, int variant,
     simt_launch(nb, 128, [&] { amb_fields_kernel(frames, n, out, pos.data(), pair.data()); });
     for (int k = 0; k < n; k++)
         if (pos[k].key != AMB_NO_KEY && (((size_t)pos[k].key << 1) | 1u) >= e->table.size()) return -1;   // test table too small
-    AmbCprSlot* table = e->table.data();
-    const int ctas = (warps + AMB_PAIR_WARPS_PER_CTA - 1) / AMB_PAIR_WARPS_PER_CTA;
-    if (variant == 1) {
-        simt_launch(ctas, 32 * AMB_PAIR_WARPS_PER_CTA, [&] { amb_pair_kernel(pos.data(), n, table, pair.data()); });
-    } else if (variant == 2) {
-        std::vector<uint32_t> keys(n);
-        simt_launch(nb, 128, [&] { amb_keys_kernel(pos.data(), n, keys.data()); });
-        simt_launch(ctas, 32 * AMB_PAIR_WARPS_PER_CTA, [&] { amb_pair_kernel_v2(keys.data(), pos.data(), n, table, pair.data()); });
-    } else {                                            // amb_v3_launch (amb_decode_v3.cuh), kernel by kernel
-        const int n_tiles = (n + AMB_V3_TILE - 1) / AMB_V3_TILE;
-        std::vector<uint32_t> cnt((size_t)AMB_V3_B * n_tiles), off((size_t)AMB_V3_B * n_tiles), tot(AMB_V3_B), base(AMB_V3_B + 1), order(n);
-        simt_launch(n_tiles, 256, [&] { amb_v3_count(pos.data(), n, n_tiles, cnt.data()); });
-        simt_launch(AMB_V3_B / 8, 256, [&] { amb_v3_rowscan(cnt.data(), n_tiles, off.data(), tot.data()); });
-        simt_launch(1, AMB_V3_B, [&] { amb_v3_basescan(tot.data(), base.data()); });
-        simt_launch(n_tiles, 256, [&] { amb_v3_scatter(pos.data(), n, n_tiles, off.data(), base.data(), order.data()); });
-        simt_launch(AMB_V3_B / 4, 128, [&] { amb_v3_pair(pos.data(), order.data(), base.data(), table, pair.data()); });
-    }
+    cudaError_t err = cudaSuccess;
+    if (amb_v3_launch(&e->v3, pos.data(), n, e->table.data(), pair.data(), nullptr, &err) < 0) return -2;
     simt_launch(nb, 128, [&] { amb_resolve_kernel(out, pos.data(), pair.data(), n, have_loc, lat, lon, e->T); });
     return 0;
 }

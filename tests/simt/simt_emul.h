@@ -192,7 +192,7 @@ static inline unsigned long long atomicMin(unsigned long long* p, unsigned long 
 static inline unsigned atomicMax(unsigned* p, unsigned v) { const unsigned o = *p; if (v > o) *p = v; return o; }
 static inline unsigned atomicMin(unsigned* p, unsigned v) { const unsigned o = *p; if (v < o) *p = v; return o; }
 
-// ---- stand-ins for the seven PTX helpers of amb_kernels.cu (mbarrier + TMA tile copy) -----------------------------
+// ---- stand-ins for the six PTX helpers of amb_kernels.cu (mbarrier + TMA tile copy) -------------------------------
 // Shared-memory "addresses" are byte offsets into the block's dynamic shared memory. An mbarrier is a counter of
 // completed phases; the tile copy happens at issue time and completes the phase (complete_tx), a waiter that finds
 // the phase incomplete yields. The copy lands with the 128-byte swizzle of CU_TENSOR_MAP_SWIZZLE_128B (16-byte chunk
@@ -230,7 +230,6 @@ static inline void tma_tile_g2s(uint32_t dst, const void* tmap, int c0, int c1, 
     simt_progress++;
 }
 static inline bool elect_one() { return (simt_cur->tid.x & 31) == 0; }
-static inline void fence_proxy_async() {}
 static inline void fence_mbar_init() {}
 
 // A thread that has exited no longer takes part in barriers (CUDA semantics for __syncthreads and *_sync with exited lanes)

@@ -1,9 +1,9 @@
-"""The decoder's KERNEL SOURCE (gr_air_modes_b200/csrc/amb_decode_kernels.cuh: fields / pairing / resolve kernels, plus
-the experimental pairing variants behind AMB_PAIR_V2 / AMB_PAIR_V3) executed on the host by a small SIMT emulator
+"""The decoder's KERNEL SOURCE (gr_air_modes_b200/csrc/amb_decode_kernels.cuh and amb_decode_v3.cuh: fields kernel, the
+five pairing kernels launched by their own launcher, resolve kernel) executed on the host by a small SIMT emulator
 (tests/simt/simt_emul.h: cooperative fibers, real barrier semantics for __syncthreads / __syncwarp / shuffles / votes /
 match) and compared with the sequential host replay of the same arithmetic and with the oracle. A CPU-side check of the
 warp-level logic - match/ballot ordering inside a 32-frame step, table hand-over between steps and batches, the stable
-partition of variant 3 - for hardware-independent bugs; the GPU tests remain the parity gate."""
+partition of the reports by owner bucket - for hardware-independent bugs; the GPU tests remain the parity gate."""
 import ctypes as C
 import os
 import subprocess
@@ -27,7 +27,7 @@ def libs(tmp_path_factory):
     e.emul_new.restype = C.c_void_p
     e.emul_new.argtypes = [C.c_int]
     e.emul_free.argtypes = [C.c_void_p]
-    e.emul_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_void_p]
+    e.emul_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_void_p]
     s.shim_new.restype = C.c_void_p
     s.shim_step.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_void_p]
     return e, s
@@ -60,7 +60,7 @@ def _traffic(n, seed, n_aircraft):
     return arr, msgs
 
 
-def _run(e, s, arr, n, variant, warps, splits, loc):
+def _run(e, s, arr, n, splits, loc):
     from gr_air_modes_b200 import decode
     have, lat, lon = (0, 0.0, 0.0) if loc is None else (1, loc[0], loc[1])
     he, hs = e.emul_new(17), s.shim_new()
@@ -73,32 +73,32 @@ def _run(e, s, arr, n, variant, warps, splits, loc):
         if c <= 0:
             break
         fr = C.c_void_p(base + 80 * pos)
-        assert e.emul_decode(he, fr, c, variant, warps, have, lat, lon, C.c_void_p(got.ctypes.data + 144 * pos)) == 0
+        assert e.emul_decode(he, fr, c, have, lat, lon, C.c_void_p(got.ctypes.data + 144 * pos)) == 0
         s.shim_step(hs, fr, c, have, lat, lon, C.c_void_p(want.ctypes.data + 144 * pos))
         pos += c
     e.emul_free(he)
     return got, want
 
 
-@pytest.mark.parametrize("variant,warps", [(1, 4), (1, 12), (2, 4), (2, 8), (3, 0)])
-def test_kernel_source_under_the_emulator_equals_sequential_replay(libs, variant, warps):
+def test_decoder_kernels_under_the_emulator_equal_sequential_replay(libs):
     e, s = libs
     n = 2500
-    arr, msgs = _traffic(n, 40 + variant, 5)
+    arr, msgs = _traffic(n, 43, 5)
     for splits in ([], [1, 31, 32, 33, 700]):
-        got, want = _run(e, s, arr, n, variant, warps, splits, [40.0, -3.0])
-        assert got.tobytes() == want.tobytes(), (variant, warps, splits)      # every byte of every record
+        got, want = _run(e, s, arr, n, splits, [40.0, -3.0])
+        assert got.tobytes() == want.tobytes(), splits      # every byte of every record
     st = want["status"]
     assert ((st & 0x10) != 0).sum() > 1200 and ((st & 0x04) != 0).sum() > 5
 
 
-def test_variant3_partition_across_tiles(libs):
-    """More than one 8192-frame tile: the stable counting sort of variant 3 must keep stream order inside every bucket."""
+def test_pairing_partition_across_tiles(libs):
+    """More than one 8192-frame tile: the stable counting sort of the pairing stage must keep stream order inside every
+    bucket."""
     from oracle import decode_oracle as do
     e, s = libs
     n = 9000
     arr, msgs = _traffic(n, 77, 40)
-    got, want = _run(e, s, arr, n, 3, 0, [8191], None)
+    got, want = _run(e, s, arr, n, [8191], None)
     assert got.tobytes() == want.tobytes()
     orc = do.decode_batch(msgs, None)
     assert [w["status"] for w in orc] == want["status"].tolist()

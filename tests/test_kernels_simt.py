@@ -69,7 +69,7 @@ def test_split_form_chain_under_the_emulator_matches_the_oracle(emul, port, rate
     (4e6, 50_000, 100, True, 5.0, 7),
 ])
 def test_fused_iq_chain_under_the_emulator_matches_the_oracle(emul, port, rate, n, nb, pmf, thr, seed):
-    """amb_process's kernels on IQ, all of them: the streaming scan kernel (its seven PTX helpers - mbarrier, 2-D TMA tile
+    """amb_process's kernels on IQ, all of them: the streaming scan kernel (its six PTX helpers - mbarrier, 2-D TMA tile
     copy - are emulated, the kernel source is the product's), prologue (tail staging), compaction, the exact and slice
     kernels in their IQ form (canonical |x|^2 / PMF / noise-floor arithmetic from the carry ++ main ++ tail segments),
     both resolvers. Detection indices, 240-chip packets and the message text equal the oracle's run over the same IQ;
