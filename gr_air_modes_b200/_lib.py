@@ -21,6 +21,9 @@ EC_ANY_MAX = 2              # option "ec_any": at most 2 flipped bits
 # AMB_FRAME_AP (include/airmodes_b200.h AMB_AP_*), option "ap_filter" = S seconds (0 = off)
 AP_NOT_CHECKED, AP_KNOWN, AP_UNKNOWN = 0, 1, 2
 AP_FILTER_MAX = 3600
+# AMB_FIELDS_LOCAL (include/airmodes_b200.h AMB_LOCAL_*), decoder option "local_cpr" = S seconds (0 = off)
+LOCAL_NOT_TRIED, LOCAL_DECODED, LOCAL_NO_REF, LOCAL_STALE, LOCAL_REJECTED = 0, 1, 2, 3, 4
+LOCAL_CPR_MAX = 600
 
 
 class Frame(C.Structure):
@@ -90,7 +93,10 @@ class WalkSummary(C.Structure):
 
 
 class Fields(C.Structure):
-    """struct amb_fields (144 bytes): one decoded message (parse.py / altitude.py / cpr.py results)."""
+    """struct amb_fields (144 bytes): one decoded message (parse.py / altitude.py / cpr.py results).
+
+    The first byte of the header's `pad_` (AMB_FIELDS_LOCAL) holds the local CPR outcome; `pad_` stays one uint64 field
+    here, so the record layout numpy sees (np.dtype(Fields)) is the one it had before local decoding existed."""
     _fields_ = [("icao", C.c_uint32), ("ecc", C.c_uint32), ("df", C.c_uint8), ("status", C.c_uint8), ("bds", C.c_uint8),
                 ("subtype", C.c_uint8), ("ca", C.c_uint8), ("fs", C.c_uint8), ("vs", C.c_uint8), ("ri", C.c_uint8),
                 ("sl", C.c_uint8), ("cc", C.c_uint8), ("dr", C.c_uint8), ("um", C.c_uint8), ("ftc", C.c_uint8),
@@ -99,6 +105,11 @@ class Fields(C.Structure):
                 ("squawk", C.c_int32), ("threat_alt", C.c_int32), ("cpr_lat", C.c_uint32), ("cpr_lon", C.c_uint32),
                 ("aux", C.c_uint32 * 4), ("ident", C.c_char * 8), ("lat", C.c_double), ("lon", C.c_double),
                 ("range", C.c_double), ("bearing", C.c_double), ("val", C.c_double * 4), ("pad_", C.c_uint64)]
+
+    @property
+    def local(self) -> int:
+        """AMB_FIELDS_LOCAL (byte 136): local CPR outcome (decoder option "local_cpr"), LOCAL_*."""
+        return self.pad_ & 0xFF
 
 
 assert C.sizeof(Frame) == 80
@@ -149,6 +160,7 @@ SYMBOLS = [
     ("amb_resolve_device", C.c_int, [_vp, _vp, _vp]),
     ("amb_join_stream", C.c_int, [_vp, _vp]),
     ("amb_decoder_create", C.c_int, [C.c_int, C.c_int, C.c_double, C.c_double, C.POINTER(_vp)]),
+    ("amb_decoder_set_option", C.c_int, [_vp, C.c_char_p, C.c_int]),
     ("amb_decoder_destroy", None, [_vp]),
     ("amb_decoder_set_location", C.c_int, [_vp, C.c_int, C.c_double, C.c_double]),
     ("amb_decoder_reset", C.c_int, [_vp]),

@@ -10,6 +10,9 @@
 //                       even and odd report of its aircraft as of that message, from the reports partitioned by owner
 //                       bucket and a direct-mapped table in HBM (2^26 x 16 B) that carries them from batch to batch
 //   amb_resolve_kernel  one thread per frame: global CPR decode, range/bearing.
+// With option "local_cpr" on, six more (amb_decode_local.cuh): amb_local_keys, the four partition kernels of the pairing
+// stage on ICAO keys, amb_local_walk - the local decode of the position messages the global decode left without a fix,
+// with a direct-mapped table of reference positions in HBM (2^24 x 24 B) carried from batch to batch.
 #include "amb_launch.h"
 #include "amb_decode_core.h"
 #include "amb_decode_kernels.cuh"
@@ -32,7 +35,10 @@ struct amb_decoder {
     // host <-> device staging: pageable caller arrays go through two pinned bounce buffers per direction so that the
     // copies run at PCIe speed and overlap the memcpy of the next piece
     void* pin[2] = {nullptr, nullptr}; cudaEvent_t pin_ev[2] = {nullptr, nullptr}; size_t pin_bytes = 0;
-    AmbV3Bufs v3;                        // scratch of the pairing stage
+    AmbV3Bufs v3;                        // scratch of the pairing stage (and of the local stage's partition)
+    int local_cpr = 0;                   // option "local_cpr" = S seconds, 0 = off
+    AmbRefPos* ltable = nullptr;         // reference position per ICAO, allocated at the first decode with the option on
+    AmbPosRec* d_lpos = nullptr; int lcap = 0;   // ICAO-keyed reports of the local stage
     uint64_t launches = 0; float ms_last = 0.f;
     std::string err;
 };
@@ -132,6 +138,7 @@ int amb_decoder_create(int device, int have_location, double lat, double lon, am
 {
     static_assert(sizeof(amb_fields) == 144, "amb_fields layout");
     static_assert(sizeof(AmbCprSlot) == 16, "table slot layout");
+    static_assert(sizeof(AmbRefPos) == 24, "reference position slot layout");
     if (!out) return AMB_ERR_INVALID;
     *out = nullptr;
     int ndev = 0;
@@ -170,6 +177,8 @@ void amb_decoder_destroy(amb_decoder* d)
     if (d->stream) cudaStreamSynchronize(d->stream);
     free_bufs(d);
     amb_v3_free(&d->v3);
+    if (d->ltable) cudaFree(d->ltable);
+    if (d->d_lpos) cudaFree(d->d_lpos);
     for (int k = 0; k < 2; k++) { if (d->pin[k]) cudaFreeHost(d->pin[k]); if (d->pin_ev[k]) cudaEventDestroy(d->pin_ev[k]); }
     if (d->table) cudaFree(d->table);
     if (d->nl_T) cudaFree(d->nl_T);
@@ -191,7 +200,35 @@ int amb_decoder_reset(amb_decoder* d)
     if (!d) return AMB_ERR_INVALID;
     DCK(cudaSetDevice(d->device));
     DCK(cudaMemsetAsync(d->table, 0xFF, AMB_TABLE_SLOTS * sizeof(AmbCprSlot), d->stream));
+    if (d->ltable) DCK(cudaMemsetAsync(d->ltable, 0xFF, AMB_LOCAL_SLOTS * sizeof(AmbRefPos), d->stream));
     DCK(cudaStreamSynchronize(d->stream));
+    return AMB_OK;
+}
+
+int amb_decoder_set_option(amb_decoder* d, const char* name, int value)
+{
+    if (!d || !name) return AMB_ERR_INVALID;
+    if (strcmp(name, "local_cpr") == 0) {
+        if (value < 0 || value > AMB_LOCAL_CPR_MAX) return dfail(d, AMB_ERR_INVALID, "local_cpr: 0 (off) .. 600 seconds");
+        d->local_cpr = value;
+        return AMB_OK;
+    }
+    return dfail(d, AMB_ERR_INVALID, "amb_decoder_set_option: unknown option");
+}
+
+// the local stage's device memory, at the first decode with the option on (the table starts empty: all NaN)
+static int ensure_local(amb_decoder* d)
+{
+    if (!d->ltable) {
+        DCK(cudaMalloc(&d->ltable, AMB_LOCAL_SLOTS * sizeof(AmbRefPos)));
+        DCK(cudaMemsetAsync(d->ltable, 0xFF, AMB_LOCAL_SLOTS * sizeof(AmbRefPos), d->stream));
+    }
+    if (d->lcap < d->cap) {
+        if (d->d_lpos) cudaFree(d->d_lpos);
+        d->d_lpos = nullptr; d->lcap = 0;
+        DCK(cudaMalloc(&d->d_lpos, (size_t)d->cap * sizeof(AmbPosRec)));
+        d->lcap = d->cap;
+    }
     return AMB_OK;
 }
 
@@ -235,6 +272,14 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
     AMB_LAUNCH((amb_resolve_kernel), nb, 128, 0, s, fields, d->d_pos, d->d_pair, n, d->have_loc, d->lat, d->lon, d->nl_T);
     DCK(cudaGetLastError());
     d->launches += 2 + (uint64_t)k;
+    if (d->local_cpr > 0) {
+        rc = ensure_local(d);
+        if (rc != AMB_OK) return rc;
+        const int kl = amb_local_launch(&d->v3, d->d_pos, d->d_lpos, n, fields, d->ltable, d->local_cpr, d->have_loc, d->lat,
+                                        d->lon, d->nl_T, s, &e);
+        if (kl < 0) return dfail(d, AMB_ERR_CUDA, "local CPR", e);
+        d->launches += (uint64_t)kl;
+    }
     if (!out_on_device) {
         rc = staged_d2h(d, out, d->d_fields, (size_t)n * sizeof(amb_fields), s);
         if (rc != AMB_OK) return rc;

@@ -353,6 +353,71 @@ AMB_HD void amb_resolve_position(amb_fields* r, const AmbPair& pr, int have_loc,
     }
 }
 
+// ---- locally referenced CPR decode (decoder option "local_cpr"; DESIGN.md §8) --------------------------------------
+// The last position of an aircraft (global or local fix) and the timestamp of its message; t is NaN when there is none.
+struct AmbRefPos { double lat, lon, t; };
+
+AMB_HD double amb_pyfmod(double a, double b)                // Python's float % for b > 0 (float_rem: fmod + sign fix-up)
+{
+    double m = fmod(a, b);
+    if (m != 0.0) { if (m < 0.0) m += b; }
+    else m = 0.0;                                           // copysign(0, b)
+    return m;
+}
+
+// cpr_resolve_local (cpr.py:75-82 with decode_lat :61-66, decode_lon :68-73, dlat :36-46, dlon :53-59), expression by
+// expression; nl() from the transition table.
+AMB_HD void amb_cpr_local(double my_lat, double my_lon, uint32_t enclat, uint32_t enclon, int ctype, int surface,
+                          const double* T, double* out_lat, double* out_lon)
+{
+    const double span = surface ? 90.0 : 360.0;
+    const double dla = span / (60 - ctype);
+    const double la2 = (double)enclat / 131072;
+    const double j = floor(my_lat / dla) + floor(0.5 + (amb_pyfmod(my_lat, dla) / dla) - la2);
+    const double lat = dla * (j + la2);
+    const int nn = (amb_nl(lat, T) - ctype) > 1 ? (amb_nl(lat, T) - ctype) : 1;
+    const double dlo = span / nn;
+    const double lo2 = (double)enclon / 131072;
+    const double m = floor(my_lon / dlo) + floor(0.5 + (amb_pyfmod(my_lon, dlo) / dlo) - lo2);
+    *out_lat = lat;
+    *out_lon = dlo * (m + lo2);
+}
+
+// One position message after the global resolve, given its aircraft's reference position `ref` as of this message
+// (updated in place). Returns the AMB_LOCAL_* outcome, which is also stored in the record.
+AMB_HD int amb_local_step(amb_fields* r, double t, AmbRefPos* ref, int max_age, int have_loc, double mylat, double mylon,
+                          const double* T)
+{
+    int v;
+    if (r->status & AMB_FS_HAS_POS) {                       // the global fix stands and becomes the reference
+        ref->lat = r->lat; ref->lon = r->lon; ref->t = t;
+        v = AMB_LOCAL_NOT_TRIED;
+    } else if (ref->t != ref->t) {
+        v = AMB_LOCAL_NO_REF;
+    } else if (!(t - ref->t >= 0.0) || t - ref->t > (double)max_age) {   // the expiry rule of amb_report_alive
+        v = AMB_LOCAL_STALE;
+    } else {
+        double lat, lon;
+        amb_cpr_local(ref->lat, ref->lon, r->cpr_lat, r->cpr_lon, r->cpr_format, r->surface, T, &lat, &lon);
+        if (lon > 180.0) lon -= 360.0;
+        else if (lon <= -180.0) lon += 360.0;
+        const double dla = (r->surface ? 90.0 : 360.0) / (60 - r->cpr_format);
+        if (fabs(lat) > 90.0 || fabs(lat - ref->lat) > dla / 2) {
+            v = AMB_LOCAL_REJECTED;
+        } else {
+            r->lat = lat; r->lon = lon; r->status |= AMB_FS_HAS_POS;
+            if (have_loc) {
+                amb_range_bearing(mylat, mylon, lat, lon, &r->range, &r->bearing);
+                r->status |= AMB_FS_HAS_RANGE;
+            }
+            ref->lat = lat; ref->lon = lon; ref->t = t;
+            v = AMB_LOCAL_DECODED;
+        }
+    }
+    AMB_FIELDS_LOCAL(r) = (uint8_t)v;
+    return v;
+}
+
 // Latest-report bookkeeping of cpr_decoder.decode for ONE message given the table state before it (cpr.py:214-229):
 // used by the pairing kernel lane by lane and, sequentially, by the host shim.
 // A stored report stamped LATER than the current message can only stem from an earlier stream (frame timestamps restart

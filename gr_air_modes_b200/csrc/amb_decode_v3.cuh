@@ -196,8 +196,9 @@ static void amb_v3_free(AmbV3Bufs* v)
     *v = AmbV3Bufs();
 }
 
-// Enqueue the five kernels; returns how many were launched (for the launch counter) or -1 with *err set.
-static int amb_v3_launch(AmbV3Bufs* v, const AmbPosRec* pos, int n, AmbCprSlot* table, AmbPair* pair, cudaStream_t s, cudaError_t* err)
+// Enqueue the four partition kernels: v->order[v->base[b] .. v->base[b+1]) = the frames whose key falls into bucket b, in
+// stream order. Also used on ICAO-keyed reports by the local CPR stage (amb_decode_local.cuh).
+static int amb_v3_partition(AmbV3Bufs* v, const AmbPosRec* pos, int n, cudaStream_t s, cudaError_t* err)
 {
     if ((*err = amb_v3_ensure(v, n)) != cudaSuccess) return -1;
     const int n_tiles = (n + AMB_V3_TILE - 1) / AMB_V3_TILE;
@@ -205,6 +206,13 @@ static int amb_v3_launch(AmbV3Bufs* v, const AmbPosRec* pos, int n, AmbCprSlot* 
     AMB_LAUNCH((amb_v3_rowscan), AMB_V3_B / 8, 256, 0, s, v->cnt, n_tiles, v->off, v->tot);
     AMB_LAUNCH((amb_v3_basescan), 1, AMB_V3_B, 0, s, v->tot, v->base);
     AMB_LAUNCH((amb_v3_scatter), n_tiles, 256, 0, s, pos, n, n_tiles, v->off, v->base, v->order);
+    return 4;
+}
+
+// Enqueue the five kernels; returns how many were launched (for the launch counter) or -1 with *err set.
+static int amb_v3_launch(AmbV3Bufs* v, const AmbPosRec* pos, int n, AmbCprSlot* table, AmbPair* pair, cudaStream_t s, cudaError_t* err)
+{
+    if (amb_v3_partition(v, pos, n, s, err) < 0) return -1;
     AMB_LAUNCH((amb_v3_pair), AMB_V3_B / 4, 128, 0, s, pos, v->order, v->base, table, pair);
     *err = cudaGetLastError();
     return *err == cudaSuccess ? 5 : -1;

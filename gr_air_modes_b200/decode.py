@@ -22,6 +22,10 @@ from ._lib import Fields, Frame, check
 FS_NO_HANDLER, FS_METRIC_ALT, FS_CPR_NO_POS, FS_CPR_STRADDLE = 0x01, 0x02, 0x04, 0x08
 FS_HAS_POS, FS_HAS_RANGE, FS_METRIC_THREAT, FS_NOT_QUEUED = 0x10, 0x20, 0x40, 0x80
 NO_ALTITUDE = -(1 << 31)
+# local CPR outcome of a record (decoder option local_cpr; include/airmodes_b200.h AMB_LOCAL_*), read by local_outcome()
+LOCAL_NOT_TRIED, LOCAL_DECODED, LOCAL_NO_REF, LOCAL_STALE, LOCAL_REJECTED = (
+    _lib.LOCAL_NOT_TRIED, _lib.LOCAL_DECODED, _lib.LOCAL_NO_REF, _lib.LOCAL_STALE, _lib.LOCAL_REJECTED)
+LOCAL_CPR_MAX = _lib.LOCAL_CPR_MAX
 
 FIELDS_DTYPE = np.dtype(Fields)
 FRAME_DTYPE = np.dtype(Frame)
@@ -49,10 +53,30 @@ def frames_from_messages(msgs):
     return arr, len(msgs)
 
 
-class batch_decoder:
-    """cpr_decoder(my_location) (cpr.py:184-190) + parser, for batches. my_location = [lat, lon] or None."""
+def local_outcome(records):
+    """AMB_FIELDS_LOCAL of a FIELDS_DTYPE record or array: LOCAL_* per record (the low byte of `pad_`)."""
+    return np.asarray(records["pad_"], dtype=np.uint64) & np.uint64(0xFF)
 
-    def __init__(self, my_location=None, device: int = 0):
+
+def check_local_cpr(seconds) -> int:
+    """Validate a local_cpr setting: an int in 0 (off) .. LOCAL_CPR_MAX seconds. Raises ValueError otherwise."""
+    try:
+        ok = not isinstance(seconds, bool) and int(seconds) == seconds and 0 <= int(seconds) <= LOCAL_CPR_MAX
+    except (TypeError, ValueError):
+        ok = False
+    if not ok:
+        raise ValueError("local_cpr: an integer number of seconds in 0 (off) .. %d, got %r" % (LOCAL_CPR_MAX, seconds))
+    return int(seconds)
+
+
+class batch_decoder:
+    """cpr_decoder(my_location) (cpr.py:184-190) + parser, for batches. my_location = [lat, lon] or None.
+
+    local_cpr = S > 0 also decodes every position message the global decode leaves without a fix relative to the
+    aircraft's last position of at most S seconds before (DESIGN.md §8); 0, the default, is the reference's decoder."""
+
+    def __init__(self, my_location=None, device: int = 0, local_cpr: int = 0):
+        local_cpr = check_local_cpr(local_cpr)
         self._lib = _lib.load()
         h = C.c_void_p()
         have, lat, lon = self._loc(my_location)
@@ -62,6 +86,9 @@ class batch_decoder:
             raise RuntimeError("libairmodes_b200: %s%s" % (self._lib.amb_strerror(rc).decode(), (" (%s)" % detail) if detail else ""))
         self._h = h
         self.my_location = my_location
+        self._local_cpr = 0
+        if local_cpr:
+            self.set_local_cpr(local_cpr)
 
     @staticmethod
     def _loc(loc):
@@ -79,7 +106,17 @@ class batch_decoder:
         self.my_location = new_location
 
     def reset(self):
+        """Forget every stored report and reference position; the local_cpr setting stays."""
         self._check(self._lib.amb_decoder_reset(self._h))
+
+    def set_local_cpr(self, seconds: int):
+        """Option local_cpr = S seconds (0 = off); applies from the next decode."""
+        seconds = check_local_cpr(seconds)
+        self._check(self._lib.amb_decoder_set_option(self._h, b"local_cpr", seconds))
+        self._local_cpr = seconds
+
+    def get_local_cpr(self) -> int:
+        return self._local_cpr
 
     def decode(self, frames, n: int | None = None) -> np.ndarray:
         """frames: ctypes Frame array / list of Frame (e.g. rx_path.frames) / numpy FRAME_DTYPE array, in stream

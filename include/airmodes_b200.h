@@ -366,21 +366,43 @@ typedef struct amb_fields {
     uint32_t cpr_lat, cpr_lon;            /* encoded 17-bit position */
     uint32_t aux[4];      /* MB bds1 = 1: acs, bcs, ecs, cfs; bds1 = 3: ara, rac, rat | mte << 1, tid (tti 1) or tidr | tidb << 8 (tti 2) */
     char ident[8];        /* BDS0,8 / MB bds1 = 2 callsign (parse.py:257-279, 374-378), no terminator */
-    double lat, lon;      /* global CPR decode (cpr.py:89-153), degrees; NaN unless AMB_FS_HAS_POS */
+    double lat, lon;      /* global CPR decode (cpr.py:89-153), or the local one (AMB_LOCAL_DECODED), degrees; NaN unless AMB_FS_HAS_POS */
     double range, bearing;/* range_bearing(my_location, position) (cpr.py:158-181): statute miles, degrees */
     double val[4];        /* BDS0,9-0: velocity, heading, vert_spd, turn_rate (parse.py:288-313)
                              BDS0,9-1: velocity, heading, vert_spd, alt_geo_diff (parse.py:315-348)
                              BDS0,9-3: mag_hdg, vel, vert_spd, geo_diff (parse.py:350-364)
                              BDS0,6  : ground_track (parse.py:283) */
-    uint64_t pad_;
+    uint64_t pad_;        /* [byte 0] local CPR outcome (AMB_FIELDS_LOCAL), the rest 0 */
 } amb_fields;             /* 144 bytes */
+
+/* Locally referenced CPR decode (amb_decoder_set_option(d, "local_cpr", S), S in 1..600 seconds). After the global
+ * decode, every queued BDS0,5 / BDS0,6 message without AMB_FS_HAS_POS is decoded relative to its aircraft's reference
+ * position - the last position (global or local) of the same 24-bit ICAO, airborne and surface alike - when that
+ * position's message lies at most S seconds back (0 <= t - ref.t <= S, t = secs + frac): cpr_resolve_local
+ * (cpr.py:61-82), longitude brought into (-180, 180] with one +/-360, rejected when |lat| > 90 or when it lies more
+ * than half a latitude zone (dlat / 2) from the reference. An accepted fix sets lat / lon and AMB_FS_HAS_POS (with a
+ * receiver location also range / bearing and AMB_FS_HAS_RANGE) and becomes the new reference; AMB_FS_CPR_NO_POS and
+ * AMB_FS_CPR_STRADDLE keep the global verdict. A global fix leaves the record as it is and becomes the reference.
+ * The outcome lives in the first byte of amb_fields.pad_ (byte 136 of the record): */
+#define AMB_FIELDS_LOCAL(r) (((uint8_t*)&(r)->pad_)[0])
+#define AMB_LOCAL_NOT_TRIED 0    /* option off, not a position message, or the global decode gave a position */
+#define AMB_LOCAL_DECODED 1      /* position from the local decode */
+#define AMB_LOCAL_NO_REF 2       /* the aircraft has no reference position */
+#define AMB_LOCAL_STALE 3        /* its reference position is more than S seconds old (or stamped later than the message) */
+#define AMB_LOCAL_REJECTED 4     /* the local decode failed the plausibility check; the reference is kept */
+#define AMB_LOCAL_CPR_MAX 600
 
 typedef struct amb_decoder amb_decoder;
 /* cpr_decoder(my_location) (cpr.py:184-190) + the parser; have_location = 0 is my_location = None. */
 AMB_API int amb_decoder_create(int device, int have_location, double lat, double lon, amb_decoder** out);
+/* "local_cpr": S = 0 (default, off) .. 600 seconds, locally referenced CPR decode (see AMB_FIELDS_LOCAL); applies from
+ * the next call. The table of reference positions (2^24 x 24 B = 384 MiB of device memory) is allocated at the first
+ * decode with the option on, written only by such decodes and cleared by amb_decoder_reset. Off changes nothing.
+ * Unknown names and out-of-range values return AMB_ERR_INVALID. */
+AMB_API int amb_decoder_set_option(amb_decoder* d, const char* name, int value);
 AMB_API void amb_decoder_destroy(amb_decoder* d);
 AMB_API int amb_decoder_set_location(amb_decoder* d, int have_location, double lat, double lon);   /* cpr.py:192-193 */
-AMB_API int amb_decoder_reset(amb_decoder* d);                      /* forget every stored report */
+AMB_API int amb_decoder_reset(amb_decoder* d);                      /* forget every stored report (and reference position) */
 /* Decode n frames (host or device array, stream order = non-decreasing time). out: n records in host memory.
  * Frames with passed == 0 get AMB_FS_NOT_QUEUED and do not touch the CPR state. */
 AMB_API int amb_decode_frames(amb_decoder* d, const amb_frame* frames, int n, int mem_kind, amb_fields* out);

@@ -111,9 +111,9 @@ class report_queue:
     python/msprint.py) - one text report per parsed message. The numbers come from the GPU batch decoder
     (gr_air_modes_b200.decode), the line format from gr_air_modes_b200.report."""
 
-    def __init__(self, location, device, out=sys.stdout):
+    def __init__(self, location, device, out=sys.stdout, local_cpr=0):
         from gr_air_modes_b200 import decode
-        self._dec = decode.batch_decoder(location, device)      # = cpr_decoder(my_position), apps/modes_rx:68
+        self._dec = decode.batch_decoder(location, device, local_cpr=local_cpr)   # = cpr_decoder(my_position), apps/modes_rx:68
         self._out, self._texts, self.count = out, [], 0
 
     def handle(self, msg):
@@ -164,6 +164,9 @@ def main(argv=None):
     ap.add_argument("--ap-filter", type=int, default=0, metavar="S",
                     help="drop address/parity replies from aircraft not confirmed by a clean DF11/DF17 in the last S "
                          "seconds, and accept DF11 replies with an II/SI code from confirmed ones; 0 = off, as the reference")
+    ap.add_argument("--local-cpr", type=int, default=0, metavar="S",
+                    help="position reports: decode a message that has no global fix relative to the aircraft's last "
+                         "position of at most S (1..600) seconds before; 0 = off, as the reference")
     args = ap.parse_args(argv)
 
     if args.source in ("uhd", "osmocom"):
@@ -187,7 +190,7 @@ def main(argv=None):
     if not args.no_print:
         if args.reports or args.location is not None:
             my_position = [float(x) for x in args.location.split(",")] if args.location is not None else None   # apps/modes_rx:64-65
-            reporter = report_queue(my_position, args.device)
+            reporter = report_queue(my_position, args.device, local_cpr=args.local_cpr)
             sinks.append(reporter)
         else:
             printer = print_queue()
