@@ -24,6 +24,10 @@ AP_FILTER_MAX = 3600
 # AMB_FIELDS_LOCAL (include/airmodes_b200.h AMB_LOCAL_*), decoder option "local_cpr" = S seconds (0 = off)
 LOCAL_NOT_TRIED, LOCAL_DECODED, LOCAL_NO_REF, LOCAL_STALE, LOCAL_REJECTED = 0, 1, 2, 3, 4
 LOCAL_CPR_MAX = 600
+# amb_aircraft.flags (include/airmodes_b200.h AMB_AC_*), decoder option "track" = S seconds (0 = off)
+AC_HAS_ALT, AC_HAS_SQUAWK, AC_HAS_IDENT, AC_HAS_POS, AC_HAS_RANGE = 0x001, 0x002, 0x004, 0x008, 0x010
+AC_HAS_VELOCITY, AC_HAS_HEADING, AC_HAS_EPS, AC_ON_GROUND = 0x020, 0x040, 0x080, 0x100
+TRACK_MAX = 3600
 
 
 class Frame(C.Structure):
@@ -112,8 +116,19 @@ class Fields(C.Structure):
         return self.pad_ & 0xFF
 
 
+class Aircraft(C.Structure):
+    """struct amb_aircraft (128 bytes): one row of the decoder's per-aircraft table (option "track")."""
+    _fields_ = [("icao", C.c_uint32), ("messages", C.c_uint32), ("first_seen", C.c_double), ("seen", C.c_double),
+                ("ref_level", C.c_float), ("flags", C.c_uint16), ("ftc", C.c_int8), ("cat", C.c_int8),
+                ("ident", C.c_char * 8), ("altitude", C.c_int32), ("squawk", C.c_int32), ("lat", C.c_double),
+                ("lon", C.c_double), ("range", C.c_double), ("bearing", C.c_double), ("pos_t", C.c_double),
+                ("speed", C.c_double), ("heading", C.c_double), ("vertical", C.c_double), ("eps", C.c_int8),
+                ("pad_", C.c_uint8 * 15)]
+
+
 assert C.sizeof(Frame) == 80
 assert C.sizeof(Fields) == 144
+assert C.sizeof(Aircraft) == 128
 
 # every symbol include/airmodes_b200.h declares: (name, restype, argtypes)
 _vp, _f32p, _u64p = C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_uint64)
@@ -166,6 +181,8 @@ SYMBOLS = [
     ("amb_decoder_reset", C.c_int, [_vp]),
     ("amb_decode_frames", C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp]),
     ("amb_decode_frames_device", C.c_int, [_vp, _vp, C.c_int, _vp]),
+    ("amb_decoder_aircraft", C.c_int, [_vp, C.c_double, _vp, C.c_int]),
+    ("amb_decoder_aircraft_device", C.c_int, [_vp, C.c_double, _vp, C.c_int]),
     ("amb_decoder_stats", C.c_int, [_vp, _u64p, _f32p]),
     ("amb_decoder_last_error", C.c_char_p, [_vp]),
     ("amb_frame_bits", C.c_uint64, [C.POINTER(Frame), C.c_int, C.c_int]),

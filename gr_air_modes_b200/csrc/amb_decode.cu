@@ -13,6 +13,9 @@
 // With option "local_cpr" on, six more (amb_decode_local.cuh): amb_local_keys, the four partition kernels of the pairing
 // stage on ICAO keys, amb_local_walk - the local decode of the position messages the global decode left without a fix,
 // with a direct-mapped table of reference positions in HBM (2^24 x 24 B) carried from batch to batch.
+// With option "track" on, six more after those (amb_decode_track.cuh): amb_track_keys, the four partition kernels on
+// address keys, amb_track_walk - the per-aircraft table, direct-mapped in HBM (2^24 x 128 B) with an occupancy bitmap;
+// amb_decoder_aircraft reads it out with three kernels of its own.
 #include "amb_launch.h"
 #include "amb_decode_core.h"
 #include "amb_decode_kernels.cuh"
@@ -38,7 +41,13 @@ struct amb_decoder {
     AmbV3Bufs v3;                        // scratch of the pairing stage (and of the local stage's partition)
     int local_cpr = 0;                   // option "local_cpr" = S seconds, 0 = off
     AmbRefPos* ltable = nullptr;         // reference position per ICAO, allocated at the first decode with the option on
-    AmbPosRec* d_lpos = nullptr; int lcap = 0;   // ICAO-keyed reports of the local stage
+    AmbPosRec* d_lpos = nullptr; int lcap = 0;   // address-keyed records of the local and the track stage
+    int track = 0;                       // option "track" = S seconds, 0 = off
+    amb_aircraft* trows = nullptr;       // one row per address, allocated at the first decode with the option on
+    unsigned* tocc = nullptr;            // which rows hold data (AMB_TRACK_WORDS words)
+    AmbTrackClock* tclk = nullptr;       // t of the latest queued record since reset
+    uint32_t* snap_cnt = nullptr;        // snapshot: per-block counts, then their scan and the total
+    amb_aircraft* d_snap = nullptr; int snap_cap = 0;   // snapshot rows on their way to host memory
     uint64_t launches = 0; float ms_last = 0.f;
     std::string err;
 };
@@ -139,6 +148,7 @@ int amb_decoder_create(int device, int have_location, double lat, double lon, am
     static_assert(sizeof(amb_fields) == 144, "amb_fields layout");
     static_assert(sizeof(AmbCprSlot) == 16, "table slot layout");
     static_assert(sizeof(AmbRefPos) == 24, "reference position slot layout");
+    static_assert(sizeof(amb_aircraft) == 128, "amb_aircraft layout");
     if (!out) return AMB_ERR_INVALID;
     *out = nullptr;
     int ndev = 0;
@@ -179,6 +189,11 @@ void amb_decoder_destroy(amb_decoder* d)
     amb_v3_free(&d->v3);
     if (d->ltable) cudaFree(d->ltable);
     if (d->d_lpos) cudaFree(d->d_lpos);
+    if (d->trows) cudaFree(d->trows);
+    if (d->tocc) cudaFree(d->tocc);
+    if (d->tclk) cudaFree(d->tclk);
+    if (d->snap_cnt) cudaFree(d->snap_cnt);
+    if (d->d_snap) cudaFree(d->d_snap);
     for (int k = 0; k < 2; k++) { if (d->pin[k]) cudaFreeHost(d->pin[k]); if (d->pin_ev[k]) cudaEventDestroy(d->pin_ev[k]); }
     if (d->table) cudaFree(d->table);
     if (d->nl_T) cudaFree(d->nl_T);
@@ -201,6 +216,11 @@ int amb_decoder_reset(amb_decoder* d)
     DCK(cudaSetDevice(d->device));
     DCK(cudaMemsetAsync(d->table, 0xFF, AMB_TABLE_SLOTS * sizeof(AmbCprSlot), d->stream));
     if (d->ltable) DCK(cudaMemsetAsync(d->ltable, 0xFF, AMB_LOCAL_SLOTS * sizeof(AmbRefPos), d->stream));
+    if (d->tocc) {                       // the rows themselves stay: a row whose bit is clear is never read
+        static const AmbTrackClock none = {NAN, 0u, 0u};
+        DCK(cudaMemsetAsync(d->tocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));
+        DCK(cudaMemcpyAsync(d->tclk, &none, sizeof none, cudaMemcpyHostToDevice, d->stream));
+    }
     DCK(cudaStreamSynchronize(d->stream));
     return AMB_OK;
 }
@@ -213,7 +233,24 @@ int amb_decoder_set_option(amb_decoder* d, const char* name, int value)
         d->local_cpr = value;
         return AMB_OK;
     }
+    if (strcmp(name, "track") == 0) {
+        if (value < 0 || value > AMB_TRACK_MAX) return dfail(d, AMB_ERR_INVALID, "track: 0 (off) .. 3600 seconds");
+        d->track = value;
+        return AMB_OK;
+    }
     return dfail(d, AMB_ERR_INVALID, "amb_decoder_set_option: unknown option");
+}
+
+// the key records of the local and the track stage, one per frame
+static int ensure_keys(amb_decoder* d)
+{
+    if (d->lcap < d->cap) {
+        if (d->d_lpos) cudaFree(d->d_lpos);
+        d->d_lpos = nullptr; d->lcap = 0;
+        DCK(cudaMalloc(&d->d_lpos, (size_t)d->cap * sizeof(AmbPosRec)));
+        d->lcap = d->cap;
+    }
+    return AMB_OK;
 }
 
 // the local stage's device memory, at the first decode with the option on (the table starts empty: all NaN)
@@ -223,13 +260,28 @@ static int ensure_local(amb_decoder* d)
         DCK(cudaMalloc(&d->ltable, AMB_LOCAL_SLOTS * sizeof(AmbRefPos)));
         DCK(cudaMemsetAsync(d->ltable, 0xFF, AMB_LOCAL_SLOTS * sizeof(AmbRefPos), d->stream));
     }
-    if (d->lcap < d->cap) {
-        if (d->d_lpos) cudaFree(d->d_lpos);
-        d->d_lpos = nullptr; d->lcap = 0;
-        DCK(cudaMalloc(&d->d_lpos, (size_t)d->cap * sizeof(AmbPosRec)));
-        d->lcap = d->cap;
+    return ensure_keys(d);
+}
+
+// the track stage's device memory, at the first decode with the option on: the rows are not initialised (the bitmap
+// starts empty), the clock starts at "nothing decoded"
+static int ensure_track(amb_decoder* d)
+{
+    if (!d->trows) {
+        cudaError_t e = cudaMalloc(&d->trows, (size_t)AMB_TRACK_ROWS * sizeof(amb_aircraft));
+        if (e != cudaSuccess) { d->trows = nullptr; return dfail(d, AMB_ERR_CUDA, "aircraft table (2 GiB)", e); }
     }
-    return AMB_OK;
+    if (!d->tclk) {
+        static const AmbTrackClock none = {NAN, 0u, 0u};
+        DCK(cudaMalloc(&d->tclk, sizeof(AmbTrackClock)));
+        DCK(cudaMemcpyAsync(d->tclk, &none, sizeof none, cudaMemcpyHostToDevice, d->stream));
+    }
+    if (!d->snap_cnt) DCK(cudaMalloc(&d->snap_cnt, (2 * AMB_TRACK_WORDS / AMB_SNAP_WORDS + 1) * sizeof(uint32_t)));
+    if (!d->tocc) {                      // last: snapshot_impl and reset take a bitmap as "everything is there"
+        DCK(cudaMalloc(&d->tocc, AMB_TRACK_WORDS * sizeof(unsigned)));
+        DCK(cudaMemsetAsync(d->tocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));
+    }
+    return ensure_keys(d);
 }
 
 static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_kind, amb_fields* out, bool out_on_device);
@@ -280,6 +332,14 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
         if (kl < 0) return dfail(d, AMB_ERR_CUDA, "local CPR", e);
         d->launches += (uint64_t)kl;
     }
+    if (d->track > 0) {
+        rc = ensure_track(d);
+        if (rc != AMB_OK) return rc;
+        const int kt = amb_track_launch(&d->v3, src, fields, d->d_pos, d->d_lpos, n, d->trows, d->tocc, d->tclk, d->track,
+                                        s, &e);
+        if (kt < 0) return dfail(d, AMB_ERR_CUDA, "aircraft table", e);
+        d->launches += (uint64_t)kt;
+    }
     if (!out_on_device) {
         rc = staged_d2h(d, out, d->d_fields, (size_t)n * sizeof(amb_fields), s);
         if (rc != AMB_OK) return rc;
@@ -289,6 +349,56 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, d->e0, d->e1) == cudaSuccess) d->ms_last = ms;
     return AMB_OK;
+}
+
+static int snapshot_impl(amb_decoder* d, double now, amb_aircraft* out, int max, bool out_on_device)
+{
+    if (!d || max < 0) return dfail(d, AMB_ERR_INVALID, "amb_decoder_aircraft: bad argument");
+    if (d->track <= 0) return dfail(d, AMB_ERR_STATE, "amb_decoder_aircraft: option track is off");
+    if (!d->tocc) return 0;                              // nothing decoded with the option on yet
+    DCK(cudaSetDevice(d->device));
+    cudaStream_t s = d->stream;
+    const unsigned nb = AMB_TRACK_WORDS / AMB_SNAP_WORDS;
+    uint32_t* off = d->snap_cnt + nb;
+    cudaError_t e = cudaSuccess;
+    if (amb_snap_count_launch(d->tocc, d->trows, d->tclk, now, d->track, AMB_TRACK_WORDS, d->snap_cnt, off, s, &e) < 0)
+        return dfail(d, AMB_ERR_CUDA, "aircraft snapshot", e);
+    d->launches += 2;
+    uint32_t total = 0;
+    DCK(cudaMemcpyAsync(&total, off + nb, sizeof total, cudaMemcpyDeviceToHost, s));
+    DCK(cudaStreamSynchronize(s));
+    if (!out) return (int)total;
+    if (total > (uint32_t)max) return dfail(d, AMB_ERR_OVERFLOW, "amb_decoder_aircraft: output buffer too small");
+    if (total == 0) return 0;
+    amb_aircraft* dst = out;
+    if (!out_on_device) {
+        if (d->snap_cap < (int)total) {
+            if (d->d_snap) cudaFree(d->d_snap);
+            d->d_snap = nullptr; d->snap_cap = 0;
+            DCK(cudaMalloc(&d->d_snap, (size_t)total * sizeof(amb_aircraft)));
+            d->snap_cap = (int)total;
+        }
+        dst = d->d_snap;
+    }
+    if (amb_snap_gather_launch(d->tocc, d->trows, d->tclk, now, d->track, AMB_TRACK_WORDS, off, dst, s, &e) < 0)
+        return dfail(d, AMB_ERR_CUDA, "aircraft snapshot", e);
+    d->launches += 1;
+    if (!out_on_device) {
+        const int rc = staged_d2h(d, out, d->d_snap, (size_t)total * sizeof(amb_aircraft), s);
+        if (rc != AMB_OK) return rc;
+    }
+    DCK(cudaStreamSynchronize(s));
+    return (int)total;
+}
+
+int amb_decoder_aircraft(amb_decoder* d, double now, amb_aircraft* out, int max)
+{
+    return snapshot_impl(d, now, out, max, false);
+}
+
+int amb_decoder_aircraft_device(amb_decoder* d, double now, amb_aircraft* out_dev, int cap)
+{
+    return snapshot_impl(d, now, out_dev, cap, true);
 }
 
 int amb_decoder_stats(amb_decoder* d, uint64_t* kernel_launches, float* ms_last)

@@ -13,11 +13,12 @@ arithmetic runs in libairmodes_b200.so on the GPU; there is no CPU implementatio
 from __future__ import annotations
 
 import ctypes as C
+import math
 
 import numpy as np
 
 from . import _lib
-from ._lib import Fields, Frame, check
+from ._lib import Aircraft, Fields, Frame, check
 
 FS_NO_HANDLER, FS_METRIC_ALT, FS_CPR_NO_POS, FS_CPR_STRADDLE = 0x01, 0x02, 0x04, 0x08
 FS_HAS_POS, FS_HAS_RANGE, FS_METRIC_THREAT, FS_NOT_QUEUED = 0x10, 0x20, 0x40, 0x80
@@ -26,9 +27,16 @@ NO_ALTITUDE = -(1 << 31)
 LOCAL_NOT_TRIED, LOCAL_DECODED, LOCAL_NO_REF, LOCAL_STALE, LOCAL_REJECTED = (
     _lib.LOCAL_NOT_TRIED, _lib.LOCAL_DECODED, _lib.LOCAL_NO_REF, _lib.LOCAL_STALE, _lib.LOCAL_REJECTED)
 LOCAL_CPR_MAX = _lib.LOCAL_CPR_MAX
+# per-aircraft table (decoder option track; include/airmodes_b200.h amb_aircraft, AMB_AC_*)
+AC_HAS_ALT, AC_HAS_SQUAWK, AC_HAS_IDENT, AC_HAS_POS, AC_HAS_RANGE = (
+    _lib.AC_HAS_ALT, _lib.AC_HAS_SQUAWK, _lib.AC_HAS_IDENT, _lib.AC_HAS_POS, _lib.AC_HAS_RANGE)
+AC_HAS_VELOCITY, AC_HAS_HEADING, AC_HAS_EPS, AC_ON_GROUND = (
+    _lib.AC_HAS_VELOCITY, _lib.AC_HAS_HEADING, _lib.AC_HAS_EPS, _lib.AC_ON_GROUND)
+TRACK_MAX = _lib.TRACK_MAX
 
 FIELDS_DTYPE = np.dtype(Fields)
 FRAME_DTYPE = np.dtype(Frame)
+AIRCRAFT_DTYPE = np.dtype(Aircraft)
 
 
 def frames_from_messages(msgs):
@@ -69,14 +77,52 @@ def check_local_cpr(seconds) -> int:
     return int(seconds)
 
 
+def check_track(seconds) -> int:
+    """Validate a track setting: an int in 0 (off) .. TRACK_MAX seconds. Raises ValueError otherwise."""
+    try:
+        ok = not isinstance(seconds, bool) and int(seconds) == seconds and 0 <= int(seconds) <= TRACK_MAX
+    except (TypeError, ValueError):
+        ok = False
+    if not ok:
+        raise ValueError("track: an integer number of seconds in 0 (off) .. %d, got %r" % (TRACK_MAX, seconds))
+    return int(seconds)
+
+
+# aircraft_to_dict: a column and the flag that says it is set
+_AC_COLUMNS = (("altitude", AC_HAS_ALT), ("squawk", AC_HAS_SQUAWK), ("ident", AC_HAS_IDENT), ("ftc", AC_HAS_IDENT),
+               ("cat", AC_HAS_IDENT), ("lat", AC_HAS_POS), ("lon", AC_HAS_POS), ("pos_t", AC_HAS_POS),
+               ("range", AC_HAS_RANGE), ("bearing", AC_HAS_RANGE), ("speed", AC_HAS_VELOCITY),
+               ("vertical", AC_HAS_VELOCITY), ("heading", AC_HAS_HEADING), ("eps", AC_HAS_EPS))
+
+
+def aircraft_to_dict(row) -> dict:
+    """One AIRCRAFT_DTYPE row -> plain dict for JSON: ident as str, a column whose flag is clear as None, on_ground as
+    bool, and rssi = 10 log10(max(1e-8, ref_level)) as the reference computes it from the slicer's level (parse.py:430)."""
+    flags = int(row["flags"])
+    d = {"icao": int(row["icao"]), "messages": int(row["messages"]), "first_seen": float(row["first_seen"]),
+         "seen": float(row["seen"]), "rssi": 10.0 * math.log10(max(1e-8, float(row["ref_level"]))),
+         "flags": flags, "on_ground": bool(flags & AC_ON_GROUND)}
+    for name, flag in _AC_COLUMNS:
+        if not flags & flag:
+            d[name] = None
+        elif name == "ident":
+            d[name] = np.asarray(row["ident"]).tobytes().rstrip(b"\0").decode("ascii", "replace")
+        else:
+            d[name] = row[name].item()
+    return d
+
+
 class batch_decoder:
     """cpr_decoder(my_location) (cpr.py:184-190) + parser, for batches. my_location = [lat, lon] or None.
 
     local_cpr = S > 0 also decodes every position message the global decode leaves without a fix relative to the
-    aircraft's last position of at most S seconds before (DESIGN.md §8); 0, the default, is the reference's decoder."""
+    aircraft's last position of at most S seconds before (DESIGN.md §8); 0, the default, is the reference's decoder.
+    track = S > 0 also keeps a per-aircraft table on the device, read with aircraft() / aircraft_device(): one row per
+    address heard in a DF17 squitter, dropped S seconds after its last message (DESIGN.md §8 "Aircraft table")."""
 
-    def __init__(self, my_location=None, device: int = 0, local_cpr: int = 0):
+    def __init__(self, my_location=None, device: int = 0, local_cpr: int = 0, track: int = 0):
         local_cpr = check_local_cpr(local_cpr)
+        track = check_track(track)
         self._lib = _lib.load()
         h = C.c_void_p()
         have, lat, lon = self._loc(my_location)
@@ -85,10 +131,14 @@ class batch_decoder:
             detail = self._lib.amb_decoder_last_error(None).decode()
             raise RuntimeError("libairmodes_b200: %s%s" % (self._lib.amb_strerror(rc).decode(), (" (%s)" % detail) if detail else ""))
         self._h = h
+        self._device = int(device)
         self.my_location = my_location
         self._local_cpr = 0
         if local_cpr:
             self.set_local_cpr(local_cpr)
+        self._track = 0
+        if track:
+            self.set_track(track)
 
     @staticmethod
     def _loc(loc):
@@ -106,7 +156,7 @@ class batch_decoder:
         self.my_location = new_location
 
     def reset(self):
-        """Forget every stored report and reference position; the local_cpr setting stays."""
+        """Forget every stored report, reference position and aircraft; the local_cpr and track settings stay."""
         self._check(self._lib.amb_decoder_reset(self._h))
 
     def set_local_cpr(self, seconds: int):
@@ -117,6 +167,42 @@ class batch_decoder:
 
     def get_local_cpr(self) -> int:
         return self._local_cpr
+
+    def set_track(self, seconds: int):
+        """Option track = S seconds (0 = off); applies from the next decode."""
+        seconds = check_track(seconds)
+        self._check(self._lib.amb_decoder_set_option(self._h, b"track", seconds))
+        self._track = seconds
+
+    def get_track(self) -> int:
+        return self._track
+
+    @staticmethod
+    def _now(now):
+        return math.nan if now is None else float(now)
+
+    def aircraft(self, now=None) -> np.ndarray:
+        """The aircraft table at time `now` (None: the t of the latest queued message decoded since reset): every row
+        heard within the last S seconds up to `now`, in ascending address, as a numpy AIRCRAFT_DTYPE array."""
+        now = self._now(now)
+        n = self._check(self._lib.amb_decoder_aircraft(self._h, now, None, 0))
+        out = np.zeros(n, dtype=AIRCRAFT_DTYPE)
+        if n:
+            n = self._check(self._lib.amb_decoder_aircraft(self._h, now, C.c_void_p(out.ctypes.data), n))
+        return out[:n]
+
+    def aircraft_device(self, now=None, out_dev=None):
+        """aircraft() into device memory: returns a CUDA uint8 tensor of 128-byte amb_aircraft rows (a view of the
+        first rows of out_dev when one is given). Only the row count crosses PCIe."""
+        import torch
+        now = self._now(now)
+        if out_dev is None:
+            n = self._check(self._lib.amb_decoder_aircraft_device(self._h, now, None, 0))
+            out_dev = torch.empty(n * 128, dtype=torch.uint8, device=torch.device("cuda", self._device))
+        torch.cuda.current_stream(out_dev.device).synchronize()          # the decoder runs on its own stream
+        n = self._check(self._lib.amb_decoder_aircraft_device(self._h, now, C.c_void_p(out_dev.data_ptr()),
+                                                              int(out_dev.numel() // 128)))
+        return out_dev[: n * 128]
 
     def decode(self, frames, n: int | None = None) -> np.ndarray:
         """frames: ctypes Frame array / list of Frame (e.g. rx_path.frames) / numpy FRAME_DTYPE array, in stream

@@ -392,14 +392,69 @@ typedef struct amb_fields {
 #define AMB_LOCAL_REJECTED 4     /* the local decode failed the plausibility check; the reference is kept */
 #define AMB_LOCAL_CPR_MAX 600
 
+/* Per-aircraft state table (amb_decoder_set_option(d, "track", S), S in 1..3600 seconds): every decode also folds its
+ * records, in stream order, into one row per 24-bit address, kept on the device. A record counts when its status has
+ * neither AMB_FS_NOT_QUEUED nor AMB_FS_NO_HANDLER; a = its icao field, t = secs + frac of its frame.
+ *   expiry    a row whose seen lies more than S before t (t - seen > S) counts as absent;
+ *   creation  without a live row, a DF17 record creates one (every column blank, first_seen = t, messages = 0); any
+ *             other record is ignored;
+ *   apply     messages += 1, seen = t, ref_level = the frame's; altitude from DF0/4/16/20 and BDS0,5 when it is not
+ *             AMB_NO_ALTITUDE; BDS0,5 clears AMB_AC_ON_GROUND (with or without an altitude), BDS0,6 sets altitude 0
+ *             and AMB_AC_ON_GROUND; squawk from DF5/21; ident,
+ *             ftc, cat from BDS0,8; lat, lon, pos_t = t from a record with AMB_FS_HAS_POS (range / bearing with
+ *             AMB_FS_HAS_RANGE, else NaN); speed, heading, vertical = val[0..2] of BDS0,9 subtypes 0 and 1; heading =
+ *             val[0] of BDS0,6; eps from BDS6,1. Nothing else changes a row.
+ * A column whose flag is clear holds NaN, AMB_NO_ALTITUDE or -1 (ident: 8 zero bytes). Every column is a copy of a
+ * record or frame value, so a row does not depend on how the stream is cut into calls. */
+#define AMB_AC_HAS_ALT 0x001
+#define AMB_AC_HAS_SQUAWK 0x002
+#define AMB_AC_HAS_IDENT 0x004       /* ident, ftc, cat */
+#define AMB_AC_HAS_POS 0x008         /* lat, lon, pos_t */
+#define AMB_AC_HAS_RANGE 0x010       /* range, bearing of that position (receiver location known) */
+#define AMB_AC_HAS_VELOCITY 0x020    /* speed, vertical */
+#define AMB_AC_HAS_HEADING 0x040
+#define AMB_AC_HAS_EPS 0x080
+#define AMB_AC_ON_GROUND 0x100       /* the last BDS0,5 / BDS0,6 was a surface report */
+#define AMB_TRACK_MAX 3600
+
+typedef struct amb_aircraft {
+    uint32_t icao;        /* the 24-bit address */
+    uint32_t messages;    /* records applied since the row was created */
+    double first_seen;    /* t of the DF17 record that created the row */
+    double seen;          /* t of the last record applied */
+    float ref_level;      /* that record's frame ref_level; rssi = 10 log10(max(1e-8, ref_level)) (parse.py:430) */
+    uint16_t flags;       /* AMB_AC_* */
+    int8_t ftc, cat;      /* BDS0,8 type code 1..4 and category */
+    char ident[8];        /* BDS0,8 callsign, no terminator */
+    int32_t altitude;     /* feet */
+    int32_t squawk;
+    double lat, lon;      /* degrees */
+    double range, bearing;/* statute miles, degrees, from the receiver location */
+    double pos_t;         /* t of the record that gave the position */
+    double speed, heading, vertical;   /* knots, degrees, feet per minute */
+    int8_t eps;           /* BDS6,1 emergency/priority status */
+    uint8_t pad_[15];     /* 0 */
+} amb_aircraft;           /* 128 bytes */
+
 typedef struct amb_decoder amb_decoder;
 /* cpr_decoder(my_location) (cpr.py:184-190) + the parser; have_location = 0 is my_location = None. */
 AMB_API int amb_decoder_create(int device, int have_location, double lat, double lon, amb_decoder** out);
 /* "local_cpr": S = 0 (default, off) .. 600 seconds, locally referenced CPR decode (see AMB_FIELDS_LOCAL); applies from
  * the next call. The table of reference positions (2^24 x 24 B = 384 MiB of device memory) is allocated at the first
  * decode with the option on, written only by such decodes and cleared by amb_decoder_reset. Off changes nothing.
+ * "track": S = 0 (default, off) .. 3600 seconds, the per-aircraft table (see amb_aircraft); applies from the next call.
+ * Rows are direct-mapped by address: 2^24 x 128 B = 2 GiB of device memory plus a 2 MiB occupancy bitmap, allocated at
+ * the first decode with the option on; only the bitmap is cleared (by amb_decoder_reset). A decode with the option on
+ * launches six kernels more (13, or 19 with "local_cpr"); with it off nothing changes.
  * Unknown names and out-of-range values return AMB_ERR_INVALID. */
 AMB_API int amb_decoder_set_option(amb_decoder* d, const char* name, int value);
+/* Snapshot of the per-aircraft table at time `now`: every row with seen <= now and now - seen <= S, in ascending
+ * address. now = NaN stands for the t of the latest queued record decoded since the last reset (kept on the device).
+ * out == NULL returns the number of rows; a buffer of fewer than that many rows returns AMB_ERR_OVERFLOW and writes
+ * nothing. Otherwise returns the number of rows written. AMB_ERR_STATE when the option "track" is off. Three kernel
+ * launches (two when nothing is written) and one 4-byte copy to the host; _device writes to device memory. */
+AMB_API int amb_decoder_aircraft(amb_decoder* d, double now, amb_aircraft* out, int max);
+AMB_API int amb_decoder_aircraft_device(amb_decoder* d, double now, amb_aircraft* out_dev, int cap);
 AMB_API void amb_decoder_destroy(amb_decoder* d);
 AMB_API int amb_decoder_set_location(amb_decoder* d, int have_location, double lat, double lon);   /* cpr.py:192-193 */
 AMB_API int amb_decoder_reset(amb_decoder* d);                      /* forget every stored report (and reference position) */

@@ -12,6 +12,7 @@ of the dl_data feed and are not re-implemented.
 
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 [-T 7.0] [-d] [-t 5556] [-n] [--reports | -l 37.4,-122.1]
     python tools/modes_rx_b200.py -s 127.0.0.1:12345 -r 4e6 --udp-idle 2.0
+    python tools/modes_rx_b200.py -s capture.cfile -r 4e6 --track 60 --aircraft aircraft.json
 
 Differences, all on the far side of rx_path:
 * live radios (-s uhd / osmocom) need GNU Radio: use gr_air_modes_b200.gr_adapter.rx_path inside modes_radio.
@@ -22,6 +23,7 @@ Differences, all on the far side of rx_path:
   in front and runs the chain at 4 Msps like modes_rx does.
 """
 import argparse
+import json
 import os
 import re
 import socket
@@ -106,15 +108,27 @@ class print_queue:
         self.count += 1
 
 
+def write_aircraft(path, rows):
+    """The aircraft table (AIRCRAFT_DTYPE rows) as a JSON list, one object per aircraft (decode.aircraft_to_dict), written
+    to a temporary file beside `path` and renamed over it, so that a reader never sees a half-written file."""
+    from gr_air_modes_b200 import decode
+    tmp = "%s.tmp%d" % (path, os.getpid())
+    with open(tmp, "w") as f:
+        json.dump([decode.aircraft_to_dict(r) for r in rows], f)
+    os.replace(tmp, path)
+
+
 class report_queue:
     """What apps/modes_rx prints by default: air_modes.output_print(cpr_dec, publisher) (apps/modes_rx:77-78,
     python/msprint.py) - one text report per parsed message. The numbers come from the GPU batch decoder
-    (gr_air_modes_b200.decode), the line format from gr_air_modes_b200.report."""
+    (gr_air_modes_b200.decode), the line format from gr_air_modes_b200.report. out=None decodes without printing;
+    aircraft=PATH writes the decoder's aircraft table (option track) to PATH after every batch."""
 
-    def __init__(self, location, device, out=sys.stdout, local_cpr=0):
+    def __init__(self, location, device, out=sys.stdout, local_cpr=0, track=0, aircraft=None, decoder=None):
         from gr_air_modes_b200 import decode
-        self._dec = decode.batch_decoder(location, device, local_cpr=local_cpr)   # = cpr_decoder(my_position), apps/modes_rx:68
-        self._out, self._texts, self.count = out, [], 0
+        self._dec = decoder if decoder is not None else \
+            decode.batch_decoder(location, device, local_cpr=local_cpr, track=track)   # = cpr_decoder(my_position), apps/modes_rx:68
+        self._out, self._texts, self.count, self._aircraft = out, [], 0, aircraft
 
     def handle(self, msg):
         text = msg.to_string()
@@ -126,17 +140,22 @@ class report_queue:
         """Decode and print everything queued since the last call (one GPU batch)."""
         from gr_air_modes_b200 import report
         if self._texts:
-            for line in report.report_lines(self._texts, self._dec.decode_messages(self._texts)):
-                self._out.write(line + "\n")
-                self.count += 1
+            recs = self._dec.decode_messages(self._texts)
+            if self._out is not None:
+                for line in report.report_lines(self._texts, recs):
+                    self._out.write(line + "\n")
+                    self.count += 1
             self._texts = []
-        self._out.flush()
+        if self._out is not None:
+            self._out.flush()
+        if self._aircraft:
+            write_aircraft(self._aircraft, self._dec.aircraft())
 
     def close(self):
         self._dec.close()
 
 
-def main(argv=None):
+def parse_args(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("-s", "--source", required=True, help="<filename> (cfile) or <ip:port> (UDP of gr_complex)")   # radio.py:94-95
     ap.add_argument("-t", "--tcp", type=int, default=None, metavar="PORT",
@@ -167,7 +186,22 @@ def main(argv=None):
     ap.add_argument("--local-cpr", type=int, default=0, metavar="S",
                     help="position reports: decode a message that has no global fix relative to the aircraft's last "
                          "position of at most S (1..600) seconds before; 0 = off, as the reference")
+    ap.add_argument("--track", type=int, default=0, metavar="S",
+                    help="keep a per-aircraft table on the GPU; an aircraft is dropped S (1..3600) seconds after its "
+                         "last message; 0 = off")
+    ap.add_argument("--aircraft", type=str, default=None, metavar="PATH",
+                    help="after every chunk, write the aircraft table to PATH as JSON, one object per aircraft "
+                         "(needs --track; decodes the messages even without --reports)")
     args = ap.parse_args(argv)
+    if not 0 <= args.track <= 3600:
+        ap.error("--track: 0 (off) .. 3600 seconds")
+    if args.aircraft and args.track <= 0:
+        ap.error("--aircraft needs --track S")
+    return args
+
+
+def main(argv=None):
+    args = parse_args(argv)
 
     if args.source in ("uhd", "osmocom"):
         raise SystemExit("live radios need GNU Radio: use gr_air_modes_b200.gr_adapter.rx_path in modes_radio (INTEGRATION.md)")
@@ -187,14 +221,19 @@ def main(argv=None):
     sinks = []
     printer = None
     reporter = None
+    my_position = [float(x) for x in args.location.split(",")] if args.location is not None else None   # apps/modes_rx:64-65
     if not args.no_print:
         if args.reports or args.location is not None:
-            my_position = [float(x) for x in args.location.split(",")] if args.location is not None else None   # apps/modes_rx:64-65
-            reporter = report_queue(my_position, args.device, local_cpr=args.local_cpr)
+            reporter = report_queue(my_position, args.device, local_cpr=args.local_cpr, track=args.track,
+                                    aircraft=args.aircraft)
             sinks.append(reporter)
         else:
             printer = print_queue()
             sinks.append(printer)
+    if args.aircraft and reporter is None:                  # the table without printed reports
+        reporter = report_queue(my_position, args.device, out=None, local_cpr=args.local_cpr, track=args.track,
+                                aircraft=args.aircraft)
+        sinks.append(reporter)
     pub = None
     if args.tcp is not None:
         from gr_air_modes_b200.zmq_pub import zmq_queue
