@@ -24,6 +24,9 @@ AP_FILTER_MAX = 3600
 # AMB_FIELDS_LOCAL (include/airmodes_b200.h AMB_LOCAL_*), decoder option "local_cpr" = S seconds (0 = off)
 LOCAL_NOT_TRIED, LOCAL_DECODED, LOCAL_NO_REF, LOCAL_STALE, LOCAL_REJECTED = 0, 1, 2, 3, 4
 LOCAL_CPR_MAX = 600
+# AMB_FIELDS_COMMB (include/airmodes_b200.h AMB_COMMB_*), decoder option "commb" = S seconds (0 = off)
+COMMB_NOT_TRIED, COMMB_DECODED, COMMB_RESOLVED, COMMB_AMBIGUOUS, COMMB_NONE = 0, 1, 2, 3, 4
+COMMB_MAX = 600
 # amb_aircraft.flags (include/airmodes_b200.h AMB_AC_*), decoder option "track" = S seconds (0 = off)
 AC_HAS_ALT, AC_HAS_SQUAWK, AC_HAS_IDENT, AC_HAS_POS, AC_HAS_RANGE = 0x001, 0x002, 0x004, 0x008, 0x010
 AC_HAS_VELOCITY, AC_HAS_HEADING, AC_HAS_EPS, AC_ON_GROUND = 0x020, 0x040, 0x080, 0x100
@@ -114,6 +117,11 @@ class Fields(C.Structure):
     def local(self) -> int:
         """AMB_FIELDS_LOCAL (byte 136): local CPR outcome (decoder option "local_cpr"), LOCAL_*."""
         return self.pad_ & 0xFF
+
+    @property
+    def commb(self) -> int:
+        """AMB_FIELDS_COMMB (byte 137): Comm-B inference outcome (decoder option "commb"), COMMB_*."""
+        return (self.pad_ >> 8) & 0xFF
 
 
 class Aircraft(C.Structure):

@@ -13,6 +13,9 @@
 // With option "local_cpr" on, six more (amb_decode_local.cuh): amb_local_keys, the four partition kernels of the pairing
 // stage on ICAO keys, amb_local_walk - the local decode of the position messages the global decode left without a fix,
 // with a direct-mapped table of reference positions in HBM (2^24 x 24 B) carried from batch to batch.
+// With option "commb" on, six more after those (amb_decode_commb.cuh): amb_commb_keys, the four partition kernels on
+// address keys, amb_commb_walk - Comm-B register inference of the DF20/21 replies the parser does not handle, with a
+// direct-mapped table of ADS-B velocities in HBM (2^24 x 24 B) carried from batch to batch.
 // With option "track" on, six more after those (amb_decode_track.cuh): amb_track_keys, the four partition kernels on
 // address keys, amb_track_walk - the per-aircraft table, direct-mapped in HBM (2^24 x 128 B) with an occupancy bitmap;
 // amb_decoder_aircraft reads it out with three kernels of its own.
@@ -42,6 +45,8 @@ struct amb_decoder {
     int local_cpr = 0;                   // option "local_cpr" = S seconds, 0 = off
     AmbRefPos* ltable = nullptr;         // reference position per ICAO, allocated at the first decode with the option on
     AmbPosRec* d_lpos = nullptr; int lcap = 0;   // address-keyed records of the local and the track stage
+    int commb = 0;                       // option "commb" = S seconds, 0 = off
+    AmbCommbRef* ctable = nullptr;       // ADS-B velocity per address, allocated at the first decode with the option on
     int track = 0;                       // option "track" = S seconds, 0 = off
     amb_aircraft* trows = nullptr;       // one row per address, allocated at the first decode with the option on
     unsigned* tocc = nullptr;            // which rows hold data (AMB_TRACK_WORDS words)
@@ -148,6 +153,7 @@ int amb_decoder_create(int device, int have_location, double lat, double lon, am
     static_assert(sizeof(amb_fields) == 144, "amb_fields layout");
     static_assert(sizeof(AmbCprSlot) == 16, "table slot layout");
     static_assert(sizeof(AmbRefPos) == 24, "reference position slot layout");
+    static_assert(sizeof(AmbCommbRef) == 24, "velocity reference slot layout");
     static_assert(sizeof(amb_aircraft) == 128, "amb_aircraft layout");
     if (!out) return AMB_ERR_INVALID;
     *out = nullptr;
@@ -189,6 +195,7 @@ void amb_decoder_destroy(amb_decoder* d)
     amb_v3_free(&d->v3);
     if (d->ltable) cudaFree(d->ltable);
     if (d->d_lpos) cudaFree(d->d_lpos);
+    if (d->ctable) cudaFree(d->ctable);
     if (d->trows) cudaFree(d->trows);
     if (d->tocc) cudaFree(d->tocc);
     if (d->tclk) cudaFree(d->tclk);
@@ -216,6 +223,7 @@ int amb_decoder_reset(amb_decoder* d)
     DCK(cudaSetDevice(d->device));
     DCK(cudaMemsetAsync(d->table, 0xFF, AMB_TABLE_SLOTS * sizeof(AmbCprSlot), d->stream));
     if (d->ltable) DCK(cudaMemsetAsync(d->ltable, 0xFF, AMB_LOCAL_SLOTS * sizeof(AmbRefPos), d->stream));
+    if (d->ctable) DCK(cudaMemsetAsync(d->ctable, 0xFF, AMB_COMMB_SLOTS * sizeof(AmbCommbRef), d->stream));
     if (d->tocc) {                       // the rows themselves stay: a row whose bit is clear is never read
         static const AmbTrackClock none = {NAN, 0u, 0u};
         DCK(cudaMemsetAsync(d->tocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));
@@ -233,6 +241,11 @@ int amb_decoder_set_option(amb_decoder* d, const char* name, int value)
         d->local_cpr = value;
         return AMB_OK;
     }
+    if (strcmp(name, "commb") == 0) {
+        if (value < 0 || value > AMB_COMMB_MAX) return dfail(d, AMB_ERR_INVALID, "commb: 0 (off) .. 600 seconds");
+        d->commb = value;
+        return AMB_OK;
+    }
     if (strcmp(name, "track") == 0) {
         if (value < 0 || value > AMB_TRACK_MAX) return dfail(d, AMB_ERR_INVALID, "track: 0 (off) .. 3600 seconds");
         d->track = value;
@@ -241,7 +254,7 @@ int amb_decoder_set_option(amb_decoder* d, const char* name, int value)
     return dfail(d, AMB_ERR_INVALID, "amb_decoder_set_option: unknown option");
 }
 
-// the key records of the local and the track stage, one per frame
+// the key records of the local, the Comm-B and the track stage, one per frame
 static int ensure_keys(amb_decoder* d)
 {
     if (d->lcap < d->cap) {
@@ -259,6 +272,17 @@ static int ensure_local(amb_decoder* d)
     if (!d->ltable) {
         DCK(cudaMalloc(&d->ltable, AMB_LOCAL_SLOTS * sizeof(AmbRefPos)));
         DCK(cudaMemsetAsync(d->ltable, 0xFF, AMB_LOCAL_SLOTS * sizeof(AmbRefPos), d->stream));
+    }
+    return ensure_keys(d);
+}
+
+// the Comm-B stage's device memory, at the first decode with the option on (the table starts empty: all NaN)
+static int ensure_commb(amb_decoder* d)
+{
+    if (!d->ctable) {
+        cudaError_t e = cudaMalloc(&d->ctable, AMB_COMMB_SLOTS * sizeof(AmbCommbRef));
+        if (e != cudaSuccess) { d->ctable = nullptr; return dfail(d, AMB_ERR_CUDA, "Comm-B velocity table (384 MiB)", e); }
+        DCK(cudaMemsetAsync(d->ctable, 0xFF, AMB_COMMB_SLOTS * sizeof(AmbCommbRef), d->stream));
     }
     return ensure_keys(d);
 }
@@ -331,6 +355,13 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
                                         d->lon, d->nl_T, s, &e);
         if (kl < 0) return dfail(d, AMB_ERR_CUDA, "local CPR", e);
         d->launches += (uint64_t)kl;
+    }
+    if (d->commb > 0) {
+        rc = ensure_commb(d);
+        if (rc != AMB_OK) return rc;
+        const int kc = amb_commb_launch(&d->v3, src, fields, d->d_pos, d->d_lpos, n, d->ctable, d->commb, s, &e);
+        if (kc < 0) return dfail(d, AMB_ERR_CUDA, "Comm-B inference", e);
+        d->launches += (uint64_t)kc;
     }
     if (d->track > 0) {
         rc = ensure_track(d);

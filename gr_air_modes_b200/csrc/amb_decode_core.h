@@ -418,6 +418,153 @@ AMB_HD int amb_local_step(amb_fields* r, double t, AmbRefPos* ref, int max_age, 
     return v;
 }
 
+// ---- Comm-B register inference (decoder option "commb"; DESIGN.md §8 "Comm-B inference") --------------------------
+// The ADS-B velocity of an address as of a message: t, speed (val[0]) and track (val[1]) of its latest DF17 BDS0,9
+// subtype 0/1 record; t is NaN when there is none.
+struct AmbCommbRef { double t, speed, track; };
+
+#define AMB_COMMB_R40 0x1u
+#define AMB_COMMB_R50 0x2u
+#define AMB_COMMB_R60 0x4u
+
+// The MB word of a record the stage tries: MB bit k (1..56) is bit 56 - k of the result.
+AMB_HD uint64_t amb_commb_mb(const amb_frame& f) { return amb_bits(amb_msg_from_frame(f), 33, 56); }
+
+AMB_HD int amb_commb_count(unsigned c) { return (int)(c & 1u) + (int)((c >> 1) & 1u) + (int)((c >> 2) & 1u); }
+
+AMB_HD unsigned amb_commb_bits(uint64_t mb, int s, int n) { return (unsigned)((mb >> (57 - s - n)) & ((1ull << n) - 1)); }
+
+// Field i of register g (0 = 4,0, 1 = 5,0, 2 = 6,0): status bit, first value bit (the sign bit of a signed field) and
+// width (sign included), packed as status | first << 8 | width << 16 | signed << 24 (the table in include/airmodes_b200.h).
+AMB_HD unsigned amb_commb_spec(int g, int i)
+{
+#define AMB_CS(st, first, w, sg) ((st) | ((first) << 8) | ((w) << 16) | ((sg) << 24))
+    switch (g * 5 + i) {
+    case 0: return AMB_CS(1, 2, 12, 0);   case 1: return AMB_CS(14, 15, 12, 0);  case 2: return AMB_CS(27, 28, 12, 0);
+    case 3: return AMB_CS(48, 49, 3, 0);  case 4: return AMB_CS(54, 55, 2, 0);
+    case 5: return AMB_CS(1, 2, 10, 1);   case 6: return AMB_CS(12, 13, 11, 1);  case 7: return AMB_CS(24, 25, 10, 0);
+    case 8: return AMB_CS(35, 36, 10, 1); case 9: return AMB_CS(46, 47, 10, 0);
+    case 10: return AMB_CS(1, 2, 11, 1);  case 11: return AMB_CS(13, 14, 10, 0); case 12: return AMB_CS(24, 25, 10, 0);
+    case 13: return AMB_CS(35, 36, 10, 1); default: return AMB_CS(46, 47, 10, 1);
+    }
+#undef AMB_CS
+}
+
+// Read register g out of mb: raw values of fields 0..4 (0 when absent) and their status bits; returns 1 when the register
+// is a candidate (status/value consistency, at least one field, reserved bits 0, plausible values).
+AMB_HD int amb_commb_read(uint64_t mb, int g, int raw[5], unsigned* mask)
+{
+    unsigned m = 0;
+    int ok = 1;
+    for (int i = 0; i < 5; i++) {
+        const unsigned sp = amb_commb_spec(g, i);
+        const int first = (int)((sp >> 8) & 0xFF), w = (int)((sp >> 16) & 0xFF);
+        const unsigned v = amb_commb_bits(mb, first, w);
+        raw[i] = 0;
+        if (amb_commb_bits(mb, (int)(sp & 0xFF), 1)) {
+            m |= 1u << i;
+            raw[i] = (sp >> 24) && (v >> (w - 1)) ? (int)v - (1 << w) : (int)v;
+        } else if (v) {
+            ok = 0;                                         // data behind a status bit of 0
+        }
+    }
+    if (!m) ok = 0;
+    const int abs0 = raw[0] < 0 ? -raw[0] : raw[0], abs3 = raw[3] < 0 ? -raw[3] : raw[3];
+    const int abs4 = raw[4] < 0 ? -raw[4] : raw[4];
+    if (g == 0) {
+        if (amb_commb_bits(mb, 40, 8) || amb_commb_bits(mb, 52, 2)) ok = 0;
+        if (raw[0] > 3125 || raw[1] > 3125 || ((m & 4u) && (raw[2] < 700 || raw[2] > 3000))) ok = 0;
+    } else if (g == 1) {
+        const int d = raw[2] - raw[4];
+        if (abs0 > 284 || raw[2] > 400 || raw[4] > 300 || ((m & 4u) && (m & 16u) && (d > 125 || d < -125))) ok = 0;
+    } else {
+        if (raw[1] > 500 || raw[2] > 250 || abs3 > 187 || abs4 > 187) ok = 0;
+    }
+    *mask = m;
+    return ok;
+}
+
+AMB_HD unsigned amb_commb_candidates(uint64_t mb)
+{
+    unsigned c = 0;
+    for (int g = 0; g < 3; g++) {
+        int raw[5]; unsigned m;
+        if (amb_commb_read(mb, g, raw, &m)) c |= 1u << g;
+    }
+    return c;
+}
+
+// The record the stage tries: queued, DF20/21, 112 bits, status exactly AMB_FS_NO_HANDLER, and an MB first byte that
+// is not one of the parser's registers (those stay the parser's, as in the reference).
+AMB_HD int amb_commb_eligible(const amb_frame& f, const amb_fields* r)
+{
+    if (!f.passed || f.nbits != 112 || r->status != AMB_FS_NO_HANDLER || (r->df != 20 && r->df != 21)) return 0;
+    const unsigned b1 = amb_commb_bits(amb_commb_mb(f), 1, 8);
+    return !((b1 & 0x0F) == 0 && (b1 >> 4) <= 3);
+}
+
+// A record that carries its address's ADS-B velocity: queued DF17 BDS0,9 subtype 0/1 with speed and track.
+AMB_HD int amb_commb_is_ref(const amb_fields* r)
+{
+    return !(r->status & AMB_FS_NOT_QUEUED) && r->df == 17 && r->bds == 0x09 && (r->subtype == 0 || r->subtype == 1) &&
+           r->val[0] == r->val[0] && r->val[1] == r->val[1];
+}
+
+// Does a 5,0 reading agree with the ADS-B speed and track? (fp64, no contraction: the decoder is built -fmad=false)
+AMB_HD int amb_commb_agree(int gs_raw, int trk_raw, double speed, double track)
+{
+    const double trk = (double)trk_raw * 90.0 / 512.0;
+    double d = fmod(fabs(trk - track), 360.0);
+    d = d < 360.0 - d ? d : 360.0 - d;
+    return fabs(2.0 * (double)gs_raw - speed) <= 20.0 && d <= 10.0;
+}
+
+// Does the reference rule apply to this word? (5,0 among several candidates, with GS and track present)
+AMB_HD int amb_commb_needs_ref(uint64_t mb, unsigned cand)
+{
+    if (!(cand & AMB_COMMB_R50) || amb_commb_count(cand) < 2) return 0;
+    int raw[5]; unsigned m;
+    amb_commb_read(mb, 1, raw, &m);
+    return (m & 0x6u) == 0x6u;
+}
+
+// Write the outcome into the record: aux = raw values of register g (g < 0: none), pad_ bytes 1..4.
+AMB_HD void amb_commb_write(amb_fields* r, uint64_t mb, unsigned cand, int outcome, int g)
+{
+    int raw[5] = {0, 0, 0, 0, 0};
+    unsigned m = 0;
+    if (g >= 0) amb_commb_read(mb, g, raw, &m);
+    r->aux[0] = (uint32_t)(uint16_t)raw[0] | ((uint32_t)(uint16_t)raw[1] << 16);   // int16_t[8], little endian
+    r->aux[1] = (uint32_t)(uint16_t)raw[2] | ((uint32_t)(uint16_t)raw[3] << 16);
+    r->aux[2] = (uint32_t)(uint16_t)raw[4];
+    r->aux[3] = 0;
+    const uint64_t keep = r->pad_ & ~0xFFFFFFFF00ull;
+    r->pad_ = keep | ((uint64_t)outcome << 8) | ((uint64_t)(g >= 0 ? 0x40 + 0x10 * g : 0) << 16) | ((uint64_t)m << 24) |
+              ((uint64_t)cand << 32);
+}
+
+// One eligible record, given its address's velocity reference as of it (ref->t NaN: none). Returns the outcome.
+AMB_HD int amb_commb_step(amb_fields* r, uint64_t mb, double t, const AmbCommbRef* ref, int max_age)
+{
+    unsigned c = amb_commb_candidates(mb);
+    const unsigned cand = c;
+    int v;
+    if (!c) v = AMB_COMMB_NONE;
+    else if (amb_commb_count(c) == 1) v = AMB_COMMB_DECODED;
+    else {
+        v = AMB_COMMB_AMBIGUOUS;
+        if (amb_commb_needs_ref(mb, c) && ref->t == ref->t && t - ref->t >= 0.0 && t - ref->t <= (double)max_age) {
+            int raw[5]; unsigned m;
+            amb_commb_read(mb, 1, raw, &m);
+            c = amb_commb_agree(raw[2], raw[1], ref->speed, ref->track) ? AMB_COMMB_R50 : (c & ~AMB_COMMB_R50);
+            if (amb_commb_count(c) == 1) v = AMB_COMMB_RESOLVED;
+        }
+    }
+    const int g = (v == AMB_COMMB_DECODED || v == AMB_COMMB_RESOLVED) ? (c == AMB_COMMB_R40 ? 0 : c == AMB_COMMB_R50 ? 1 : 2) : -1;
+    amb_commb_write(r, mb, cand, v, g);
+    return v;
+}
+
 // Latest-report bookkeeping of cpr_decoder.decode for ONE message given the table state before it (cpr.py:214-229):
 // used by the pairing kernel lane by lane and, sequentially, by the host shim.
 // A stored report stamped LATER than the current message can only stem from an earlier stream (frame timestamps restart

@@ -42,4 +42,5 @@ __global__ void __launch_bounds__(128) amb_resolve_kernel(amb_fields* __restrict
 
 #include "amb_decode_v3.cuh"
 #include "amb_decode_local.cuh"
+#include "amb_decode_commb.cuh"
 #include "amb_decode_track.cuh"

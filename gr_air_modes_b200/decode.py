@@ -27,6 +27,10 @@ NO_ALTITUDE = -(1 << 31)
 LOCAL_NOT_TRIED, LOCAL_DECODED, LOCAL_NO_REF, LOCAL_STALE, LOCAL_REJECTED = (
     _lib.LOCAL_NOT_TRIED, _lib.LOCAL_DECODED, _lib.LOCAL_NO_REF, _lib.LOCAL_STALE, _lib.LOCAL_REJECTED)
 LOCAL_CPR_MAX = _lib.LOCAL_CPR_MAX
+# Comm-B inference outcome of a record (decoder option commb; include/airmodes_b200.h AMB_COMMB_*), read by commb_outcome()
+COMMB_NOT_TRIED, COMMB_DECODED, COMMB_RESOLVED, COMMB_AMBIGUOUS, COMMB_NONE = (
+    _lib.COMMB_NOT_TRIED, _lib.COMMB_DECODED, _lib.COMMB_RESOLVED, _lib.COMMB_AMBIGUOUS, _lib.COMMB_NONE)
+COMMB_MAX = _lib.COMMB_MAX
 # per-aircraft table (decoder option track; include/airmodes_b200.h amb_aircraft, AMB_AC_*)
 AC_HAS_ALT, AC_HAS_SQUAWK, AC_HAS_IDENT, AC_HAS_POS, AC_HAS_RANGE = (
     _lib.AC_HAS_ALT, _lib.AC_HAS_SQUAWK, _lib.AC_HAS_IDENT, _lib.AC_HAS_POS, _lib.AC_HAS_RANGE)
@@ -77,6 +81,53 @@ def check_local_cpr(seconds) -> int:
     return int(seconds)
 
 
+def check_commb(seconds) -> int:
+    """Validate a commb setting: an int in 0 (off) .. COMMB_MAX seconds. Raises ValueError otherwise."""
+    try:
+        ok = not isinstance(seconds, bool) and int(seconds) == seconds and 0 <= int(seconds) <= COMMB_MAX
+    except (TypeError, ValueError):
+        ok = False
+    if not ok:
+        raise ValueError("commb: an integer number of seconds in 0 (off) .. %d, got %r" % (COMMB_MAX, seconds))
+    return int(seconds)
+
+
+def commb_outcome(records):
+    """AMB_FIELDS_COMMB of a FIELDS_DTYPE record or array: COMMB_* per record (byte 1 of `pad_`)."""
+    return (np.asarray(records["pad_"], dtype=np.uint64) >> np.uint64(8)) & np.uint64(0xFF)
+
+
+# commb_values: per register, the names of fields 0..4 and their LSBs (include/airmodes_b200.h, DESIGN.md §8)
+COMMB_FIELDS = {
+    0x40: (("mcp_alt", 16.0), ("fms_alt", 16.0), ("baro", 0.1), ("modes", 1), ("alt_source", 1)),
+    0x50: (("roll", 45.0 / 256), ("track", 90.0 / 512), ("gs", 2.0), ("track_rate", 8.0 / 256), ("tas", 2.0)),
+    0x60: (("heading", 90.0 / 512), ("ias", 1.0), ("mach", 2.048 / 512), ("baro_rate", 32.0), ("inertial_rate", 32.0)),
+}
+
+
+def commb_values(record):
+    """The register a DECODED / RESOLVED record carries, as named physical values: {"bds": 0x40 / 0x50 / 0x60, name:
+    value or None for an absent field}. Degrees, knots, feet, mb (baro = 800 + 0.1 raw), Mach, ft/min and deg/s; the
+    mode bits (VNAV = 4, ALT = 2, APP = 1) and the target altitude source stay integers. None for any other record.
+    `record`: a FIELDS_DTYPE record or the dict from record_to_dict()."""
+    pad = int(record["pad_"])
+    if (pad >> 8) & 0xFF not in (COMMB_DECODED, COMMB_RESOLVED):
+        return None
+    reg, mask = (pad >> 16) & 0xFF, (pad >> 24) & 0xFF
+    words = [int(x) for x in record["aux"]]
+    raw = [((words[i // 2] >> (16 * (i % 2))) & 0xFFFF) for i in range(5)]
+    raw = [x - 0x10000 if x & 0x8000 else x for x in raw]
+    out = {"bds": reg}
+    for i, (name, lsb) in enumerate(COMMB_FIELDS[reg]):
+        if not mask & (1 << i):
+            out[name] = None
+        elif isinstance(lsb, int):
+            out[name] = raw[i]
+        else:
+            out[name] = raw[i] * lsb + (800.0 if name == "baro" else 0.0)
+    return out
+
+
 def check_track(seconds) -> int:
     """Validate a track setting: an int in 0 (off) .. TRACK_MAX seconds. Raises ValueError otherwise."""
     try:
@@ -118,10 +169,14 @@ class batch_decoder:
     local_cpr = S > 0 also decodes every position message the global decode leaves without a fix relative to the
     aircraft's last position of at most S seconds before (DESIGN.md §8); 0, the default, is the reference's decoder.
     track = S > 0 also keeps a per-aircraft table on the device, read with aircraft() / aircraft_device(): one row per
-    address heard in a DF17 squitter, dropped S seconds after its last message (DESIGN.md §8 "Aircraft table")."""
+    address heard in a DF17 squitter, dropped S seconds after its last message (DESIGN.md §8 "Aircraft table").
+    commb = S > 0 also infers the register (BDS 4,0 / 5,0 / 6,0) of the DF20/21 replies the parser does not handle,
+    with the address's ADS-B velocity of at most S seconds before deciding between 5,0 and the others; read with
+    commb_outcome() / commb_values() (DESIGN.md §8 "Comm-B inference")."""
 
-    def __init__(self, my_location=None, device: int = 0, local_cpr: int = 0, track: int = 0):
+    def __init__(self, my_location=None, device: int = 0, local_cpr: int = 0, track: int = 0, commb: int = 0):
         local_cpr = check_local_cpr(local_cpr)
+        commb = check_commb(commb)
         track = check_track(track)
         self._lib = _lib.load()
         h = C.c_void_p()
@@ -139,6 +194,9 @@ class batch_decoder:
         self._track = 0
         if track:
             self.set_track(track)
+        self._commb = 0
+        if commb:
+            self.set_commb(commb)
 
     @staticmethod
     def _loc(loc):
@@ -156,7 +214,7 @@ class batch_decoder:
         self.my_location = new_location
 
     def reset(self):
-        """Forget every stored report, reference position and aircraft; the local_cpr and track settings stay."""
+        """Forget every stored report, reference position, velocity and aircraft; the option settings stay."""
         self._check(self._lib.amb_decoder_reset(self._h))
 
     def set_local_cpr(self, seconds: int):
@@ -176,6 +234,15 @@ class batch_decoder:
 
     def get_track(self) -> int:
         return self._track
+
+    def set_commb(self, seconds: int):
+        """Option commb = S seconds (0 = off); applies from the next decode."""
+        seconds = check_commb(seconds)
+        self._check(self._lib.amb_decoder_set_option(self._h, b"commb", seconds))
+        self._commb = seconds
+
+    def get_commb(self) -> int:
+        return self._commb
 
     @staticmethod
     def _now(now):

@@ -47,6 +47,25 @@ def prefix(reference: float, secs: int, frac: float) -> str:
     return "(%i %.8f) " % (rssi, secs + frac)
 
 
+# Comm-B inference (decoder option commb): per register, its title and (name, format) of the fields that are present
+_COMMB_TEXT = {
+    0x40: ("BDS4,0 selected vertical intention", (("mcp_alt", "MCP alt %ift"), ("fms_alt", "FMS alt %ift"),
+                                                  ("baro", "baro %.1fmb"), ("modes", "modes %i"),
+                                                  ("alt_source", "alt source %i"))),
+    0x50: ("BDS5,0 track and turn report", (("roll", "roll %.1f"), ("track", "track %.1f"), ("gs", "GS %ikt"),
+                                            ("track_rate", "track rate %.2f"), ("tas", "TAS %ikt"))),
+    0x60: ("BDS6,0 heading and speed report", (("heading", "heading %.1f"), ("ias", "IAS %ikt"), ("mach", "Mach %.3f"),
+                                               ("baro_rate", "baro rate %ift/min"),
+                                               ("inertial_rate", "inertial rate %ift/min"))),
+}
+
+
+def _commb_text(df, ecc, v):
+    title, fields = _COMMB_TEXT[v["bds"]]
+    parts = [fmt % v[name] for name, fmt in fields if v[name] is not None]
+    return "Type %i %s from %x: %s" % (df, title, ecc, " ".join(parts))
+
+
 def format_report(message: str, r) -> str | None:
     """One slicer message string + its decoded record -> the line output_print would print, or None where the
     reference prints nothing. `r`: a FIELDS_DTYPE record or the dict from decode.record_to_dict()."""
@@ -54,6 +73,10 @@ def format_report(message: str, r) -> str | None:
         r = _d.record_to_dict(r)
     _, _, ref, secs, frac = message.split()
     st, df, ecc = r["status"], r["df"], r["ecc"]
+    if st == _d.FS_NO_HANDLER and df in (20, 21):
+        v = _d.commb_values(r)                      # decoder option commb: an inferred BDS 4,0 / 5,0 / 6,0 register
+        if v is not None:
+            return prefix(float(ref), int(secs), float(frac)) + _commb_text(df, ecc, v)
     if st & (_d.FS_NO_HANDLER | _d.FS_NOT_QUEUED):
         return None                                 # the parser raised: nothing is published (parse.py:431-434)
     out = prefix(float(ref), int(secs), float(frac))

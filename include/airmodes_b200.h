@@ -372,7 +372,7 @@ typedef struct amb_fields {
                              BDS0,9-1: velocity, heading, vert_spd, alt_geo_diff (parse.py:315-348)
                              BDS0,9-3: mag_hdg, vel, vert_spd, geo_diff (parse.py:350-364)
                              BDS0,6  : ground_track (parse.py:283) */
-    uint64_t pad_;        /* [byte 0] local CPR outcome (AMB_FIELDS_LOCAL), the rest 0 */
+    uint64_t pad_;        /* [byte 0] local CPR outcome (AMB_FIELDS_LOCAL), [1..4] Comm-B (AMB_FIELDS_COMMB*), the rest 0 */
 } amb_fields;             /* 144 bytes */
 
 /* Locally referenced CPR decode (amb_decoder_set_option(d, "local_cpr", S), S in 1..600 seconds). After the global
@@ -391,6 +391,40 @@ typedef struct amb_fields {
 #define AMB_LOCAL_STALE 3        /* its reference position is more than S seconds old (or stamped later than the message) */
 #define AMB_LOCAL_REJECTED 4     /* the local decode failed the plausibility check; the reference is kept */
 #define AMB_LOCAL_CPR_MAX 600
+
+/* Comm-B register inference (amb_decoder_set_option(d, "commb", S), S in 1..600 seconds). The parser accepts an MB word
+ * only when its first byte names register 0,0 / 1,0 / 2,0 / 3,0 (parse.py:180-190); the Enhanced Surveillance replies
+ * (BDS 4,0 / 5,0 / 6,0) say nothing of their register and stay AMB_FS_NO_HANDLER. With the option on, a queued 112-bit
+ * DF20/21 record whose status is exactly AMB_FS_NO_HANDLER and whose MB first byte is not one of the parser's registers
+ * is tried. MB bits are numbered 1..56 (MB bit k = message bit 32 + k); a signed field is a sign bit and n magnitude
+ * bits read as two's complement. Fields 0..4 (status bit, value bits, LSB):
+ *   4,0  0 MCP/FCU selected altitude 1, 2-13, 16 ft   1 FMS selected altitude 14, 15-26, 16 ft
+ *        2 baro setting - 800 mb 27, 28-39, 0.1 mb   3 VNAV/ALT/APP mode bits 48, 49-51   4 target altitude source 54, 55-56
+ *        reserved (must be 0) 40-47, 52-53
+ *   5,0  0 roll 1, s2 3-11, 45/256 deg   1 true track 12, s13 14-23, 90/512 deg   2 ground speed 24, 25-34, 2 kt
+ *        3 track angle rate 35, s36 37-45, 8/256 deg/s   4 true airspeed 46, 47-56, 2 kt
+ *   6,0  0 magnetic heading 1, s2 3-12, 90/512 deg   1 IAS 13, 14-23, 1 kt   2 Mach 24, 25-34, 2.048/512
+ *        3 baro altitude rate 35, s36 37-45, 32 ft/min   4 inertial vertical rate 46, s47 48-56, 32 ft/min
+ * A register is a candidate when every field whose status bit is 0 has all its value bits 0, at least one status bit
+ * is 1, the reserved bits are 0, and every present field is plausible (raw units): 4,0 selected altitudes <= 3125, baro
+ * 700..3000; 5,0 |roll| <= 284, GS <= 400, TAS <= 300, |GS - TAS| <= 125 when both are present; 6,0 IAS <= 500,
+ * Mach <= 250, |baro rate| and |inertial rate| <= 187. One candidate: AMB_COMMB_DECODED. Several: when 5,0 is among them
+ * with GS and track present and the address (icao) has a reference - the latest earlier queued DF17 BDS0,9 subtype 0/1
+ * record of that icao with val[0], val[1] not NaN, taken when 0 <= t - t_ref <= S (t = secs + frac) - 5,0 is kept alone
+ * when |2 gs - val[0]| <= 20 kt and the track difference (fmod(|track - val[1]|, 360), folded to 0..180) is <= 10 deg,
+ * else dropped; one register left: AMB_COMMB_RESOLVED. Otherwise AMB_COMMB_AMBIGUOUS. The status and every other field
+ * of the record stay as they are; the option writes only aux and bytes 1..4 of pad_: */
+#define AMB_FIELDS_COMMB(r) (((uint8_t*)&(r)->pad_)[1])        /* outcome, AMB_COMMB_* */
+#define AMB_FIELDS_COMMB_REG(r) (((uint8_t*)&(r)->pad_)[2])    /* 0x40 / 0x50 / 0x60 when DECODED or RESOLVED, else 0 */
+#define AMB_FIELDS_COMMB_MASK(r) (((uint8_t*)&(r)->pad_)[3])   /* bit i = status bit of field i of that register */
+#define AMB_FIELDS_COMMB_CAND(r) (((uint8_t*)&(r)->pad_)[4])   /* candidates: bit 0 = 4,0, bit 1 = 5,0, bit 2 = 6,0 */
+#define AMB_FIELDS_COMMB_RAW(r, i) (((int16_t*)(r)->aux)[i])   /* raw value of field i (0 when absent); 5..7 are 0 */
+#define AMB_COMMB_NOT_TRIED 0    /* option off, or not an eligible record */
+#define AMB_COMMB_DECODED 1      /* exactly one candidate register */
+#define AMB_COMMB_RESOLVED 2     /* several, one left after the test against the aircraft's ADS-B velocity */
+#define AMB_COMMB_AMBIGUOUS 3    /* several, and the velocity test could not apply or left more than one */
+#define AMB_COMMB_NONE 4         /* no candidate */
+#define AMB_COMMB_MAX 600
 
 /* Per-aircraft state table (amb_decoder_set_option(d, "track", S), S in 1..3600 seconds): every decode also folds its
  * records, in stream order, into one row per 24-bit address, kept on the device. A record counts when its status has
@@ -446,6 +480,10 @@ AMB_API int amb_decoder_create(int device, int have_location, double lat, double
  * Rows are direct-mapped by address: 2^24 x 128 B = 2 GiB of device memory plus a 2 MiB occupancy bitmap, allocated at
  * the first decode with the option on; only the bitmap is cleared (by amb_decoder_reset). A decode with the option on
  * launches six kernels more (13, or 19 with "local_cpr"); with it off nothing changes.
+ * "commb": S = 0 (default, off) .. 600 seconds, Comm-B register inference (see AMB_FIELDS_COMMB); applies from the next
+ * call. The ADS-B velocity per address (2^24 x 24 B = 384 MiB of device memory) is allocated at the first decode with
+ * the option on and cleared by amb_decoder_reset. A decode with the option on launches six kernels more; off changes
+ * nothing.
  * Unknown names and out-of-range values return AMB_ERR_INVALID. */
 AMB_API int amb_decoder_set_option(amb_decoder* d, const char* name, int value);
 /* Snapshot of the per-aircraft table at time `now`: every row with seen <= now and now - seen <= S, in ascending
