@@ -1,6 +1,7 @@
 """In-tree build of libairmodes_b200.so (nvcc, sm_90a only). Cross-compiles without a GPU."""
 from __future__ import annotations
 
+import glob
 import os
 import shutil
 import subprocess
@@ -9,7 +10,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libairmodes_b200.so")
 SOURCES = ["amb_kernels.cu", "amb_api.cu", "amb_decode.cu"]
-HEADERS = ["amb_internal.h", "amb_launch.h", "amb_params.h", "amb_decode_core.h", "amb_decode_kernels.cuh", "amb_decode_v3.cuh", "amb_decode_local.cuh", "amb_decode_commb.cuh", "amb_decode_track.cuh", "amb_order_kernels.cuh", os.path.join("..", "..", "include", "airmodes_b200.h")]
+HEADERS = sorted(glob.glob(os.path.join(CSRC, "*.h")) + glob.glob(os.path.join(CSRC, "*.cuh"))) + \
+    [os.path.join(HERE, "..", "include", "airmodes_b200.h")]
 # amb_decode.cu follows cpr.py operation by operation in IEEE double: no fused multiply-add contraction there
 EXTRA_FLAGS = {"amb_decode.cu": ["-fmad=false"]}
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

@@ -1,7 +1,8 @@
 // Batch field decode (SURVEY.md 8 row f4): kernels + C ABI of amb_decoder (include/airmodes_b200.h).
-// The per-message arithmetic is in amb_decode_core.h, the kernels in amb_decode_kernels.cuh and amb_decode_v3.cuh
-// (launch-free headers, so that tests/simt can run the same kernel source under a host emulator); this file holds the
-// per-aircraft report table and the host orchestration. Compiled with -fmad=false: latitude/longitude follow cpr.py
+// The per-message arithmetic is in amb_decode_core.h, the kernels and amb_decode_launch - the one launch sequence of a
+// decode - in amb_decode_kernels.cuh and the stage headers it includes (launch-free headers, so that tests/simt can run
+// the same kernel source and sequence under a host emulator); this file allocates the tables and buffers the stages
+// need, copies the frames in and the records out. Compiled with -fmad=false: latitude/longitude follow cpr.py
 // operation by operation in IEEE double, nothing may be contracted. Citations are file:line under gr-air-modes/python.
 //
 // Seven launches per decode, in stream order:
@@ -33,24 +34,13 @@ struct amb_decoder {
     int device = 0;
     cudaStream_t stream = nullptr;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
-    int have_loc = 0; double lat = 0.0, lon = 0.0;
-    AmbCprSlot* table = nullptr;
-    double* nl_T = nullptr;              // device copy of the NL transition table
-    amb_frame* d_frames = nullptr; amb_fields* d_fields = nullptr; AmbPosRec* d_pos = nullptr; AmbPair* d_pair = nullptr;
-    int cap = 0;
+    AmbDecodeState st;                   // the stages' tables, scratch and options (amb_decode_kernels.cuh)
+    amb_frame* d_frames = nullptr; amb_fields* d_fields = nullptr;
+    int cap = 0;                         // frames d_frames, d_fields, st.pos and st.pair hold
+    int kcap = 0;                        // frames st.keys holds
     // host <-> device staging: pageable caller arrays go through two pinned bounce buffers per direction so that the
     // copies run at PCIe speed and overlap the memcpy of the next piece
     void* pin[2] = {nullptr, nullptr}; cudaEvent_t pin_ev[2] = {nullptr, nullptr}; size_t pin_bytes = 0;
-    AmbV3Bufs v3;                        // scratch of the pairing stage (and of the local stage's partition)
-    int local_cpr = 0;                   // option "local_cpr" = S seconds, 0 = off
-    AmbRefPos* ltable = nullptr;         // reference position per ICAO, allocated at the first decode with the option on
-    AmbPosRec* d_lpos = nullptr; int lcap = 0;   // address-keyed records of the local and the track stage
-    int commb = 0;                       // option "commb" = S seconds, 0 = off
-    AmbCommbRef* ctable = nullptr;       // ADS-B velocity per address, allocated at the first decode with the option on
-    int track = 0;                       // option "track" = S seconds, 0 = off
-    amb_aircraft* trows = nullptr;       // one row per address, allocated at the first decode with the option on
-    unsigned* tocc = nullptr;            // which rows hold data (AMB_TRACK_WORDS words)
-    AmbTrackClock* tclk = nullptr;       // t of the latest queued record since reset
     uint32_t* snap_cnt = nullptr;        // snapshot: per-block counts, then their scan and the total
     amb_aircraft* d_snap = nullptr; int snap_cap = 0;   // snapshot rows on their way to host memory
     uint64_t launches = 0; float ms_last = 0.f;
@@ -127,9 +117,9 @@ static void free_bufs(amb_decoder* d)
 {
     if (d->d_frames) cudaFree(d->d_frames);
     if (d->d_fields) cudaFree(d->d_fields);
-    if (d->d_pos) cudaFree(d->d_pos);
-    if (d->d_pair) cudaFree(d->d_pair);
-    d->d_frames = nullptr; d->d_fields = nullptr; d->d_pos = nullptr; d->d_pair = nullptr; d->cap = 0;
+    if (d->st.pos) cudaFree(d->st.pos);
+    if (d->st.pair) cudaFree(d->st.pair);
+    d->d_frames = nullptr; d->d_fields = nullptr; d->st.pos = nullptr; d->st.pair = nullptr; d->cap = 0;
 }
 
 static int ensure_cap(amb_decoder* d, int n)
@@ -140,8 +130,8 @@ static int ensure_cap(amb_decoder* d, int n)
     free_bufs(d);
     DCK(cudaMalloc(&d->d_frames, (size_t)cap * sizeof(amb_frame)));
     DCK(cudaMalloc(&d->d_fields, (size_t)cap * sizeof(amb_fields)));
-    DCK(cudaMalloc(&d->d_pos, (size_t)cap * sizeof(AmbPosRec)));
-    DCK(cudaMalloc(&d->d_pair, (size_t)cap * sizeof(AmbPair)));
+    DCK(cudaMalloc(&d->st.pos, (size_t)cap * sizeof(AmbPosRec)));
+    DCK(cudaMalloc(&d->st.pair, (size_t)cap * sizeof(AmbPair)));
     d->cap = cap;
     return AMB_OK;
 }
@@ -165,19 +155,19 @@ int amb_decoder_create(int device, int have_location, double lat, double lon, am
     amb_decoder* d = new (std::nothrow) amb_decoder();
     if (!d) return AMB_ERR_INVALID;
     d->device = device;
-    d->have_loc = have_location ? 1 : 0; d->lat = lat; d->lon = lon;
+    d->st.have_loc = have_location ? 1 : 0; d->st.lat = lat; d->st.lon = lon;
     int rc = AMB_OK;
     do {
         if (cudaSetDevice(device) != cudaSuccess) { rc = AMB_ERR_NO_DEVICE; break; }
         if (cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking) != cudaSuccess ||
             cudaEventCreate(&d->e0) != cudaSuccess || cudaEventCreate(&d->e1) != cudaSuccess) { rc = AMB_ERR_CUDA; break; }
-        cudaError_t e = cudaMalloc(&d->table, AMB_TABLE_SLOTS * sizeof(AmbCprSlot));
+        cudaError_t e = cudaMalloc(&d->st.table, AMB_TABLE_SLOTS * sizeof(AmbCprSlot));
         if (e != cudaSuccess) { rc = dfail(d, AMB_ERR_CUDA, "report table (1 GiB)", e); break; }
-        if (cudaMalloc(&d->nl_T, AMB_NL_MAX * sizeof(double)) != cudaSuccess) { rc = AMB_ERR_CUDA; break; }
+        if (cudaMalloc(&d->st.nl_T, AMB_NL_MAX * sizeof(double)) != cudaSuccess) { rc = AMB_ERR_CUDA; break; }
         double T[AMB_NL_MAX];
         amb_build_nl_table(T);                          // cpr.py:46-51 through the host libm, once
-        if (cudaMemcpyAsync(d->nl_T, T, sizeof T, cudaMemcpyHostToDevice, d->stream) != cudaSuccess ||
-            cudaMemsetAsync(d->table, 0xFF, AMB_TABLE_SLOTS * sizeof(AmbCprSlot), d->stream) != cudaSuccess ||
+        if (cudaMemcpyAsync(d->st.nl_T, T, sizeof T, cudaMemcpyHostToDevice, d->stream) != cudaSuccess ||
+            cudaMemsetAsync(d->st.table, 0xFF, AMB_TABLE_SLOTS * sizeof(AmbCprSlot), d->stream) != cudaSuccess ||
             cudaStreamSynchronize(d->stream) != cudaSuccess) { rc = AMB_ERR_CUDA; break; }
     } while (0);
     if (rc != AMB_OK) { g_create_err = d->err.empty() ? "CUDA resource creation failed" : d->err; amb_decoder_destroy(d); return rc; }
@@ -192,18 +182,18 @@ void amb_decoder_destroy(amb_decoder* d)
     cudaSetDevice(d->device);
     if (d->stream) cudaStreamSynchronize(d->stream);
     free_bufs(d);
-    amb_v3_free(&d->v3);
-    if (d->ltable) cudaFree(d->ltable);
-    if (d->d_lpos) cudaFree(d->d_lpos);
-    if (d->ctable) cudaFree(d->ctable);
-    if (d->trows) cudaFree(d->trows);
-    if (d->tocc) cudaFree(d->tocc);
-    if (d->tclk) cudaFree(d->tclk);
+    amb_v3_free(&d->st.v3);
+    if (d->st.ltable) cudaFree(d->st.ltable);
+    if (d->st.keys) cudaFree(d->st.keys);
+    if (d->st.ctable) cudaFree(d->st.ctable);
+    if (d->st.trows) cudaFree(d->st.trows);
+    if (d->st.tocc) cudaFree(d->st.tocc);
+    if (d->st.tclk) cudaFree(d->st.tclk);
     if (d->snap_cnt) cudaFree(d->snap_cnt);
     if (d->d_snap) cudaFree(d->d_snap);
     for (int k = 0; k < 2; k++) { if (d->pin[k]) cudaFreeHost(d->pin[k]); if (d->pin_ev[k]) cudaEventDestroy(d->pin_ev[k]); }
-    if (d->table) cudaFree(d->table);
-    if (d->nl_T) cudaFree(d->nl_T);
+    if (d->st.table) cudaFree(d->st.table);
+    if (d->st.nl_T) cudaFree(d->st.nl_T);
     if (d->e0) cudaEventDestroy(d->e0);
     if (d->e1) cudaEventDestroy(d->e1);
     if (d->stream) cudaStreamDestroy(d->stream);
@@ -213,7 +203,7 @@ void amb_decoder_destroy(amb_decoder* d)
 int amb_decoder_set_location(amb_decoder* d, int have_location, double lat, double lon)
 {
     if (!d) return AMB_ERR_INVALID;
-    d->have_loc = have_location ? 1 : 0; d->lat = lat; d->lon = lon;
+    d->st.have_loc = have_location ? 1 : 0; d->st.lat = lat; d->st.lon = lon;
     return AMB_OK;
 }
 
@@ -221,13 +211,13 @@ int amb_decoder_reset(amb_decoder* d)
 {
     if (!d) return AMB_ERR_INVALID;
     DCK(cudaSetDevice(d->device));
-    DCK(cudaMemsetAsync(d->table, 0xFF, AMB_TABLE_SLOTS * sizeof(AmbCprSlot), d->stream));
-    if (d->ltable) DCK(cudaMemsetAsync(d->ltable, 0xFF, AMB_LOCAL_SLOTS * sizeof(AmbRefPos), d->stream));
-    if (d->ctable) DCK(cudaMemsetAsync(d->ctable, 0xFF, AMB_COMMB_SLOTS * sizeof(AmbCommbRef), d->stream));
-    if (d->tocc) {                       // the rows themselves stay: a row whose bit is clear is never read
+    DCK(cudaMemsetAsync(d->st.table, 0xFF, AMB_TABLE_SLOTS * sizeof(AmbCprSlot), d->stream));
+    if (d->st.ltable) DCK(cudaMemsetAsync(d->st.ltable, 0xFF, AMB_LOCAL_SLOTS * sizeof(AmbRefPos), d->stream));
+    if (d->st.ctable) DCK(cudaMemsetAsync(d->st.ctable, 0xFF, AMB_COMMB_SLOTS * sizeof(AmbCommbRef), d->stream));
+    if (d->st.tocc) {                    // the rows themselves stay: a row whose bit is clear is never read
         static const AmbTrackClock none = {NAN, 0u, 0u};
-        DCK(cudaMemsetAsync(d->tocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));
-        DCK(cudaMemcpyAsync(d->tclk, &none, sizeof none, cudaMemcpyHostToDevice, d->stream));
+        DCK(cudaMemsetAsync(d->st.tocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));
+        DCK(cudaMemcpyAsync(d->st.tclk, &none, sizeof none, cudaMemcpyHostToDevice, d->stream));
     }
     DCK(cudaStreamSynchronize(d->stream));
     return AMB_OK;
@@ -235,20 +225,20 @@ int amb_decoder_reset(amb_decoder* d)
 
 int amb_decoder_set_option(amb_decoder* d, const char* name, int value)
 {
+    static const struct { const char* name; int max; int AmbDecodeState::*seconds; } options[] = {
+        {"local_cpr", AMB_LOCAL_CPR_MAX, &AmbDecodeState::local_cpr},
+        {"commb", AMB_COMMB_MAX, &AmbDecodeState::commb},
+        {"track", AMB_TRACK_MAX, &AmbDecodeState::track},
+    };
     if (!d || !name) return AMB_ERR_INVALID;
-    if (strcmp(name, "local_cpr") == 0) {
-        if (value < 0 || value > AMB_LOCAL_CPR_MAX) return dfail(d, AMB_ERR_INVALID, "local_cpr: 0 (off) .. 600 seconds");
-        d->local_cpr = value;
-        return AMB_OK;
-    }
-    if (strcmp(name, "commb") == 0) {
-        if (value < 0 || value > AMB_COMMB_MAX) return dfail(d, AMB_ERR_INVALID, "commb: 0 (off) .. 600 seconds");
-        d->commb = value;
-        return AMB_OK;
-    }
-    if (strcmp(name, "track") == 0) {
-        if (value < 0 || value > AMB_TRACK_MAX) return dfail(d, AMB_ERR_INVALID, "track: 0 (off) .. 3600 seconds");
-        d->track = value;
+    for (const auto& o : options) {
+        if (strcmp(name, o.name) != 0) continue;
+        if (value < 0 || value > o.max) {
+            char what[64];
+            snprintf(what, sizeof what, "%s: 0 (off) .. %d seconds", o.name, o.max);
+            return dfail(d, AMB_ERR_INVALID, what);
+        }
+        d->st.*o.seconds = value;
         return AMB_OK;
     }
     return dfail(d, AMB_ERR_INVALID, "amb_decoder_set_option: unknown option");
@@ -257,11 +247,11 @@ int amb_decoder_set_option(amb_decoder* d, const char* name, int value)
 // the key records of the local, the Comm-B and the track stage, one per frame
 static int ensure_keys(amb_decoder* d)
 {
-    if (d->lcap < d->cap) {
-        if (d->d_lpos) cudaFree(d->d_lpos);
-        d->d_lpos = nullptr; d->lcap = 0;
-        DCK(cudaMalloc(&d->d_lpos, (size_t)d->cap * sizeof(AmbPosRec)));
-        d->lcap = d->cap;
+    if (d->kcap < d->cap) {
+        if (d->st.keys) cudaFree(d->st.keys);
+        d->st.keys = nullptr; d->kcap = 0;
+        DCK(cudaMalloc(&d->st.keys, (size_t)d->cap * sizeof(AmbPosRec)));
+        d->kcap = d->cap;
     }
     return AMB_OK;
 }
@@ -269,9 +259,9 @@ static int ensure_keys(amb_decoder* d)
 // the local stage's device memory, at the first decode with the option on (the table starts empty: all NaN)
 static int ensure_local(amb_decoder* d)
 {
-    if (!d->ltable) {
-        DCK(cudaMalloc(&d->ltable, AMB_LOCAL_SLOTS * sizeof(AmbRefPos)));
-        DCK(cudaMemsetAsync(d->ltable, 0xFF, AMB_LOCAL_SLOTS * sizeof(AmbRefPos), d->stream));
+    if (!d->st.ltable) {
+        DCK(cudaMalloc(&d->st.ltable, AMB_LOCAL_SLOTS * sizeof(AmbRefPos)));
+        DCK(cudaMemsetAsync(d->st.ltable, 0xFF, AMB_LOCAL_SLOTS * sizeof(AmbRefPos), d->stream));
     }
     return ensure_keys(d);
 }
@@ -279,10 +269,10 @@ static int ensure_local(amb_decoder* d)
 // the Comm-B stage's device memory, at the first decode with the option on (the table starts empty: all NaN)
 static int ensure_commb(amb_decoder* d)
 {
-    if (!d->ctable) {
-        cudaError_t e = cudaMalloc(&d->ctable, AMB_COMMB_SLOTS * sizeof(AmbCommbRef));
-        if (e != cudaSuccess) { d->ctable = nullptr; return dfail(d, AMB_ERR_CUDA, "Comm-B velocity table (384 MiB)", e); }
-        DCK(cudaMemsetAsync(d->ctable, 0xFF, AMB_COMMB_SLOTS * sizeof(AmbCommbRef), d->stream));
+    if (!d->st.ctable) {
+        cudaError_t e = cudaMalloc(&d->st.ctable, AMB_COMMB_SLOTS * sizeof(AmbCommbRef));
+        if (e != cudaSuccess) { d->st.ctable = nullptr; return dfail(d, AMB_ERR_CUDA, "Comm-B velocity table (384 MiB)", e); }
+        DCK(cudaMemsetAsync(d->st.ctable, 0xFF, AMB_COMMB_SLOTS * sizeof(AmbCommbRef), d->stream));
     }
     return ensure_keys(d);
 }
@@ -291,19 +281,19 @@ static int ensure_commb(amb_decoder* d)
 // starts empty), the clock starts at "nothing decoded"
 static int ensure_track(amb_decoder* d)
 {
-    if (!d->trows) {
-        cudaError_t e = cudaMalloc(&d->trows, (size_t)AMB_TRACK_ROWS * sizeof(amb_aircraft));
-        if (e != cudaSuccess) { d->trows = nullptr; return dfail(d, AMB_ERR_CUDA, "aircraft table (2 GiB)", e); }
+    if (!d->st.trows) {
+        cudaError_t e = cudaMalloc(&d->st.trows, (size_t)AMB_TRACK_ROWS * sizeof(amb_aircraft));
+        if (e != cudaSuccess) { d->st.trows = nullptr; return dfail(d, AMB_ERR_CUDA, "aircraft table (2 GiB)", e); }
     }
-    if (!d->tclk) {
+    if (!d->st.tclk) {
         static const AmbTrackClock none = {NAN, 0u, 0u};
-        DCK(cudaMalloc(&d->tclk, sizeof(AmbTrackClock)));
-        DCK(cudaMemcpyAsync(d->tclk, &none, sizeof none, cudaMemcpyHostToDevice, d->stream));
+        DCK(cudaMalloc(&d->st.tclk, sizeof(AmbTrackClock)));
+        DCK(cudaMemcpyAsync(d->st.tclk, &none, sizeof none, cudaMemcpyHostToDevice, d->stream));
     }
     if (!d->snap_cnt) DCK(cudaMalloc(&d->snap_cnt, (2 * AMB_TRACK_WORDS / AMB_SNAP_WORDS + 1) * sizeof(uint32_t)));
-    if (!d->tocc) {                      // last: snapshot_impl and reset take a bitmap as "everything is there"
-        DCK(cudaMalloc(&d->tocc, AMB_TRACK_WORDS * sizeof(unsigned)));
-        DCK(cudaMemsetAsync(d->tocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));
+    if (!d->st.tocc) {                   // last: snapshot_impl and reset take a bitmap as "everything is there"
+        DCK(cudaMalloc(&d->st.tocc, AMB_TRACK_WORDS * sizeof(unsigned)));
+        DCK(cudaMemsetAsync(d->st.tocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));
     }
     return ensure_keys(d);
 }
@@ -329,6 +319,9 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
     if (n == 0) return AMB_OK;
     DCK(cudaSetDevice(d->device));
     int rc = ensure_cap(d, n);
+    if (rc == AMB_OK && d->st.local_cpr > 0) rc = ensure_local(d);
+    if (rc == AMB_OK && d->st.commb > 0) rc = ensure_commb(d);
+    if (rc == AMB_OK && d->st.track > 0) rc = ensure_track(d);
     if (rc != AMB_OK) return rc;
     cudaStream_t s = d->stream;
     amb_fields* const fields = out_on_device ? out : d->d_fields;
@@ -339,38 +332,14 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
         if (rc != AMB_OK) return rc;
         src = d->d_frames;
     }
-    const int nb = (n + 127) / 128;
-    AMB_LAUNCH((amb_fields_kernel), nb, 128, 0, s, src, n, fields, d->d_pos, d->d_pair);
-    DCK(cudaGetLastError());
     cudaError_t e = cudaSuccess;
-    const int k = amb_v3_launch(&d->v3, d->d_pos, n, d->table, d->d_pair, s, &e);
-    if (k < 0) return dfail(d, AMB_ERR_CUDA, "pairing", e);
-    AMB_LAUNCH((amb_resolve_kernel), nb, 128, 0, s, fields, d->d_pos, d->d_pair, n, d->have_loc, d->lat, d->lon, d->nl_T);
-    DCK(cudaGetLastError());
-    d->launches += 2 + (uint64_t)k;
-    if (d->local_cpr > 0) {
-        rc = ensure_local(d);
-        if (rc != AMB_OK) return rc;
-        const int kl = amb_local_launch(&d->v3, d->d_pos, d->d_lpos, n, fields, d->ltable, d->local_cpr, d->have_loc, d->lat,
-                                        d->lon, d->nl_T, s, &e);
-        if (kl < 0) return dfail(d, AMB_ERR_CUDA, "local CPR", e);
-        d->launches += (uint64_t)kl;
+    const int k = amb_decode_launch(&d->st, src, n, fields, s, &e);
+    if (k < 0) {
+        static const char* const stage[] = {"cudaGetLastError()", "pairing", "cudaGetLastError()", "local CPR",
+                                            "Comm-B inference", "aircraft table"};   // by -AMB_STAGE_* - 1
+        return dfail(d, AMB_ERR_CUDA, stage[-k - 1], e);
     }
-    if (d->commb > 0) {
-        rc = ensure_commb(d);
-        if (rc != AMB_OK) return rc;
-        const int kc = amb_commb_launch(&d->v3, src, fields, d->d_pos, d->d_lpos, n, d->ctable, d->commb, s, &e);
-        if (kc < 0) return dfail(d, AMB_ERR_CUDA, "Comm-B inference", e);
-        d->launches += (uint64_t)kc;
-    }
-    if (d->track > 0) {
-        rc = ensure_track(d);
-        if (rc != AMB_OK) return rc;
-        const int kt = amb_track_launch(&d->v3, src, fields, d->d_pos, d->d_lpos, n, d->trows, d->tocc, d->tclk, d->track,
-                                        s, &e);
-        if (kt < 0) return dfail(d, AMB_ERR_CUDA, "aircraft table", e);
-        d->launches += (uint64_t)kt;
-    }
+    d->launches += (uint64_t)k;
     if (!out_on_device) {
         rc = staged_d2h(d, out, d->d_fields, (size_t)n * sizeof(amb_fields), s);
         if (rc != AMB_OK) return rc;
@@ -385,14 +354,15 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
 static int snapshot_impl(amb_decoder* d, double now, amb_aircraft* out, int max, bool out_on_device)
 {
     if (!d || max < 0) return dfail(d, AMB_ERR_INVALID, "amb_decoder_aircraft: bad argument");
-    if (d->track <= 0) return dfail(d, AMB_ERR_STATE, "amb_decoder_aircraft: option track is off");
-    if (!d->tocc) return 0;                              // nothing decoded with the option on yet
+    if (d->st.track <= 0) return dfail(d, AMB_ERR_STATE, "amb_decoder_aircraft: option track is off");
+    if (!d->st.tocc) return 0;                           // nothing decoded with the option on yet
     DCK(cudaSetDevice(d->device));
     cudaStream_t s = d->stream;
     const unsigned nb = AMB_TRACK_WORDS / AMB_SNAP_WORDS;
     uint32_t* off = d->snap_cnt + nb;
     cudaError_t e = cudaSuccess;
-    if (amb_snap_count_launch(d->tocc, d->trows, d->tclk, now, d->track, AMB_TRACK_WORDS, d->snap_cnt, off, s, &e) < 0)
+    if (amb_snap_count_launch(d->st.tocc, d->st.trows, d->st.tclk, now, d->st.track, AMB_TRACK_WORDS, d->snap_cnt, off,
+                              s, &e) < 0)
         return dfail(d, AMB_ERR_CUDA, "aircraft snapshot", e);
     d->launches += 2;
     uint32_t total = 0;
@@ -411,7 +381,7 @@ static int snapshot_impl(amb_decoder* d, double now, amb_aircraft* out, int max,
         }
         dst = d->d_snap;
     }
-    if (amb_snap_gather_launch(d->tocc, d->trows, d->tclk, now, d->track, AMB_TRACK_WORDS, off, dst, s, &e) < 0)
+    if (amb_snap_gather_launch(d->st.tocc, d->st.trows, d->st.tclk, now, d->st.track, AMB_TRACK_WORDS, off, dst, s, &e) < 0)
         return dfail(d, AMB_ERR_CUDA, "aircraft snapshot", e);
     d->launches += 1;
     if (!out_on_device) {

@@ -70,26 +70,34 @@ def local_outcome(records):
     return np.asarray(records["pad_"], dtype=np.uint64) & np.uint64(0xFF)
 
 
-def check_local_cpr(seconds) -> int:
-    """Validate a local_cpr setting: an int in 0 (off) .. LOCAL_CPR_MAX seconds. Raises ValueError otherwise."""
+# the decoder options (amb_decoder_set_option) and their maxima in seconds
+OPTION_MAX = {"local_cpr": LOCAL_CPR_MAX, "track": TRACK_MAX, "commb": COMMB_MAX}
+
+
+def check_option(name: str, seconds) -> int:
+    """Validate a setting of decoder option `name`: an int in 0 (off) .. OPTION_MAX[name] seconds. Raises ValueError
+    otherwise."""
+    top = OPTION_MAX[name]
     try:
-        ok = not isinstance(seconds, bool) and int(seconds) == seconds and 0 <= int(seconds) <= LOCAL_CPR_MAX
+        ok = not isinstance(seconds, bool) and int(seconds) == seconds and 0 <= int(seconds) <= top
     except (TypeError, ValueError):
         ok = False
     if not ok:
-        raise ValueError("local_cpr: an integer number of seconds in 0 (off) .. %d, got %r" % (LOCAL_CPR_MAX, seconds))
+        raise ValueError("%s: an integer number of seconds in 0 (off) .. %d, got %r" % (name, top, seconds))
     return int(seconds)
+
+
+# check_option bound to one option, under the names the module has always exported
+def check_local_cpr(seconds) -> int:
+    return check_option("local_cpr", seconds)
 
 
 def check_commb(seconds) -> int:
-    """Validate a commb setting: an int in 0 (off) .. COMMB_MAX seconds. Raises ValueError otherwise."""
-    try:
-        ok = not isinstance(seconds, bool) and int(seconds) == seconds and 0 <= int(seconds) <= COMMB_MAX
-    except (TypeError, ValueError):
-        ok = False
-    if not ok:
-        raise ValueError("commb: an integer number of seconds in 0 (off) .. %d, got %r" % (COMMB_MAX, seconds))
-    return int(seconds)
+    return check_option("commb", seconds)
+
+
+def check_track(seconds) -> int:
+    return check_option("track", seconds)
 
 
 def commb_outcome(records):
@@ -128,17 +136,6 @@ def commb_values(record):
     return out
 
 
-def check_track(seconds) -> int:
-    """Validate a track setting: an int in 0 (off) .. TRACK_MAX seconds. Raises ValueError otherwise."""
-    try:
-        ok = not isinstance(seconds, bool) and int(seconds) == seconds and 0 <= int(seconds) <= TRACK_MAX
-    except (TypeError, ValueError):
-        ok = False
-    if not ok:
-        raise ValueError("track: an integer number of seconds in 0 (off) .. %d, got %r" % (TRACK_MAX, seconds))
-    return int(seconds)
-
-
 # aircraft_to_dict: a column and the flag that says it is set
 _AC_COLUMNS = (("altitude", AC_HAS_ALT), ("squawk", AC_HAS_SQUAWK), ("ident", AC_HAS_IDENT), ("ftc", AC_HAS_IDENT),
                ("cat", AC_HAS_IDENT), ("lat", AC_HAS_POS), ("lon", AC_HAS_POS), ("pos_t", AC_HAS_POS),
@@ -175,9 +172,8 @@ class batch_decoder:
     commb_outcome() / commb_values() (DESIGN.md §8 "Comm-B inference")."""
 
     def __init__(self, my_location=None, device: int = 0, local_cpr: int = 0, track: int = 0, commb: int = 0):
-        local_cpr = check_local_cpr(local_cpr)
-        commb = check_commb(commb)
-        track = check_track(track)
+        settings = {"local_cpr": check_option("local_cpr", local_cpr), "track": check_option("track", track),
+                    "commb": check_option("commb", commb)}
         self._lib = _lib.load()
         h = C.c_void_p()
         have, lat, lon = self._loc(my_location)
@@ -188,15 +184,10 @@ class batch_decoder:
         self._h = h
         self._device = int(device)
         self.my_location = my_location
-        self._local_cpr = 0
-        if local_cpr:
-            self.set_local_cpr(local_cpr)
-        self._track = 0
-        if track:
-            self.set_track(track)
-        self._commb = 0
-        if commb:
-            self.set_commb(commb)
+        self._options = dict.fromkeys(OPTION_MAX, 0)
+        for name, seconds in settings.items():
+            if seconds:
+                self._set_option(name, seconds)
 
     @staticmethod
     def _loc(loc):
@@ -217,32 +208,31 @@ class batch_decoder:
         """Forget every stored report, reference position, velocity and aircraft; the option settings stay."""
         self._check(self._lib.amb_decoder_reset(self._h))
 
+    def _set_option(self, name, seconds):
+        seconds = check_option(name, seconds)
+        self._check(self._lib.amb_decoder_set_option(self._h, name.encode(), seconds))
+        self._options[name] = seconds
+
     def set_local_cpr(self, seconds: int):
         """Option local_cpr = S seconds (0 = off); applies from the next decode."""
-        seconds = check_local_cpr(seconds)
-        self._check(self._lib.amb_decoder_set_option(self._h, b"local_cpr", seconds))
-        self._local_cpr = seconds
+        self._set_option("local_cpr", seconds)
 
     def get_local_cpr(self) -> int:
-        return self._local_cpr
+        return self._options["local_cpr"]
 
     def set_track(self, seconds: int):
         """Option track = S seconds (0 = off); applies from the next decode."""
-        seconds = check_track(seconds)
-        self._check(self._lib.amb_decoder_set_option(self._h, b"track", seconds))
-        self._track = seconds
+        self._set_option("track", seconds)
 
     def get_track(self) -> int:
-        return self._track
+        return self._options["track"]
 
     def set_commb(self, seconds: int):
         """Option commb = S seconds (0 = off); applies from the next decode."""
-        seconds = check_commb(seconds)
-        self._check(self._lib.amb_decoder_set_option(self._h, b"commb", seconds))
-        self._commb = seconds
+        self._set_option("commb", seconds)
 
     def get_commb(self) -> int:
-        return self._commb
+        return self._options["commb"]
 
     @staticmethod
     def _now(now):

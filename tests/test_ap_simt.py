@@ -2,7 +2,6 @@
 the same recipe as tests/test_ec_simt.py): the fused chain on small fleet scenes, against the oracle plus the checkers
 of tests/ec_oracle.py, tests/ec_any_oracle.py and tests/ap_oracle.py."""
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -11,8 +10,8 @@ import pytest
 import gr_air_modes_b200 as am
 from gr_air_modes_b200 import _lib, synth
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import emul_build  # noqa: E402
 import ap_cases as apc  # noqa: E402
 import ap_oracle as apo  # noqa: E402
 import ec_cases as ecc  # noqa: E402
@@ -20,9 +19,7 @@ import ec_cases as ecc  # noqa: E402
 
 @pytest.fixture(scope="module", autouse=True)
 def emulated_library(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("libsimt_ap") / "libairmodes_b200_emulated.so")
-    subprocess.run(["g++", "-std=c++17", "-O1", "-U_FORTIFY_SOURCE", "-ffp-contract=off", "-Wno-unknown-pragmas", "-Wno-psabi", "-shared", "-fPIC",
-                    "-o", out, os.path.join(ROOT, "tests", "simt", "library_emul.cc")], check=True)
+    out = emul_build.build(tmp_path_factory, emul_build.LIBRARY_EMUL)
     saved = (_lib.LIB_PATH, _lib._lib)
     _lib.LIB_PATH, _lib._lib = out, None
     try:

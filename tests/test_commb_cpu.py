@@ -5,7 +5,6 @@ FIELDS_DTYPE (compiled on the host), commb_values, the report line and the CLI's
 import ctypes as C
 import os
 import re
-import subprocess
 import sys
 
 import numpy as np
@@ -16,10 +15,11 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 import commb_cases as cc  # noqa: E402
 import commb_oracle as co  # noqa: E402
+import emul_build  # noqa: E402
 import track_cases as tc  # noqa: E402
 
 CORE_SHIM = r"""
-#include "amb_decode_core.h"
+#include "%s"
 extern "C" int shim_agree(int gs, int trk, double speed, double track) { return amb_commb_agree(gs, trk, speed, track); }
 extern "C" unsigned shim_candidates(uint64_t mb) { return amb_commb_candidates(mb); }
 extern "C" void shim_layout(size_t* out)
@@ -42,13 +42,9 @@ extern "C" void shim_write(amb_fields* r, uint64_t mb, unsigned cand, int outcom
 
 @pytest.fixture(scope="module")
 def core(tmp_path_factory):
-    d = tmp_path_factory.mktemp("commb_core")
-    src = d / "shim.cc"
-    src.write_text(CORE_SHIM)
-    lib = str(d / "libshim.so")
-    subprocess.run(["g++", "-std=c++17", "-O1", "-ffp-contract=off", "-shared", "-fPIC",
-                    "-I" + os.path.join(ROOT, "gr_air_modes_b200", "csrc"), "-o", lib, str(src)], check=True)
-    s = C.CDLL(lib)
+    src = tmp_path_factory.mktemp("commb_core") / "shim.cc"
+    src.write_text(CORE_SHIM % os.path.join(ROOT, "gr_air_modes_b200", "csrc", "amb_decode_core.h"))
+    s = C.CDLL(emul_build.build(tmp_path_factory, src))
     s.shim_agree.argtypes = [C.c_int, C.c_int, C.c_double, C.c_double]
     s.shim_candidates.argtypes = [C.c_uint64]
     s.shim_candidates.restype = C.c_uint
@@ -157,10 +153,7 @@ def test_report_line():
 @pytest.fixture(scope="module")
 def emulated(tmp_path_factory):
     from gr_air_modes_b200 import _lib
-    out = str(tmp_path_factory.mktemp("libsimt_commb") / "libairmodes_b200_emulated.so")
-    subprocess.run(["g++", "-std=c++17", "-O1", "-U_FORTIFY_SOURCE", "-ffp-contract=off", "-Wno-unknown-pragmas",
-                    "-Wno-psabi", "-shared", "-fPIC", "-o", out, os.path.join(ROOT, "tests", "simt", "library_emul.cc")],
-                   check=True)
+    out = emul_build.build(tmp_path_factory, emul_build.LIBRARY_EMUL)
     saved = (_lib.LIB_PATH, _lib._lib)
     _lib.LIB_PATH, _lib._lib = out, None
     try:

@@ -60,12 +60,8 @@ def test_decode_oracle_matches_live_reference_on_fresh_seeds(ref_py):
 @pytest.fixture(scope="module")
 def shim(tmp_path_factory):
     import ctypes as C
-    import subprocess
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    out = str(tmp_path_factory.mktemp("shim") / "libdecode_shim.so")
-    subprocess.run(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", out,
-                    os.path.join(root, "tests", "decode_host_shim.cc")], check=True)
-    lib = C.CDLL(out)
+    import emul_build
+    lib = C.CDLL(emul_build.build(tmp_path_factory, os.path.join(emul_build.ROOT, "tests", "decode_host_shim.cc")))
     lib.shim_decode.restype = C.c_int
     lib.shim_decode.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_void_p]
     lib.shim_nl.restype = C.c_int

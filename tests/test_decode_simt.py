@@ -1,36 +1,27 @@
 """The decoder's KERNEL SOURCE (gr_air_modes_b200/csrc/amb_decode_kernels.cuh and amb_decode_v3.cuh: fields kernel, the
-five pairing kernels launched by their own launcher, resolve kernel) executed on the host by a small SIMT emulator
-(tests/simt/simt_emul.h: cooperative fibers, real barrier semantics for __syncthreads / __syncwarp / shuffles / votes /
-match) and compared with the sequential host replay of the same arithmetic and with the oracle. A CPU-side check of the
-warp-level logic - match/ballot ordering inside a 32-frame step, table hand-over between steps and batches, the stable
-partition of the reports by owner bucket - for hardware-independent bugs; the GPU tests remain the parity gate."""
+five pairing kernels, resolve kernel, enqueued by the decoder's own amb_decode_launch with every option off) executed on
+the host by a small SIMT emulator (tests/simt/simt_emul.h: cooperative fibers, real barrier semantics for
+__syncthreads / __syncwarp / shuffles / votes / match) and compared with the sequential host replay of the same
+arithmetic and with the oracle. A CPU-side check of the warp-level logic - match/ballot ordering inside a 32-frame
+step, table hand-over between steps and batches, the stable partition of the reports by owner bucket - for
+hardware-independent bugs; the GPU tests remain the parity gate."""
 import ctypes as C
 import os
-import subprocess
 import sys
 
 import numpy as np
 import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import emul_build  # noqa: E402
 
 
 @pytest.fixture(scope="module")
 def libs(tmp_path_factory):
-    d = tmp_path_factory.mktemp("simt")
-    emul, shim = str(d / "libdecode_emul.so"), str(d / "libdecode_shim.so")
-    flags = ["g++", "-std=c++17", "-O1", "-U_FORTIFY_SOURCE", "-ffp-contract=off", "-Wno-unknown-pragmas", "-shared", "-fPIC"]
-    subprocess.run(flags + ["-o", emul, os.path.join(ROOT, "tests", "simt", "decode_emul.cc")], check=True)
-    subprocess.run(flags + ["-o", shim, os.path.join(ROOT, "tests", "decode_host_shim.cc")], check=True)
-    e, s = C.CDLL(emul), C.CDLL(shim)
-    e.emul_new.restype = C.c_void_p
-    e.emul_new.argtypes = [C.c_int]
-    e.emul_free.argtypes = [C.c_void_p]
-    e.emul_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_void_p]
+    s = C.CDLL(emul_build.build(tmp_path_factory, os.path.join(emul_build.ROOT, "tests", "decode_host_shim.cc")))
     s.shim_new.restype = C.c_void_p
     s.shim_step.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_void_p]
-    return e, s
+    return emul_build.decode_emul(tmp_path_factory), s
 
 
 def _traffic(n, seed, n_aircraft):
@@ -73,7 +64,7 @@ def _run(e, s, arr, n, splits, loc):
         if c <= 0:
             break
         fr = C.c_void_p(base + 80 * pos)
-        assert e.emul_decode(he, fr, c, have, lat, lon, C.c_void_p(got.ctypes.data + 144 * pos)) == 0
+        assert e.emul_decode(he, fr, c, have, lat, lon, 0, 0, 0, C.c_void_p(got.ctypes.data + 144 * pos)) == 0
         s.shim_step(hs, fr, c, have, lat, lon, C.c_void_p(want.ctypes.data + 144 * pos))
         pos += c
     e.emul_free(he)

@@ -2,7 +2,6 @@
 (tests/simt/library_emul.cc, the same recipe as tests/test_ec_simt.py): the split-form slicer on constructed packets and
 the fused chain on a small IQ scene, against the oracle plus the brute-force checkers."""
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -11,8 +10,8 @@ import pytest
 import gr_air_modes_b200 as am
 from gr_air_modes_b200 import _lib
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import emul_build  # noqa: E402
 import ec_any_cases as eac  # noqa: E402
 import ec_any_oracle as ea  # noqa: E402
 import ec_cases as ecc  # noqa: E402
@@ -21,9 +20,7 @@ import ec_oracle as eo  # noqa: E402
 
 @pytest.fixture(scope="module", autouse=True)
 def emulated_library(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("libsimt_ec_any") / "libairmodes_b200_emulated.so")
-    subprocess.run(["g++", "-std=c++17", "-O1", "-U_FORTIFY_SOURCE", "-ffp-contract=off", "-Wno-unknown-pragmas", "-Wno-psabi", "-shared", "-fPIC",
-                    "-o", out, os.path.join(ROOT, "tests", "simt", "library_emul.cc")], check=True)
+    out = emul_build.build(tmp_path_factory, emul_build.LIBRARY_EMUL)
     saved = (_lib.LIB_PATH, _lib._lib)
     _lib.LIB_PATH, _lib._lib = out, None
     try:

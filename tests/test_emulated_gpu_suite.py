@@ -14,16 +14,16 @@ import os
 import subprocess
 import sys
 
+import emul_build
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EXCLUDE = ("full_size or config0 or c_abi_example or cli_ or randomised_stress or time_sharded_speculative or "
            "host_ingest_paths or sc16_input or torch_input or device_resident_decode or device_side_drain or "
            "without_leaving_the_device")   # the last six need pinned / CUDA tensors; test_library_simt.py has their emulated twins
 
 
-def test_gpu_parity_tests_pass_against_the_emulated_library(tmp_path):
-    lib = str(tmp_path / "libairmodes_b200_emulated.so")
-    subprocess.run(["g++", "-std=c++17", "-O1", "-U_FORTIFY_SOURCE", "-ffp-contract=off", "-Wno-unknown-pragmas", "-Wno-psabi",
-                    "-shared", "-fPIC", "-o", lib, os.path.join(ROOT, "tests", "simt", "library_emul.cc")], check=True)
+def test_gpu_parity_tests_pass_against_the_emulated_library(tmp_path_factory):
+    lib = emul_build.build(tmp_path_factory, emul_build.LIBRARY_EMUL)
     env = dict(os.environ, AMB_TEST_EMULATED_LIB=lib)
     workers = str(max(1, min(6, (os.cpu_count() or 2) - 1)))
     cmd = [sys.executable, "-m", "pytest", os.path.join(ROOT, "tests", "test_gpu_parity.py"),

@@ -5,7 +5,6 @@ tests make through amb_preamble_process / amb_slicer_process / amb_device_crc, h
 hardware-independent bugs in the warp-level logic and in the launch configuration; the GPU tests remain the gate."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -13,15 +12,14 @@ import pytest
 from gr_air_modes_b200 import synth
 from oracle import cpu_oracle as co
 
+import emul_build
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
 def emul(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("ksimt") / "libkernels_emul.so")
-    subprocess.run(["g++", "-std=c++17", "-O1", "-U_FORTIFY_SOURCE", "-ffp-contract=off", "-Wno-unknown-pragmas", "-Wno-psabi", "-shared", "-fPIC",
-                    "-o", out, os.path.join(ROOT, "tests", "simt", "kernels_emul.cc")], check=True)
-    lib = C.CDLL(out)
+    lib = C.CDLL(emul_build.build(tmp_path_factory, os.path.join(ROOT, "tests", "simt", "kernels_emul.cc")))
     lib.emul_preamble.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_float, C.c_int, C.c_int, C.c_void_p,
                                   C.c_void_p, C.c_int, C.c_void_p]
     lib.emul_process_iq.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_int, C.c_int, C.c_int,

@@ -10,7 +10,6 @@ package itself only ever binds gr_air_modes_b200/libairmodes_b200.so and has no 
 It is not thread-safe (one emulated device, global fiber state): everything here is sequential.
 """
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -22,14 +21,13 @@ from oracle import cpu_oracle as co
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import emul_build  # noqa: E402
 from ref_golden import same_chips  # noqa: E402
 
 
 @pytest.fixture(scope="module", autouse=True)
 def emulated_library(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("libsimt") / "libairmodes_b200_emulated.so")
-    subprocess.run(["g++", "-std=c++17", "-O1", "-U_FORTIFY_SOURCE", "-ffp-contract=off", "-Wno-unknown-pragmas", "-Wno-psabi", "-shared", "-fPIC",
-                    "-o", out, os.path.join(ROOT, "tests", "simt", "library_emul.cc")], check=True)
+    out = emul_build.build(tmp_path_factory, emul_build.LIBRARY_EMUL)
     saved = (_lib.LIB_PATH, _lib._lib)
     _lib.LIB_PATH, _lib._lib = out, None
     try:

@@ -7,7 +7,6 @@ import gzip
 import json
 import os
 import re
-import subprocess
 import sys
 
 import pytest
@@ -17,6 +16,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "local_cpr_golden.json.gz")
 REF = os.path.join(os.environ.get("AMB_REFERENCE_TREE", "/root/reference"), "python")
 
+import emul_build  # noqa: E402
 import local_cpr_oracle as lo  # noqa: E402
 
 
@@ -27,10 +27,7 @@ def _golden():
 
 @pytest.fixture(scope="module")
 def shim(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("shim_local") / "libdecode_shim.so")
-    subprocess.run(["g++", "-std=c++17", "-O1", "-ffp-contract=off", "-shared", "-fPIC", "-o", out,
-                    os.path.join(ROOT, "tests", "local_cpr_host_shim.cc")], check=True)
-    s = C.CDLL(out)
+    s = C.CDLL(emul_build.build(tmp_path_factory, os.path.join(ROOT, "tests", "local_cpr_host_shim.cc")))
     s.shim_cpr_local.argtypes = [C.c_double, C.c_double, C.c_uint32, C.c_uint32, C.c_int, C.c_int, C.POINTER(C.c_double)]
     s.shim_sizeof_fields.restype = C.c_int
     return s

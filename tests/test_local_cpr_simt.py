@@ -1,5 +1,5 @@
-"""The local CPR stage's KERNEL SOURCE (gr_air_modes_b200/csrc/amb_decode_local.cuh, launched by its own launcher after
-the fields, pairing and resolve kernels) on the host under the SIMT emulator (tests/simt/simt_emul.h), against the
+"""The local CPR stage's KERNEL SOURCE (gr_air_modes_b200/csrc/amb_decode_local.cuh, enqueued by the decoder's own
+amb_decode_launch after the fields, pairing and resolve kernels) on the host under the SIMT emulator (tests/simt/simt_emul.h), against the
 sequential replay of the same arithmetic (tests/local_cpr_host_shim.cc) byte for byte and against the brute-force checker
 (tests/local_cpr_oracle.py) record for record: decode_cases scenes in several batch splits (single messages, cuts at
 31/32/33 inside a 32-message step), a bucket holding many aircraft, and one aircraft with far more than 32 consecutive
@@ -7,39 +7,25 @@ local fixes. A copy of the kernel whose lanes read the table instead of their pr
 import ctypes as C
 import os
 import shutil
-import subprocess
 import sys
 
 import numpy as np
 import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-FLAGS = ["g++", "-std=c++17", "-O1", "-U_FORTIFY_SOURCE", "-ffp-contract=off", "-Wno-unknown-pragmas", "-shared", "-fPIC"]
-
+import emul_build  # noqa: E402
 import local_cpr_cases as lc  # noqa: E402
 import local_cpr_oracle as lo  # noqa: E402
 
-
-def _bind_emul(path):
-    e = C.CDLL(path)
-    e.emul_local_new.restype = C.c_void_p
-    e.emul_local_new.argtypes = [C.c_int]
-    e.emul_local_free.argtypes = [C.c_void_p]
-    e.emul_decode_local.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_void_p]
-    return e
+ROOT = emul_build.ROOT
 
 
 @pytest.fixture(scope="module")
 def libs(tmp_path_factory):
-    d = tmp_path_factory.mktemp("simt_local")
-    emul, shim = str(d / "libdecode_emul.so"), str(d / "libdecode_shim.so")
-    subprocess.run(FLAGS + ["-o", emul, os.path.join(ROOT, "tests", "simt", "decode_local_emul.cc")], check=True)
-    subprocess.run(FLAGS + ["-o", shim, os.path.join(ROOT, "tests", "local_cpr_host_shim.cc")], check=True)
-    s = C.CDLL(shim)
+    s = C.CDLL(emul_build.build(tmp_path_factory, os.path.join(ROOT, "tests", "local_cpr_host_shim.cc")))
     s.shim_local_new.restype = C.c_void_p
     s.shim_local_step.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_void_p]
-    return _bind_emul(emul), s
+    return emul_build.decode_emul(tmp_path_factory), s
 
 
 def _run(e, s, msgs, loc, S, splits):
@@ -47,7 +33,7 @@ def _run(e, s, msgs, loc, S, splits):
     from gr_air_modes_b200 import decode
     arr, n = decode.frames_from_messages(msgs)
     have, lat, lon = (0, 0.0, 0.0) if loc is None else (1, loc[0], loc[1])
-    he = e.emul_local_new(17)
+    he = e.emul_new(17)
     hs = s.shim_local_new() if s is not None else None
     got = np.zeros(n, dtype=decode.FIELDS_DTYPE)
     want = np.zeros(n, dtype=decode.FIELDS_DTYPE)
@@ -57,11 +43,11 @@ def _run(e, s, msgs, loc, S, splits):
         if c <= 0:
             break
         fr = C.c_void_p(base + 80 * pos)
-        assert e.emul_decode_local(he, fr, c, have, lat, lon, S, C.c_void_p(got.ctypes.data + 144 * pos)) == 0
+        assert e.emul_decode(he, fr, c, have, lat, lon, S, 0, 0, C.c_void_p(got.ctypes.data + 144 * pos)) == 0
         if hs is not None:
             s.shim_local_step(hs, fr, c, have, lat, lon, S, C.c_void_p(want.ctypes.data + 144 * pos))
         pos += c
-    e.emul_local_free(he)
+    e.emul_free(he)
     return got, want
 
 
@@ -132,7 +118,7 @@ def test_one_aircraft_with_a_long_local_chain(libs):
     assert best > 64
 
 
-def test_a_chain_that_reads_the_table_instead_of_its_predecessor_is_caught(libs, tmp_path):
+def test_a_chain_that_reads_the_table_instead_of_its_predecessor_is_caught(tmp_path, tmp_path_factory):
     """Mutation: every lane takes its reference from the table, none from the previous member of its group."""
     for sub in ("gr_air_modes_b200/csrc", "include", "tests/simt"):
         shutil.copytree(os.path.join(ROOT, sub), str(tmp_path / sub))
@@ -141,9 +127,7 @@ def test_a_chain_that_reads_the_table_instead_of_its_predecessor_is_caught(libs,
     a, b = "if (mine && rank == 0) {", "if (mine && (rank == 0 || (fields[k].status & AMB_FS_HAS_POS))) {"
     assert src.count(a) == 1 and src.count(b) == 1
     p.write_text(src.replace(a, "if (mine) {").replace(b, "if (mine) {"))
-    lib = str(tmp_path / "libbroken.so")
-    subprocess.run(FLAGS + ["-o", lib, str(tmp_path / "tests/simt/decode_local_emul.cc")], check=True)
-    e = _bind_emul(lib)
+    e = emul_build.decode_emul(tmp_path_factory, tmp_path / "tests/simt/decode_emul.cc")
     msgs = lc.chain_scene(n_local=100)
     got, _ = _run(e, None, msgs, None, 5, [])
     with pytest.raises(AssertionError):

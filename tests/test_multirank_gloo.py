@@ -259,12 +259,9 @@ def _emul_worker(rank, world, port_no, lib_path, ret):
     dist.destroy_process_group()
 
 
-def test_both_multi_gpu_modes_world2_with_the_emulated_library(tmp_path):
-    import subprocess
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    lib = str(tmp_path / "libairmodes_b200_emulated.so")
-    subprocess.run(["g++", "-std=c++17", "-O1", "-U_FORTIFY_SOURCE", "-ffp-contract=off", "-Wno-unknown-pragmas", "-Wno-psabi",
-                    "-shared", "-fPIC", "-o", lib, os.path.join(root, "tests", "simt", "library_emul.cc")], check=True)
+def test_both_multi_gpu_modes_world2_with_the_emulated_library(tmp_path_factory):
+    import emul_build
+    lib = emul_build.build(tmp_path_factory, emul_build.LIBRARY_EMUL)
     mgr = mp.Manager()
     ret = mgr.dict()
     mp.spawn(_emul_worker, args=(2, _free_port(), lib, ret), nprocs=2, join=True)

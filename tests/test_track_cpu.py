@@ -16,6 +16,7 @@ import pytest
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
+import emul_build  # noqa: E402
 import track_cases as tc  # noqa: E402
 import track_oracle as to  # noqa: E402
 
@@ -87,10 +88,7 @@ def test_aircraft_to_dict():
 @pytest.fixture(scope="module")
 def emulated(tmp_path_factory):
     from gr_air_modes_b200 import _lib
-    out = str(tmp_path_factory.mktemp("libsimt_track") / "libairmodes_b200_emulated.so")
-    subprocess.run(["g++", "-std=c++17", "-O1", "-U_FORTIFY_SOURCE", "-ffp-contract=off", "-Wno-unknown-pragmas",
-                    "-Wno-psabi", "-shared", "-fPIC", "-o", out, os.path.join(ROOT, "tests", "simt", "library_emul.cc")],
-                   check=True)
+    out = emul_build.build(tmp_path_factory, emul_build.LIBRARY_EMUL)
     saved = (_lib.LIB_PATH, _lib._lib)
     _lib.LIB_PATH, _lib._lib = out, None
     try:

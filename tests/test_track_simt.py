@@ -1,71 +1,54 @@
-"""The aircraft table's KERNEL SOURCE (gr_air_modes_b200/csrc/amb_decode_track.cuh, launched by its own launchers after the
-fields, pairing, resolve and local CPR kernels) on the host under the SIMT emulator (tests/simt/simt_emul.h), against
-the sequential checker (tests/track_oracle.py) fed with the same records: after every batch and at the end, in several
-batch splits (single messages, cuts at 31/32/33 inside a 32-record step, random sizes), for aircraft that fall silent
-and come back, a bucket of 32 aircraft and one address with far more than 32 records in a row. A copy of the walk that
-skips the expiry test must fail."""
+"""The aircraft table's KERNEL SOURCE (gr_air_modes_b200/csrc/amb_decode_track.cuh, enqueued by the decoder's own
+amb_decode_launch after the fields, pairing, resolve, local CPR and Comm-B kernels, and read out by its snapshot
+launchers) on the host under the SIMT emulator (tests/simt/simt_emul.h), against the sequential checker
+(tests/track_oracle.py) fed with the same records: after every batch and at the end, in several batch splits (single
+messages, cuts at 31/32/33 inside a 32-record step, random sizes), for aircraft that fall silent and come back, a bucket
+of 32 aircraft and one address with far more than 32 records in a row. A copy of the walk that skips the expiry test
+must fail."""
 import ctypes as C
 import math
 import os
 import shutil
-import subprocess
 import sys
 
 import numpy as np
 import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-FLAGS = ["g++", "-std=c++17", "-O1", "-U_FORTIFY_SOURCE", "-ffp-contract=off", "-Wno-unknown-pragmas", "-shared", "-fPIC"]
 WORDS = 1024                    # bitmap words the snapshot scans: addresses below 2^15, like the emulated tables
 
+import emul_build  # noqa: E402
 import local_cpr_cases as lc  # noqa: E402
 import track_cases as tc  # noqa: E402
 import track_oracle as to  # noqa: E402
 
-
-def _bind(path):
-    e = C.CDLL(path)
-    e.emul_track_new.restype = C.c_void_p
-    e.emul_track_new.argtypes = [C.c_int]
-    e.emul_track_free.argtypes = [C.c_void_p]
-    e.emul_track_reset.argtypes = [C.c_void_p]
-    e.emul_decode_track.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_int,
-                                    C.c_void_p]
-    e.emul_track_snapshot.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_uint, C.c_void_p, C.c_int]
-    return e
-
-
-def _build(src, out):
-    subprocess.run(FLAGS + ["-o", out, src], check=True)
-    return _bind(out)
+ROOT = emul_build.ROOT
 
 
 @pytest.fixture(scope="module")
 def emul(tmp_path_factory):
-    d = tmp_path_factory.mktemp("simt_track")
-    return _build(os.path.join(ROOT, "tests", "simt", "decode_track_emul.cc"), str(d / "libdecode_track_emul.so"))
+    return emul_build.decode_emul(tmp_path_factory)
 
 
 def _snapshot(e, h, now, S):
     from gr_air_modes_b200 import decode
-    n = e.emul_track_snapshot(h, math.nan if now is None else now, S, WORDS, None, 0)
+    n = e.emul_snapshot(h, math.nan if now is None else now, S, WORDS, None, 0)
     assert n >= 0
     out = np.zeros(n, dtype=decode.AIRCRAFT_DTYPE)
     if n:
-        assert e.emul_track_snapshot(h, math.nan if now is None else now, S, WORDS, C.c_void_p(out.ctypes.data), n - 1) == -5
-        assert e.emul_track_snapshot(h, math.nan if now is None else now, S, WORDS, C.c_void_p(out.ctypes.data), n) == n
+        assert e.emul_snapshot(h, math.nan if now is None else now, S, WORDS, C.c_void_p(out.ctypes.data), n - 1) == -5
+        assert e.emul_snapshot(h, math.nan if now is None else now, S, WORDS, C.c_void_p(out.ctypes.data), n) == n
     return out
 
 
-def _run(e, msgs, loc, S, splits, local_S=0, each=False):
+def _run(e, msgs, loc, S, splits, local_S=0, each=False, commb_S=0):
     """Decode in batches cut at `splits` with the table on; compare with the checker after every batch (each=True) and
     at the end (now = the latest record, the middle of the stream, and just past the end). Returns the final snapshot."""
     from gr_air_modes_b200 import decode
     frames = tc.frames_of(msgs)
     n = len(frames)
     have, lat, lon = (0, 0.0, 0.0) if loc is None else (1, loc[0], loc[1])
-    h = e.emul_track_new(17)
+    h = e.emul_new(17)
     assert h
     tr = to.Tracker(S)
     recs = np.zeros(n, dtype=decode.FIELDS_DTYPE)
@@ -74,8 +57,8 @@ def _run(e, msgs, loc, S, splits, local_S=0, each=False):
         c = min(c, n - pos)
         if c <= 0:
             break
-        assert e.emul_decode_track(h, C.c_void_p(frames.ctypes.data + 80 * pos), c, have, lat, lon, local_S, S,
-                                   C.c_void_p(recs.ctypes.data + 144 * pos)) == 0
+        assert e.emul_decode(h, C.c_void_p(frames.ctypes.data + 80 * pos), c, have, lat, lon, local_S, commb_S, S,
+                             C.c_void_p(recs.ctypes.data + 144 * pos)) == 0
         tr.feed(frames[pos:pos + c], recs[pos:pos + c])
         if each:
             to.assert_rows_equal(_snapshot(e, h, None, S), tr.snapshot_array(), ("batch at", pos))
@@ -85,23 +68,24 @@ def _run(e, msgs, loc, S, splits, local_S=0, each=False):
     to.assert_rows_equal(final, tr.snapshot_array(), "end")
     for now in (ts[n // 2], ts[-1] + S / 2):
         to.assert_rows_equal(_snapshot(e, h, now, S), tr.snapshot_array(now), ("now", now))
-    e.emul_track_reset(h)
-    assert e.emul_track_snapshot(h, math.nan, S, WORDS, None, 0) == 0
-    assert e.emul_track_snapshot(h, ts[-1], S, WORDS, None, 0) == 0
-    e.emul_track_free(h)
+    e.emul_reset(h)
+    assert e.emul_snapshot(h, math.nan, S, WORDS, None, 0) == 0
+    assert e.emul_snapshot(h, ts[-1], S, WORDS, None, 0) == 0
+    e.emul_free(h)
     return final, recs
 
 
 SPLITS = ([], [1] * 40 + [31, 32, 33, 31, 65])
 
 
-@pytest.mark.parametrize("seed", [1, 2])
-def test_life_scene_in_batch_splits(emul, seed):
+@pytest.mark.parametrize("seed,commb_S", [(1, 0), (2, 0), (1, 30), (2, 30)], ids=["1", "2", "1+commb", "2+commb"])
+def test_life_scene_in_batch_splits(emul, seed, commb_S):
+    """Alone, and with the Comm-B stage also on (+commb), as amb_decode_frames runs them."""
     msgs = tc.life_scene(seed=seed)
     loc = [51.5, -0.2] if seed == 1 else None
     finals = []
     for splits in SPLITS:
-        final, _ = _run(emul, msgs, loc, 20, splits, each=bool(splits))
+        final, _ = _run(emul, msgs, loc, 20, splits, each=bool(splits), commb_S=commb_S)
         finals.append(final)
     to.assert_rows_equal(finals[0], finals[1], "splits")
     assert len(finals[0]) >= 4
@@ -145,7 +129,7 @@ def test_one_address_with_long_runs_in_a_step(emul):
         _run(emul, msgs, None, 3, splits, each=True)
 
 
-def test_a_walk_without_the_expiry_test_is_caught(tmp_path):
+def test_a_walk_without_the_expiry_test_is_caught(tmp_path, tmp_path_factory):
     """Mutation: a row never expires, so a record after a silence keeps the old row instead of starting a new one (or
     of being ignored)."""
     for sub in ("gr_air_modes_b200/csrc", "include", "tests/simt"):
@@ -155,6 +139,6 @@ def test_a_walk_without_the_expiry_test_is_caught(tmp_path):
     a = "const bool alive = live && !(t - seen > (double)max_age);"
     assert src.count(a) == 1
     p.write_text(src.replace(a, "const bool alive = live;"))
-    e = _build(str(tmp_path / "tests/simt/decode_track_emul.cc"), str(tmp_path / "libbroken.so"))
+    e = emul_build.decode_emul(tmp_path_factory, tmp_path / "tests/simt/decode_emul.cc")
     with pytest.raises(AssertionError):
         _run(e, tc.burst_scene(), None, 3, [])
