@@ -227,7 +227,9 @@ AMB_HD void amb_decode_fields(const amb_frame& f, amb_fields* r, AmbPosRec* pos)
                 double tr = (double)((int)amb_bits(m, 35, 6) * 15) / 62;
                 if (amb_bits(m, 34, 1)) tr = 0 - tr;
                 int ns = (int)amb_bits(m, 23, 11) - 1, ew = (int)amb_bits(m, 11, 11) - 1;
-                const double vel = hypot((double)ns, (double)ew);
+                // hypot of integers: the root of the exact integer sum is correctly rounded (device hypot is not: one
+                // ulp off in about a quarter of the words, perfect squares included) - DESIGN.md §8
+                const double vel = sqrt((double)(ns * ns + ew * ew));
                 if (amb_bits(m, 10, 1)) ew = 0 - ew;
                 if (amb_bits(m, 22, 1)) ns = 0 - ns;
                 double hdg = atan2((double)ew, (double)ns) * (180.0 / M_PI);
@@ -241,7 +243,7 @@ AMB_HD void amb_decode_fields(const amb_frame& f, amb_fields* r, AmbPosRec* pos)
                 if (amb_bits(m, 37, 1)) vs = 0 - vs;
                 double ns = (double)(int)amb_bits(m, 26, 10), ew = (double)(int)amb_bits(m, 15, 10);
                 if (sub == 2) { ns *= 4; ew *= 4; }
-                const double vel = hypot(ns, ew);
+                const double vel = sqrt(ns * ns + ew * ew);                 // exact sum (< 2^25), as above
                 if (amb_bits(m, 14, 1)) ew = 0 - ew;
                 double hdg = (ns == 0) ? 0.0 : atan(ew / ns) * (180.0 / M_PI);
                 if (amb_bits(m, 25, 1)) hdg = 180 - hdg;

@@ -213,6 +213,73 @@ def burst_scene(seed=4):
     return _msgs(ev)
 
 
+# ---- the decision rules at their ties (tests/test_decode_fp_edges_*.py) -------------------------------------------------
+def pythagorean(max_c=478):
+    """(a, b, c) with a^2 + b^2 = c^2 and c even: every primitive triple doubled and scaled, (6,8,10)k, (10,24,26)k,
+    (16,30,34)k, ..., up to c = max_c (so that GS = (c + 22) / 2 stays at most 250 raw, 6,0's Mach limit on the same
+    bits: the word must stay a 6,0 candidate too)."""
+    out = set()
+    for m in range(2, 40):
+        for n in range(1, m):
+            if (m - n) % 2 == 1 and math.gcd(m, n) == 1:
+                a, b, c = m * m - n * n, 2 * m * n, m * m + n * n
+                for k in range(2, max_c // c + 1, 2):
+                    out.add((a * k, b * k, c * k))
+    return sorted(out)
+
+
+def velocity_word(sub, ns, ew):
+    """DF17 BDS0,9 subtype 0 or 1 with signed north and east speeds `ns`, `ew` kt."""
+    b = dc.Bits(56).put(1, 5, 19).put(6, 3, sub)
+    if sub == 0:
+        b.put(10, 1, ew < 0).put(11, 11, abs(ew) + 1).put(22, 1, ns < 0).put(23, 11, abs(ns) + 1).put(42, 9, 3)
+    else:
+        b.put(14, 1, ew < 0).put(15, 10, abs(ew)).put(25, 1, ns < 0).put(26, 10, abs(ns)).put(38, 9, 5)
+    return b.v
+
+
+# 5,0 track raw values of a word that is also a 6,0 candidate: 6,0's IAS field overlays 5,0's track, so the track is 0
+# (IAS absent) or negative with its low ten bits, the IAS, at most 500
+TRK_AMBIGUOUS = np.concatenate([[0], np.arange(-1024, -523)])
+
+
+def track_gap(trk_raw, track):
+    """amb_commb_agree's track difference d of a 5,0 track raw value against an ADS-B track, in degrees."""
+    d = math.fmod(abs(trk_raw * 90.0 / 512.0 - track), 360.0)
+    return min(d, 360.0 - d)
+
+
+def tie_scene(every=1, seed=6):
+    """Pythagorean velocities with an even hypotenuse c (exact integer speeds), both orders of (a, b), all four sign
+    combinations, subtypes 0 and 1; after each, on the same address, 5,0/6,0-ambiguous DF20 words with
+    2 GS - c = -22, -20, 20, 22 and the track nearest the velocity's, then with 2 GS = c and the tracks whose difference d
+    is nearest 10 deg from below and from above. `every`: keep every n-th velocity. Returns (msgs, cases): cases[k] =
+    (kind, delta) for a reply ("speed", 2 GS - c) / ("track", d), None for a velocity."""
+    rng = np.random.default_rng(seed)
+    ev, t, aa = [], 1.0, 0x300000
+    vels = [(sub, sn * a, se * b, c) for a0, b0, c in pythagorean() for a, b in ((a0, b0), (b0, a0))
+            for sn in (1, -1) for se in (1, -1) for sub in (0, 1)]
+    for sub, ns, ew, c in vels[::every]:
+        track = math.atan2(ew, ns) * (180.0 / math.pi) % 360.0
+        gaps = np.array([track_gap(int(x), track) for x in TRK_AMBIGUOUS])
+        ev.append((t, *dc.df17(aa, velocity_word(sub, ns, ew)), None))
+        words = []
+        if gaps.min() <= 9.0:
+            trk = int(TRK_AMBIGUOUS[int(np.argmin(gaps))])
+            words += [((c + delta) // 2, trk, ("speed", delta)) for delta in (-22, -20, 20, 22) if c + delta >= 0]
+        for side in (gaps <= 10.0, gaps > 10.0):
+            near = np.flatnonzero(side & (np.abs(gaps - 10.0) < 0.2))
+            if len(near):
+                k = near[np.argmin(np.abs(gaps[near] - 10.0))]
+                words.append((c // 2, int(TRK_AMBIGUOUS[k]), ("track", float(gaps[k]))))
+        for j, (gs, trk, case) in enumerate(words):
+            ev.append((t + 0.01 * (j + 1), *reply(20, aa, ambiguous_word(rng, gs=gs, trk=trk), rng), case))
+        aa += 1
+        t += 0.1
+    ev.sort(key=lambda e: e[0])
+    return [(fr.hex(), ecc, int(t), float(np.float64(t - int(t)))) for t, fr, ecc, _ in ev], [e[3] for e in ev]
+
+
 # ---- a synthetic fleet (tools/commb_yield.py, the GPU stress) -----------------------------------------------------------
 def _q(x, lsb, lo, hi):
     return int(max(lo, min(hi, round(x / lsb))))
