@@ -27,6 +27,10 @@ LOCAL_CPR_MAX = 600
 # AMB_FIELDS_COMMB (include/airmodes_b200.h AMB_COMMB_*), decoder option "commb" = S seconds (0 = off)
 COMMB_NOT_TRIED, COMMB_DECODED, COMMB_RESOLVED, COMMB_AMBIGUOUS, COMMB_NONE = 0, 1, 2, 3, 4
 COMMB_MAX = 600
+# AMB_FIELDS_ES (include/airmodes_b200.h AMB_ES_*), decoder option "opstatus" = S seconds (0 = off)
+ES_NOT_TRIED, ES_OPSTATUS, ES_TARGET_STATE, ES_NIC, ES_NUC, ES_UNSUPPORTED = 0, 1, 2, 3, 4, 5
+ES_NO_VERSION = 0xFF
+OPSTATUS_MAX = 600
 # amb_aircraft.flags (include/airmodes_b200.h AMB_AC_*), decoder option "track" = S seconds (0 = off)
 AC_HAS_ALT, AC_HAS_SQUAWK, AC_HAS_IDENT, AC_HAS_POS, AC_HAS_RANGE = 0x001, 0x002, 0x004, 0x008, 0x010
 AC_HAS_VELOCITY, AC_HAS_HEADING, AC_HAS_EPS, AC_ON_GROUND = 0x020, 0x040, 0x080, 0x100
@@ -122,6 +126,11 @@ class Fields(C.Structure):
     def commb(self) -> int:
         """AMB_FIELDS_COMMB (byte 137): Comm-B inference outcome (decoder option "commb"), COMMB_*."""
         return (self.pad_ >> 8) & 0xFF
+
+    @property
+    def es(self) -> int:
+        """AMB_FIELDS_ES (byte 141): op status / integrity outcome (decoder option "opstatus"), ES_*."""
+        return (self.pad_ >> 40) & 0xFF
 
 
 class Aircraft(C.Structure):

@@ -20,6 +20,9 @@
 // With option "track" on, six more after those (amb_decode_track.cuh): amb_track_keys, the four partition kernels on
 // address keys, amb_track_walk - the per-aircraft table, direct-mapped in HBM (2^24 x 128 B) with an occupancy bitmap;
 // amb_decoder_aircraft reads it out with three kernels of its own.
+// With option "opstatus" on, six more between the Comm-B and the track stage (amb_decode_opstatus.cuh):
+// amb_opstatus_keys, the four partition kernels on address keys, amb_opstatus_walk - DF17 TC 29 / 31 decoded, and NIC / Rc
+// or NUCp for every position, with a direct-mapped table of op status in HBM (2^24 x 24 B) carried from batch to batch.
 #include "amb_launch.h"
 #include "amb_decode_core.h"
 #include "amb_decode_kernels.cuh"
@@ -144,6 +147,7 @@ int amb_decoder_create(int device, int have_location, double lat, double lon, am
     static_assert(sizeof(AmbCprSlot) == 16, "table slot layout");
     static_assert(sizeof(AmbRefPos) == 24, "reference position slot layout");
     static_assert(sizeof(AmbCommbRef) == 24, "velocity reference slot layout");
+    static_assert(sizeof(AmbOpsSlot) == 24, "op status slot layout");
     static_assert(sizeof(amb_aircraft) == 128, "amb_aircraft layout");
     if (!out) return AMB_ERR_INVALID;
     *out = nullptr;
@@ -186,6 +190,7 @@ void amb_decoder_destroy(amb_decoder* d)
     if (d->st.ltable) cudaFree(d->st.ltable);
     if (d->st.keys) cudaFree(d->st.keys);
     if (d->st.ctable) cudaFree(d->st.ctable);
+    if (d->st.otable) cudaFree(d->st.otable);
     if (d->st.trows) cudaFree(d->st.trows);
     if (d->st.tocc) cudaFree(d->st.tocc);
     if (d->st.tclk) cudaFree(d->st.tclk);
@@ -214,6 +219,7 @@ int amb_decoder_reset(amb_decoder* d)
     DCK(cudaMemsetAsync(d->st.table, 0xFF, AMB_TABLE_SLOTS * sizeof(AmbCprSlot), d->stream));
     if (d->st.ltable) DCK(cudaMemsetAsync(d->st.ltable, 0xFF, AMB_LOCAL_SLOTS * sizeof(AmbRefPos), d->stream));
     if (d->st.ctable) DCK(cudaMemsetAsync(d->st.ctable, 0xFF, AMB_COMMB_SLOTS * sizeof(AmbCommbRef), d->stream));
+    if (d->st.otable) DCK(cudaMemsetAsync(d->st.otable, 0xFF, AMB_OPS_SLOTS * sizeof(AmbOpsSlot), d->stream));
     if (d->st.tocc) {                    // the rows themselves stay: a row whose bit is clear is never read
         static const AmbTrackClock none = {NAN, 0u, 0u};
         DCK(cudaMemsetAsync(d->st.tocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));
@@ -229,6 +235,7 @@ int amb_decoder_set_option(amb_decoder* d, const char* name, int value)
         {"local_cpr", AMB_LOCAL_CPR_MAX, &AmbDecodeState::local_cpr},
         {"commb", AMB_COMMB_MAX, &AmbDecodeState::commb},
         {"track", AMB_TRACK_MAX, &AmbDecodeState::track},
+        {"opstatus", AMB_OPSTATUS_MAX, &AmbDecodeState::opstatus},
     };
     if (!d || !name) return AMB_ERR_INVALID;
     for (const auto& o : options) {
@@ -244,7 +251,7 @@ int amb_decoder_set_option(amb_decoder* d, const char* name, int value)
     return dfail(d, AMB_ERR_INVALID, "amb_decoder_set_option: unknown option");
 }
 
-// the key records of the local, the Comm-B and the track stage, one per frame
+// the key records of the local, the Comm-B, the op-status and the track stage, one per frame
 static int ensure_keys(amb_decoder* d)
 {
     if (d->kcap < d->cap) {
@@ -273,6 +280,17 @@ static int ensure_commb(amb_decoder* d)
         cudaError_t e = cudaMalloc(&d->st.ctable, AMB_COMMB_SLOTS * sizeof(AmbCommbRef));
         if (e != cudaSuccess) { d->st.ctable = nullptr; return dfail(d, AMB_ERR_CUDA, "Comm-B velocity table (384 MiB)", e); }
         DCK(cudaMemsetAsync(d->st.ctable, 0xFF, AMB_COMMB_SLOTS * sizeof(AmbCommbRef), d->stream));
+    }
+    return ensure_keys(d);
+}
+
+// the op-status stage's device memory, at the first decode with the option on (the table starts empty: all NaN)
+static int ensure_opstatus(amb_decoder* d)
+{
+    if (!d->st.otable) {
+        cudaError_t e = cudaMalloc(&d->st.otable, AMB_OPS_SLOTS * sizeof(AmbOpsSlot));
+        if (e != cudaSuccess) { d->st.otable = nullptr; return dfail(d, AMB_ERR_CUDA, "op status table (384 MiB)", e); }
+        DCK(cudaMemsetAsync(d->st.otable, 0xFF, AMB_OPS_SLOTS * sizeof(AmbOpsSlot), d->stream));
     }
     return ensure_keys(d);
 }
@@ -321,6 +339,7 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
     int rc = ensure_cap(d, n);
     if (rc == AMB_OK && d->st.local_cpr > 0) rc = ensure_local(d);
     if (rc == AMB_OK && d->st.commb > 0) rc = ensure_commb(d);
+    if (rc == AMB_OK && d->st.opstatus > 0) rc = ensure_opstatus(d);
     if (rc == AMB_OK && d->st.track > 0) rc = ensure_track(d);
     if (rc != AMB_OK) return rc;
     cudaStream_t s = d->stream;
@@ -336,7 +355,7 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
     const int k = amb_decode_launch(&d->st, src, n, fields, s, &e);
     if (k < 0) {
         static const char* const stage[] = {"cudaGetLastError()", "pairing", "cudaGetLastError()", "local CPR",
-                                            "Comm-B inference", "aircraft table"};   // by -AMB_STAGE_* - 1
+                                            "Comm-B inference", "aircraft table", "op status"};   // by -AMB_STAGE_* - 1
         return dfail(d, AMB_ERR_CUDA, stage[-k - 1], e);
     }
     d->launches += (uint64_t)k;

@@ -567,6 +567,138 @@ AMB_HD int amb_commb_step(amb_fields* r, uint64_t mb, double t, const AmbCommbRe
     return v;
 }
 
+// ---- ADS-B operational status, target state and position integrity (decoder option "opstatus"; DESIGN.md §8
+// "Operational status and NIC") ---------------------------------------------------------------------------------------
+// An address's op status as of a message: t_any / any of its latest op-status record (either subtype), t_surf / surf of
+// its latest surface one; t is NaN when there is none. any = version | NIC-A << 8, surf = NIC-C. Also the table slot.
+struct AmbOpsSlot { double t_any, t_surf; uint32_t any, surf; };
+
+// What the stage makes of a record before the lookup (amb_es_classify)
+#define AMB_ES_KIND_NONE 0u
+#define AMB_ES_KIND_AIR 1u        // airborne op status (a writer)
+#define AMB_ES_KIND_SURF 2u       // surface op status (a writer of both references)
+#define AMB_ES_KIND_POS 3u        // BDS0,5 / BDS0,6 position
+
+// NIC and Rc (metres, NaN = unknown) of a position's type code given its two supplements: (NIC-A, NIC-B) for airborne
+// type codes 9-18, (NIC-A, NIC-C) for surface 5-8. DO-260B as pyModeS tabulates it; a combination the table does not
+// list is NIC 0, Rc unknown.
+AMB_HD int amb_nic_table(int tc, int sa, int sb, float* rc)
+{
+    const int s = sa * 2 + sb;                      // (0,0) 0, (0,1) 1, (1,0) 2, (1,1) 3
+    int nic = 0;
+    float r = NAN;
+    switch (tc) {
+    case 9: case 5:   nic = 11; r = 7.5f; break;
+    case 10: case 6:  nic = 10; r = 25.0f; break;
+    case 11:          if (s == 3) { nic = 9; r = 75.0f; } else if (s == 0) { nic = 8; r = 185.2f; } break;
+    case 7:           if (s == 2) { nic = 9; r = 75.0f; } else if (s == 0) { nic = 8; r = 185.2f; } break;
+    case 12:          nic = 7; r = 370.4f; break;
+    case 13:          if (s == 1) { nic = 6; r = 555.6f; } else if (s == 0) { nic = 6; r = 926.0f; }
+                      else if (s == 3) { nic = 6; r = 1111.2f; } break;
+    case 8:           if (s == 3) { nic = 7; r = 370.4f; } else if (s == 2) { nic = 6; r = 555.6f; }
+                      else if (s == 1) { nic = 6; r = 1111.2f; } break;
+    case 14:          nic = 5; r = 1852.0f; break;
+    case 16:          if (s == 3) { nic = 3; r = 7408.0f; } else if (s == 0) { nic = 2; r = 14816.0f; } break;
+    case 17:          nic = 1; r = 37040.0f; break;
+    default:          break;                        // 18: NIC 0, Rc unknown
+    }
+    *rc = r;
+    return nic;
+}
+
+// NUCp of a position's type code: airborne 9..18 -> 9..0 (15 is no position), surface 5..8 -> 9..6
+AMB_HD int amb_nucp(int tc) { return tc <= 8 ? 14 - tc : 18 - tc; }
+
+AMB_HD uint32_t amb_u8x4(unsigned b0, unsigned b1, unsigned b2, unsigned b3)
+{
+    return (uint32_t)(b0 & 0xFF) | ((uint32_t)(b1 & 0xFF) << 8) | ((uint32_t)(b2 & 0xFF) << 16) | ((uint32_t)(b3 & 0xFF) << 24);
+}
+
+// Write the stage's fields into a record: aux, and pad_ bytes 5..7 (bytes 0..4 stay the local CPR and Comm-B stages')
+AMB_HD void amb_es_write(amb_fields* r, const uint32_t aux[4], int outcome, int version, int nic)
+{
+    for (int k = 0; k < 4; k++) r->aux[k] = aux[k];
+    const uint64_t keep = r->pad_ & 0xFFFFFFFFFFull;
+    r->pad_ = keep | ((uint64_t)(outcome & 0xFF) << 40) | ((uint64_t)(version & 0xFF) << 48) | ((uint64_t)(nic & 0xFF) << 56);
+}
+
+// The ME field of a DF17 frame: ME bit k (1..56) is bit 56 - k of the result (read with amb_commb_bits)
+AMB_HD uint64_t amb_es_me(const amb_frame& f) { return amb_bits(amb_msg_from_frame(f), 33, 56); }
+
+// Decode a queued DF17 TC 29 / TC 31 record in place (AMB_ES_OPSTATUS / _TARGET_STATE / _UNSUPPORTED) and classify
+// every record for the lookup: AMB_ES_KIND_*. *info, *extra = version | NIC-A << 8 and NIC-C (0 for an airborne one)
+// of a writer, type code and ME bit 8 (NIC-B) of a position.
+AMB_HD unsigned amb_es_classify(const amb_frame& f, amb_fields* r, uint32_t* info, uint32_t* extra)
+{
+    *info = 0; *extra = 0;
+    if (!f.passed || r->df != 17 || (r->status & AMB_FS_NOT_QUEUED)) return AMB_ES_KIND_NONE;
+    const uint64_t me = amb_es_me(f);
+    if (r->bds == 0x05 || r->bds == 0x06) {
+        *info = r->ftc; *extra = amb_commb_bits(me, 8, 1);
+        return AMB_ES_KIND_POS;
+    }
+    if (r->status != AMB_FS_NO_HANDLER) return AMB_ES_KIND_NONE;
+    const unsigned tc = amb_commb_bits(me, 1, 5);
+    uint32_t aux[4] = {0, 0, 0, 0};
+    if (tc == 31) {
+        const unsigned sub = amb_commb_bits(me, 6, 3), ver = amb_commb_bits(me, 41, 3);
+        if (sub > 1 || ver > 2) { amb_es_write(r, aux, AMB_ES_UNSUPPORTED, (int)ver, 0); return AMB_ES_KIND_NONE; }
+        aux[0] = amb_commb_bits(me, 9, 16) | (amb_commb_bits(me, 25, 16) << 16);     // capability class, operational mode
+        unsigned nica = 0, nicc = 0;
+        aux[1] = amb_u8x4(sub, 0, 0, 0);
+        if (ver > 0) {                               // version 0 has another layout: its slots stay 0
+            nica = amb_commb_bits(me, 44, 1);
+            aux[1] = amb_u8x4(sub, nica, amb_commb_bits(me, 45, 4), amb_commb_bits(me, 49, 2));
+            aux[2] = amb_u8x4(amb_commb_bits(me, 51, 2), amb_commb_bits(me, 53, 1), amb_commb_bits(me, 54, 1),
+                              amb_commb_bits(me, 55, 1));
+            if (sub == 1) {
+                nicc = amb_commb_bits(me, 20, 1);
+                aux[3] = amb_u8x4(nicc, amb_commb_bits(me, 21, 4), 0, 0);
+            }
+        }
+        amb_es_write(r, aux, AMB_ES_OPSTATUS, (int)ver, 0);
+        *info = ver | (nica << 8); *extra = nicc;
+        return sub ? AMB_ES_KIND_SURF : AMB_ES_KIND_AIR;
+    }
+    if (tc == 29) {
+        if (amb_commb_bits(me, 6, 2) != 1) { amb_es_write(r, aux, AMB_ES_UNSUPPORTED, AMB_ES_NO_VERSION, 0); return AMB_ES_KIND_NONE; }
+        aux[0] = amb_commb_bits(me, 10, 11) | (amb_commb_bits(me, 21, 9) << 16);   // selected altitude, baro setting
+        aux[1] = amb_commb_bits(me, 31, 9) | (amb_u8x4(0, 0, amb_commb_bits(me, 8, 1), amb_commb_bits(me, 9, 1)));
+        aux[2] = amb_u8x4(amb_commb_bits(me, 30, 1), amb_commb_bits(me, 40, 4), amb_commb_bits(me, 44, 1),
+                          amb_commb_bits(me, 45, 2));
+        aux[3] = amb_commb_bits(me, 47, 8);
+        amb_es_write(r, aux, AMB_ES_TARGET_STATE, 2, 0);
+    }
+    return AMB_ES_KIND_NONE;
+}
+
+// One position record, given its address's op status as of it. tc = its type code, nicb = its ME bit 8.
+AMB_HD int amb_es_position(amb_fields* r, int tc, int nicb, double t, const AmbOpsSlot* ref, int max_age)
+{
+    const bool a_ok = ref->t_any == ref->t_any && t - ref->t_any >= 0.0 && t - ref->t_any <= (double)max_age;
+    const bool c_ok = ref->t_surf == ref->t_surf && t - ref->t_surf >= 0.0 && t - ref->t_surf <= (double)max_age;
+    const int ver = (int)(ref->any & 0xFF);
+    uint32_t aux[4] = {0, 0, 0, 0};
+    if (!a_ok || ver == 0) {
+        aux[1] = 0x7FC00000u;                        // Rc unknown: float32 NaN
+        amb_es_write(r, aux, AMB_ES_NUC, a_ok ? 0 : AMB_ES_NO_VERSION, amb_nucp(tc));
+        return AMB_ES_NUC;
+    }
+    const int surface = tc <= 8;
+    const int a = (int)((ref->any >> 8) & 1);
+    const int b = surface ? 0 : (ver == 2 ? nicb : a);
+    const int c = (surface && ver == 2 && c_ok) ? (int)(ref->surf & 1) : 0;
+    float rc = NAN;
+    int nic = 0;
+    if (!(ver == 1 && tc == 8)) nic = amb_nic_table(tc, a, surface ? c : b, &rc);   // version 1: TC 8 is NIC 0
+    union { float f; uint32_t u; } bitsof;
+    bitsof.f = rc;
+    aux[0] = amb_u8x4(a, b, c, 0);
+    aux[1] = rc == rc ? bitsof.u : 0x7FC00000u;
+    amb_es_write(r, aux, AMB_ES_NIC, ver, nic);
+    return AMB_ES_NIC;
+}
+
 // Latest-report bookkeeping of cpr_decoder.decode for ONE message given the table state before it (cpr.py:214-229):
 // used by the pairing kernel lane by lane and, sequentially, by the host shim.
 // A stored report stamped LATER than the current message can only stem from an earlier stream (frame timestamps restart

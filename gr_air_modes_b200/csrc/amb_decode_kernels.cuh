@@ -43,6 +43,7 @@ __global__ void __launch_bounds__(128) amb_resolve_kernel(amb_fields* __restrict
 #include "amb_decode_v3.cuh"
 #include "amb_decode_local.cuh"
 #include "amb_decode_commb.cuh"
+#include "amb_decode_opstatus.cuh"
 #include "amb_decode_track.cuh"
 
 // ---- launch sequence ----------------------------------------------------------------------------------------------
@@ -53,11 +54,13 @@ struct AmbDecodeState {
     double* nl_T = nullptr;              // NL transition table, AMB_NL_MAX
     AmbV3Bufs v3;                        // pairing scratch, reused by the partitions of the stages after it
     AmbPosRec* pos = nullptr; AmbPair* pair = nullptr;   // one per frame
-    AmbPosRec* keys = nullptr;           // one per frame: address-keyed records of the local, Comm-B and track stage
+    AmbPosRec* keys = nullptr;           // one per frame: address-keyed records of the local, Comm-B, op-status and track stage
     int local_cpr = 0;                   // option "local_cpr" = S seconds, 0 = off
     AmbRefPos* ltable = nullptr;         // reference position per ICAO, AMB_LOCAL_SLOTS
     int commb = 0;                       // option "commb" = S seconds, 0 = off
     AmbCommbRef* ctable = nullptr;       // ADS-B velocity per address, AMB_COMMB_SLOTS
+    int opstatus = 0;                    // option "opstatus" = S seconds, 0 = off
+    AmbOpsSlot* otable = nullptr;        // latest op status per address, AMB_OPS_SLOTS
     int track = 0;                       // option "track" = S seconds, 0 = off
     amb_aircraft* trows = nullptr;       // one row per address, AMB_TRACK_ROWS
     unsigned* tocc = nullptr;            // which rows hold data, AMB_TRACK_WORDS
@@ -67,11 +70,11 @@ struct AmbDecodeState {
 
 // What amb_decode_launch returns when a stage fails to launch.
 enum { AMB_STAGE_FIELDS = -1, AMB_STAGE_PAIRING = -2, AMB_STAGE_RESOLVE = -3, AMB_STAGE_LOCAL = -4,
-       AMB_STAGE_COMMB = -5, AMB_STAGE_TRACK = -6 };
+       AMB_STAGE_COMMB = -5, AMB_STAGE_TRACK = -6, AMB_STAGE_OPSTATUS = -7 };
 
 // Enqueue one decode of the n frames into the n records on stream s, in this order: fields, pairing, resolve, then the
-// local CPR, Comm-B and track stages whose S is > 0. Returns how many kernels were launched (7, plus 6 per stage that
-// is on), or an AMB_STAGE_* code with *err set.
+// local CPR, Comm-B, op-status and track stages whose S is > 0. Returns how many kernels were launched (7, plus 6 per
+// stage that is on), or an AMB_STAGE_* code with *err set.
 static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n, amb_fields* fields, cudaStream_t s,
                              cudaError_t* err)
 {
@@ -94,6 +97,11 @@ static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n,
         const int kc = amb_commb_launch(&st->v3, frames, fields, st->pos, st->keys, n, st->ctable, st->commb, s, err);
         if (kc < 0) return AMB_STAGE_COMMB;
         k += kc;
+    }
+    if (st->opstatus > 0) {
+        const int ko = amb_opstatus_launch(&st->v3, frames, fields, st->pos, st->keys, n, st->otable, st->opstatus, s, err);
+        if (ko < 0) return AMB_STAGE_OPSTATUS;
+        k += ko;
     }
     if (st->track > 0) {
         const int kt = amb_track_launch(&st->v3, frames, fields, st->pos, st->keys, n, st->trows, st->tocc, st->tclk,

@@ -31,6 +31,12 @@ LOCAL_CPR_MAX = _lib.LOCAL_CPR_MAX
 COMMB_NOT_TRIED, COMMB_DECODED, COMMB_RESOLVED, COMMB_AMBIGUOUS, COMMB_NONE = (
     _lib.COMMB_NOT_TRIED, _lib.COMMB_DECODED, _lib.COMMB_RESOLVED, _lib.COMMB_AMBIGUOUS, _lib.COMMB_NONE)
 COMMB_MAX = _lib.COMMB_MAX
+# op status / integrity outcome of a record (decoder option opstatus; include/airmodes_b200.h AMB_ES_*), read by
+# opstatus_outcome()
+ES_NOT_TRIED, ES_OPSTATUS, ES_TARGET_STATE, ES_NIC, ES_NUC, ES_UNSUPPORTED = (
+    _lib.ES_NOT_TRIED, _lib.ES_OPSTATUS, _lib.ES_TARGET_STATE, _lib.ES_NIC, _lib.ES_NUC, _lib.ES_UNSUPPORTED)
+ES_NO_VERSION = _lib.ES_NO_VERSION
+OPSTATUS_MAX = _lib.OPSTATUS_MAX
 # per-aircraft table (decoder option track; include/airmodes_b200.h amb_aircraft, AMB_AC_*)
 AC_HAS_ALT, AC_HAS_SQUAWK, AC_HAS_IDENT, AC_HAS_POS, AC_HAS_RANGE = (
     _lib.AC_HAS_ALT, _lib.AC_HAS_SQUAWK, _lib.AC_HAS_IDENT, _lib.AC_HAS_POS, _lib.AC_HAS_RANGE)
@@ -71,7 +77,7 @@ def local_outcome(records):
 
 
 # the decoder options (amb_decoder_set_option) and their maxima in seconds
-OPTION_MAX = {"local_cpr": LOCAL_CPR_MAX, "track": TRACK_MAX, "commb": COMMB_MAX}
+OPTION_MAX = {"local_cpr": LOCAL_CPR_MAX, "track": TRACK_MAX, "commb": COMMB_MAX, "opstatus": OPSTATUS_MAX}
 
 
 def check_option(name: str, seconds) -> int:
@@ -98,6 +104,10 @@ def check_commb(seconds) -> int:
 
 def check_track(seconds) -> int:
     return check_option("track", seconds)
+
+
+def check_opstatus(seconds) -> int:
+    return check_option("opstatus", seconds)
 
 
 def commb_outcome(records):
@@ -136,6 +146,61 @@ def commb_values(record):
     return out
 
 
+def opstatus_outcome(records):
+    """AMB_FIELDS_ES of a FIELDS_DTYPE record or array: ES_* per record (byte 5 of `pad_`)."""
+    return (np.asarray(records["pad_"], dtype=np.uint64) >> np.uint64(40)) & np.uint64(0xFF)
+
+
+def _aux_bytes(record):
+    return np.asarray([int(x) for x in record["aux"]], dtype="<u4").view(np.uint8)
+
+
+def opstatus_values(record):
+    """What the decoder option opstatus wrote into a record, as named values; None for a record it did not decode.
+      OPSTATUS      {"kind": "opstatus", "version", "subtype" (0 airborne, 1 surface), "capability", "op_mode" (the
+                    16-bit words)}, and for versions 1 and 2 "nic_a", "nacp", "gva", "sil", "hrd", "sil_supplement",
+                    "nic_baro" (airborne) or "trk_hdg" (surface), "nic_c" and "length_width" (surface)
+      TARGET_STATE  {"kind": "target_state", "version": 2, "alt_source" ("MCP/FCU" / "FMS"), "selected_alt" (ft),
+                    "baro" (mb), "heading" (deg; None when absent), "nacp", "nic_baro", "sil", "sil_supplement",
+                    "autopilot", "vnav", "alt_hold", "approach", "lnav" (bool, None when the mode status bit is 0),
+                    "tcas" (bool)}
+      NIC / NUC     {"kind": "nic" / "nuc", "version" (None when there is no op status), "nic" or "nucp", "nic_a",
+                    "nic_b", "nic_c", "rc" (m, None when unknown)}
+    `record`: a FIELDS_DTYPE record or the dict from record_to_dict()."""
+    pad = int(record["pad_"])
+    es, ver, nic = (pad >> 40) & 0xFF, (pad >> 48) & 0xFF, (pad >> 56) & 0xFF
+    b = _aux_bytes(record)
+    u16 = b.view("<u2")
+    if es == ES_OPSTATUS:
+        out = {"kind": "opstatus", "version": ver, "subtype": int(b[4]), "capability": int(u16[0]),
+               "op_mode": int(u16[1])}
+        if ver:
+            out.update(nic_a=int(b[5]), nacp=int(b[6]), gva=int(b[7]), sil=int(b[8]), hrd=int(b[10]),
+                       sil_supplement=int(b[11]))
+            if b[4]:
+                out.update(trk_hdg=int(b[9]), nic_c=int(b[12]), length_width=int(b[13]))
+            else:
+                out["nic_baro"] = int(b[9])
+        return out
+    if es == ES_TARGET_STATE:
+        alt, baro, hdg, modes = int(u16[0]), int(u16[1]), int(u16[2]), int(b[12])
+        valid = bool(modes & 0x80)
+        out = {"kind": "target_state", "version": ver, "alt_source": "FMS" if b[7] else "MCP/FCU",
+               "selected_alt": None if alt == 0 else (alt - 1) * 32, "baro": None if baro == 0 else 800.0 + (baro - 1) * 0.8,
+               "heading": hdg * 180.0 / 256 if b[8] else None, "nacp": int(b[9]), "nic_baro": int(b[10]),
+               "sil": int(b[11]), "sil_supplement": int(b[6])}
+        for name, bit in (("autopilot", 0x40), ("vnav", 0x20), ("alt_hold", 0x10), ("approach", 0x04), ("lnav", 0x01)):
+            out[name] = bool(modes & bit) if valid else None
+        out["tcas"] = bool(modes & 0x02)
+        return out
+    if es in (ES_NIC, ES_NUC):
+        rc = float(b[4:8].view("<f4")[0])
+        return {"kind": "nic" if es == ES_NIC else "nuc", "version": None if ver == ES_NO_VERSION else ver,
+                ("nic" if es == ES_NIC else "nucp"): nic, "nic_a": int(b[0]), "nic_b": int(b[1]), "nic_c": int(b[2]),
+                "rc": None if math.isnan(rc) else rc}
+    return None
+
+
 # aircraft_to_dict: a column and the flag that says it is set
 _AC_COLUMNS = (("altitude", AC_HAS_ALT), ("squawk", AC_HAS_SQUAWK), ("ident", AC_HAS_IDENT), ("ftc", AC_HAS_IDENT),
                ("cat", AC_HAS_IDENT), ("lat", AC_HAS_POS), ("lon", AC_HAS_POS), ("pos_t", AC_HAS_POS),
@@ -169,11 +234,15 @@ class batch_decoder:
     address heard in a DF17 squitter, dropped S seconds after its last message (DESIGN.md §8 "Aircraft table").
     commb = S > 0 also infers the register (BDS 4,0 / 5,0 / 6,0) of the DF20/21 replies the parser does not handle,
     with the address's ADS-B velocity of at most S seconds before deciding between 5,0 and the others; read with
-    commb_outcome() / commb_values() (DESIGN.md §8 "Comm-B inference")."""
+    commb_outcome() / commb_values() (DESIGN.md §8 "Comm-B inference").
+    opstatus = S > 0 also decodes the DF17 operational status (TC 31) and target state (TC 29 subtype 1) squitters, and
+    gives every DF17 position its NIC and containment radius from the address's op status of at most S seconds before,
+    or its NUCp; read with opstatus_outcome() / opstatus_values() (DESIGN.md §8 "Operational status and NIC")."""
 
-    def __init__(self, my_location=None, device: int = 0, local_cpr: int = 0, track: int = 0, commb: int = 0):
+    def __init__(self, my_location=None, device: int = 0, local_cpr: int = 0, track: int = 0, commb: int = 0,
+                 opstatus: int = 0):
         settings = {"local_cpr": check_option("local_cpr", local_cpr), "track": check_option("track", track),
-                    "commb": check_option("commb", commb)}
+                    "commb": check_option("commb", commb), "opstatus": check_option("opstatus", opstatus)}
         self._lib = _lib.load()
         h = C.c_void_p()
         have, lat, lon = self._loc(my_location)
@@ -205,7 +274,8 @@ class batch_decoder:
         self.my_location = new_location
 
     def reset(self):
-        """Forget every stored report, reference position, velocity and aircraft; the option settings stay."""
+        """Forget every stored report, reference position, velocity, op status and aircraft; the option settings
+        stay."""
         self._check(self._lib.amb_decoder_reset(self._h))
 
     def _set_option(self, name, seconds):
@@ -233,6 +303,13 @@ class batch_decoder:
 
     def get_commb(self) -> int:
         return self._options["commb"]
+
+    def set_opstatus(self, seconds: int):
+        """Option opstatus = S seconds (0 = off); applies from the next decode."""
+        self._set_option("opstatus", seconds)
+
+    def get_opstatus(self) -> int:
+        return self._options["opstatus"]
 
     @staticmethod
     def _now(now):

@@ -66,6 +66,33 @@ def _commb_text(df, ecc, v):
     return "Type %i %s from %x: %s" % (df, title, ecc, " ".join(parts))
 
 
+def _opstatus_text(icao, v):
+    """Decoder option opstatus: one line for a decoded TC 31 (BDS6,5) or TC 29 subtype 1 (BDS6,2) squitter."""
+    if v["kind"] == "opstatus":
+        out = "Type 17 BDS6,5 (operational status) from %x version %i %s capability %04x mode %04x" % (
+            icao, v["version"], "surface" if v["subtype"] else "airborne", v["capability"], v["op_mode"])
+        if v["version"]:
+            out += " NIC-A %i NACp %i SIL %i" % (v["nic_a"], v["nacp"], v["sil"])
+            if v["subtype"]:
+                out += " NIC-C %i TRK/HDG %i L/W %i" % (v["nic_c"], v["trk_hdg"], v["length_width"])
+            else:
+                out += " GVA %i NICbaro %i" % (v["gva"], v["nic_baro"])
+            out += " HRD %i SIL supp %i" % (v["hrd"], v["sil_supplement"])
+        return out
+    out = "Type 17 BDS6,2 (target state) from %x" % icao
+    if v["selected_alt"] is not None:
+        out += " selected alt %ift (%s)" % (v["selected_alt"], v["alt_source"])
+    if v["baro"] is not None:
+        out += " baro %.1fmb" % v["baro"]
+    if v["heading"] is not None:
+        out += " heading %.1f" % v["heading"]
+    modes = [name for name, key in (("AP", "autopilot"), ("VNAV", "vnav"), ("ALT", "alt_hold"), ("APP", "approach"),
+                                    ("LNAV", "lnav"), ("TCAS", "tcas")) if v[key]]
+    if modes:
+        out += " modes " + " ".join(modes)
+    return out + " NACp %i NICbaro %i SIL %i" % (v["nacp"], v["nic_baro"], v["sil"])
+
+
 def format_report(message: str, r) -> str | None:
     """One slicer message string + its decoded record -> the line output_print would print, or None where the
     reference prints nothing. `r`: a FIELDS_DTYPE record or the dict from decode.record_to_dict()."""
@@ -77,6 +104,10 @@ def format_report(message: str, r) -> str | None:
         v = _d.commb_values(r)                      # decoder option commb: an inferred BDS 4,0 / 5,0 / 6,0 register
         if v is not None:
             return prefix(float(ref), int(secs), float(frac)) + _commb_text(df, ecc, v)
+    if st == _d.FS_NO_HANDLER and df == 17:
+        v = _d.opstatus_values(r)                   # decoder option opstatus: a decoded TC 31 / TC 29 squitter
+        if v is not None:
+            return prefix(float(ref), int(secs), float(frac)) + _opstatus_text(r["icao"], v)
     if st & (_d.FS_NO_HANDLER | _d.FS_NOT_QUEUED):
         return None                                 # the parser raised: nothing is published (parse.py:431-434)
     out = prefix(float(ref), int(secs), float(frac))

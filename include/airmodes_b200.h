@@ -372,7 +372,7 @@ typedef struct amb_fields {
                              BDS0,9-1: velocity, heading, vert_spd, alt_geo_diff (parse.py:315-348)
                              BDS0,9-3: mag_hdg, vel, vert_spd, geo_diff (parse.py:350-364)
                              BDS0,6  : ground_track (parse.py:283) */
-    uint64_t pad_;        /* [byte 0] local CPR outcome (AMB_FIELDS_LOCAL), [1..4] Comm-B (AMB_FIELDS_COMMB*), the rest 0 */
+    uint64_t pad_;        /* [byte 0] local CPR (AMB_FIELDS_LOCAL), [1..4] Comm-B (AMB_FIELDS_COMMB*), [5..7] AMB_FIELDS_ES* */
 } amb_fields;             /* 144 bytes */
 
 /* Locally referenced CPR decode (amb_decoder_set_option(d, "local_cpr", S), S in 1..600 seconds). After the global
@@ -425,6 +425,71 @@ typedef struct amb_fields {
 #define AMB_COMMB_AMBIGUOUS 3    /* several, and the velocity test could not apply or left more than one */
 #define AMB_COMMB_NONE 4         /* no candidate */
 #define AMB_COMMB_MAX 600
+
+/* ADS-B operational status, target state and position integrity (amb_decoder_set_option(d, "opstatus", S), S in
+ * 1..600 seconds). The parser has no handler for DF17 type codes 29 and 31; with the option on, the queued DF17 records
+ * below are decoded. ME bits are numbered 1..56 (ME bit k = message bit 32 + k); t = secs + frac. DF18 is not touched.
+ *   TC 31, ME 6-8 subtype 0 (airborne) or 1 (surface), version ME 41-43 in 0..2: AMB_ES_OPSTATUS (aircraft operational
+ *         status, BDS6,5); any other subtype or version: AMB_ES_UNSUPPORTED.
+ *   TC 29, ME 6-7 = 1: AMB_ES_TARGET_STATE (target state and status, BDS6,2, version 2); subtypes 0, 2, 3:
+ *         AMB_ES_UNSUPPORTED.
+ *   BDS0,5 (TC 9-18 but 15) and BDS0,6 (TC 5-8), with or without a fix: A = the latest earlier AMB_ES_OPSTATUS record of
+ *         the same icao (either subtype, in stream order, since amb_decoder_reset), counted when 0 <= t - t_A <= S;
+ *         C = the same over surface ones. Version (of A) 1 or 2: AMB_ES_NIC with NIC and Rc from DESIGN.md §8's tables
+ *         by type code and supplements: NIC-A from A; NIC-B = ME 8 of an airborne position for version 2, NIC-A for
+ *         version 1; NIC-C from C for version 2 (0 when C does not count), 0 for version 1, where surface TC 8 is NIC 0
+ *         with Rc unknown. A combination the tables do not list is NIC 0, Rc unknown. Version 0 or no A: AMB_ES_NUC,
+ *         NUCp by type code (airborne 18 - TC, surface 14 - TC), Rc unknown.
+ * Status stays AMB_FS_NO_HANDLER for TC 29 / 31. The option writes only aux and bytes 5..7 of pad_ of these records
+ * (every other DF17 record keeps aux = 0 and pad_ bytes 5..7 = 0): */
+#define AMB_FIELDS_ES(r) (((uint8_t*)&(r)->pad_)[5])          /* outcome, AMB_ES_* */
+#define AMB_FIELDS_ES_VERSION(r) (((uint8_t*)&(r)->pad_)[6])  /* TC 31: its version (ME 41-43); TC 29 subtype 1: 2;
+                                                                 position: A's version; else AMB_ES_NO_VERSION */
+#define AMB_FIELDS_ES_NIC(r) (((uint8_t*)&(r)->pad_)[7])      /* position: NIC (AMB_ES_NIC) or NUCp (AMB_ES_NUC); else 0 */
+#define AMB_ES_NOT_TRIED 0       /* option off, or not one of the records above */
+#define AMB_ES_OPSTATUS 1        /* TC 31 decoded into aux */
+#define AMB_ES_TARGET_STATE 2    /* TC 29 subtype 1 decoded into aux */
+#define AMB_ES_NIC 3             /* position with NIC and Rc */
+#define AMB_ES_NUC 4             /* position with NUCp only (version 0, or no op status within S) */
+#define AMB_ES_UNSUPPORTED 5     /* TC 31 of another subtype or version, TC 29 of another subtype: aux is 0 */
+#define AMB_ES_NO_VERSION 0xff
+#define AMB_OPSTATUS_MAX 600
+/* aux of AMB_ES_OPSTATUS (raw fields; version 0 has another layout: only SUBTYPE, CC and OM are written, the rest is 0) */
+#define AMB_FIELDS_OPS_CC(r) (((uint16_t*)(r)->aux)[0])        /* capability class, ME 9-24 */
+#define AMB_FIELDS_OPS_OM(r) (((uint16_t*)(r)->aux)[1])        /* operational mode, ME 25-40 */
+#define AMB_FIELDS_OPS_SUBTYPE(r) (((uint8_t*)(r)->aux)[4])    /* 0 airborne, 1 surface */
+#define AMB_FIELDS_OPS_NIC_A(r) (((uint8_t*)(r)->aux)[5])      /* ME 44 */
+#define AMB_FIELDS_OPS_NACP(r) (((uint8_t*)(r)->aux)[6])       /* ME 45-48 */
+#define AMB_FIELDS_OPS_GVA(r) (((uint8_t*)(r)->aux)[7])        /* ME 49-50 */
+#define AMB_FIELDS_OPS_SIL(r) (((uint8_t*)(r)->aux)[8])        /* ME 51-52 */
+#define AMB_FIELDS_OPS_NIC_BARO(r) (((uint8_t*)(r)->aux)[9])   /* ME 53: NICbaro (airborne), TRK/HDG (surface) */
+#define AMB_FIELDS_OPS_HRD(r) (((uint8_t*)(r)->aux)[10])       /* ME 54 */
+#define AMB_FIELDS_OPS_SIL_SUPP(r) (((uint8_t*)(r)->aux)[11])  /* ME 55 */
+#define AMB_FIELDS_OPS_NIC_C(r) (((uint8_t*)(r)->aux)[12])     /* surface: ME 20 (last capability-class bit); else 0 */
+#define AMB_FIELDS_OPS_LW(r) (((uint8_t*)(r)->aux)[13])        /* surface: length/width code ME 21-24; else 0 */
+/* aux of AMB_ES_TARGET_STATE (raw fields) */
+#define AMB_FIELDS_TS_ALT(r) (((uint16_t*)(r)->aux)[0])        /* selected altitude ME 10-20: 0 no data, else (n-1) * 32 ft */
+#define AMB_FIELDS_TS_BARO(r) (((uint16_t*)(r)->aux)[1])       /* baro setting ME 21-29: 0 no data, else 800 + (n-1) * 0.8 mb */
+#define AMB_FIELDS_TS_HDG(r) (((uint16_t*)(r)->aux)[2])        /* selected heading ME 31-39 (sign included): n * 180/256 deg */
+#define AMB_FIELDS_TS_SIL_SUPP(r) (((uint8_t*)(r)->aux)[6])    /* ME 8 */
+#define AMB_FIELDS_TS_ALT_TYPE(r) (((uint8_t*)(r)->aux)[7])    /* ME 9: 0 MCP/FCU, 1 FMS */
+#define AMB_FIELDS_TS_HDG_STATUS(r) (((uint8_t*)(r)->aux)[8])  /* ME 30: 1 = the heading is valid */
+#define AMB_FIELDS_TS_NACP(r) (((uint8_t*)(r)->aux)[9])        /* ME 40-43 */
+#define AMB_FIELDS_TS_NIC_BARO(r) (((uint8_t*)(r)->aux)[10])   /* ME 44 */
+#define AMB_FIELDS_TS_SIL(r) (((uint8_t*)(r)->aux)[11])        /* ME 45-46 */
+#define AMB_FIELDS_TS_MODES(r) (((uint8_t*)(r)->aux)[12])      /* ME 47 (bit 7) .. ME 54 (bit 0): AMB_TS_* */
+#define AMB_TS_MODE_STATUS 0x80  /* ME 47: the mode bits below (but TCAS) are valid */
+#define AMB_TS_AUTOPILOT 0x40
+#define AMB_TS_VNAV 0x20
+#define AMB_TS_ALT_HOLD 0x10
+#define AMB_TS_APPROACH 0x04     /* 0x08 is ME 51, reserved */
+#define AMB_TS_TCAS 0x02         /* TCAS/ACAS operational */
+#define AMB_TS_LNAV 0x01
+/* aux of AMB_ES_NIC / AMB_ES_NUC (a position): the supplements used (0 where unused, all 0 for NUC) and Rc */
+#define AMB_FIELDS_POS_NIC_A(r) (((uint8_t*)(r)->aux)[0])
+#define AMB_FIELDS_POS_NIC_B(r) (((uint8_t*)(r)->aux)[1])      /* airborne only */
+#define AMB_FIELDS_POS_NIC_C(r) (((uint8_t*)(r)->aux)[2])      /* surface, version 2 only */
+#define AMB_FIELDS_POS_RC(r) (((float*)(r)->aux)[1])           /* containment radius, metres; NaN = unknown */
 
 /* Per-aircraft state table (amb_decoder_set_option(d, "track", S), S in 1..3600 seconds): every decode also folds its
  * records, in stream order, into one row per 24-bit address, kept on the device. A record counts when its status has
@@ -484,6 +549,10 @@ AMB_API int amb_decoder_create(int device, int have_location, double lat, double
  * call. The ADS-B velocity per address (2^24 x 24 B = 384 MiB of device memory) is allocated at the first decode with
  * the option on and cleared by amb_decoder_reset. A decode with the option on launches six kernels more; off changes
  * nothing.
+ * "opstatus": S = 0 (default, off) .. 600 seconds, ADS-B op status, target state and position integrity (see
+ * AMB_FIELDS_ES); applies from the next call. The latest op status per address (2^24 x 24 B = 384 MiB of device memory)
+ * is allocated at the first decode with the option on and cleared by amb_decoder_reset. A decode with the option on
+ * launches six kernels more; off changes nothing.
  * Unknown names and out-of-range values return AMB_ERR_INVALID. */
 AMB_API int amb_decoder_set_option(amb_decoder* d, const char* name, int value);
 /* Snapshot of the per-aircraft table at time `now`: every row with seen <= now and now - seen <= S, in ascending
@@ -495,7 +564,8 @@ AMB_API int amb_decoder_aircraft(amb_decoder* d, double now, amb_aircraft* out, 
 AMB_API int amb_decoder_aircraft_device(amb_decoder* d, double now, amb_aircraft* out_dev, int cap);
 AMB_API void amb_decoder_destroy(amb_decoder* d);
 AMB_API int amb_decoder_set_location(amb_decoder* d, int have_location, double lat, double lon);   /* cpr.py:192-193 */
-AMB_API int amb_decoder_reset(amb_decoder* d);                      /* forget every stored report (and reference position) */
+AMB_API int amb_decoder_reset(amb_decoder* d);                      /* forget every stored report, reference position,
+                                                                       velocity, op status and aircraft */
 /* Decode n frames (host or device array, stream order = non-decreasing time). out: n records in host memory.
  * Frames with passed == 0 get AMB_FS_NOT_QUEUED and do not touch the CPR state. */
 AMB_API int amb_decode_frames(amb_decoder* d, const amb_frame* frames, int n, int mem_kind, amb_fields* out);

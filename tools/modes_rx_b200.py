@@ -14,6 +14,7 @@ of the dl_data feed and are not re-implemented.
     python tools/modes_rx_b200.py -s 127.0.0.1:12345 -r 4e6 --udp-idle 2.0
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 --track 60 --aircraft aircraft.json
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 --reports --commb 30
+    python tools/modes_rx_b200.py -s capture.cfile -r 4e6 --reports --opstatus 60
 
 Differences, all on the far side of rx_path:
 * live radios (-s uhd / osmocom) need GNU Radio: use gr_air_modes_b200.gr_adapter.rx_path inside modes_radio.
@@ -125,10 +126,12 @@ class report_queue:
     (gr_air_modes_b200.decode), the line format from gr_air_modes_b200.report. out=None decodes without printing;
     aircraft=PATH writes the decoder's aircraft table (option track) to PATH after every batch."""
 
-    def __init__(self, location, device, out=sys.stdout, local_cpr=0, track=0, aircraft=None, decoder=None, commb=0):
+    def __init__(self, location, device, out=sys.stdout, local_cpr=0, track=0, aircraft=None, decoder=None, commb=0,
+                 opstatus=0):
         from gr_air_modes_b200 import decode
         self._dec = decoder if decoder is not None else \
-            decode.batch_decoder(location, device, local_cpr=local_cpr, track=track, commb=commb)   # = cpr_decoder(my_position), apps/modes_rx:68
+            decode.batch_decoder(location, device, local_cpr=local_cpr, track=track, commb=commb,
+                                 opstatus=opstatus)   # = cpr_decoder(my_position), apps/modes_rx:68
         self._out, self._texts, self.count, self._aircraft = out, [], 0, aircraft
 
     def handle(self, msg):
@@ -187,6 +190,9 @@ def parse_args(argv=None):
     ap.add_argument("--commb", type=int, default=0, metavar="S",
                     help="text reports: infer the register (BDS 4,0 / 5,0 / 6,0) of DF20/21 replies the parser does not "
                          "handle, with the aircraft's ADS-B velocity of at most S (1..600) seconds before; 0 = off")
+    ap.add_argument("--opstatus", type=int, default=0, metavar="S",
+                    help="text reports: decode ADS-B operational status (TC 31) and target state (TC 29) squitters, and "
+                         "rate positions by the aircraft's op status of at most S (1..600) seconds before; 0 = off")
     ap.add_argument("--local-cpr", type=int, default=0, metavar="S",
                     help="position reports: decode a message that has no global fix relative to the aircraft's last "
                          "position of at most S (1..600) seconds before; 0 = off, as the reference")
@@ -205,6 +211,10 @@ def parse_args(argv=None):
         ap.error("--commb: 0 (off) .. 600 seconds")
     if args.commb and not (args.reports or args.location is not None):
         ap.error("--commb needs --reports or -l")
+    if not 0 <= args.opstatus <= 600:
+        ap.error("--opstatus: 0 (off) .. 600 seconds")
+    if args.opstatus and not (args.reports or args.location is not None):
+        ap.error("--opstatus needs --reports or -l")
     return args
 
 
@@ -233,7 +243,7 @@ def main(argv=None):
     if not args.no_print:
         if args.reports or args.location is not None:
             reporter = report_queue(my_position, args.device, local_cpr=args.local_cpr, track=args.track, commb=args.commb,
-                                    aircraft=args.aircraft)
+                                    opstatus=args.opstatus, aircraft=args.aircraft)
             sinks.append(reporter)
         else:
             printer = print_queue()
