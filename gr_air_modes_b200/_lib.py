@@ -35,6 +35,10 @@ OPSTATUS_MAX = 600
 AC_HAS_ALT, AC_HAS_SQUAWK, AC_HAS_IDENT, AC_HAS_POS, AC_HAS_RANGE = 0x001, 0x002, 0x004, 0x008, 0x010
 AC_HAS_VELOCITY, AC_HAS_HEADING, AC_HAS_EPS, AC_ON_GROUND = 0x020, 0x040, 0x080, 0x100
 TRACK_MAX = 3600
+# amb_aircraft_ext.shown (include/airmodes_b200.h AMB_AXG_*), decoder option "track_ext" = S2 seconds (0 = off)
+AXG_OPS, AXG_TS, AXG_INTEG, AXG_B40, AXG_B50, AXG_B60 = 0x01, 0x02, 0x04, 0x08, 0x10, 0x20
+AXG_N = 6
+TRACK_EXT_MAX = 3600
 
 
 class Frame(C.Structure):
@@ -143,9 +147,20 @@ class Aircraft(C.Structure):
                 ("pad_", C.c_uint8 * 15)]
 
 
+class AircraftExt(C.Structure):
+    """struct amb_aircraft_ext (144 bytes): the op-status and Comm-B groups beside one aircraft row (option
+    "track_ext"); t[i] is the time of the group with bit 1 << i."""
+    _fields_ = [("icao", C.c_uint32), ("shown", C.c_uint8), ("ops_version", C.c_uint8), ("integ_es", C.c_uint8),
+                ("integ_version", C.c_uint8), ("t", C.c_double * 6), ("ops", C.c_uint32 * 4), ("ts", C.c_uint32 * 4),
+                ("integ", C.c_uint32 * 2), ("integ_nic", C.c_uint8), ("commb_mask", C.c_uint8 * 3),
+                ("commb_outcome", C.c_uint8 * 3), ("pad0_", C.c_uint8), ("commb", (C.c_int16 * 5) * 3),
+                ("pad_", C.c_uint8 * 10)]
+
+
 assert C.sizeof(Frame) == 80
 assert C.sizeof(Fields) == 144
 assert C.sizeof(Aircraft) == 128
+assert C.sizeof(AircraftExt) == 144
 
 # every symbol include/airmodes_b200.h declares: (name, restype, argtypes)
 _vp, _f32p, _u64p = C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_uint64)
@@ -200,6 +215,8 @@ SYMBOLS = [
     ("amb_decode_frames_device", C.c_int, [_vp, _vp, C.c_int, _vp]),
     ("amb_decoder_aircraft", C.c_int, [_vp, C.c_double, _vp, C.c_int]),
     ("amb_decoder_aircraft_device", C.c_int, [_vp, C.c_double, _vp, C.c_int]),
+    ("amb_decoder_aircraft_ext", C.c_int, [_vp, C.c_double, _vp, _vp, C.c_int]),
+    ("amb_decoder_aircraft_ext_device", C.c_int, [_vp, C.c_double, _vp, _vp, C.c_int]),
     ("amb_decoder_stats", C.c_int, [_vp, _u64p, _f32p]),
     ("amb_decoder_last_error", C.c_char_p, [_vp]),
     ("amb_frame_bits", C.c_uint64, [C.POINTER(Frame), C.c_int, C.c_int]),

@@ -23,6 +23,10 @@
 // With option "opstatus" on, six more between the Comm-B and the track stage (amb_decode_opstatus.cuh):
 // amb_opstatus_keys, the four partition kernels on address keys, amb_opstatus_walk - DF17 TC 29 / 31 decoded, and NIC / Rc
 // or NUCp for every position, with a direct-mapped table of op status in HBM (2^24 x 24 B) carried from batch to batch.
+// With options "track" and "track_ext" both on, six more after the track stage (amb_decode_track_ext.cuh):
+// amb_track_ext_keys, the four partition kernels on address keys, amb_track_ext_walk - the op-status and Comm-B groups
+// of every address, direct-mapped in HBM (2^24 x 144 B) with an occupancy bitmap; amb_decoder_aircraft_ext reads them
+// out beside the aircraft rows with amb_snap_count, amb_snap_scan and amb_snap_gather_ext.
 #include "amb_launch.h"
 #include "amb_decode_core.h"
 #include "amb_decode_kernels.cuh"
@@ -46,6 +50,7 @@ struct amb_decoder {
     void* pin[2] = {nullptr, nullptr}; cudaEvent_t pin_ev[2] = {nullptr, nullptr}; size_t pin_bytes = 0;
     uint32_t* snap_cnt = nullptr;        // snapshot: per-block counts, then their scan and the total
     amb_aircraft* d_snap = nullptr; int snap_cap = 0;   // snapshot rows on their way to host memory
+    amb_aircraft_ext* d_xsnap = nullptr; int xsnap_cap = 0;   // ... and their extensions
     uint64_t launches = 0; float ms_last = 0.f;
     std::string err;
 };
@@ -149,6 +154,10 @@ int amb_decoder_create(int device, int have_location, double lat, double lon, am
     static_assert(sizeof(AmbCommbRef) == 24, "velocity reference slot layout");
     static_assert(sizeof(AmbOpsSlot) == 24, "op status slot layout");
     static_assert(sizeof(amb_aircraft) == 128, "amb_aircraft layout");
+    static_assert(sizeof(amb_aircraft_ext) == 144 && sizeof(amb_aircraft_ext) % 16 == 0, "amb_aircraft_ext layout");
+    static_assert(offsetof(amb_aircraft_ext, t) == 8 && offsetof(amb_aircraft_ext, ops) == 56 &&
+                  offsetof(amb_aircraft_ext, integ_nic) == 96 && offsetof(amb_aircraft_ext, commb) == 104,
+                  "amb_aircraft_ext layout");
     if (!out) return AMB_ERR_INVALID;
     *out = nullptr;
     int ndev = 0;
@@ -194,6 +203,9 @@ void amb_decoder_destroy(amb_decoder* d)
     if (d->st.trows) cudaFree(d->st.trows);
     if (d->st.tocc) cudaFree(d->st.tocc);
     if (d->st.tclk) cudaFree(d->st.tclk);
+    if (d->st.xrows) cudaFree(d->st.xrows);
+    if (d->st.xocc) cudaFree(d->st.xocc);
+    if (d->d_xsnap) cudaFree(d->d_xsnap);
     if (d->snap_cnt) cudaFree(d->snap_cnt);
     if (d->d_snap) cudaFree(d->d_snap);
     for (int k = 0; k < 2; k++) { if (d->pin[k]) cudaFreeHost(d->pin[k]); if (d->pin_ev[k]) cudaEventDestroy(d->pin_ev[k]); }
@@ -225,6 +237,7 @@ int amb_decoder_reset(amb_decoder* d)
         DCK(cudaMemsetAsync(d->st.tocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));
         DCK(cudaMemcpyAsync(d->st.tclk, &none, sizeof none, cudaMemcpyHostToDevice, d->stream));
     }
+    if (d->st.xocc) DCK(cudaMemsetAsync(d->st.xocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));   // likewise
     DCK(cudaStreamSynchronize(d->stream));
     return AMB_OK;
 }
@@ -236,6 +249,7 @@ int amb_decoder_set_option(amb_decoder* d, const char* name, int value)
         {"commb", AMB_COMMB_MAX, &AmbDecodeState::commb},
         {"track", AMB_TRACK_MAX, &AmbDecodeState::track},
         {"opstatus", AMB_OPSTATUS_MAX, &AmbDecodeState::opstatus},
+        {"track_ext", AMB_TRACK_EXT_MAX, &AmbDecodeState::track_ext},
     };
     if (!d || !name) return AMB_ERR_INVALID;
     for (const auto& o : options) {
@@ -316,6 +330,21 @@ static int ensure_track(amb_decoder* d)
     return ensure_keys(d);
 }
 
+// the track extension's device memory, at the first decode with it and the track stage on: the rows are not
+// initialised (the bitmap starts empty)
+static int ensure_track_ext(amb_decoder* d)
+{
+    if (!d->st.xrows) {
+        cudaError_t e = cudaMalloc(&d->st.xrows, (size_t)AMB_TRACK_ROWS * sizeof(amb_aircraft_ext));
+        if (e != cudaSuccess) { d->st.xrows = nullptr; return dfail(d, AMB_ERR_CUDA, "aircraft table extension (2.25 GiB)", e); }
+    }
+    if (!d->st.xocc) {                   // last: snapshot_impl and reset take a bitmap as "everything is there"
+        DCK(cudaMalloc(&d->st.xocc, AMB_TRACK_WORDS * sizeof(unsigned)));
+        DCK(cudaMemsetAsync(d->st.xocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));
+    }
+    return AMB_OK;
+}
+
 static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_kind, amb_fields* out, bool out_on_device);
 
 int amb_decode_frames(amb_decoder* d, const amb_frame* frames, int n, int mem_kind, amb_fields* out)
@@ -341,6 +370,7 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
     if (rc == AMB_OK && d->st.commb > 0) rc = ensure_commb(d);
     if (rc == AMB_OK && d->st.opstatus > 0) rc = ensure_opstatus(d);
     if (rc == AMB_OK && d->st.track > 0) rc = ensure_track(d);
+    if (rc == AMB_OK && d->st.track > 0 && d->st.track_ext > 0) rc = ensure_track_ext(d);
     if (rc != AMB_OK) return rc;
     cudaStream_t s = d->stream;
     amb_fields* const fields = out_on_device ? out : d->d_fields;
@@ -355,7 +385,8 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
     const int k = amb_decode_launch(&d->st, src, n, fields, s, &e);
     if (k < 0) {
         static const char* const stage[] = {"cudaGetLastError()", "pairing", "cudaGetLastError()", "local CPR",
-                                            "Comm-B inference", "aircraft table", "op status"};   // by -AMB_STAGE_* - 1
+                                            "Comm-B inference", "aircraft table", "op status",
+                                            "aircraft table extension"};   // by -AMB_STAGE_* - 1
         return dfail(d, AMB_ERR_CUDA, stage[-k - 1], e);
     }
     d->launches += (uint64_t)k;
@@ -370,10 +401,18 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
     return AMB_OK;
 }
 
-static int snapshot_impl(amb_decoder* d, double now, amb_aircraft* out, int max, bool out_on_device)
+// with_ext: amb_decoder_aircraft_ext(_device), ext[] beside out[]; else amb_decoder_aircraft(_device)
+static int snapshot_impl(amb_decoder* d, double now, amb_aircraft* out, amb_aircraft_ext* ext, int max, bool out_on_device,
+                         bool with_ext)
 {
-    if (!d || max < 0) return dfail(d, AMB_ERR_INVALID, "amb_decoder_aircraft: bad argument");
-    if (d->st.track <= 0) return dfail(d, AMB_ERR_STATE, "amb_decoder_aircraft: option track is off");
+    const char* fn = with_ext ? "amb_decoder_aircraft_ext" : "amb_decoder_aircraft";
+    char what[96];
+    if (!d || max < 0 || (with_ext && out && !ext)) {
+        snprintf(what, sizeof what, "%s: bad argument", fn);
+        return dfail(d, AMB_ERR_INVALID, what);
+    }
+    if (d->st.track <= 0) { snprintf(what, sizeof what, "%s: option track is off", fn); return dfail(d, AMB_ERR_STATE, what); }
+    if (with_ext && d->st.track_ext <= 0) return dfail(d, AMB_ERR_STATE, "amb_decoder_aircraft_ext: option track_ext is off");
     if (!d->st.tocc) return 0;                           // nothing decoded with the option on yet
     DCK(cudaSetDevice(d->device));
     cudaStream_t s = d->stream;
@@ -388,9 +427,10 @@ static int snapshot_impl(amb_decoder* d, double now, amb_aircraft* out, int max,
     DCK(cudaMemcpyAsync(&total, off + nb, sizeof total, cudaMemcpyDeviceToHost, s));
     DCK(cudaStreamSynchronize(s));
     if (!out) return (int)total;
-    if (total > (uint32_t)max) return dfail(d, AMB_ERR_OVERFLOW, "amb_decoder_aircraft: output buffer too small");
+    if (total > (uint32_t)max) { snprintf(what, sizeof what, "%s: output buffer too small", fn); return dfail(d, AMB_ERR_OVERFLOW, what); }
     if (total == 0) return 0;
     amb_aircraft* dst = out;
+    amb_aircraft_ext* xdst = ext;
     if (!out_on_device) {
         if (d->snap_cap < (int)total) {
             if (d->d_snap) cudaFree(d->d_snap);
@@ -398,13 +438,24 @@ static int snapshot_impl(amb_decoder* d, double now, amb_aircraft* out, int max,
             DCK(cudaMalloc(&d->d_snap, (size_t)total * sizeof(amb_aircraft)));
             d->snap_cap = (int)total;
         }
+        if (with_ext && d->xsnap_cap < (int)total) {
+            if (d->d_xsnap) cudaFree(d->d_xsnap);
+            d->d_xsnap = nullptr; d->xsnap_cap = 0;
+            DCK(cudaMalloc(&d->d_xsnap, (size_t)total * sizeof(amb_aircraft_ext)));
+            d->xsnap_cap = (int)total;
+        }
         dst = d->d_snap;
+        xdst = d->d_xsnap;
     }
-    if (amb_snap_gather_launch(d->st.tocc, d->st.trows, d->st.tclk, now, d->st.track, AMB_TRACK_WORDS, off, dst, s, &e) < 0)
-        return dfail(d, AMB_ERR_CUDA, "aircraft snapshot", e);
+    const int k = with_ext ? amb_snap_gather_ext_launch(d->st.tocc, d->st.trows, d->st.tclk, now, d->st.track, AMB_TRACK_WORDS,
+                                                   off, dst, d->st.xocc, d->st.xrows, d->st.track_ext, xdst, s, &e)
+                      : amb_snap_gather_launch(d->st.tocc, d->st.trows, d->st.tclk, now, d->st.track, AMB_TRACK_WORDS, off,
+                                               dst, s, &e);
+    if (k < 0) return dfail(d, AMB_ERR_CUDA, "aircraft snapshot", e);
     d->launches += 1;
     if (!out_on_device) {
-        const int rc = staged_d2h(d, out, d->d_snap, (size_t)total * sizeof(amb_aircraft), s);
+        int rc = staged_d2h(d, out, d->d_snap, (size_t)total * sizeof(amb_aircraft), s);
+        if (rc == AMB_OK && with_ext) rc = staged_d2h(d, ext, d->d_xsnap, (size_t)total * sizeof(amb_aircraft_ext), s);
         if (rc != AMB_OK) return rc;
     }
     DCK(cudaStreamSynchronize(s));
@@ -413,12 +464,22 @@ static int snapshot_impl(amb_decoder* d, double now, amb_aircraft* out, int max,
 
 int amb_decoder_aircraft(amb_decoder* d, double now, amb_aircraft* out, int max)
 {
-    return snapshot_impl(d, now, out, max, false);
+    return snapshot_impl(d, now, out, nullptr, max, false, false);
 }
 
 int amb_decoder_aircraft_device(amb_decoder* d, double now, amb_aircraft* out_dev, int cap)
 {
-    return snapshot_impl(d, now, out_dev, cap, true);
+    return snapshot_impl(d, now, out_dev, nullptr, cap, true, false);
+}
+
+int amb_decoder_aircraft_ext(amb_decoder* d, double now, amb_aircraft* out, amb_aircraft_ext* ext, int max)
+{
+    return snapshot_impl(d, now, out, ext, max, false, true);
+}
+
+int amb_decoder_aircraft_ext_device(amb_decoder* d, double now, amb_aircraft* out_dev, amb_aircraft_ext* ext_dev, int cap)
+{
+    return snapshot_impl(d, now, out_dev, ext_dev, cap, true, true);
 }
 
 int amb_decoder_stats(amb_decoder* d, uint64_t* kernel_launches, float* ms_last)

@@ -45,6 +45,7 @@ __global__ void __launch_bounds__(128) amb_resolve_kernel(amb_fields* __restrict
 #include "amb_decode_commb.cuh"
 #include "amb_decode_opstatus.cuh"
 #include "amb_decode_track.cuh"
+#include "amb_decode_track_ext.cuh"
 
 // ---- launch sequence ----------------------------------------------------------------------------------------------
 // What the stages of one decode read and write besides the frames and the records: amb_decoder keeps one in device
@@ -65,16 +66,20 @@ struct AmbDecodeState {
     amb_aircraft* trows = nullptr;       // one row per address, AMB_TRACK_ROWS
     unsigned* tocc = nullptr;            // which rows hold data, AMB_TRACK_WORDS
     AmbTrackClock* tclk = nullptr;       // t of the latest queued record since reset
+    int track_ext = 0;                   // option "track_ext" = S2 seconds, 0 = off; runs only while track is on too
+    amb_aircraft_ext* xrows = nullptr;   // one extension row per address, AMB_TRACK_ROWS
+    unsigned* xocc = nullptr;            // which extension rows were written since reset, AMB_TRACK_WORDS
     int have_loc = 0; double lat = 0.0, lon = 0.0;      // receiver location
 };
 
 // What amb_decode_launch returns when a stage fails to launch.
 enum { AMB_STAGE_FIELDS = -1, AMB_STAGE_PAIRING = -2, AMB_STAGE_RESOLVE = -3, AMB_STAGE_LOCAL = -4,
-       AMB_STAGE_COMMB = -5, AMB_STAGE_TRACK = -6, AMB_STAGE_OPSTATUS = -7 };
+       AMB_STAGE_COMMB = -5, AMB_STAGE_TRACK = -6, AMB_STAGE_OPSTATUS = -7, AMB_STAGE_TRACK_EXT = -8 };
 
 // Enqueue one decode of the n frames into the n records on stream s, in this order: fields, pairing, resolve, then the
-// local CPR, Comm-B, op-status and track stages whose S is > 0. Returns how many kernels were launched (7, plus 6 per
-// stage that is on), or an AMB_STAGE_* code with *err set.
+// local CPR, Comm-B, op-status and track stages whose S is > 0, and the track extension when track and track_ext are
+// both > 0. Returns how many kernels were launched (7, plus 6 per stage that is on), or an AMB_STAGE_* code with *err
+// set.
 static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n, amb_fields* fields, cudaStream_t s,
                              cudaError_t* err)
 {
@@ -108,6 +113,11 @@ static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n,
                                         st->track, s, err);
         if (kt < 0) return AMB_STAGE_TRACK;
         k += kt;
+        if (st->track_ext > 0) {
+            const int kx = amb_track_ext_launch(&st->v3, fields, st->pos, st->keys, n, st->xrows, st->xocc, s, err);
+            if (kx < 0) return AMB_STAGE_TRACK_EXT;
+            k += kx;
+        }
     }
     return k;
 }

@@ -225,7 +225,9 @@ __device__ __forceinline__ bool amb_track_shown(const amb_aircraft* rows, unsign
 }
 
 // Rows to show among this thread's four bitmap words, and their exclusive prefix over the 256 threads of the block.
-__device__ __forceinline__ unsigned amb_snap_thread(const unsigned* occ, const amb_aircraft* rows, const AmbTrackClock* clk,
+// Static, so that each library compiled from this header - and each host-emulated one, where the __shared__ array
+// becomes a function-local static - calls its own copy.
+static __device__ __forceinline__ unsigned amb_snap_thread(const unsigned* occ, const amb_aircraft* rows, const AmbTrackClock* clk,
                                                     double now, int max_age, unsigned* before)
 {
     __shared__ unsigned ws[8];

@@ -18,7 +18,7 @@ import math
 import numpy as np
 
 from . import _lib
-from ._lib import Aircraft, Fields, Frame, check
+from ._lib import Aircraft, AircraftExt, Fields, Frame, check
 
 FS_NO_HANDLER, FS_METRIC_ALT, FS_CPR_NO_POS, FS_CPR_STRADDLE = 0x01, 0x02, 0x04, 0x08
 FS_HAS_POS, FS_HAS_RANGE, FS_METRIC_THREAT, FS_NOT_QUEUED = 0x10, 0x20, 0x40, 0x80
@@ -43,10 +43,15 @@ AC_HAS_ALT, AC_HAS_SQUAWK, AC_HAS_IDENT, AC_HAS_POS, AC_HAS_RANGE = (
 AC_HAS_VELOCITY, AC_HAS_HEADING, AC_HAS_EPS, AC_ON_GROUND = (
     _lib.AC_HAS_VELOCITY, _lib.AC_HAS_HEADING, _lib.AC_HAS_EPS, _lib.AC_ON_GROUND)
 TRACK_MAX = _lib.TRACK_MAX
+# extension of the per-aircraft table (decoder option track_ext; include/airmodes_b200.h amb_aircraft_ext, AMB_AXG_*)
+AXG_OPS, AXG_TS, AXG_INTEG, AXG_B40, AXG_B50, AXG_B60 = (
+    _lib.AXG_OPS, _lib.AXG_TS, _lib.AXG_INTEG, _lib.AXG_B40, _lib.AXG_B50, _lib.AXG_B60)
+TRACK_EXT_MAX = _lib.TRACK_EXT_MAX
 
 FIELDS_DTYPE = np.dtype(Fields)
 FRAME_DTYPE = np.dtype(Frame)
 AIRCRAFT_DTYPE = np.dtype(Aircraft)
+AIRCRAFT_EXT_DTYPE = np.dtype(AircraftExt)
 
 
 def frames_from_messages(msgs):
@@ -77,7 +82,8 @@ def local_outcome(records):
 
 
 # the decoder options (amb_decoder_set_option) and their maxima in seconds
-OPTION_MAX = {"local_cpr": LOCAL_CPR_MAX, "track": TRACK_MAX, "commb": COMMB_MAX, "opstatus": OPSTATUS_MAX}
+OPTION_MAX = {"local_cpr": LOCAL_CPR_MAX, "track": TRACK_MAX, "commb": COMMB_MAX, "opstatus": OPSTATUS_MAX,
+              "track_ext": TRACK_EXT_MAX}
 
 
 def check_option(name: str, seconds) -> int:
@@ -225,6 +231,44 @@ def aircraft_to_dict(row) -> dict:
     return d
 
 
+# aircraft_ext_to_dict: the key of each group, in the order of the AXG_* bits
+_AXG_KEYS = ("opstatus", "target_state", "integrity", "bds40", "bds50", "bds60")
+
+
+def _group_record(ext, i) -> dict:
+    """The `pad_` and `aux` slots of the record that wrote group i of an AIRCRAFT_EXT_DTYPE row, rebuilt from the copy
+    the group keeps (every slot the group does not keep is 0)."""
+    words = [0, 0, 0, 0]
+    if i == 0:
+        words, pad = [int(x) for x in ext["ops"]], (ES_OPSTATUS << 40) | (int(ext["ops_version"]) << 48)
+    elif i == 1:
+        words, pad = [int(x) for x in ext["ts"]], (ES_TARGET_STATE << 40) | (2 << 48)
+    elif i == 2:
+        words[:2] = [int(x) for x in ext["integ"]]
+        pad = (int(ext["integ_es"]) << 40) | (int(ext["integ_version"]) << 48) | (int(ext["integ_nic"]) << 56)
+    else:
+        c = i - 3
+        raw = [int(x) & 0xFFFF for x in ext["commb"][c]] + [0]
+        words = [raw[0] | raw[1] << 16, raw[2] | raw[3] << 16, raw[4], 0]
+        pad = (int(ext["commb_outcome"][c]) << 8) | ((0x40 + 0x10 * c) << 16) | (int(ext["commb_mask"][c]) << 24)
+    return {"pad_": pad, "aux": words}
+
+
+def aircraft_ext_to_dict(row, ext) -> dict:
+    """One AIRCRAFT_DTYPE row and its AIRCRAFT_EXT_DTYPE extension -> aircraft_to_dict(row) plus the keys "opstatus",
+    "target_state", "integrity", "bds40", "bds50" and "bds60": None for a group that is not shown, else {"t": the time of
+    the record that wrote it} merged with opstatus_values() / commb_values() of that record."""
+    d = aircraft_to_dict(row)
+    shown = int(ext["shown"])
+    for i, key in enumerate(_AXG_KEYS):
+        if not shown & (1 << i):
+            d[key] = None
+            continue
+        rec = _group_record(ext, i)
+        d[key] = {"t": float(ext["t"][i]), **(opstatus_values(rec) if i < 3 else commb_values(rec))}
+    return d
+
+
 class batch_decoder:
     """cpr_decoder(my_location) (cpr.py:184-190) + parser, for batches. my_location = [lat, lon] or None.
 
@@ -237,12 +281,16 @@ class batch_decoder:
     commb_outcome() / commb_values() (DESIGN.md §8 "Comm-B inference").
     opstatus = S > 0 also decodes the DF17 operational status (TC 31) and target state (TC 29 subtype 1) squitters, and
     gives every DF17 position its NIC and containment radius from the address's op status of at most S seconds before,
-    or its NUCp; read with opstatus_outcome() / opstatus_values() (DESIGN.md §8 "Operational status and NIC")."""
+    or its NUCp; read with opstatus_outcome() / opstatus_values() (DESIGN.md §8 "Operational status and NIC").
+    track_ext = S2 > 0, with track on, also keeps beside every aircraft row the latest op status, target state, position
+    integrity and Comm-B 4,0 / 5,0 / 6,0 of the address, each shown for S2 seconds; read with aircraft_ext() /
+    aircraft_ext_device() (DESIGN.md §8 "Aircraft table extension")."""
 
     def __init__(self, my_location=None, device: int = 0, local_cpr: int = 0, track: int = 0, commb: int = 0,
-                 opstatus: int = 0):
+                 opstatus: int = 0, track_ext: int = 0):
         settings = {"local_cpr": check_option("local_cpr", local_cpr), "track": check_option("track", track),
-                    "commb": check_option("commb", commb), "opstatus": check_option("opstatus", opstatus)}
+                    "commb": check_option("commb", commb), "opstatus": check_option("opstatus", opstatus),
+                    "track_ext": check_option("track_ext", track_ext)}
         self._lib = _lib.load()
         h = C.c_void_p()
         have, lat, lon = self._loc(my_location)
@@ -311,6 +359,13 @@ class batch_decoder:
     def get_opstatus(self) -> int:
         return self._options["opstatus"]
 
+    def set_track_ext(self, seconds: int):
+        """Option track_ext = S2 seconds (0 = off); applies from the next decode, while track is on too."""
+        self._set_option("track_ext", seconds)
+
+    def get_track_ext(self) -> int:
+        return self._options["track_ext"]
+
     @staticmethod
     def _now(now):
         return math.nan if now is None else float(now)
@@ -337,6 +392,37 @@ class batch_decoder:
         n = self._check(self._lib.amb_decoder_aircraft_device(self._h, now, C.c_void_p(out_dev.data_ptr()),
                                                               int(out_dev.numel() // 128)))
         return out_dev[: n * 128]
+
+    def aircraft_ext(self, now=None):
+        """aircraft(now) and the extension of every row: (AIRCRAFT_DTYPE rows, AIRCRAFT_EXT_DTYPE rows), ext[i] beside
+        rows[i]. Needs the options track and track_ext on."""
+        now = self._now(now)
+        n = self._check(self._lib.amb_decoder_aircraft_ext(self._h, now, None, None, 0))
+        out = np.zeros(n, dtype=AIRCRAFT_DTYPE)
+        ext = np.zeros(n, dtype=AIRCRAFT_EXT_DTYPE)
+        if n:
+            n = self._check(self._lib.amb_decoder_aircraft_ext(self._h, now, C.c_void_p(out.ctypes.data),
+                                                               C.c_void_p(ext.ctypes.data), n))
+        return out[:n], ext[:n]
+
+    def aircraft_ext_device(self, now=None, out_dev=None, ext_dev=None):
+        """aircraft_ext() into device memory: returns two CUDA uint8 tensors, of 128-byte amb_aircraft rows and of
+        144-byte amb_aircraft_ext rows (views of the first rows of out_dev / ext_dev when they are given; give both or
+        neither). Only the row count crosses PCIe."""
+        import torch
+        now = self._now(now)
+        if (out_dev is None) != (ext_dev is None):
+            raise ValueError("aircraft_ext_device: give both out_dev and ext_dev, or neither")
+        if out_dev is None:
+            n = self._check(self._lib.amb_decoder_aircraft_ext_device(self._h, now, None, None, 0))
+            dev = torch.device("cuda", self._device)
+            out_dev = torch.empty(n * 128, dtype=torch.uint8, device=dev)
+            ext_dev = torch.empty(n * 144, dtype=torch.uint8, device=dev)
+        torch.cuda.current_stream(out_dev.device).synchronize()          # the decoder runs on its own stream
+        cap = int(min(out_dev.numel() // 128, ext_dev.numel() // 144))
+        n = self._check(self._lib.amb_decoder_aircraft_ext_device(self._h, now, C.c_void_p(out_dev.data_ptr()),
+                                                                  C.c_void_p(ext_dev.data_ptr()), cap))
+        return out_dev[: n * 128], ext_dev[: n * 144]
 
     def decode(self, frames, n: int | None = None) -> np.ndarray:
         """frames: ctypes Frame array / list of Frame (e.g. rx_path.frames) / numpy FRAME_DTYPE array, in stream

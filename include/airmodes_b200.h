@@ -535,6 +535,58 @@ typedef struct amb_aircraft {
     uint8_t pad_[15];     /* 0 */
 } amb_aircraft;           /* 128 bytes */
 
+/* Extension of the per-aircraft table (amb_decoder_set_option(d, "track_ext", S2), S2 in 1..3600 seconds; it has an
+ * effect only while "track" is on too): what the "opstatus" and "commb" options write into the records, kept per
+ * address in six groups. A group holds a copy of the latest record, in stream order, that writes it; its time is that
+ * record's t = secs + frac. Every record writes at most one group; a = its icao field:
+ *   OPS    a queued record with AMB_FIELDS_ES == AMB_ES_OPSTATUS (needs "opstatus"): aux and its version byte;
+ *   TS     AMB_FIELDS_ES == AMB_ES_TARGET_STATE (needs "opstatus"): aux;
+ *   INTEG  AMB_FIELDS_ES == AMB_ES_NIC or AMB_ES_NUC, and AMB_FS_HAS_POS (needs "opstatus"): aux[0..1], the outcome,
+ *          version and NIC bytes. With "opstatus" on from the start, every position the base row takes is rated, so a
+ *          shown INTEG group comes from the record that gave the row its position: t[INTEG] == pos_t;
+ *   B40 / B50 / B60  AMB_FIELDS_COMMB == AMB_COMMB_DECODED or AMB_COMMB_RESOLVED with register 0x40 / 0x50 / 0x60
+ *          (needs "commb"): the five raw fields, the status mask and the outcome.
+ * A snapshot (amb_decoder_aircraft_ext) returns exactly the rows amb_decoder_aircraft would, and beside each row its
+ * extension, in which a group is shown when t >= the row's first_seen (it arrived while this row existed), t <= now and
+ * now - t <= S2. A group that is not shown has t = NaN and every byte of its fields 0, so snapshots compare byte for
+ * byte. amb_decoder_reset forgets every group. */
+#define AMB_AXG_OPS 0x01
+#define AMB_AXG_TS 0x02
+#define AMB_AXG_INTEG 0x04
+#define AMB_AXG_B40 0x08
+#define AMB_AXG_B50 0x10
+#define AMB_AXG_B60 0x20
+#define AMB_AXG_N 6              /* group i has bit 1 << i and time t[i] */
+#define AMB_TRACK_EXT_MAX 3600
+
+typedef struct amb_aircraft_ext {
+    uint32_t icao;        /* the row's address */
+    uint8_t shown;        /* AMB_AXG_* of the groups shown */
+    uint8_t ops_version;  /* OPS: AMB_FIELDS_ES_VERSION of its record */
+    uint8_t integ_es;     /* INTEG: AMB_FIELDS_ES of its record (AMB_ES_NIC / AMB_ES_NUC) */
+    uint8_t integ_version;/* INTEG: AMB_FIELDS_ES_VERSION of its record */
+    double t[6];          /* t of each group's record, by group index; NaN when not shown */
+    uint32_t ops[4];      /* OPS: the record's aux, byte for byte (AMB_AXG_OPS_BYTE) */
+    uint32_t ts[4];       /* TS: the record's aux, byte for byte (AMB_AXG_TS_BYTE) */
+    uint32_t integ[2];    /* INTEG: aux[0..1] of the record (AMB_AXG_INTEG_BYTE, AMB_AXG_INTEG_RC) */
+    uint8_t integ_nic;    /* INTEG: AMB_FIELDS_ES_NIC of its record */
+    uint8_t commb_mask[3];/* B40 / B50 / B60: AMB_FIELDS_COMMB_MASK of its record */
+    uint8_t commb_outcome[3]; /* B40 / B50 / B60: AMB_FIELDS_COMMB of its record */
+    uint8_t pad0_;        /* 0 */
+    int16_t commb[3][5];  /* B40 / B50 / B60: AMB_FIELDS_COMMB_RAW(0..4) of its record */
+    uint8_t pad_[10];     /* 0 */
+} amb_aircraft_ext;       /* 144 bytes */
+/* The groups' payloads at the byte offsets the record macros use (x is an amb_aircraft_ext*): byte i of OPS is
+ * ((uint8_t*)aux)[i] of its record, so AMB_FIELDS_OPS_NACP reads AMB_AXG_OPS_BYTE(x, 6), AMB_FIELDS_TS_MODES
+ * AMB_AXG_TS_BYTE(x, 12), AMB_FIELDS_POS_NIC_B AMB_AXG_INTEG_BYTE(x, 1); the 16-bit words likewise. */
+#define AMB_AXG_OPS_BYTE(x, i) (((const uint8_t*)(x)->ops)[i])
+#define AMB_AXG_OPS_WORD(x, i) (((const uint16_t*)(x)->ops)[i])      /* 0: capability class, 1: operational mode */
+#define AMB_AXG_TS_BYTE(x, i) (((const uint8_t*)(x)->ts)[i])
+#define AMB_AXG_TS_WORD(x, i) (((const uint16_t*)(x)->ts)[i])        /* 0: selected altitude, 1: baro, 2: heading */
+#define AMB_AXG_INTEG_BYTE(x, i) (((const uint8_t*)(x)->integ)[i])   /* 0: NIC-A, 1: NIC-B, 2: NIC-C */
+#define AMB_AXG_INTEG_RC(x) (((const float*)(x)->integ)[1])          /* containment radius, metres; NaN = unknown */
+#define AMB_AXG_COMMB_RAW(x, g, i) ((x)->commb[g][i])   /* g = 0 (4,0), 1 (5,0), 2 (6,0); raw field i = 0..4 */
+
 typedef struct amb_decoder amb_decoder;
 /* cpr_decoder(my_location) (cpr.py:184-190) + the parser; have_location = 0 is my_location = None. */
 AMB_API int amb_decoder_create(int device, int have_location, double lat, double lon, amb_decoder** out);
@@ -553,6 +605,10 @@ AMB_API int amb_decoder_create(int device, int have_location, double lat, double
  * AMB_FIELDS_ES); applies from the next call. The latest op status per address (2^24 x 24 B = 384 MiB of device memory)
  * is allocated at the first decode with the option on and cleared by amb_decoder_reset. A decode with the option on
  * launches six kernels more; off changes nothing.
+ * "track_ext": S2 = 0 (default, off) .. 3600 seconds, the extension of the per-aircraft table (see amb_aircraft_ext);
+ * applies from the next call, and only while "track" is on too. Rows are direct-mapped by address: 2^24 x 144 B =
+ * 2.25 GiB of device memory plus a 2 MiB bitmap, allocated at the first decode with both options on; only the bitmap is
+ * cleared (by amb_decoder_reset). A decode with both on launches six kernels more; off changes nothing.
  * Unknown names and out-of-range values return AMB_ERR_INVALID. */
 AMB_API int amb_decoder_set_option(amb_decoder* d, const char* name, int value);
 /* Snapshot of the per-aircraft table at time `now`: every row with seen <= now and now - seen <= S, in ascending
@@ -562,10 +618,18 @@ AMB_API int amb_decoder_set_option(amb_decoder* d, const char* name, int value);
  * launches (two when nothing is written) and one 4-byte copy to the host; _device writes to device memory. */
 AMB_API int amb_decoder_aircraft(amb_decoder* d, double now, amb_aircraft* out, int max);
 AMB_API int amb_decoder_aircraft_device(amb_decoder* d, double now, amb_aircraft* out_dev, int cap);
+/* The same snapshot with the extension beside it: out[] is byte for byte what amb_decoder_aircraft writes, ext[i] the
+ * groups of out[i] shown at `now` (see amb_aircraft_ext). out == NULL returns the number of rows; too small a buffer
+ * returns AMB_ERR_OVERFLOW and writes nothing. AMB_ERR_STATE unless both "track" and "track_ext" are on. Three kernel
+ * launches (two when nothing is written) and one 4-byte copy to the host; _device writes both arrays to device memory. */
+AMB_API int amb_decoder_aircraft_ext(amb_decoder* d, double now, amb_aircraft* out, amb_aircraft_ext* ext, int max);
+AMB_API int amb_decoder_aircraft_ext_device(amb_decoder* d, double now, amb_aircraft* out_dev, amb_aircraft_ext* ext_dev,
+                                            int cap);
 AMB_API void amb_decoder_destroy(amb_decoder* d);
 AMB_API int amb_decoder_set_location(amb_decoder* d, int have_location, double lat, double lon);   /* cpr.py:192-193 */
 AMB_API int amb_decoder_reset(amb_decoder* d);                      /* forget every stored report, reference position,
-                                                                       velocity, op status and aircraft */
+                                                                       velocity, op status, aircraft and extension
+                                                                       group */
 /* Decode n frames (host or device array, stream order = non-decreasing time). out: n records in host memory.
  * Frames with passed == 0 get AMB_FS_NOT_QUEUED and do not touch the CPR state. */
 AMB_API int amb_decode_frames(amb_decoder* d, const amb_frame* frames, int n, int mem_kind, amb_fields* out);

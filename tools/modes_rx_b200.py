@@ -13,6 +13,8 @@ of the dl_data feed and are not re-implemented.
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 [-T 7.0] [-d] [-t 5556] [-n] [--reports | -l 37.4,-122.1]
     python tools/modes_rx_b200.py -s 127.0.0.1:12345 -r 4e6 --udp-idle 2.0
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 --track 60 --aircraft aircraft.json
+    python tools/modes_rx_b200.py -s capture.cfile -r 4e6 --track 60 --track-ext 60 --opstatus 30 --commb 30 \
+        --aircraft aircraft.json
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 --reports --commb 30
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 --reports --opstatus 60
 
@@ -110,13 +112,17 @@ class print_queue:
         self.count += 1
 
 
-def write_aircraft(path, rows):
-    """The aircraft table (AIRCRAFT_DTYPE rows) as a JSON list, one object per aircraft (decode.aircraft_to_dict), written
-    to a temporary file beside `path` and renamed over it, so that a reader never sees a half-written file."""
+def write_aircraft(path, rows, ext=None):
+    """The aircraft table (AIRCRAFT_DTYPE rows) as a JSON list, one object per aircraft (decode.aircraft_to_dict, or
+    decode.aircraft_ext_to_dict with the extension rows `ext`), written to a temporary file beside `path` and renamed
+    over it, so that a reader never sees a half-written file."""
     from gr_air_modes_b200 import decode
     tmp = "%s.tmp%d" % (path, os.getpid())
     with open(tmp, "w") as f:
-        json.dump([decode.aircraft_to_dict(r) for r in rows], f)
+        if ext is None:
+            json.dump([decode.aircraft_to_dict(r) for r in rows], f)
+        else:
+            json.dump([decode.aircraft_ext_to_dict(r, x) for r, x in zip(rows, ext)], f)
     os.replace(tmp, path)
 
 
@@ -124,15 +130,17 @@ class report_queue:
     """What apps/modes_rx prints by default: air_modes.output_print(cpr_dec, publisher) (apps/modes_rx:77-78,
     python/msprint.py) - one text report per parsed message. The numbers come from the GPU batch decoder
     (gr_air_modes_b200.decode), the line format from gr_air_modes_b200.report. out=None decodes without printing;
-    aircraft=PATH writes the decoder's aircraft table (option track) to PATH after every batch."""
+    aircraft=PATH writes the decoder's aircraft table (option track) to PATH after every batch, with the extension of
+    every row when track_ext is on."""
 
     def __init__(self, location, device, out=sys.stdout, local_cpr=0, track=0, aircraft=None, decoder=None, commb=0,
-                 opstatus=0):
+                 opstatus=0, track_ext=0):
         from gr_air_modes_b200 import decode
         self._dec = decoder if decoder is not None else \
             decode.batch_decoder(location, device, local_cpr=local_cpr, track=track, commb=commb,
-                                 opstatus=opstatus)   # = cpr_decoder(my_position), apps/modes_rx:68
+                                 opstatus=opstatus, track_ext=track_ext)   # = cpr_decoder(my_position), apps/modes_rx:68
         self._out, self._texts, self.count, self._aircraft = out, [], 0, aircraft
+        self._ext = track_ext > 0
 
     def handle(self, msg):
         text = msg.to_string()
@@ -152,7 +160,9 @@ class report_queue:
             self._texts = []
         if self._out is not None:
             self._out.flush()
-        if self._aircraft:
+        if self._aircraft and self._ext:
+            write_aircraft(self._aircraft, *self._dec.aircraft_ext())
+        elif self._aircraft:
             write_aircraft(self._aircraft, self._dec.aircraft())
 
     def close(self):
@@ -202,18 +212,27 @@ def parse_args(argv=None):
     ap.add_argument("--aircraft", type=str, default=None, metavar="PATH",
                     help="after every chunk, write the aircraft table to PATH as JSON, one object per aircraft "
                          "(needs --track; decodes the messages even without --reports)")
+    ap.add_argument("--track-ext", type=int, default=0, metavar="S",
+                    help="keep beside every aircraft the latest op status, target state, position integrity (with "
+                         "--opstatus) and Comm-B 4,0 / 5,0 / 6,0 (with --commb), each shown for S (1..3600) seconds, and "
+                         "write them with --aircraft (needs --track); 0 = off")
     args = ap.parse_args(argv)
     if not 0 <= args.track <= 3600:
         ap.error("--track: 0 (off) .. 3600 seconds")
     if args.aircraft and args.track <= 0:
         ap.error("--aircraft needs --track S")
+    if not 0 <= args.track_ext <= 3600:
+        ap.error("--track-ext: 0 (off) .. 3600 seconds")
+    if args.track_ext and args.track <= 0:
+        ap.error("--track-ext needs --track S")
+    with_table = bool(args.aircraft and args.track_ext)     # the extension shows what --commb / --opstatus decode
     if not 0 <= args.commb <= 600:
         ap.error("--commb: 0 (off) .. 600 seconds")
-    if args.commb and not (args.reports or args.location is not None):
+    if args.commb and not (args.reports or args.location is not None or with_table):
         ap.error("--commb needs --reports or -l")
     if not 0 <= args.opstatus <= 600:
         ap.error("--opstatus: 0 (off) .. 600 seconds")
-    if args.opstatus and not (args.reports or args.location is not None):
+    if args.opstatus and not (args.reports or args.location is not None or with_table):
         ap.error("--opstatus needs --reports or -l")
     return args
 
@@ -243,14 +262,15 @@ def main(argv=None):
     if not args.no_print:
         if args.reports or args.location is not None:
             reporter = report_queue(my_position, args.device, local_cpr=args.local_cpr, track=args.track, commb=args.commb,
-                                    opstatus=args.opstatus, aircraft=args.aircraft)
+                                    opstatus=args.opstatus, aircraft=args.aircraft, track_ext=args.track_ext)
             sinks.append(reporter)
         else:
             printer = print_queue()
             sinks.append(printer)
     if args.aircraft and reporter is None:                  # the table without printed reports
         reporter = report_queue(my_position, args.device, out=None, local_cpr=args.local_cpr, track=args.track,
-                                aircraft=args.aircraft)
+                                aircraft=args.aircraft, **({"commb": args.commb, "opstatus": args.opstatus,
+                                                            "track_ext": args.track_ext} if args.track_ext else {}))
         sinks.append(reporter)
     pub = None
     if args.tcp is not None:
