@@ -39,6 +39,9 @@ TRACK_MAX = 3600
 AXG_OPS, AXG_TS, AXG_INTEG, AXG_B40, AXG_B50, AXG_B60 = 0x01, 0x02, 0x04, 0x08, 0x10, 0x20
 AXG_N = 6
 TRACK_EXT_MAX = 3600
+# SBS-1 feed (decoder options sbs1, sbs1_tz; include/airmodes_b200.h AMB_SBS1_TZ_*)
+SBS1_TZ_MIN, SBS1_TZ_MAX = -720, 840
+ERR_OVERFLOW = -5                # AMB_ERR_OVERFLOW: the buffer is too small (amb_decoder_sbs1 reports the size needed)
 
 
 class Frame(C.Structure):
@@ -217,6 +220,8 @@ SYMBOLS = [
     ("amb_decoder_aircraft_device", C.c_int, [_vp, C.c_double, _vp, C.c_int]),
     ("amb_decoder_aircraft_ext", C.c_int, [_vp, C.c_double, _vp, _vp, C.c_int]),
     ("amb_decoder_aircraft_ext_device", C.c_int, [_vp, C.c_double, _vp, _vp, C.c_int]),
+    ("amb_decoder_sbs1", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("amb_decoder_sbs1_device", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("amb_decoder_stats", C.c_int, [_vp, _u64p, _f32p]),
     ("amb_decoder_last_error", C.c_char_p, [_vp]),
     ("amb_frame_bits", C.c_uint64, [C.POINTER(Frame), C.c_int, C.c_int]),

@@ -27,6 +27,10 @@
 // amb_track_ext_keys, the four partition kernels on address keys, amb_track_ext_walk - the op-status and Comm-B groups
 // of every address, direct-mapped in HBM (2^24 x 144 B) with an occupancy bitmap; amb_decoder_aircraft_ext reads them
 // out beside the aircraft rows with amb_snap_count, amb_snap_scan and amb_snap_gather_ext.
+// With option "sbs1" on, ten more after every other stage (amb_decode_sbs1.cuh): amb_sbs1_keys, the four partition
+// kernels on address keys, amb_sbs1_walk, amb_sbs1_ids - the aircraft ids of sbs1.py, with a direct-mapped table of the
+// latest id per address in HBM (2^24 x 8 B) carried from batch to batch - and amb_sbs1_format, amb_sbs1_scan,
+// amb_sbs1_gather, which write the call's SBS-1 lines and pack them on the device; amb_decoder_sbs1 copies them out.
 #include "amb_launch.h"
 #include "amb_decode_core.h"
 #include "amb_decode_kernels.cuh"
@@ -51,11 +55,23 @@ struct amb_decoder {
     uint32_t* snap_cnt = nullptr;        // snapshot: per-block counts, then their scan and the total
     amb_aircraft* d_snap = nullptr; int snap_cap = 0;   // snapshot rows on their way to host memory
     amb_aircraft_ext* d_xsnap = nullptr; int xsnap_cap = 0;   // ... and their extensions
+    int scap = 0;                        // frames st.sb holds
+    int sbs1_nb = -1;                    // blocks of lines of the last decode (its byte total is st.sb.boff[sbs1_nb]);
+                                         // -1: the last decode wrote no lines
     uint64_t launches = 0; float ms_last = 0.f;
     std::string err;
 };
 
 static thread_local std::string g_create_err;          // why the last amb_decoder_create on this thread failed
+
+static void free_sbs1_bufs(amb_decoder* d)
+{
+    AmbSbs1Bufs& b = d->st.sb;
+    void* const all[] = {b.src, b.gid, b.flag, b.slots, b.len, b.bsum, b.boff, b.text};
+    for (void* p : all) if (p) cudaFree(p);
+    b = AmbSbs1Bufs();
+    d->scap = 0;
+}
 
 static int dfail(amb_decoder* d, int code, const char* what, cudaError_t e = cudaSuccess)
 {
@@ -205,6 +221,9 @@ void amb_decoder_destroy(amb_decoder* d)
     if (d->st.tclk) cudaFree(d->st.tclk);
     if (d->st.xrows) cudaFree(d->st.xrows);
     if (d->st.xocc) cudaFree(d->st.xocc);
+    free_sbs1_bufs(d);
+    if (d->st.stable) cudaFree(d->st.stable);
+    if (d->st.sctr) cudaFree(d->st.sctr);
     if (d->d_xsnap) cudaFree(d->d_xsnap);
     if (d->snap_cnt) cudaFree(d->snap_cnt);
     if (d->d_snap) cudaFree(d->d_snap);
@@ -238,6 +257,9 @@ int amb_decoder_reset(amb_decoder* d)
         DCK(cudaMemcpyAsync(d->st.tclk, &none, sizeof none, cudaMemcpyHostToDevice, d->stream));
     }
     if (d->st.xocc) DCK(cudaMemsetAsync(d->st.xocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));   // likewise
+    if (d->st.sctr)                      // ids up to G are dead from now on: no table memset
+        DCK(cudaMemcpyAsync(&d->st.sctr->base, &d->st.sctr->G, sizeof(unsigned long long), cudaMemcpyDeviceToDevice,
+                            d->stream));
     DCK(cudaStreamSynchronize(d->stream));
     return AMB_OK;
 }
@@ -252,6 +274,17 @@ int amb_decoder_set_option(amb_decoder* d, const char* name, int value)
         {"track_ext", AMB_TRACK_EXT_MAX, &AmbDecodeState::track_ext},
     };
     if (!d || !name) return AMB_ERR_INVALID;
+    if (strcmp(name, "sbs1") == 0) {
+        if (value != 0 && value != 1) return dfail(d, AMB_ERR_INVALID, "sbs1: 0 (off) or 1 (on)");
+        d->st.sbs1 = value;
+        return AMB_OK;
+    }
+    if (strcmp(name, "sbs1_tz") == 0) {
+        if (value < AMB_SBS1_TZ_MIN || value > AMB_SBS1_TZ_MAX)
+            return dfail(d, AMB_ERR_INVALID, "sbs1_tz: -720 .. 840 minutes");
+        d->st.sbs1_tz = value;
+        return AMB_OK;
+    }
     for (const auto& o : options) {
         if (strcmp(name, o.name) != 0) continue;
         if (value < 0 || value > o.max) {
@@ -345,6 +378,36 @@ static int ensure_track_ext(amb_decoder* d)
     return AMB_OK;
 }
 
+// the SBS-1 stage's device memory: the id table and counter at the first decode with the option on (the table starts
+// with no id, the counter at 0), the per-frame scratch as the frame capacity grows
+static int ensure_sbs1(amb_decoder* d)
+{
+    if (!d->st.stable) {
+        cudaError_t e = cudaMalloc(&d->st.stable, (size_t)AMB_SBS1_SLOTS * sizeof(unsigned long long));
+        if (e != cudaSuccess) { d->st.stable = nullptr; return dfail(d, AMB_ERR_CUDA, "SBS-1 id table (128 MiB)", e); }
+        DCK(cudaMemsetAsync(d->st.stable, 0, (size_t)AMB_SBS1_SLOTS * sizeof(unsigned long long), d->stream));
+    }
+    if (!d->st.sctr) {
+        DCK(cudaMalloc(&d->st.sctr, sizeof(AmbSbs1Ctr)));
+        DCK(cudaMemsetAsync(d->st.sctr, 0, sizeof(AmbSbs1Ctr), d->stream));
+    }
+    if (d->scap < d->cap) {
+        free_sbs1_bufs(d);
+        const size_t n = (size_t)d->cap, nb = (n + 127) / 128, chunks = (n + AMB_SBS1_CHUNK - 1) / AMB_SBS1_CHUNK;
+        AmbSbs1Bufs& b = d->st.sb;
+        DCK(cudaMalloc(&b.src, n * sizeof(unsigned long long)));
+        DCK(cudaMalloc(&b.gid, n * sizeof(unsigned long long)));
+        DCK(cudaMalloc(&b.flag, chunks * sizeof(unsigned long long)));
+        DCK(cudaMalloc(&b.slots, n * AMB_SBS1_STRIDE));
+        DCK(cudaMalloc(&b.len, n * sizeof(uint32_t)));
+        DCK(cudaMalloc(&b.bsum, nb * sizeof(uint32_t)));
+        DCK(cudaMalloc(&b.boff, (nb + 1) * sizeof(unsigned long long)));
+        DCK(cudaMalloc(&b.text, n * AMB_SBS1_STRIDE));
+        d->scap = d->cap;
+    }
+    return ensure_keys(d);
+}
+
 static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_kind, amb_fields* out, bool out_on_device);
 
 int amb_decode_frames(amb_decoder* d, const amb_frame* frames, int n, int mem_kind, amb_fields* out)
@@ -363,14 +426,16 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
 {
     if (!d || n < 0 || (n > 0 && (!frames || !out)) || (mem_kind != AMB_MEM_HOST && mem_kind != AMB_MEM_DEVICE))
         return dfail(d, AMB_ERR_INVALID, "amb_decode_frames: bad argument");
-    if (n == 0) return AMB_OK;
+    if (n == 0) { d->sbs1_nb = -1; return AMB_OK; }
     DCK(cudaSetDevice(d->device));
+    d->sbs1_nb = -1;
     int rc = ensure_cap(d, n);
     if (rc == AMB_OK && d->st.local_cpr > 0) rc = ensure_local(d);
     if (rc == AMB_OK && d->st.commb > 0) rc = ensure_commb(d);
     if (rc == AMB_OK && d->st.opstatus > 0) rc = ensure_opstatus(d);
     if (rc == AMB_OK && d->st.track > 0) rc = ensure_track(d);
     if (rc == AMB_OK && d->st.track > 0 && d->st.track_ext > 0) rc = ensure_track_ext(d);
+    if (rc == AMB_OK && d->st.sbs1 > 0) rc = ensure_sbs1(d);
     if (rc != AMB_OK) return rc;
     cudaStream_t s = d->stream;
     amb_fields* const fields = out_on_device ? out : d->d_fields;
@@ -386,10 +451,11 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
     if (k < 0) {
         static const char* const stage[] = {"cudaGetLastError()", "pairing", "cudaGetLastError()", "local CPR",
                                             "Comm-B inference", "aircraft table", "op status",
-                                            "aircraft table extension"};   // by -AMB_STAGE_* - 1
+                                            "aircraft table extension", "SBS-1 feed"};   // by -AMB_STAGE_* - 1
         return dfail(d, AMB_ERR_CUDA, stage[-k - 1], e);
     }
     d->launches += (uint64_t)k;
+    if (d->st.sbs1 > 0) d->sbs1_nb = (n + 127) / 128;
     if (!out_on_device) {
         rc = staged_d2h(d, out, d->d_fields, (size_t)n * sizeof(amb_fields), s);
         if (rc != AMB_OK) return rc;
@@ -480,6 +546,40 @@ int amb_decoder_aircraft_ext(amb_decoder* d, double now, amb_aircraft* out, amb_
 int amb_decoder_aircraft_ext_device(amb_decoder* d, double now, amb_aircraft* out_dev, amb_aircraft_ext* ext_dev, int cap)
 {
     return snapshot_impl(d, now, out_dev, ext_dev, cap, true, true);
+}
+
+// the last decode's lines into out (host or device memory)
+static int sbs1_impl(amb_decoder* d, char* out, size_t cap, size_t* n_bytes, bool out_on_device)
+{
+    if (!d || !n_bytes || (cap > 0 && !out)) return dfail(d, AMB_ERR_INVALID, "amb_decoder_sbs1: bad argument");
+    *n_bytes = 0;
+    if (d->st.sbs1 <= 0) return dfail(d, AMB_ERR_STATE, "amb_decoder_sbs1: option sbs1 is off");
+    if (d->sbs1_nb < 0) return AMB_OK;                   // no decode with the option on since it was set
+    DCK(cudaSetDevice(d->device));
+    cudaStream_t s = d->stream;
+    unsigned long long total = 0;
+    DCK(cudaMemcpyAsync(&total, d->st.sb.boff + d->sbs1_nb, sizeof total, cudaMemcpyDeviceToHost, s));
+    DCK(cudaStreamSynchronize(s));
+    *n_bytes = (size_t)total;
+    if (total > cap) return dfail(d, AMB_ERR_OVERFLOW, "amb_decoder_sbs1: output buffer too small");
+    if (total == 0) return AMB_OK;
+    if (out_on_device) DCK(cudaMemcpyAsync(out, d->st.sb.text, (size_t)total, cudaMemcpyDeviceToDevice, s));
+    else {
+        int rc = staged_d2h(d, out, d->st.sb.text, (size_t)total, s);
+        if (rc != AMB_OK) return rc;
+    }
+    DCK(cudaStreamSynchronize(s));
+    return AMB_OK;
+}
+
+int amb_decoder_sbs1(amb_decoder* d, char* out, size_t cap, size_t* n_bytes)
+{
+    return sbs1_impl(d, out, cap, n_bytes, false);
+}
+
+int amb_decoder_sbs1_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes)
+{
+    return sbs1_impl(d, out_dev, cap, n_bytes, true);
 }
 
 int amb_decoder_stats(amb_decoder* d, uint64_t* kernel_launches, float* ms_last)

@@ -46,6 +46,7 @@ __global__ void __launch_bounds__(128) amb_resolve_kernel(amb_fields* __restrict
 #include "amb_decode_opstatus.cuh"
 #include "amb_decode_track.cuh"
 #include "amb_decode_track_ext.cuh"
+#include "amb_decode_sbs1.cuh"
 
 // ---- launch sequence ----------------------------------------------------------------------------------------------
 // What the stages of one decode read and write besides the frames and the records: amb_decoder keeps one in device
@@ -69,17 +70,23 @@ struct AmbDecodeState {
     int track_ext = 0;                   // option "track_ext" = S2 seconds, 0 = off; runs only while track is on too
     amb_aircraft_ext* xrows = nullptr;   // one extension row per address, AMB_TRACK_ROWS
     unsigned* xocc = nullptr;            // which extension rows were written since reset, AMB_TRACK_WORDS
+    int sbs1 = 0;                        // option "sbs1": 1 = on, 0 = off
+    int sbs1_tz = 0;                     // option "sbs1_tz": minutes added to UTC in the lines' date and time
+    unsigned long long* stable = nullptr;   // latest aircraft id per address (a global value, 0 = none), AMB_SBS1_SLOTS
+    AmbSbs1Ctr* sctr = nullptr;          // the id counter and the base recorded at reset
+    AmbSbs1Bufs sb;                      // the stage's per-call scratch and the packed lines, one entry per frame
     int have_loc = 0; double lat = 0.0, lon = 0.0;      // receiver location
 };
 
 // What amb_decode_launch returns when a stage fails to launch.
 enum { AMB_STAGE_FIELDS = -1, AMB_STAGE_PAIRING = -2, AMB_STAGE_RESOLVE = -3, AMB_STAGE_LOCAL = -4,
-       AMB_STAGE_COMMB = -5, AMB_STAGE_TRACK = -6, AMB_STAGE_OPSTATUS = -7, AMB_STAGE_TRACK_EXT = -8 };
+       AMB_STAGE_COMMB = -5, AMB_STAGE_TRACK = -6, AMB_STAGE_OPSTATUS = -7, AMB_STAGE_TRACK_EXT = -8,
+       AMB_STAGE_SBS1 = -9 };
 
 // Enqueue one decode of the n frames into the n records on stream s, in this order: fields, pairing, resolve, then the
 // local CPR, Comm-B, op-status and track stages whose S is > 0, and the track extension when track and track_ext are
-// both > 0. Returns how many kernels were launched (7, plus 6 per stage that is on), or an AMB_STAGE_* code with *err
-// set.
+// both > 0, then the SBS-1 feed when sbs1 is on. Returns how many kernels were launched (7, plus 6 per stage that is
+// on, plus 10 for the SBS-1 feed), or an AMB_STAGE_* code with *err set.
 static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n, amb_fields* fields, cudaStream_t s,
                              cudaError_t* err)
 {
@@ -118,6 +125,12 @@ static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n,
             if (kx < 0) return AMB_STAGE_TRACK_EXT;
             k += kx;
         }
+    }
+    if (st->sbs1 > 0) {
+        const int ks = amb_sbs1_launch(&st->v3, frames, fields, st->keys, n, st->stable, st->sctr, &st->sb, st->sbs1_tz,
+                                       s, err);
+        if (ks < 0) return AMB_STAGE_SBS1;
+        k += ks;
     }
     return k;
 }

@@ -47,6 +47,8 @@ TRACK_MAX = _lib.TRACK_MAX
 AXG_OPS, AXG_TS, AXG_INTEG, AXG_B40, AXG_B50, AXG_B60 = (
     _lib.AXG_OPS, _lib.AXG_TS, _lib.AXG_INTEG, _lib.AXG_B40, _lib.AXG_B50, _lib.AXG_B60)
 TRACK_EXT_MAX = _lib.TRACK_EXT_MAX
+# SBS-1 feed (decoder options sbs1 and sbs1_tz; include/airmodes_b200.h AMB_SBS1_TZ_*)
+SBS1_TZ_MIN, SBS1_TZ_MAX = _lib.SBS1_TZ_MIN, _lib.SBS1_TZ_MAX
 
 FIELDS_DTYPE = np.dtype(Fields)
 FRAME_DTYPE = np.dtype(Frame)
@@ -114,6 +116,25 @@ def check_track(seconds) -> int:
 
 def check_opstatus(seconds) -> int:
     return check_option("opstatus", seconds)
+
+
+def check_sbs1(on) -> int:
+    """Validate a setting of decoder option sbs1: False / True or 0 / 1. Raises ValueError otherwise."""
+    if isinstance(on, (bool, np.bool_)) or (isinstance(on, (int, np.integer)) and int(on) in (0, 1)):
+        return int(on)
+    raise ValueError("sbs1: False / True (0 / 1), got %r" % (on,))
+
+
+def check_sbs1_tz(minutes) -> int:
+    """Validate a setting of decoder option sbs1_tz: an int in SBS1_TZ_MIN .. SBS1_TZ_MAX minutes. Raises ValueError
+    otherwise."""
+    try:
+        ok = not isinstance(minutes, bool) and int(minutes) == minutes and SBS1_TZ_MIN <= int(minutes) <= SBS1_TZ_MAX
+    except (TypeError, ValueError):
+        ok = False
+    if not ok:
+        raise ValueError("sbs1_tz: an integer number of minutes in %d .. %d, got %r" % (SBS1_TZ_MIN, SBS1_TZ_MAX, minutes))
+    return int(minutes)
 
 
 def commb_outcome(records):
@@ -284,13 +305,18 @@ class batch_decoder:
     or its NUCp; read with opstatus_outcome() / opstatus_values() (DESIGN.md §8 "Operational status and NIC").
     track_ext = S2 > 0, with track on, also keeps beside every aircraft row the latest op status, target state, position
     integrity and Comm-B 4,0 / 5,0 / 6,0 of the address, each shown for S2 seconds; read with aircraft_ext() /
-    aircraft_ext_device() (DESIGN.md §8 "Aircraft table extension")."""
+    aircraft_ext_device() (DESIGN.md §8 "Aircraft table extension").
+    sbs1 = True also writes, on the device, the SBS-1 (BaseStation) lines the reference's output_sbs1 would send for the
+    decoded messages, with aircraft ids carried from call to call and the date and time of each frame's stamp shifted
+    by sbs1_tz minutes; read the last decode's lines with sbs1_text() / sbs1_text_device() (DESIGN.md §8 "SBS-1
+    feed")."""
 
     def __init__(self, my_location=None, device: int = 0, local_cpr: int = 0, track: int = 0, commb: int = 0,
-                 opstatus: int = 0, track_ext: int = 0):
+                 opstatus: int = 0, track_ext: int = 0, sbs1=False, sbs1_tz: int = 0):
         settings = {"local_cpr": check_option("local_cpr", local_cpr), "track": check_option("track", track),
                     "commb": check_option("commb", commb), "opstatus": check_option("opstatus", opstatus),
                     "track_ext": check_option("track_ext", track_ext)}
+        sbs1, sbs1_tz = check_sbs1(sbs1), check_sbs1_tz(sbs1_tz)
         self._lib = _lib.load()
         h = C.c_void_p()
         have, lat, lon = self._loc(my_location)
@@ -305,6 +331,11 @@ class batch_decoder:
         for name, seconds in settings.items():
             if seconds:
                 self._set_option(name, seconds)
+        self._sbs1, self._sbs1_tz = 0, 0
+        if sbs1:
+            self.set_sbs1(True)
+        if sbs1_tz:
+            self.set_sbs1_tz(sbs1_tz)
 
     @staticmethod
     def _loc(loc):
@@ -365,6 +396,49 @@ class batch_decoder:
 
     def get_track_ext(self) -> int:
         return self._options["track_ext"]
+
+    def set_sbs1(self, on):
+        """Option sbs1 on (True) or off (False); applies from the next decode."""
+        on = check_sbs1(on)
+        self._check(self._lib.amb_decoder_set_option(self._h, b"sbs1", on))
+        self._sbs1 = on
+
+    def get_sbs1(self) -> bool:
+        return bool(self._sbs1)
+
+    def set_sbs1_tz(self, minutes: int):
+        """Option sbs1_tz = minutes added to UTC in the SBS-1 date and time (0 = UTC); applies from the next decode."""
+        minutes = check_sbs1_tz(minutes)
+        self._check(self._lib.amb_decoder_set_option(self._h, b"sbs1_tz", minutes))
+        self._sbs1_tz = minutes
+
+    def get_sbs1_tz(self) -> int:
+        return self._sbs1_tz
+
+    def sbs1_text(self) -> bytes:
+        """The SBS-1 lines of the last decode, concatenated ("\\r\\n" after each). Needs the option sbs1 on."""
+        n = C.c_size_t()
+        rc = self._lib.amb_decoder_sbs1(self._h, None, 0, C.byref(n))
+        if rc == _lib.ERR_OVERFLOW:
+            buf = C.create_string_buffer(n.value)
+            self._check(self._lib.amb_decoder_sbs1(self._h, buf, n.value, C.byref(n)))
+            return buf.raw[: n.value]
+        self._check(rc)
+        return b""
+
+    def sbs1_text_device(self, out_dev) -> int:
+        """sbs1_text() into out_dev, a CUDA uint8 tensor; returns the byte count. Only the count crosses PCIe. Raises
+        RuntimeError (with the size needed) when out_dev is too small."""
+        import torch
+        if out_dev.dtype != torch.uint8 or not out_dev.is_cuda or not out_dev.is_contiguous():
+            raise ValueError("sbs1_text_device: out_dev must be a contiguous CUDA uint8 tensor")
+        n = C.c_size_t()
+        torch.cuda.current_stream(out_dev.device).synchronize()          # the decoder runs on its own stream
+        rc = self._lib.amb_decoder_sbs1_device(self._h, C.c_void_p(out_dev.data_ptr()), int(out_dev.numel()), C.byref(n))
+        if rc == _lib.ERR_OVERFLOW:
+            raise RuntimeError("sbs1_text_device: %d bytes needed, out_dev holds %d" % (n.value, out_dev.numel()))
+        self._check(rc)
+        return int(n.value)
 
     @staticmethod
     def _now(now):

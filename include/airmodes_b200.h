@@ -587,6 +587,29 @@ typedef struct amb_aircraft_ext {
 #define AMB_AXG_INTEG_RC(x) (((const float*)(x)->integ)[1])          /* containment radius, metres; NaN = unknown */
 #define AMB_AXG_COMMB_RAW(x, g, i) ((x)->commb[g][i])   /* g = 0 (4,0), 1 (5,0), 2 (6,0); raw field i = 0..4 */
 
+/* SBS-1 (BaseStation) feed (amb_decoder_set_option(d, "sbs1", 1)): every decode also writes the lines that the
+ * reference's output_sbs1 (python/sbs1.py, modes_rx -P) would send for its records, in record order, continuing across
+ * calls since the last amb_decoder_reset. t = secs + frac of the record's frame.
+ *   published  a record counts when its frame was queued, its status lacks AMB_FS_NO_HANDLER, its df is 0, 4, 5, 11 or
+ *              17 and its icao fits in 24 bits; icao is the address (the AP syndrome for DF0/4/5, AA for DF11/17).
+ *   ids        every published record takes an aircraft id before anything else, as get_aircraft_id (sbs1.py:73-90):
+ *              with n ids handed out since the reset, the address's id is live when it was assigned since the reset and
+ *              id > n - 10000; a live id is reused, otherwise the record gets n + 1 (the first id after a reset is 1).
+ *   lines      MSG,7 (DF0), MSG,5 (DF4), MSG,6 (DF5), MSG,8 (DF11), MSG,1 (BDS0,8), MSG,2 (BDS0,6), MSG,3 (BDS0,5),
+ *              MSG,4 (BDS0,9 subtype 1), each ending in "\r\n", field for field as pp0 .. pp17 format them (%.5f / %.1f
+ *              round the exact binary value half to even, %i of a float truncates). No line, but an id is taken, for
+ *              DF0/4 with AMB_FS_METRIC_ALT, BDS0,5 / 0,6 without AMB_FS_HAS_POS (a local fix counts), BDS0,9 subtypes 0
+ *              and 3, BDS6,1 and BDS0,8 whose cat is out of range for its ftc.
+ *   date/time  from the frame's stamp, not a wall clock: secs += int(frac), frac -= int(frac); milliseconds
+ *              max(0, min(999, floor(frac * 1000))) (a negative frac counts as 0); the proleptic Gregorian date of
+ *              secs + 60 * sbs1_tz. Outside 1970-01-01 .. 9999-12-31 23:59:59, or for a frac that is not finite, the four
+ *              date/time fields are empty.
+ * The ids live in a direct-mapped table in device memory (2^24 x 8 B = 128 MiB), allocated at the first decode with the
+ * option on; a reset only records where the ids of the new stream begin. A decode with the option on launches ten
+ * kernels more; with it off nothing changes. */
+#define AMB_SBS1_TZ_MIN (-720)
+#define AMB_SBS1_TZ_MAX 840
+
 typedef struct amb_decoder amb_decoder;
 /* cpr_decoder(my_location) (cpr.py:184-190) + the parser; have_location = 0 is my_location = None. */
 AMB_API int amb_decoder_create(int device, int have_location, double lat, double lon, amb_decoder** out);
@@ -609,6 +632,8 @@ AMB_API int amb_decoder_create(int device, int have_location, double lat, double
  * applies from the next call, and only while "track" is on too. Rows are direct-mapped by address: 2^24 x 144 B =
  * 2.25 GiB of device memory plus a 2 MiB bitmap, allocated at the first decode with both options on; only the bitmap is
  * cleared (by amb_decoder_reset). A decode with both on launches six kernels more; off changes nothing.
+ * "sbs1": 0 (default, off) or 1, the SBS-1 feed (see AMB_SBS1_TZ_MIN); applies from the next call.
+ * "sbs1_tz": AMB_SBS1_TZ_MIN .. AMB_SBS1_TZ_MAX minutes (default 0, UTC) added to the stamp in the SBS-1 date and time.
  * Unknown names and out-of-range values return AMB_ERR_INVALID. */
 AMB_API int amb_decoder_set_option(amb_decoder* d, const char* name, int value);
 /* Snapshot of the per-aircraft table at time `now`: every row with seen <= now and now - seen <= S, in ascending
@@ -625,6 +650,12 @@ AMB_API int amb_decoder_aircraft_device(amb_decoder* d, double now, amb_aircraft
 AMB_API int amb_decoder_aircraft_ext(amb_decoder* d, double now, amb_aircraft* out, amb_aircraft_ext* ext, int max);
 AMB_API int amb_decoder_aircraft_ext_device(amb_decoder* d, double now, amb_aircraft* out_dev, amb_aircraft_ext* ext_dev,
                                             int cap);
+/* The SBS-1 lines of the last decode, concatenated, into out (cap bytes; no terminator); *n_bytes = their length.
+ * AMB_ERR_STATE when the option "sbs1" is off; a buffer of fewer than *n_bytes bytes returns AMB_ERR_OVERFLOW with
+ * nothing written (out may then be NULL with cap 0). One 8-byte copy to the host, then the text; _device copies the text
+ * to device memory instead, so only the byte count crosses PCIe. */
+AMB_API int amb_decoder_sbs1(amb_decoder* d, char* out, size_t cap, size_t* n_bytes);
+AMB_API int amb_decoder_sbs1_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes);
 AMB_API void amb_decoder_destroy(amb_decoder* d);
 AMB_API int amb_decoder_set_location(amb_decoder* d, int have_location, double lat, double lon);   /* cpr.py:192-193 */
 AMB_API int amb_decoder_reset(amb_decoder* d);                      /* forget every stored report, reference position,

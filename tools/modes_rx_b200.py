@@ -7,8 +7,10 @@ gr_complex), and the same two outlets for the slicer's messages: printed to stdo
 ("<hex> <crc> <ref> <secs> <frac>", what lands on the gr.msg_queue) and published as ZMQ "dl_data"
 (radio.py:79-87) on tcp://*:PORT with -t. With --reports / -l LAT,LON stdout carries what apps/modes_rx prints by
 default instead: the text reports of python/msprint.py, decoded on the GPU (gr_air_modes_b200.decode: parse.py,
-altitude.py, cpr.py for whole batches). KML, SBS-1 and FlightGear outputs are the reference's own pure-Python consumers
-of the dl_data feed and are not re-implemented.
+altitude.py, cpr.py for whole batches). With -P [PORT] the SBS-1 (BaseStation) feed of apps/modes_rx -P is served on
+TCP port PORT (default 30003): the lines are formed on the GPU by the decoder (gr_air_modes_b200.decode, option sbs1)
+with the date and time of each message's stamp in the host's local time, and sent by gr_air_modes_b200.sbs1. KML and
+FlightGear outputs are the reference's own pure-Python consumers of the dl_data feed and are not re-implemented.
 
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 [-T 7.0] [-d] [-t 5556] [-n] [--reports | -l 37.4,-122.1]
     python tools/modes_rx_b200.py -s 127.0.0.1:12345 -r 4e6 --udp-idle 2.0
@@ -17,6 +19,7 @@ of the dl_data feed and are not re-implemented.
         --aircraft aircraft.json
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 --reports --commb 30
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 --reports --opstatus 60
+    python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -l 37.4,-122.1 -P 30003
 
 Differences, all on the far side of rx_path:
 * live radios (-s uhd / osmocom) need GNU Radio: use gr_air_modes_b200.gr_adapter.rx_path inside modes_radio.
@@ -131,16 +134,19 @@ class report_queue:
     python/msprint.py) - one text report per parsed message. The numbers come from the GPU batch decoder
     (gr_air_modes_b200.decode), the line format from gr_air_modes_b200.report. out=None decodes without printing;
     aircraft=PATH writes the decoder's aircraft table (option track) to PATH after every batch, with the extension of
-    every row when track_ext is on."""
+    every row when track_ext is on; sbs1=server (gr_air_modes_b200.sbs1.sbs1_server) sends the batch's SBS-1 lines to
+    it, with the date and time shifted by sbs1_tz minutes."""
 
     def __init__(self, location, device, out=sys.stdout, local_cpr=0, track=0, aircraft=None, decoder=None, commb=0,
-                 opstatus=0, track_ext=0):
+                 opstatus=0, track_ext=0, sbs1=None, sbs1_tz=0):
         from gr_air_modes_b200 import decode
         self._dec = decoder if decoder is not None else \
             decode.batch_decoder(location, device, local_cpr=local_cpr, track=track, commb=commb,
-                                 opstatus=opstatus, track_ext=track_ext)   # = cpr_decoder(my_position), apps/modes_rx:68
+                                 opstatus=opstatus, track_ext=track_ext, sbs1=sbs1 is not None,
+                                 sbs1_tz=sbs1_tz)   # = cpr_decoder(my_position), apps/modes_rx:68
         self._out, self._texts, self.count, self._aircraft = out, [], 0, aircraft
         self._ext = track_ext > 0
+        self._sbs1 = sbs1
 
     def handle(self, msg):
         text = msg.to_string()
@@ -153,6 +159,8 @@ class report_queue:
         from gr_air_modes_b200 import report
         if self._texts:
             recs = self._dec.decode_messages(self._texts)
+            if self._sbs1 is not None:
+                self._sbs1.send(self._dec.sbs1_text())
             if self._out is not None:
                 for line in report.report_lines(self._texts, recs):
                     self._out.write(line + "\n")
@@ -167,6 +175,16 @@ class report_queue:
 
     def close(self):
         self._dec.close()
+        if self._sbs1 is not None:
+            self._sbs1.close()
+
+
+def local_utc_offset_minutes() -> int:
+    """The host's current UTC offset in minutes, as datetime.now() writes local time in the reference's lines
+    (sbs1.py:113-115), within the decoder's -720 .. 840."""
+    import datetime
+    off = datetime.datetime.now().astimezone().utcoffset()
+    return max(-720, min(840, int(off.total_seconds() // 60)))
 
 
 def parse_args(argv=None):
@@ -216,7 +234,19 @@ def parse_args(argv=None):
                     help="keep beside every aircraft the latest op status, target state, position integrity (with "
                          "--opstatus) and Comm-B 4,0 / 5,0 / 6,0 (with --commb), each shown for S (1..3600) seconds, and "
                          "write them with --aircraft (needs --track); 0 = off")
+    ap.add_argument("-P", "--sbs1", type=int, nargs="?", const=30003, default=None, metavar="PORT",
+                    help="serve the SBS-1 (BaseStation) feed on TCP port PORT (default 30003), as apps/modes_rx -P; "
+                         "decodes the messages even without --reports")                                          # apps/modes_rx:48,84-85
+    ap.add_argument("--sbs1-wait", type=float, default=0.0, metavar="S",
+                    help="with -P: wait up to S seconds for the first SBS-1 client before reading the source (for "
+                         "replaying a recording); 0 = start at once, as modes_rx")
     args = ap.parse_args(argv)
+    if args.sbs1 is not None and not 0 < args.sbs1 < 65536:
+        ap.error("--sbs1: a TCP port 1 .. 65535")
+    if not 0 <= args.sbs1_wait <= 3600:
+        ap.error("--sbs1-wait: 0 .. 3600 seconds")
+    if args.sbs1_wait and args.sbs1 is None:
+        ap.error("--sbs1-wait needs -P")
     if not 0 <= args.track <= 3600:
         ap.error("--track: 0 (off) .. 3600 seconds")
     if args.aircraft and args.track <= 0:
@@ -259,18 +289,26 @@ def main(argv=None):
     printer = None
     reporter = None
     my_position = [float(x) for x in args.location.split(",")] if args.location is not None else None   # apps/modes_rx:64-65
+    server = None
+    if args.sbs1 is not None:
+        from gr_air_modes_b200.sbs1 import sbs1_server
+        server = sbs1_server(args.sbs1)                                                                            # apps/modes_rx:84-85
+        if args.sbs1_wait and not server.wait_for_client(args.sbs1_wait):
+            print("# no SBS-1 client within %g s, starting anyway" % args.sbs1_wait, file=sys.stderr)
+    feed = {"sbs1": server, "sbs1_tz": local_utc_offset_minutes()} if server is not None else {}
     if not args.no_print:
         if args.reports or args.location is not None:
             reporter = report_queue(my_position, args.device, local_cpr=args.local_cpr, track=args.track, commb=args.commb,
-                                    opstatus=args.opstatus, aircraft=args.aircraft, track_ext=args.track_ext)
+                                    opstatus=args.opstatus, aircraft=args.aircraft, track_ext=args.track_ext, **feed)
             sinks.append(reporter)
         else:
             printer = print_queue()
             sinks.append(printer)
-    if args.aircraft and reporter is None:                  # the table without printed reports
+    if (args.aircraft or server is not None) and reporter is None:   # the table or the feed without printed reports
         reporter = report_queue(my_position, args.device, out=None, local_cpr=args.local_cpr, track=args.track,
                                 aircraft=args.aircraft, **({"commb": args.commb, "opstatus": args.opstatus,
-                                                            "track_ext": args.track_ext} if args.track_ext else {}))
+                                                            "track_ext": args.track_ext} if args.track_ext else {}),
+                                **feed)
         sinks.append(reporter)
     pub = None
     if args.tcp is not None:
