@@ -1,8 +1,9 @@
 // Batch field decode (SURVEY.md 8 row f4): kernels + C ABI of amb_decoder (include/airmodes_b200.h).
-// The per-message arithmetic is in amb_decode_core.h, the kernels and amb_decode_launch - the one launch sequence of a
-// decode - in amb_decode_kernels.cuh and the stage headers it includes (launch-free headers, so that tests/simt can run
-// the same kernel source and sequence under a host emulator); this file allocates the tables and buffers the stages
-// need, copies the frames in and the records out. Compiled with -fmad=false: latitude/longitude follow cpr.py
+// The per-message arithmetic is in amb_decode_core.h, the kernels, amb_decode_launch - the one launch sequence of a
+// decode - and the stages' memory (amb_decode_prepare / amb_decode_reset / amb_decode_free) in amb_decode_kernels.cuh
+// and the stage headers it includes (launch-free headers, so that tests/simt can run the same kernel source, sequence
+// and memory rules under a host emulator); this file keeps the frames, records and snapshot rows on their way between
+// the caller and the stages, copies the frames in and the records out. Compiled with -fmad=false: latitude/longitude follow cpr.py
 // operation by operation in IEEE double, nothing may be contracted. Citations are file:line under gr-air-modes/python.
 //
 // Seven launches per decode, in stream order:
@@ -45,17 +46,14 @@ struct amb_decoder {
     int device = 0;
     cudaStream_t stream = nullptr;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
-    AmbDecodeState st;                   // the stages' tables, scratch and options (amb_decode_kernels.cuh)
+    AmbDecodeState st;                   // the stages' memory and options (amb_decode_kernels.cuh)
     amb_frame* d_frames = nullptr; amb_fields* d_fields = nullptr;
-    int cap = 0;                         // frames d_frames, d_fields, st.pos and st.pair hold
-    int kcap = 0;                        // frames st.keys holds
+    int cap = 0;                         // frames d_frames and d_fields hold
     // host <-> device staging: pageable caller arrays go through two pinned bounce buffers per direction so that the
     // copies run at PCIe speed and overlap the memcpy of the next piece
     void* pin[2] = {nullptr, nullptr}; cudaEvent_t pin_ev[2] = {nullptr, nullptr}; size_t pin_bytes = 0;
-    uint32_t* snap_cnt = nullptr;        // snapshot: per-block counts, then their scan and the total
     amb_aircraft* d_snap = nullptr; int snap_cap = 0;   // snapshot rows on their way to host memory
     amb_aircraft_ext* d_xsnap = nullptr; int xsnap_cap = 0;   // ... and their extensions
-    int scap = 0;                        // frames st.sb holds
     int sbs1_nb = -1;                    // blocks of lines of the last decode (its byte total is st.sb.boff[sbs1_nb]);
                                          // -1: the last decode wrote no lines
     uint64_t launches = 0; float ms_last = 0.f;
@@ -63,15 +61,6 @@ struct amb_decoder {
 };
 
 static thread_local std::string g_create_err;          // why the last amb_decoder_create on this thread failed
-
-static void free_sbs1_bufs(amb_decoder* d)
-{
-    AmbSbs1Bufs& b = d->st.sb;
-    void* const all[] = {b.src, b.gid, b.flag, b.slots, b.len, b.bsum, b.boff, b.text};
-    for (void* p : all) if (p) cudaFree(p);
-    b = AmbSbs1Bufs();
-    d->scap = 0;
-}
 
 static int dfail(amb_decoder* d, int code, const char* what, cudaError_t e = cudaSuccess)
 {
@@ -90,7 +79,7 @@ static int dfail(amb_decoder* d, int code, const char* what, cudaError_t e = cud
 extern "C" void amb_parallel_memcpy(void* dst, const void* src, size_t n);      // amb_api.cu (the ingest copy threads)
 #define AMB_DEC_PIECE ((size_t)8 << 20)
 
-static int ensure_pinned(amb_decoder* d)
+static int alloc_pinned(amb_decoder* d)
 {
     if (d->pin[0]) return AMB_OK;
     for (int k = 0; k < 2; k++) {
@@ -104,7 +93,7 @@ static int ensure_pinned(amb_decoder* d)
 // pageable host -> device through the pinned pieces (memcpy of piece k+1 overlaps the DMA of piece k)
 static int staged_h2d(amb_decoder* d, void* dst, const void* src, size_t bytes, cudaStream_t s)
 {
-    int rc = ensure_pinned(d); if (rc) return rc;
+    int rc = alloc_pinned(d); if (rc) return rc;
     size_t off = 0; int k = 0;
     while (off < bytes) {
         const size_t m = bytes - off < AMB_DEC_PIECE ? bytes - off : AMB_DEC_PIECE;
@@ -120,7 +109,7 @@ static int staged_h2d(amb_decoder* d, void* dst, const void* src, size_t bytes, 
 // device -> pageable host: the DMA of piece i overlaps the memcpy of piece i-1 out of its pinned buffer
 static int staged_d2h(amb_decoder* d, void* dst, const void* src, size_t bytes, cudaStream_t s)
 {
-    int rc = ensure_pinned(d); if (rc) return rc;
+    int rc = alloc_pinned(d); if (rc) return rc;
     const size_t np = (bytes + AMB_DEC_PIECE - 1) / AMB_DEC_PIECE;
     for (size_t i = 0; i <= np; i++) {
         if (i < np) {
@@ -141,22 +130,21 @@ static void free_bufs(amb_decoder* d)
 {
     if (d->d_frames) cudaFree(d->d_frames);
     if (d->d_fields) cudaFree(d->d_fields);
-    if (d->st.pos) cudaFree(d->st.pos);
-    if (d->st.pair) cudaFree(d->st.pair);
-    d->d_frames = nullptr; d->d_fields = nullptr; d->st.pos = nullptr; d->st.pair = nullptr; d->cap = 0;
+    d->d_frames = nullptr; d->d_fields = nullptr; d->cap = 0;
 }
 
-static int ensure_cap(amb_decoder* d, int n)
+// the stages' memory for n frames (amb_decode_prepare), and the frames and records as many as the stages hold
+static int prepare(amb_decoder* d, int n)
 {
-    if (n <= d->cap) return AMB_OK;
-    int cap = d->cap ? d->cap : 4096;
-    while (cap < n) cap *= 2;
-    free_bufs(d);
-    DCK(cudaMalloc(&d->d_frames, (size_t)cap * sizeof(amb_frame)));
-    DCK(cudaMalloc(&d->d_fields, (size_t)cap * sizeof(amb_fields)));
-    DCK(cudaMalloc(&d->st.pos, (size_t)cap * sizeof(AmbPosRec)));
-    DCK(cudaMalloc(&d->st.pair, (size_t)cap * sizeof(AmbPair)));
-    d->cap = cap;
+    cudaError_t e = cudaSuccess;
+    const int k = amb_decode_prepare(&d->st, n, d->stream, &e);
+    if (k < 0) return dfail(d, AMB_ERR_CUDA, amb_stage_names[-k - 1].memory, e);
+    if (d->cap < d->st.cap) {
+        free_bufs(d);
+        DCK(cudaMalloc(&d->d_frames, (size_t)d->st.cap * sizeof(amb_frame)));
+        DCK(cudaMalloc(&d->d_fields, (size_t)d->st.cap * sizeof(amb_fields)));
+        d->cap = d->st.cap;
+    }
     return AMB_OK;
 }
 
@@ -190,14 +178,8 @@ int amb_decoder_create(int device, int have_location, double lat, double lon, am
         if (cudaSetDevice(device) != cudaSuccess) { rc = AMB_ERR_NO_DEVICE; break; }
         if (cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking) != cudaSuccess ||
             cudaEventCreate(&d->e0) != cudaSuccess || cudaEventCreate(&d->e1) != cudaSuccess) { rc = AMB_ERR_CUDA; break; }
-        cudaError_t e = cudaMalloc(&d->st.table, AMB_TABLE_SLOTS * sizeof(AmbCprSlot));
-        if (e != cudaSuccess) { rc = dfail(d, AMB_ERR_CUDA, "report table (1 GiB)", e); break; }
-        if (cudaMalloc(&d->st.nl_T, AMB_NL_MAX * sizeof(double)) != cudaSuccess) { rc = AMB_ERR_CUDA; break; }
-        double T[AMB_NL_MAX];
-        amb_build_nl_table(T);                          // cpr.py:46-51 through the host libm, once
-        if (cudaMemcpyAsync(d->st.nl_T, T, sizeof T, cudaMemcpyHostToDevice, d->stream) != cudaSuccess ||
-            cudaMemsetAsync(d->st.table, 0xFF, AMB_TABLE_SLOTS * sizeof(AmbCprSlot), d->stream) != cudaSuccess ||
-            cudaStreamSynchronize(d->stream) != cudaSuccess) { rc = AMB_ERR_CUDA; break; }
+        if ((rc = prepare(d, 0)) != AMB_OK) break;      // the report and NL tables now, so that a lack of memory shows here
+        if (cudaStreamSynchronize(d->stream) != cudaSuccess) { rc = AMB_ERR_CUDA; break; }
     } while (0);
     if (rc != AMB_OK) { g_create_err = d->err.empty() ? "CUDA resource creation failed" : d->err; amb_decoder_destroy(d); return rc; }
     g_create_err.clear();
@@ -211,25 +193,10 @@ void amb_decoder_destroy(amb_decoder* d)
     cudaSetDevice(d->device);
     if (d->stream) cudaStreamSynchronize(d->stream);
     free_bufs(d);
-    amb_v3_free(&d->st.v3);
-    if (d->st.ltable) cudaFree(d->st.ltable);
-    if (d->st.keys) cudaFree(d->st.keys);
-    if (d->st.ctable) cudaFree(d->st.ctable);
-    if (d->st.otable) cudaFree(d->st.otable);
-    if (d->st.trows) cudaFree(d->st.trows);
-    if (d->st.tocc) cudaFree(d->st.tocc);
-    if (d->st.tclk) cudaFree(d->st.tclk);
-    if (d->st.xrows) cudaFree(d->st.xrows);
-    if (d->st.xocc) cudaFree(d->st.xocc);
-    free_sbs1_bufs(d);
-    if (d->st.stable) cudaFree(d->st.stable);
-    if (d->st.sctr) cudaFree(d->st.sctr);
+    amb_decode_free(&d->st);
     if (d->d_xsnap) cudaFree(d->d_xsnap);
-    if (d->snap_cnt) cudaFree(d->snap_cnt);
     if (d->d_snap) cudaFree(d->d_snap);
     for (int k = 0; k < 2; k++) { if (d->pin[k]) cudaFreeHost(d->pin[k]); if (d->pin_ev[k]) cudaEventDestroy(d->pin_ev[k]); }
-    if (d->st.table) cudaFree(d->st.table);
-    if (d->st.nl_T) cudaFree(d->st.nl_T);
     if (d->e0) cudaEventDestroy(d->e0);
     if (d->e1) cudaEventDestroy(d->e1);
     if (d->stream) cudaStreamDestroy(d->stream);
@@ -247,19 +214,9 @@ int amb_decoder_reset(amb_decoder* d)
 {
     if (!d) return AMB_ERR_INVALID;
     DCK(cudaSetDevice(d->device));
-    DCK(cudaMemsetAsync(d->st.table, 0xFF, AMB_TABLE_SLOTS * sizeof(AmbCprSlot), d->stream));
-    if (d->st.ltable) DCK(cudaMemsetAsync(d->st.ltable, 0xFF, AMB_LOCAL_SLOTS * sizeof(AmbRefPos), d->stream));
-    if (d->st.ctable) DCK(cudaMemsetAsync(d->st.ctable, 0xFF, AMB_COMMB_SLOTS * sizeof(AmbCommbRef), d->stream));
-    if (d->st.otable) DCK(cudaMemsetAsync(d->st.otable, 0xFF, AMB_OPS_SLOTS * sizeof(AmbOpsSlot), d->stream));
-    if (d->st.tocc) {                    // the rows themselves stay: a row whose bit is clear is never read
-        static const AmbTrackClock none = {NAN, 0u, 0u};
-        DCK(cudaMemsetAsync(d->st.tocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));
-        DCK(cudaMemcpyAsync(d->st.tclk, &none, sizeof none, cudaMemcpyHostToDevice, d->stream));
-    }
-    if (d->st.xocc) DCK(cudaMemsetAsync(d->st.xocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));   // likewise
-    if (d->st.sctr)                      // ids up to G are dead from now on: no table memset
-        DCK(cudaMemcpyAsync(&d->st.sctr->base, &d->st.sctr->G, sizeof(unsigned long long), cudaMemcpyDeviceToDevice,
-                            d->stream));
+    cudaError_t e = cudaSuccess;
+    const int k = amb_decode_reset(&d->st, d->stream, &e);
+    if (k < 0) return dfail(d, AMB_ERR_CUDA, amb_stage_names[-k - 1].memory, e);
     DCK(cudaStreamSynchronize(d->stream));
     return AMB_OK;
 }
@@ -298,116 +255,6 @@ int amb_decoder_set_option(amb_decoder* d, const char* name, int value)
     return dfail(d, AMB_ERR_INVALID, "amb_decoder_set_option: unknown option");
 }
 
-// the key records of the local, the Comm-B, the op-status and the track stage, one per frame
-static int ensure_keys(amb_decoder* d)
-{
-    if (d->kcap < d->cap) {
-        if (d->st.keys) cudaFree(d->st.keys);
-        d->st.keys = nullptr; d->kcap = 0;
-        DCK(cudaMalloc(&d->st.keys, (size_t)d->cap * sizeof(AmbPosRec)));
-        d->kcap = d->cap;
-    }
-    return AMB_OK;
-}
-
-// the local stage's device memory, at the first decode with the option on (the table starts empty: all NaN)
-static int ensure_local(amb_decoder* d)
-{
-    if (!d->st.ltable) {
-        DCK(cudaMalloc(&d->st.ltable, AMB_LOCAL_SLOTS * sizeof(AmbRefPos)));
-        DCK(cudaMemsetAsync(d->st.ltable, 0xFF, AMB_LOCAL_SLOTS * sizeof(AmbRefPos), d->stream));
-    }
-    return ensure_keys(d);
-}
-
-// the Comm-B stage's device memory, at the first decode with the option on (the table starts empty: all NaN)
-static int ensure_commb(amb_decoder* d)
-{
-    if (!d->st.ctable) {
-        cudaError_t e = cudaMalloc(&d->st.ctable, AMB_COMMB_SLOTS * sizeof(AmbCommbRef));
-        if (e != cudaSuccess) { d->st.ctable = nullptr; return dfail(d, AMB_ERR_CUDA, "Comm-B velocity table (384 MiB)", e); }
-        DCK(cudaMemsetAsync(d->st.ctable, 0xFF, AMB_COMMB_SLOTS * sizeof(AmbCommbRef), d->stream));
-    }
-    return ensure_keys(d);
-}
-
-// the op-status stage's device memory, at the first decode with the option on (the table starts empty: all NaN)
-static int ensure_opstatus(amb_decoder* d)
-{
-    if (!d->st.otable) {
-        cudaError_t e = cudaMalloc(&d->st.otable, AMB_OPS_SLOTS * sizeof(AmbOpsSlot));
-        if (e != cudaSuccess) { d->st.otable = nullptr; return dfail(d, AMB_ERR_CUDA, "op status table (384 MiB)", e); }
-        DCK(cudaMemsetAsync(d->st.otable, 0xFF, AMB_OPS_SLOTS * sizeof(AmbOpsSlot), d->stream));
-    }
-    return ensure_keys(d);
-}
-
-// the track stage's device memory, at the first decode with the option on: the rows are not initialised (the bitmap
-// starts empty), the clock starts at "nothing decoded"
-static int ensure_track(amb_decoder* d)
-{
-    if (!d->st.trows) {
-        cudaError_t e = cudaMalloc(&d->st.trows, (size_t)AMB_TRACK_ROWS * sizeof(amb_aircraft));
-        if (e != cudaSuccess) { d->st.trows = nullptr; return dfail(d, AMB_ERR_CUDA, "aircraft table (2 GiB)", e); }
-    }
-    if (!d->st.tclk) {
-        static const AmbTrackClock none = {NAN, 0u, 0u};
-        DCK(cudaMalloc(&d->st.tclk, sizeof(AmbTrackClock)));
-        DCK(cudaMemcpyAsync(d->st.tclk, &none, sizeof none, cudaMemcpyHostToDevice, d->stream));
-    }
-    if (!d->snap_cnt) DCK(cudaMalloc(&d->snap_cnt, (2 * AMB_TRACK_WORDS / AMB_SNAP_WORDS + 1) * sizeof(uint32_t)));
-    if (!d->st.tocc) {                   // last: snapshot_impl and reset take a bitmap as "everything is there"
-        DCK(cudaMalloc(&d->st.tocc, AMB_TRACK_WORDS * sizeof(unsigned)));
-        DCK(cudaMemsetAsync(d->st.tocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));
-    }
-    return ensure_keys(d);
-}
-
-// the track extension's device memory, at the first decode with it and the track stage on: the rows are not
-// initialised (the bitmap starts empty)
-static int ensure_track_ext(amb_decoder* d)
-{
-    if (!d->st.xrows) {
-        cudaError_t e = cudaMalloc(&d->st.xrows, (size_t)AMB_TRACK_ROWS * sizeof(amb_aircraft_ext));
-        if (e != cudaSuccess) { d->st.xrows = nullptr; return dfail(d, AMB_ERR_CUDA, "aircraft table extension (2.25 GiB)", e); }
-    }
-    if (!d->st.xocc) {                   // last: snapshot_impl and reset take a bitmap as "everything is there"
-        DCK(cudaMalloc(&d->st.xocc, AMB_TRACK_WORDS * sizeof(unsigned)));
-        DCK(cudaMemsetAsync(d->st.xocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), d->stream));
-    }
-    return AMB_OK;
-}
-
-// the SBS-1 stage's device memory: the id table and counter at the first decode with the option on (the table starts
-// with no id, the counter at 0), the per-frame scratch as the frame capacity grows
-static int ensure_sbs1(amb_decoder* d)
-{
-    if (!d->st.stable) {
-        cudaError_t e = cudaMalloc(&d->st.stable, (size_t)AMB_SBS1_SLOTS * sizeof(unsigned long long));
-        if (e != cudaSuccess) { d->st.stable = nullptr; return dfail(d, AMB_ERR_CUDA, "SBS-1 id table (128 MiB)", e); }
-        DCK(cudaMemsetAsync(d->st.stable, 0, (size_t)AMB_SBS1_SLOTS * sizeof(unsigned long long), d->stream));
-    }
-    if (!d->st.sctr) {
-        DCK(cudaMalloc(&d->st.sctr, sizeof(AmbSbs1Ctr)));
-        DCK(cudaMemsetAsync(d->st.sctr, 0, sizeof(AmbSbs1Ctr), d->stream));
-    }
-    if (d->scap < d->cap) {
-        free_sbs1_bufs(d);
-        const size_t n = (size_t)d->cap, nb = (n + 127) / 128, chunks = (n + AMB_SBS1_CHUNK - 1) / AMB_SBS1_CHUNK;
-        AmbSbs1Bufs& b = d->st.sb;
-        DCK(cudaMalloc(&b.src, n * sizeof(unsigned long long)));
-        DCK(cudaMalloc(&b.gid, n * sizeof(unsigned long long)));
-        DCK(cudaMalloc(&b.flag, chunks * sizeof(unsigned long long)));
-        DCK(cudaMalloc(&b.slots, n * AMB_SBS1_STRIDE));
-        DCK(cudaMalloc(&b.len, n * sizeof(uint32_t)));
-        DCK(cudaMalloc(&b.bsum, nb * sizeof(uint32_t)));
-        DCK(cudaMalloc(&b.boff, (nb + 1) * sizeof(unsigned long long)));
-        DCK(cudaMalloc(&b.text, n * AMB_SBS1_STRIDE));
-        d->scap = d->cap;
-    }
-    return ensure_keys(d);
-}
-
 static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_kind, amb_fields* out, bool out_on_device);
 
 int amb_decode_frames(amb_decoder* d, const amb_frame* frames, int n, int mem_kind, amb_fields* out)
@@ -429,13 +276,7 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
     if (n == 0) { d->sbs1_nb = -1; return AMB_OK; }
     DCK(cudaSetDevice(d->device));
     d->sbs1_nb = -1;
-    int rc = ensure_cap(d, n);
-    if (rc == AMB_OK && d->st.local_cpr > 0) rc = ensure_local(d);
-    if (rc == AMB_OK && d->st.commb > 0) rc = ensure_commb(d);
-    if (rc == AMB_OK && d->st.opstatus > 0) rc = ensure_opstatus(d);
-    if (rc == AMB_OK && d->st.track > 0) rc = ensure_track(d);
-    if (rc == AMB_OK && d->st.track > 0 && d->st.track_ext > 0) rc = ensure_track_ext(d);
-    if (rc == AMB_OK && d->st.sbs1 > 0) rc = ensure_sbs1(d);
+    int rc = prepare(d, n);
     if (rc != AMB_OK) return rc;
     cudaStream_t s = d->stream;
     amb_fields* const fields = out_on_device ? out : d->d_fields;
@@ -448,12 +289,7 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
     }
     cudaError_t e = cudaSuccess;
     const int k = amb_decode_launch(&d->st, src, n, fields, s, &e);
-    if (k < 0) {
-        static const char* const stage[] = {"cudaGetLastError()", "pairing", "cudaGetLastError()", "local CPR",
-                                            "Comm-B inference", "aircraft table", "op status",
-                                            "aircraft table extension", "SBS-1 feed"};   // by -AMB_STAGE_* - 1
-        return dfail(d, AMB_ERR_CUDA, stage[-k - 1], e);
-    }
+    if (k < 0) return dfail(d, AMB_ERR_CUDA, amb_stage_names[-k - 1].launch, e);
     d->launches += (uint64_t)k;
     if (d->st.sbs1 > 0) d->sbs1_nb = (n + 127) / 128;
     if (!out_on_device) {
@@ -483,9 +319,9 @@ static int snapshot_impl(amb_decoder* d, double now, amb_aircraft* out, amb_airc
     DCK(cudaSetDevice(d->device));
     cudaStream_t s = d->stream;
     const unsigned nb = AMB_TRACK_WORDS / AMB_SNAP_WORDS;
-    uint32_t* off = d->snap_cnt + nb;
+    uint32_t* off = d->st.snap_cnt + nb;
     cudaError_t e = cudaSuccess;
-    if (amb_snap_count_launch(d->st.tocc, d->st.trows, d->st.tclk, now, d->st.track, AMB_TRACK_WORDS, d->snap_cnt, off,
+    if (amb_snap_count_launch(d->st.tocc, d->st.trows, d->st.tclk, now, d->st.track, AMB_TRACK_WORDS, d->st.snap_cnt, off,
                               s, &e) < 0)
         return dfail(d, AMB_ERR_CUDA, "aircraft snapshot", e);
     d->launches += 2;

@@ -1,8 +1,11 @@
 // The kernels of the batch field decoder (SURVEY.md 8 row f4): amb_fields_kernel and amb_resolve_kernel here, the CPR
-// pairing stage between them in amb_decode_v3.cuh. The host orchestration and the C ABI are in amb_decode.cu, the
-// per-message arithmetic in amb_decode_core.h. Kept in headers without any <<< >>> launch so that tests/simt/ can
-// compile the very same kernel source for the host under a small SIMT emulator (CPU-side check of the warp-level logic;
-// the GPU tests remain the parity gate).
+// pairing stage between them in amb_decode_v3.cuh, the optional stages in the headers included below; then the state
+// every stage reads and writes, its lifecycle (amb_decode_prepare, amb_decode_reset, amb_decode_free) and the one launch
+// sequence of a decode (amb_decode_launch). The staging of frames and records and the C ABI are in amb_decode.cu, the
+// per-message arithmetic in amb_decode_core.h. Kept in headers without any <<< >>> launch, and with the state's memory
+// handled through cudaMalloc / cudaMemsetAsync / cudaMemcpyAsync / cudaFree only, so that tests/simt/ can compile the
+// very same kernel source and state handling for the host under a small SIMT emulator (CPU-side check of the
+// warp-level logic; the GPU tests remain the parity gate).
 #pragma once
 #include "amb_decode_core.h"
 
@@ -48,17 +51,22 @@ __global__ void __launch_bounds__(128) amb_resolve_kernel(amb_fields* __restrict
 #include "amb_decode_track_ext.cuh"
 #include "amb_decode_sbs1.cuh"
 
-// ---- launch sequence ----------------------------------------------------------------------------------------------
-// What the stages of one decode read and write besides the frames and the records: amb_decoder keeps one in device
-// memory, tests/simt/decode_emul.cc one in host memory. A stage's tables are only touched while its S is > 0.
+// ---- state and launch sequence ------------------------------------------------------------------------------------
+// What the stages of one decode read and write besides the frames and the records, and the one owner of that memory:
+// amb_decoder keeps one in device memory, tests/simt/decode_emul.cc one in host memory, and both allocate, clear and
+// free it with amb_decode_prepare, amb_decode_reset and amb_decode_free below. A stage's tables are only allocated and
+// touched while its S is > 0.
 struct AmbDecodeState {
-    AmbCprSlot* table = nullptr;         // pairing: latest even / odd report per (ICAO, surface), AMB_TABLE_SLOTS
+    AmbCprSlot* table = nullptr;         // pairing: latest even / odd report per (ICAO, surface), table_slots
+    size_t table_slots = AMB_TABLE_SLOTS, local_slots = AMB_LOCAL_SLOTS;   // smaller only in the emulator's tests
     double* nl_T = nullptr;              // NL transition table, AMB_NL_MAX
     AmbV3Bufs v3;                        // pairing scratch, reused by the partitions of the stages after it
     AmbPosRec* pos = nullptr; AmbPair* pair = nullptr;   // one per frame
+    int cap = 0;                         // frames pos and pair hold
     AmbPosRec* keys = nullptr;           // one per frame: address-keyed records of the local, Comm-B, op-status and track stage
+    int kcap = 0;                        // frames keys holds
     int local_cpr = 0;                   // option "local_cpr" = S seconds, 0 = off
-    AmbRefPos* ltable = nullptr;         // reference position per ICAO, AMB_LOCAL_SLOTS
+    AmbRefPos* ltable = nullptr;         // reference position per ICAO, local_slots
     int commb = 0;                       // option "commb" = S seconds, 0 = off
     AmbCommbRef* ctable = nullptr;       // ADS-B velocity per address, AMB_COMMB_SLOTS
     int opstatus = 0;                    // option "opstatus" = S seconds, 0 = off
@@ -67,6 +75,7 @@ struct AmbDecodeState {
     amb_aircraft* trows = nullptr;       // one row per address, AMB_TRACK_ROWS
     unsigned* tocc = nullptr;            // which rows hold data, AMB_TRACK_WORDS
     AmbTrackClock* tclk = nullptr;       // t of the latest queued record since reset
+    uint32_t* snap_cnt = nullptr;        // snapshot: per-block counts, then their scan and the total
     int track_ext = 0;                   // option "track_ext" = S2 seconds, 0 = off; runs only while track is on too
     amb_aircraft_ext* xrows = nullptr;   // one extension row per address, AMB_TRACK_ROWS
     unsigned* xocc = nullptr;            // which extension rows were written since reset, AMB_TRACK_WORDS
@@ -75,13 +84,155 @@ struct AmbDecodeState {
     unsigned long long* stable = nullptr;   // latest aircraft id per address (a global value, 0 = none), AMB_SBS1_SLOTS
     AmbSbs1Ctr* sctr = nullptr;          // the id counter and the base recorded at reset
     AmbSbs1Bufs sb;                      // the stage's per-call scratch and the packed lines, one entry per frame
+    int scap = 0;                        // frames sb holds
     int have_loc = 0; double lat = 0.0, lon = 0.0;      // receiver location
 };
 
-// What amb_decode_launch returns when a stage fails to launch.
+// What amb_decode_prepare, amb_decode_reset and amb_decode_launch return when a stage's memory or launch fails.
 enum { AMB_STAGE_FIELDS = -1, AMB_STAGE_PAIRING = -2, AMB_STAGE_RESOLVE = -3, AMB_STAGE_LOCAL = -4,
        AMB_STAGE_COMMB = -5, AMB_STAGE_TRACK = -6, AMB_STAGE_OPSTATUS = -7, AMB_STAGE_TRACK_EXT = -8,
        AMB_STAGE_SBS1 = -9 };
+
+// By -AMB_STAGE_* - 1: what a failed launch of the stage reports, and what a failure of its memory reports.
+static const struct { const char* launch; const char* memory; } amb_stage_names[] = {
+    {"cudaGetLastError()", "per-frame records"},
+    {"pairing", "report table (1 GiB)"},
+    {"cudaGetLastError()", "NL transition table"},
+    {"local CPR", "reference position table (384 MiB)"},
+    {"Comm-B inference", "Comm-B velocity table (384 MiB)"},
+    {"aircraft table", "aircraft table (2 GiB)"},
+    {"op status", "op status table (384 MiB)"},
+    {"aircraft table extension", "aircraft table extension (2.25 GiB)"},
+    {"SBS-1 feed", "SBS-1 id table (128 MiB)"},
+};
+
+// cudaMalloc, then every byte set to `fill` unless it is < 0; *p is NULL after a failed cudaMalloc
+template <typename T> static cudaError_t amb_decode_alloc(T** p, size_t bytes, int fill, cudaStream_t s)
+{
+    const cudaError_t e = cudaMalloc(p, bytes);
+    if (e != cudaSuccess) { *p = nullptr; return e; }
+    return fill < 0 ? cudaSuccess : cudaMemsetAsync(*p, fill, bytes, s);
+}
+
+static void amb_sbs1_bufs_free(AmbSbs1Bufs* b)
+{
+    void* const all[] = {b->src, b->gid, b->flag, b->slots, b->len, b->bsum, b->boff, b->text};
+    for (void* p : all) cudaFree(p);
+    *b = AmbSbs1Bufs();
+}
+
+#define AMB_STAGE_TRY(stage, call) do { if ((*err = (call)) != cudaSuccess) return (stage); } while (0)
+
+// Allocate on stream s what the stages that are on need for a decode of n frames (n = 0: only the pairing and NL
+// tables, which every decode needs): the per-frame records, from 4096 frames up, doubling; the address-keyed records
+// once a stage that partitions them is on; each stage's table, bitmap, clock and counter at its first decode with the
+// option on, filled as an empty one (the track extension only while track is on too); the SBS-1 scratch as the frame
+// capacity grows. Returns 0, or the AMB_STAGE_* code of the stage whose memory could not be had, with *err set.
+static int amb_decode_prepare(AmbDecodeState* st, int n, cudaStream_t s, cudaError_t* err)
+{
+    if (!st->table) AMB_STAGE_TRY(AMB_STAGE_PAIRING, amb_decode_alloc(&st->table, st->table_slots * sizeof(AmbCprSlot), 0xFF, s));
+    if (!st->nl_T) {
+        double T[AMB_NL_MAX];
+        amb_build_nl_table(T);                          // cpr.py:46-51 through the host libm, once
+        AMB_STAGE_TRY(AMB_STAGE_RESOLVE, amb_decode_alloc(&st->nl_T, sizeof T, -1, s));
+        AMB_STAGE_TRY(AMB_STAGE_RESOLVE, cudaMemcpyAsync(st->nl_T, T, sizeof T, cudaMemcpyHostToDevice, s));
+    }
+    if (n > st->cap) {
+        int cap = st->cap ? st->cap : 4096;
+        while (cap < n) cap *= 2;
+        cudaFree(st->pos); cudaFree(st->pair);
+        st->pos = nullptr; st->pair = nullptr; st->cap = 0;
+        AMB_STAGE_TRY(AMB_STAGE_FIELDS, amb_decode_alloc(&st->pos, (size_t)cap * sizeof(AmbPosRec), -1, s));
+        AMB_STAGE_TRY(AMB_STAGE_FIELDS, amb_decode_alloc(&st->pair, (size_t)cap * sizeof(AmbPair), -1, s));
+        st->cap = cap;
+    }
+    if ((st->local_cpr > 0 || st->commb > 0 || st->opstatus > 0 || st->track > 0 || st->sbs1 > 0) && st->kcap < st->cap) {
+        cudaFree(st->keys);
+        st->keys = nullptr; st->kcap = 0;
+        AMB_STAGE_TRY(AMB_STAGE_FIELDS, amb_decode_alloc(&st->keys, (size_t)st->cap * sizeof(AmbPosRec), -1, s));
+        st->kcap = st->cap;
+    }
+    if (st->local_cpr > 0 && !st->ltable)               // the tables start empty: all NaN
+        AMB_STAGE_TRY(AMB_STAGE_LOCAL, amb_decode_alloc(&st->ltable, st->local_slots * sizeof(AmbRefPos), 0xFF, s));
+    if (st->commb > 0 && !st->ctable)
+        AMB_STAGE_TRY(AMB_STAGE_COMMB, amb_decode_alloc(&st->ctable, AMB_COMMB_SLOTS * sizeof(AmbCommbRef), 0xFF, s));
+    if (st->opstatus > 0 && !st->otable)
+        AMB_STAGE_TRY(AMB_STAGE_OPSTATUS, amb_decode_alloc(&st->otable, AMB_OPS_SLOTS * sizeof(AmbOpsSlot), 0xFF, s));
+    if (st->track > 0) {                                // rows are not initialised: the bitmaps start empty
+        static const AmbTrackClock none = {NAN, 0u, 0u};   // "nothing decoded"
+        if (!st->trows)
+            AMB_STAGE_TRY(AMB_STAGE_TRACK, amb_decode_alloc(&st->trows, (size_t)AMB_TRACK_ROWS * sizeof(amb_aircraft), -1, s));
+        if (!st->tclk) {
+            AMB_STAGE_TRY(AMB_STAGE_TRACK, amb_decode_alloc(&st->tclk, sizeof none, -1, s));
+            AMB_STAGE_TRY(AMB_STAGE_TRACK, cudaMemcpyAsync(st->tclk, &none, sizeof none, cudaMemcpyHostToDevice, s));
+        }
+        if (!st->snap_cnt)
+            AMB_STAGE_TRY(AMB_STAGE_TRACK, amb_decode_alloc(&st->snap_cnt, (2 * AMB_TRACK_WORDS / AMB_SNAP_WORDS + 1) *
+                                                                               sizeof(uint32_t), -1, s));
+        if (!st->tocc)                                  // last: a snapshot and a reset take a bitmap as "everything is there"
+            AMB_STAGE_TRY(AMB_STAGE_TRACK, amb_decode_alloc(&st->tocc, AMB_TRACK_WORDS * sizeof(unsigned), 0, s));
+        if (st->track_ext > 0 && !st->xrows)
+            AMB_STAGE_TRY(AMB_STAGE_TRACK_EXT, amb_decode_alloc(&st->xrows, (size_t)AMB_TRACK_ROWS * sizeof(amb_aircraft_ext),
+                                                                -1, s));
+        if (st->track_ext > 0 && !st->xocc)             // last, likewise
+            AMB_STAGE_TRY(AMB_STAGE_TRACK_EXT, amb_decode_alloc(&st->xocc, AMB_TRACK_WORDS * sizeof(unsigned), 0, s));
+    }
+    if (st->sbs1 > 0) {                                 // no id yet, the counter at 0
+        if (!st->stable)
+            AMB_STAGE_TRY(AMB_STAGE_SBS1, amb_decode_alloc(&st->stable, (size_t)AMB_SBS1_SLOTS * sizeof(unsigned long long),
+                                                           0, s));
+        if (!st->sctr) AMB_STAGE_TRY(AMB_STAGE_SBS1, amb_decode_alloc(&st->sctr, sizeof(AmbSbs1Ctr), 0, s));
+        if (st->scap < st->cap) {
+            amb_sbs1_bufs_free(&st->sb);
+            st->scap = 0;
+            const size_t c = (size_t)st->cap, nb = (c + 127) / 128, chunks = (c + AMB_SBS1_CHUNK - 1) / AMB_SBS1_CHUNK;
+            AmbSbs1Bufs& b = st->sb;
+            AMB_STAGE_TRY(AMB_STAGE_SBS1, amb_decode_alloc(&b.src, c * sizeof(unsigned long long), -1, s));
+            AMB_STAGE_TRY(AMB_STAGE_SBS1, amb_decode_alloc(&b.gid, c * sizeof(unsigned long long), -1, s));
+            AMB_STAGE_TRY(AMB_STAGE_SBS1, amb_decode_alloc(&b.flag, chunks * sizeof(unsigned long long), -1, s));
+            AMB_STAGE_TRY(AMB_STAGE_SBS1, amb_decode_alloc(&b.slots, c * AMB_SBS1_STRIDE, -1, s));
+            AMB_STAGE_TRY(AMB_STAGE_SBS1, amb_decode_alloc(&b.len, c * sizeof(uint32_t), -1, s));
+            AMB_STAGE_TRY(AMB_STAGE_SBS1, amb_decode_alloc(&b.bsum, nb * sizeof(uint32_t), -1, s));
+            AMB_STAGE_TRY(AMB_STAGE_SBS1, amb_decode_alloc(&b.boff, (nb + 1) * sizeof(unsigned long long), -1, s));
+            AMB_STAGE_TRY(AMB_STAGE_SBS1, amb_decode_alloc(&b.text, c * AMB_SBS1_STRIDE, -1, s));
+            st->scap = st->cap;
+        }
+    }
+    return 0;
+}
+
+// amb_decoder_reset on stream s, for whatever is allocated: every table empty again. The rows of the aircraft table
+// and its extension stay (a row whose bit is clear is never read), and so does the SBS-1 id table (ids up to G are
+// dead once base = G). Returns 0, or the AMB_STAGE_* code of the stage whose memory could not be cleared, with *err set.
+static int amb_decode_reset(AmbDecodeState* st, cudaStream_t s, cudaError_t* err)
+{
+    static const AmbTrackClock none = {NAN, 0u, 0u};
+    if (st->table) AMB_STAGE_TRY(AMB_STAGE_PAIRING, cudaMemsetAsync(st->table, 0xFF, st->table_slots * sizeof(AmbCprSlot), s));
+    if (st->ltable) AMB_STAGE_TRY(AMB_STAGE_LOCAL, cudaMemsetAsync(st->ltable, 0xFF, st->local_slots * sizeof(AmbRefPos), s));
+    if (st->ctable) AMB_STAGE_TRY(AMB_STAGE_COMMB, cudaMemsetAsync(st->ctable, 0xFF, AMB_COMMB_SLOTS * sizeof(AmbCommbRef), s));
+    if (st->otable) AMB_STAGE_TRY(AMB_STAGE_OPSTATUS, cudaMemsetAsync(st->otable, 0xFF, AMB_OPS_SLOTS * sizeof(AmbOpsSlot), s));
+    if (st->tocc) {
+        AMB_STAGE_TRY(AMB_STAGE_TRACK, cudaMemsetAsync(st->tocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), s));
+        AMB_STAGE_TRY(AMB_STAGE_TRACK, cudaMemcpyAsync(st->tclk, &none, sizeof none, cudaMemcpyHostToDevice, s));
+    }
+    if (st->xocc) AMB_STAGE_TRY(AMB_STAGE_TRACK_EXT, cudaMemsetAsync(st->xocc, 0, AMB_TRACK_WORDS * sizeof(unsigned), s));
+    if (st->sctr)
+        AMB_STAGE_TRY(AMB_STAGE_SBS1, cudaMemcpyAsync(&st->sctr->base, &st->sctr->G, sizeof(unsigned long long),
+                                                      cudaMemcpyDeviceToDevice, s));
+    return 0;
+}
+#undef AMB_STAGE_TRY
+
+// Free everything the state owns and leave it as a new one (the caller has synchronised with its last use).
+static void amb_decode_free(AmbDecodeState* st)
+{
+    void* const all[] = {st->table, st->nl_T, st->pos, st->pair, st->keys, st->ltable, st->ctable, st->otable, st->trows,
+                         st->tocc, st->tclk, st->snap_cnt, st->xrows, st->xocc, st->stable, st->sctr};
+    for (void* p : all) cudaFree(p);
+    amb_v3_free(&st->v3);
+    amb_sbs1_bufs_free(&st->sb);
+    *st = AmbDecodeState();
+}
 
 // Enqueue one decode of the n frames into the n records on stream s, in this order: fields, pairing, resolve, then the
 // local CPR, Comm-B, op-status and track stages whose S is > 0, and the track extension when track and track_ext are

@@ -3,6 +3,7 @@ tests/simt and the host shims of the decode core, each compiled once per pytest 
 import ctypes as C
 import hashlib
 import os
+import shutil
 import subprocess
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -29,6 +30,19 @@ def build(tmp_path_factory, src) -> str:
     return _built[src]
 
 
+class EmulOpts(C.Structure):
+    """The options of one emulated decode (struct EmulOpts of tests/simt/decode_emul.cc): the receiver location and
+    every stage's S, 0 = off."""
+    _fields_ = [("have_loc", C.c_int), ("lat", C.c_double), ("lon", C.c_double), ("local_cpr", C.c_int),
+                ("commb", C.c_int), ("opstatus", C.c_int), ("track", C.c_int), ("track_ext", C.c_int), ("sbs1", C.c_int),
+                ("sbs1_tz", C.c_int)]
+
+
+def opts(loc=None, **stages):
+    """EmulOpts with the receiver at loc = (lat, lon) (None: no location) and the given stages on, e.g. commb=30."""
+    return EmulOpts(0, 0.0, 0.0, **stages) if loc is None else EmulOpts(1, loc[0], loc[1], **stages)
+
+
 def decode_emul(tmp_path_factory, src=DECODE_EMUL):
     """The decoder harness tests/simt/decode_emul.cc (or a patched copy at `src`), built and bound."""
     e = C.CDLL(build(tmp_path_factory, src))
@@ -36,7 +50,23 @@ def decode_emul(tmp_path_factory, src=DECODE_EMUL):
     e.emul_new.argtypes = [C.c_int]
     e.emul_free.argtypes = [C.c_void_p]
     e.emul_reset.argtypes = [C.c_void_p]
-    e.emul_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, C.c_int,
-                              C.c_void_p]
-    e.emul_snapshot.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_uint, C.c_void_p, C.c_int]
+    e.emul_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(EmulOpts), C.c_void_p]
+    e.emul_snapshot.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int, C.c_uint, C.c_void_p, C.c_void_p, C.c_int]
+    e.emul_sbs1_text.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    e.emul_sbs1_ids.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     return e
+
+
+def mutant(tmp_path, tmp_path_factory, rel, old, new):
+    """The harness built from a copy of the sources under tmp_path in which the text `old`, which must occur exactly
+    once in the file `rel` (relative to the repository), reads `new`. old and new may also be tuples of such texts,
+    patched in turn."""
+    for sub in ("gr_air_modes_b200/csrc", "include", "tests/simt"):
+        shutil.copytree(os.path.join(ROOT, sub), str(tmp_path / sub))
+    p = tmp_path / rel
+    src = p.read_text()
+    for a, b in zip(*((old, new) if isinstance(old, tuple) else ((old,), (new,)))):
+        assert src.count(a) == 1, a
+        src = src.replace(a, b)
+    p.write_text(src)
+    return decode_emul(tmp_path_factory, tmp_path / "tests/simt/decode_emul.cc")

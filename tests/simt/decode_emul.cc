@@ -1,116 +1,121 @@
 // TEST HARNESS (not a product path): runs the decoder's kernel source - gr_air_modes_b200/csrc/amb_decode_kernels.cuh
-// and the stage headers it includes - on the host under tests/simt/simt_emul.h, through the decoder's own launch
-// sequence amb_decode_launch: fields, pairing, resolve, and the local CPR, Comm-B and track stages whose S is > 0.
-// tests/test_decode_simt.py, test_local_cpr_simt.py, test_commb_simt.py and test_track_simt.py build it with plain g++
-// (tests/emul_build.py).
+// and the stage headers it includes - on the host under tests/simt/simt_emul.h, with the decoder's own state and launch
+// sequence: amb_decode_prepare allocates what the stages that are on need (host memory here), amb_decode_launch enqueues
+// fields, pairing, resolve and every stage that is on, and amb_decode_reset / amb_decode_free are what
+// amb_decoder_reset / amb_decoder_destroy run. The tests/test_*_simt.py modules build it with plain g++ and bind it
+// through tests/emul_build.py.
 #include "simt_emul.h"
 
 #include "../../gr_air_modes_b200/csrc/amb_decode_kernels.cuh"
 
-#include <sys/mman.h>
-
 #include <algorithm>
-#include <vector>
 
-// The pairing table and the local stage's table are indexed by ICAO below 2^log2_slots (the tests keep the position
-// squitters' addresses small). The velocity table and the aircraft rows span all 2^24 addresses like the decoder's,
-// since a DF20/21 record's address is its AP syndrome; they are allocated at the first decode with their stage on, the
-// rows in a reserve-only mapping (only the pages of rows that are written get memory).
-struct Emul {
-    AmbDecodeState st;                                  // kept across calls, like the decoder's
-    std::vector<AmbCprSlot> table;
-    double T[AMB_NL_MAX];
-    std::vector<AmbRefPos> ltable;
-    std::vector<AmbCommbRef> ctable;
-    std::vector<unsigned> occ;
-    AmbTrackClock clk;
-    std::vector<uint32_t> snap;
-    std::vector<AmbPosRec> pos, keys;
-    std::vector<AmbPair> pair;
+// The options of one decode, as amb_decoder_set_location and amb_decoder_set_option set them (emul_build.EmulOpts).
+struct EmulOpts {
+    int have_loc; double lat, lon;
+    int local_cpr, commb, opstatus, track, track_ext, sbs1, sbs1_tz;
 };
 
-static const size_t kRowBytes = (size_t)AMB_TRACK_ROWS * sizeof(amb_aircraft);
+struct Emul {
+    AmbDecodeState st;                                  // kept across calls, like the decoder's
+};
 
-// amb_decoder_reset: every table empty again, the aircraft rows stay (a row whose bit is clear is never read)
-extern "C" void emul_reset(void* h)
-{
-    Emul* e = static_cast<Emul*>(h);
-    memset(e->table.data(), 0xFF, e->table.size() * sizeof(AmbCprSlot));
-    memset(e->ltable.data(), 0xFF, e->ltable.size() * sizeof(AmbRefPos));
-    if (!e->ctable.empty()) memset(e->ctable.data(), 0xFF, e->ctable.size() * sizeof(AmbCommbRef));
-    std::fill(e->occ.begin(), e->occ.end(), 0u);
-    e->clk.last_t = NAN; e->clk.last_k = 0; e->clk.pad_ = 0;
-}
-
+// The pairing table and the local stage's table hold 2^log2_slots entries (the tests keep the position squitters'
+// addresses small); every other table spans all 2^24 addresses like the decoder's.
 extern "C" void* emul_new(int log2_slots)
 {
     Emul* e = new Emul();
-    e->table.resize((size_t)1 << log2_slots);
-    e->ltable.resize((size_t)1 << log2_slots);
-    amb_build_nl_table(e->T);
-    e->st.table = e->table.data();
-    e->st.nl_T = e->T;
-    e->st.ltable = e->ltable.data();
-    e->st.tclk = &e->clk;
-    emul_reset(e);
+    e->st.table_slots = e->st.local_slots = (size_t)1 << log2_slots;
+    cudaError_t err = cudaSuccess;
+    if (amb_decode_prepare(&e->st, 0, nullptr, &err) < 0) { amb_decode_free(&e->st); delete e; return nullptr; }
     return e;
 }
 
 extern "C" void emul_free(void* h)
 {
     Emul* e = static_cast<Emul*>(h);
-    if (e->st.trows) munmap(e->st.trows, kRowBytes);
-    amb_v3_free(&e->st.v3);
+    amb_decode_free(&e->st);
     delete e;
 }
 
-// amb_decode_frames: returns 0, or -1 when a position squitter's address does not fit the test's tables
-extern "C" int emul_decode(void* h, const amb_frame* frames, int n, int have_loc, double lat, double lon, int local_S,
-                           int commb_S, int track_S, amb_fields* out)
+extern "C" void emul_reset(void* h)
 {
-    Emul* e = static_cast<Emul*>(h);
+    cudaError_t err = cudaSuccess;
+    amb_decode_reset(&static_cast<Emul*>(h)->st, nullptr, &err);
+}
+
+// amb_decode_frames: returns 0, -1 when a position squitter's address does not fit the test's tables, -2 when a stage
+// fails to launch, -3 when the stages' memory cannot be had
+extern "C" int emul_decode(void* h, const amb_frame* frames, int n, const EmulOpts* o, amb_fields* out)
+{
+    AmbDecodeState& st = static_cast<Emul*>(h)->st;
     if (n <= 0) return 0;
     for (int k = 0; k < n; k++) {
         amb_fields r; AmbPosRec p;
         amb_decode_fields(frames[k], &r, &p);
-        if (p.key != AMB_NO_KEY && (((size_t)p.key << 1) | 1u) >= e->table.size()) return -1;   // test table too small
+        if (p.key != AMB_NO_KEY && (((size_t)p.key << 1) | 1u) >= st.table_slots) return -1;   // test table too small
     }
-    if (commb_S > 0 && e->ctable.empty()) {
-        e->ctable.resize((size_t)AMB_COMMB_SLOTS);
-        memset(e->ctable.data(), 0xFF, e->ctable.size() * sizeof(AmbCommbRef));
-        e->st.ctable = e->ctable.data();
-    }
-    if (track_S > 0 && !e->st.trows) {
-        void* p = mmap(nullptr, kRowBytes, PROT_READ | PROT_WRITE, MAP_PRIVATE | MAP_ANONYMOUS | MAP_NORESERVE, -1, 0);
-        if (p == MAP_FAILED) return -3;
-        memset(p, 0xA5, 4096 * 4);                      // rows are never cleared: the first ones start as garbage
-        e->st.trows = static_cast<amb_aircraft*>(p);
-        e->occ.assign(AMB_TRACK_WORDS, 0u);
-        e->st.tocc = e->occ.data();
-        e->snap.assign(2 * AMB_TRACK_WORDS / AMB_SNAP_WORDS + 1, 0u);
-    }
-    e->pos.resize(n); e->pair.resize(n); e->keys.resize(n);
-    e->st.pos = e->pos.data(); e->st.pair = e->pair.data(); e->st.keys = e->keys.data();
-    e->st.have_loc = have_loc; e->st.lat = lat; e->st.lon = lon;
-    e->st.local_cpr = local_S; e->st.commb = commb_S; e->st.track = track_S;
+    st.have_loc = o->have_loc; st.lat = o->lat; st.lon = o->lon;
+    st.local_cpr = o->local_cpr; st.commb = o->commb; st.opstatus = o->opstatus; st.track = o->track;
+    st.track_ext = o->track_ext; st.sbs1 = o->sbs1; st.sbs1_tz = o->sbs1_tz;
+    const bool had_rows = st.trows, had_xrows = st.xrows;
     cudaError_t err = cudaSuccess;
-    return amb_decode_launch(&e->st, frames, n, out, nullptr, &err) < 0 ? -2 : 0;
+    if (amb_decode_prepare(&st, n, nullptr, &err) < 0) return -3;
+    // rows are never cleared: the first ones start as garbage
+    if (!had_rows && st.trows) memset(st.trows, 0xA5, 4096 * 4);
+    if (!had_xrows && st.xrows) memset(st.xrows, 0xA5, 4096 * 4);
+    if (st.sbs1 > 0) {                                  // the SBS-1 scratch poisoned before every call: no kernel may
+        AmbSbs1Bufs& b = st.sb;                         // read what an earlier call left there
+        const size_t c = (size_t)st.scap, nb = (c + 127) / 128, chunks = (c + AMB_SBS1_CHUNK - 1) / AMB_SBS1_CHUNK;
+        std::fill_n(b.src, c, 0xDEADBEEFull); std::fill_n(b.gid, c, 0xDEADBEEFull);
+        std::fill_n(b.flag, chunks, 0xDEADBEEFull);
+        memset(b.slots, '?', c * AMB_SBS1_STRIDE); memset(b.text, '?', c * AMB_SBS1_STRIDE);
+        std::fill_n(b.len, c, 7u); std::fill_n(b.bsum, nb, 7u); std::fill_n(b.boff, nb + 1, 7ull);
+    }
+    return amb_decode_launch(&st, frames, n, out, nullptr, &err) < 0 ? -2 : 0;
 }
 
-// amb_decoder_aircraft over the first `words` bitmap words (a multiple of AMB_SNAP_WORDS): out == NULL returns the count.
-extern "C" int emul_snapshot(void* h, double now, int S, unsigned words, amb_aircraft* out, int max)
+// amb_decoder_aircraft (ext == NULL) or amb_decoder_aircraft_ext over the first `words` bitmap words (a multiple of
+// AMB_SNAP_WORDS): out == NULL returns the count, too small a `max` -5.
+extern "C" int emul_snapshot(void* h, double now, int S, int S2, unsigned words, amb_aircraft* out, amb_aircraft_ext* ext,
+                             int max)
 {
-    Emul* e = static_cast<Emul*>(h);
-    if (!e->st.trows) return 0;                         // nothing decoded with the track stage on yet
+    const AmbDecodeState& st = static_cast<Emul*>(h)->st;
+    if (!st.tocc) return 0;                             // nothing decoded with the track stage on yet
     const unsigned nb = words / AMB_SNAP_WORDS;
-    uint32_t* off = e->snap.data() + nb;
+    uint32_t* off = st.snap_cnt + nb;
     cudaError_t err = cudaSuccess;
-    if (amb_snap_count_launch(e->st.tocc, e->st.trows, &e->clk, now, S, words, e->snap.data(), off, nullptr, &err) < 0)
-        return -1;
+    if (amb_snap_count_launch(st.tocc, st.trows, st.tclk, now, S, words, st.snap_cnt, off, nullptr, &err) < 0) return -1;
     const int total = (int)off[nb];
     if (!out) return total;
     if (total > max) return -5;
-    if (total && amb_snap_gather_launch(e->st.tocc, e->st.trows, &e->clk, now, S, words, off, out, nullptr, &err) < 0)
-        return -1;
-    return total;
+    if (total == 0) return 0;
+    const int k = ext ? amb_snap_gather_ext_launch(st.tocc, st.trows, st.tclk, now, S, words, off, out, st.xocc, st.xrows,
+                                                   S2, ext, nullptr, &err)
+                      : amb_snap_gather_launch(st.tocc, st.trows, st.tclk, now, S, words, off, out, nullptr, &err);
+    return k < 0 ? -1 : total;
+}
+
+// amb_decoder_sbs1 after a decode of n frames with the option on: its packed lines into text; returns 0, or -5 when
+// they do not fit `cap` (*n_bytes = their length either way)
+extern "C" int emul_sbs1_text(void* h, int n, char* text, size_t cap, size_t* n_bytes)
+{
+    const AmbDecodeState& st = static_cast<Emul*>(h)->st;
+    *n_bytes = 0;
+    if (n <= 0) return 0;
+    const size_t total = (size_t)st.sb.boff[(n + 127) / 128];
+    *n_bytes = total;
+    if (total > cap) return -5;
+    memcpy(text, st.sb.text, total);
+    return 0;
+}
+
+// the ids of the last call's published records, in stream order (count returned)
+extern "C" int emul_sbs1_ids(void* h, const amb_fields* recs, int n, unsigned long long* ids)
+{
+    const AmbDecodeState& st = static_cast<Emul*>(h)->st;
+    int m = 0;
+    for (int k = 0; k < n; k++)
+        if (amb_sbs1_published(&recs[k])) ids[m++] = st.sb.gid[k] - st.sctr->base;
+    return m;
 }

@@ -6,7 +6,6 @@ random sizes), alone and with the local CPR and track stages also on. Two mutant
 the table instead of an earlier same-address lane, and an age test with < for <=."""
 import ctypes as C
 import os
-import shutil
 import sys
 
 import numpy as np
@@ -18,8 +17,6 @@ import commb_oracle as co  # noqa: E402
 import emul_build  # noqa: E402
 import track_cases as tc  # noqa: E402
 
-ROOT = emul_build.ROOT
-
 
 @pytest.fixture(scope="module")
 def emul(tmp_path_factory):
@@ -30,6 +27,7 @@ def _decode(e, frames, S, splits, local_S=0, track_S=0):
     """Records of the emulated decode cut at `splits` (S = 0: the option off)."""
     from gr_air_modes_b200 import decode
     n = len(frames)
+    opts = emul_build.opts(local_cpr=local_S, commb=S, track=track_S)
     h = e.emul_new(17)
     assert h
     recs = np.zeros(n, dtype=decode.FIELDS_DTYPE)
@@ -38,7 +36,7 @@ def _decode(e, frames, S, splits, local_S=0, track_S=0):
         c = min(c, n - pos)
         if c <= 0:
             break
-        assert e.emul_decode(h, C.c_void_p(frames.ctypes.data + 80 * pos), c, 0, 0.0, 0.0, local_S, S, track_S,
+        assert e.emul_decode(h, C.c_void_p(frames.ctypes.data + 80 * pos), c, opts,
                              C.c_void_p(recs.ctypes.data + 144 * pos)) == 0
         pos += c
     e.emul_free(h)
@@ -90,28 +88,18 @@ def test_a_bucket_of_32_aircraft(emul):
     assert np.sum(co.outcome_of(got) == co.RESOLVED) > 100
 
 
-def _mutant(tmp_path, tmp_path_factory, rel, old, new):
-    for sub in ("gr_air_modes_b200/csrc", "include", "tests/simt"):
-        shutil.copytree(os.path.join(ROOT, sub), str(tmp_path / sub))
-    p = tmp_path / rel
-    src = p.read_text()
-    assert src.count(old) == 1
-    p.write_text(src.replace(old, new))
-    return emul_build.decode_emul(tmp_path_factory, tmp_path / "tests/simt/decode_emul.cc")
-
-
 def test_a_walk_reading_the_table_instead_of_an_earlier_lane_is_caught(tmp_path, tmp_path_factory):
     """Mutation: a record whose velocity came earlier in the same 32-record step reads the table, which holds the
     velocity of an earlier step (or none)."""
-    e = _mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_commb.cuh", "            if (!before) {",
-                "            if (true) {")
+    e = emul_build.mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_commb.cuh",
+                          "            if (!before) {", "            if (true) {")
     with pytest.raises(AssertionError):
         _check(e, cc.burst_scene(), 3, [])
 
 
 def test_an_age_test_with_less_than_is_caught(tmp_path, tmp_path_factory):
     """Mutation: a reference exactly S seconds old no longer counts."""
-    e = _mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_core.h", "t - ref->t <= (double)max_age",
-                "t - ref->t < (double)max_age")
+    e = emul_build.mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_core.h",
+                          "t - ref->t <= (double)max_age", "t - ref->t < (double)max_age")
     with pytest.raises(AssertionError):
         _check(e, cc.reference_scene(S=30), 30, [])

@@ -6,7 +6,6 @@ sequential replay of the same arithmetic (tests/local_cpr_host_shim.cc) byte for
 local fixes. A copy of the kernel whose lanes read the table instead of their predecessor's fix must fail."""
 import ctypes as C
 import os
-import shutil
 import sys
 
 import numpy as np
@@ -33,6 +32,7 @@ def _run(e, s, msgs, loc, S, splits):
     from gr_air_modes_b200 import decode
     arr, n = decode.frames_from_messages(msgs)
     have, lat, lon = (0, 0.0, 0.0) if loc is None else (1, loc[0], loc[1])
+    opts = emul_build.opts(loc, local_cpr=S)
     he = e.emul_new(17)
     hs = s.shim_local_new() if s is not None else None
     got = np.zeros(n, dtype=decode.FIELDS_DTYPE)
@@ -43,7 +43,7 @@ def _run(e, s, msgs, loc, S, splits):
         if c <= 0:
             break
         fr = C.c_void_p(base + 80 * pos)
-        assert e.emul_decode(he, fr, c, have, lat, lon, S, 0, 0, C.c_void_p(got.ctypes.data + 144 * pos)) == 0
+        assert e.emul_decode(he, fr, c, opts, C.c_void_p(got.ctypes.data + 144 * pos)) == 0
         if hs is not None:
             s.shim_local_step(hs, fr, c, have, lat, lon, S, C.c_void_p(want.ctypes.data + 144 * pos))
         pos += c
@@ -120,14 +120,9 @@ def test_one_aircraft_with_a_long_local_chain(libs):
 
 def test_a_chain_that_reads_the_table_instead_of_its_predecessor_is_caught(tmp_path, tmp_path_factory):
     """Mutation: every lane takes its reference from the table, none from the previous member of its group."""
-    for sub in ("gr_air_modes_b200/csrc", "include", "tests/simt"):
-        shutil.copytree(os.path.join(ROOT, sub), str(tmp_path / sub))
-    p = tmp_path / "gr_air_modes_b200/csrc/amb_decode_local.cuh"
-    src = p.read_text()
-    a, b = "if (mine && rank == 0) {", "if (mine && (rank == 0 || (fields[k].status & AMB_FS_HAS_POS))) {"
-    assert src.count(a) == 1 and src.count(b) == 1
-    p.write_text(src.replace(a, "if (mine) {").replace(b, "if (mine) {"))
-    e = emul_build.decode_emul(tmp_path_factory, tmp_path / "tests/simt/decode_emul.cc")
+    e = emul_build.mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_local.cuh",
+                          ("if (mine && rank == 0) {", "if (mine && (rank == 0 || (fields[k].status & AMB_FS_HAS_POS))) {"),
+                          ("if (mine) {", "if (mine) {"))
     msgs = lc.chain_scene(n_local=100)
     got, _ = _run(e, None, msgs, None, 5, [])
     with pytest.raises(AssertionError):

@@ -1,6 +1,6 @@
 """The SBS-1 stage's KERNEL SOURCE (gr_air_modes_b200/csrc/amb_decode_sbs1.cuh, enqueued by the decoder's own
 amb_decode_launch after every other stage) on the host under the SIMT emulator (tests/simt/simt_emul.h), through
-tests/simt/decode_sbs1_emul.cc - the track-extension harness plus this option - against the sequential checker
+the decoder harness tests/simt/decode_emul.cc, against the sequential checker
 (tests/sbs1_oracle.py) fed with the same frames and the decoder's own records: the text byte for byte and every id,
 across single messages, cuts at 31/32/33 and random splits, with local_cpr / commb / opstatus / track on and off; the
 window crossed across calls, inside one call, in a cascade, and by one call of more than 10000 new addresses; a reset
@@ -8,7 +8,6 @@ followed by earlier timestamps. Four mutants must fail: a walk that reads the ta
 plain scan that ignores expiry inside a call, round-half-up formatting and rounded milliseconds."""
 import ctypes as C
 import os
-import shutil
 import sys
 
 import numpy as np
@@ -20,23 +19,10 @@ import sbs1_cases as sc  # noqa: E402
 import sbs1_oracle as so  # noqa: E402
 import track_cases as tc  # noqa: E402
 
-ROOT = emul_build.ROOT
-HARNESS = os.path.join(ROOT, "tests", "simt", "decode_sbs1_emul.cc")
-
-
-def _bind(e):
-    e.emul_decode_sbs1.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_int,
-                                   C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t,
-                                   C.POINTER(C.c_size_t)]
-    e.emul_sbs1_ids.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
-    e.emul_reset_sbs1.argtypes = [C.c_void_p]
-    e.emul_free_sbs1.argtypes = [C.c_void_p]
-    return e
-
 
 @pytest.fixture(scope="module")
 def emul(tmp_path_factory):
-    return _bind(emul_build.decode_emul(tmp_path_factory, HARNESS))
+    return emul_build.decode_emul(tmp_path_factory)
 
 
 LOC = (47.9, 11.1)                                       # receiver location: surface positions need one
@@ -49,8 +35,10 @@ def _call(e, h, frames, opts, tz, chk):
     buf = C.create_string_buffer(max(1, n * 192))
     nb = C.c_size_t()
     local_S, commb_S, opstatus_S, track_S = opts
-    assert e.emul_decode_sbs1(h, C.c_void_p(frames.ctypes.data), n, 1, LOC[0], LOC[1], local_S, commb_S, opstatus_S, track_S,
-                              20 if track_S else 0, 1, tz, C.c_void_p(recs.ctypes.data), buf, len(buf), C.byref(nb)) == 0
+    o = emul_build.opts(LOC, local_cpr=local_S, commb=commb_S, opstatus=opstatus_S, track=track_S,
+                        track_ext=20 if track_S else 0, sbs1=1, sbs1_tz=tz)
+    assert e.emul_decode(h, C.c_void_p(frames.ctypes.data), n, o, C.c_void_p(recs.ctypes.data)) == 0
+    assert e.emul_sbs1_text(h, n, buf, len(buf), C.byref(nb)) == 0
     want_ids = []
     want = chk.feed(frames, recs, want_ids)
     got = buf.raw[: nb.value]
@@ -77,10 +65,10 @@ def _run(e, calls, opts=(0, 0, 0, 0), tz=0, resets=()):
     out = []
     for i, frames in enumerate(calls):
         if i in resets:
-            e.emul_reset_sbs1(h)
+            e.emul_reset(h)
             chk.reset()
         out.append(_call(e, h, frames, opts, tz, chk))
-    e.emul_free_sbs1(h)
+    e.emul_free(h)
     return b"".join(out), chk
 
 
@@ -141,40 +129,30 @@ def test_reset_then_earlier_stamps(emul):
     assert text.count(b"MSG,") > 0
 
 
-def _mutant(tmp_path, tmp_path_factory, rel, old, new):
-    for sub in ("gr_air_modes_b200/csrc", "include", "tests/simt"):
-        shutil.copytree(os.path.join(ROOT, sub), str(tmp_path / sub))
-    p = tmp_path / rel
-    src = p.read_text()
-    assert src.count(old) == 1
-    p.write_text(src.replace(old, new))
-    return _bind(emul_build.decode_emul(tmp_path_factory, tmp_path / "tests/simt/decode_sbs1_emul.cc"))
-
-
 def test_a_walk_reading_the_table_instead_of_the_earlier_lane_is_caught(tmp_path, tmp_path_factory):
-    e = _mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_sbs1.cuh",
-                "src[k] = before ? (AMB_SBS1_MARK | pk) : slot;", "src[k] = slot; (void)pk;")
+    e = emul_build.mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_sbs1.cuh",
+                          "src[k] = before ? (AMB_SBS1_MARK | pk) : slot;", "src[k] = slot; (void)pk;")
     with pytest.raises(AssertionError):
         _run(e, [tc.frames_of(sc.mix_scene())])
 
 
 def test_a_plain_scan_ignoring_expiry_inside_a_call_is_caught(tmp_path, tmp_path_factory):
-    e = _mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_sbs1.cuh",
-                "amb_sbs1_live(g, G0, base) != amb_sbs1_live(g, G0 + AMB_SBS1_CHUNK, base)) s_amb = 1u;",
-                "false) s_amb = 1u;")
+    e = emul_build.mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_sbs1.cuh",
+                          "amb_sbs1_live(g, G0, base) != amb_sbs1_live(g, G0 + AMB_SBS1_CHUNK, base)) s_amb = 1u;",
+                          "false) s_amb = 1u;")
     with pytest.raises(AssertionError):
         _run(e, [tc.frames_of(m, unqueued_every=0) for m in sc.window_calls()])
 
 
 def test_round_half_up_is_caught(tmp_path, tmp_path_factory):
-    e = _mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_sbs1_format.h",
-                "if (rem > half || (rem == half && (q & 1))) q++;", "if (rem >= half) q++;")
+    e = emul_build.mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_sbs1_format.h",
+                          "if (rem > half || (rem == half && (q & 1))) q++;", "if (rem >= half) q++;")
     with pytest.raises(AssertionError):
         _run(e, [tc.frames_of(sc.mix_scene())])
 
 
 def test_rounded_milliseconds_are_caught(tmp_path, tmp_path_factory):
-    e = _mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_sbs1_format.h",
-                "double msf = floor(f * 1000.0);", "double msf = rint(f * 1000.0);")
+    e = emul_build.mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_sbs1_format.h",
+                          "double msf = floor(f * 1000.0);", "double msf = rint(f * 1000.0);")
     with pytest.raises(AssertionError):
         _run(e, [tc.frames_of(sc.mix_scene())])

@@ -1,15 +1,15 @@
 """The aircraft table extension's KERNEL SOURCE (gr_air_modes_b200/csrc/amb_decode_track_ext.cuh, enqueued by the
 decoder's own amb_decode_launch after the track stage, and read out by amb_snap_count / amb_snap_scan /
-amb_snap_gather_ext) on the host under the SIMT emulator (tests/simt/simt_emul.h), through
-tests/simt/decode_track_ext_emul.cc - the op-status harness plus this option - against the sequential checker
+amb_snap_gather_ext) on the host under the SIMT emulator (tests/simt/simt_emul.h), through the decoder harness
+tests/simt/decode_emul.cc, against the sequential checker
 (tests/track_ext_oracle.py) fed with the same frames and the decoder's own records: snapshots byte for byte after every
 batch and at the end, in several batch splits (single messages, cuts at 31/32/33 inside a 32-record step, random sizes),
-with the local CPR stage on and off. Three mutants must fail: a walk that keeps the first writer of a group instead of
-the last, a snapshot without the first_seen test, and a reset that leaves groups visible."""
+with the local CPR stage on and off. Four mutants must fail: a walk that keeps the first writer of a group instead of
+the last, a snapshot without the first_seen test, a walk that leaves groups of an earlier stream visible after a reset,
+and a reset that leaves the extension's bitmap as it was."""
 import ctypes as C
 import math
 import os
-import shutil
 import sys
 
 import numpy as np
@@ -21,23 +21,12 @@ import track_cases as tc  # noqa: E402
 import track_ext_cases as xc  # noqa: E402
 import track_ext_oracle as xo  # noqa: E402
 
-ROOT = emul_build.ROOT
-HARNESS = os.path.join(ROOT, "tests", "simt", "decode_track_ext_emul.cc")
 OPSTATUS_S, COMMB_S = 30, 30
-
-
-def _bind(e):
-    e.emul_decode_ext.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_int,
-                                  C.c_int, C.c_int, C.c_int, C.c_void_p]
-    e.emul_snapshot_ext.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int, C.c_uint, C.c_void_p, C.c_void_p, C.c_int]
-    e.emul_reset_ext.argtypes = [C.c_void_p]
-    e.emul_free_ext.argtypes = [C.c_void_p]
-    return e
 
 
 @pytest.fixture(scope="module")
 def emul(tmp_path_factory):
-    return _bind(emul_build.decode_emul(tmp_path_factory, HARNESS))
+    return emul_build.decode_emul(tmp_path_factory)
 
 
 def _words(frames):
@@ -51,22 +40,22 @@ def _words(frames):
 def _snapshot(e, h, now, S, S2, words):
     from gr_air_modes_b200 import decode
     now = math.nan if now is None else now
-    n = e.emul_snapshot_ext(h, now, S, S2, words, None, None, 0)
+    n = e.emul_snapshot(h, now, S, S2, words, None, None, 0)
     assert n >= 0
     out = np.zeros(n, dtype=decode.AIRCRAFT_DTYPE)
     ext = np.zeros(n, dtype=decode.AIRCRAFT_EXT_DTYPE)
     if n:
-        assert e.emul_snapshot_ext(h, now, S, S2, words, C.c_void_p(out.ctypes.data), C.c_void_p(ext.ctypes.data),
-                                   n - 1) == -5
+        assert e.emul_snapshot(h, now, S, S2, words, C.c_void_p(out.ctypes.data), C.c_void_p(ext.ctypes.data),
+                               n - 1) == -5
         assert not ext.view(np.uint8).any()
-        assert e.emul_snapshot_ext(h, now, S, S2, words, C.c_void_p(out.ctypes.data), C.c_void_p(ext.ctypes.data),
-                                   n) == n
+        assert e.emul_snapshot(h, now, S, S2, words, C.c_void_p(out.ctypes.data), C.c_void_p(ext.ctypes.data),
+                               n) == n
     return out, ext
 
 
 def _decode(e, h, frames, local_S, S, S2, recs):
-    assert e.emul_decode_ext(h, C.c_void_p(frames.ctypes.data), len(frames), 0, 0.0, 0.0, local_S, COMMB_S, OPSTATUS_S,
-                             S, S2, C.c_void_p(recs.ctypes.data)) == 0
+    opts = emul_build.opts(local_cpr=local_S, commb=COMMB_S, opstatus=OPSTATUS_S, track=S, track_ext=S2)
+    assert e.emul_decode(h, C.c_void_p(frames.ctypes.data), len(frames), opts, C.c_void_p(recs.ctypes.data)) == 0
 
 
 def _run(e, msgs, S, S2, splits, local_S=0, each=False):
@@ -96,7 +85,7 @@ def _run(e, msgs, S, S2, splits, local_S=0, each=False):
     xo.assert_snapshots_equal(final, chk.snapshot_arrays(), "end")
     for now in (ts[n // 2], ts[-1] + S2 / 2):
         xo.assert_snapshots_equal(_snapshot(e, h, now, S, S2, words), chk.snapshot_arrays(now), ("now", now))
-    e.emul_free_ext(h)
+    e.emul_free(h)
     return final
 
 
@@ -153,7 +142,7 @@ def test_a_group_exactly_S2_old_is_shown_and_one_2_to_the_minus_40_older_is_not(
     recs = np.zeros(len(frames), dtype=decode.FIELDS_DTYPE)
     _decode(emul, h, frames, 0, 60, 30, recs)
     rows, ext = _snapshot(emul, h, now, 60, 30, 1024)
-    emul.emul_free_ext(h)
+    emul.emul_free(h)
     xo.assert_snapshots_equal((rows, ext), xo.replay(frames, recs, 60, 30, now), "age edge")
     assert len(rows) == 1
     assert ext["shown"][0] & 0x01 and ext["t"][0][0] == now - 30            # OPS: exactly S2 old
@@ -177,9 +166,9 @@ def _reset_run(e, S=60, S2=600):
     chk = xo.ExtTracker(S, S2)
     for fr, reset in ((fa, False), (fb, True)):
         if reset:
-            e.emul_reset_ext(h)
+            e.emul_reset(h)
             chk.reset()
-            assert e.emul_snapshot_ext(h, math.nan, S, S2, 1024, None, None, 0) == 0
+            assert e.emul_snapshot(h, math.nan, S, S2, 1024, None, None, 0) == 0
         recs = np.zeros(len(fr), dtype=decode.FIELDS_DTYPE)
         _decode(e, h, fr, 0, S, S2, recs)
         chk.feed(fr, recs)
@@ -187,34 +176,24 @@ def _reset_run(e, S=60, S2=600):
         got = _snapshot(e, h, now, S, S2, 1024)
         xo.assert_snapshots_equal(got, chk.snapshot_arrays(now), ("after reset", now))
         assert len(got[0]) == 2 and not np.any(got[1]["shown"].astype(int) & ~AXG_INTEG)
-    e.emul_free_ext(h)
+    e.emul_free(h)
 
 
 def test_reset_forgets_every_group(emul):
     _reset_run(emul)
 
 
-def _mutant(tmp_path, tmp_path_factory, rel, old, new):
-    for sub in ("gr_air_modes_b200/csrc", "include", "tests/simt"):
-        shutil.copytree(os.path.join(ROOT, sub), str(tmp_path / sub))
-    p = tmp_path / rel
-    src = p.read_text()
-    assert src.count(old) == 1
-    p.write_text(src.replace(old, new))
-    return _bind(emul_build.decode_emul(tmp_path_factory, tmp_path / "tests/simt/decode_track_ext_emul.cc"))
-
-
 def test_a_walk_keeping_the_first_writer_is_caught(tmp_path, tmp_path_factory):
-    e = _mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_track_ext.cuh",
-                "if (g == q && (int)lane == 31 - __clz(w)) last = true;",
-                "if (g == q && (int)lane == __ffs(w) - 1) last = true;")
+    e = emul_build.mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_track_ext.cuh",
+                          "if (g == q && (int)lane == 31 - __clz(w)) last = true;",
+                          "if (g == q && (int)lane == __ffs(w) - 1) last = true;")
     with pytest.raises(AssertionError):
         _run(e, xc.burst_scene(), 20, 60, [])
 
 
 def test_a_snapshot_without_the_first_seen_test_is_caught(tmp_path, tmp_path_factory):
-    e = _mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_track_ext.cuh",
-                "if (t >= first && t <= now", "if (t == t && t <= now")
+    e = emul_build.mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_track_ext.cuh",
+                          "if (t >= first && t <= now", "if (t == t && t <= now")
     with pytest.raises(AssertionError):
         _run(e, xc.absence_scene(S=10), 10, 600, [])
 
@@ -222,7 +201,16 @@ def test_a_snapshot_without_the_first_seen_test_is_caught(tmp_path, tmp_path_fac
 def test_a_reset_leaving_groups_visible_is_caught(tmp_path, tmp_path_factory):
     """Mutation: a row written for the first time since reset keeps the times of the groups this step does not
     write, so stream A's groups show after the reset."""
-    e = _mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_track_ext.cuh",
-                "if (!((wrote >> q) & 1u)) row->t[q] = NAN;", "(void)wrote;")
+    e = emul_build.mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_track_ext.cuh",
+                          "if (!((wrote >> q) & 1u)) row->t[q] = NAN;", "(void)wrote;")
+    with pytest.raises(AssertionError):
+        _reset_run(e)
+
+
+def test_a_reset_leaving_the_extension_bitmap_is_caught(tmp_path, tmp_path_factory):
+    """Mutation: amb_decode_reset - the decoder's own reset, which the harness runs - leaves the extension's bitmap as
+    it was, so stream B's rows count as written since the reset and keep stream A's groups."""
+    e = emul_build.mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_kernels.cuh",
+                          "if (st->xocc) AMB_STAGE_TRY", "if (false) AMB_STAGE_TRY")
     with pytest.raises(AssertionError):
         _reset_run(e)

@@ -8,7 +8,6 @@ must fail."""
 import ctypes as C
 import math
 import os
-import shutil
 import sys
 
 import numpy as np
@@ -22,8 +21,6 @@ import local_cpr_cases as lc  # noqa: E402
 import track_cases as tc  # noqa: E402
 import track_oracle as to  # noqa: E402
 
-ROOT = emul_build.ROOT
-
 
 @pytest.fixture(scope="module")
 def emul(tmp_path_factory):
@@ -32,12 +29,14 @@ def emul(tmp_path_factory):
 
 def _snapshot(e, h, now, S):
     from gr_air_modes_b200 import decode
-    n = e.emul_snapshot(h, math.nan if now is None else now, S, WORDS, None, 0)
+    n = e.emul_snapshot(h, math.nan if now is None else now, S, 0, WORDS, None, None, 0)
     assert n >= 0
     out = np.zeros(n, dtype=decode.AIRCRAFT_DTYPE)
     if n:
-        assert e.emul_snapshot(h, math.nan if now is None else now, S, WORDS, C.c_void_p(out.ctypes.data), n - 1) == -5
-        assert e.emul_snapshot(h, math.nan if now is None else now, S, WORDS, C.c_void_p(out.ctypes.data), n) == n
+        assert e.emul_snapshot(h, math.nan if now is None else now, S, 0, WORDS, C.c_void_p(out.ctypes.data), None,
+                               n - 1) == -5
+        assert e.emul_snapshot(h, math.nan if now is None else now, S, 0, WORDS, C.c_void_p(out.ctypes.data), None,
+                               n) == n
     return out
 
 
@@ -47,7 +46,7 @@ def _run(e, msgs, loc, S, splits, local_S=0, each=False, commb_S=0):
     from gr_air_modes_b200 import decode
     frames = tc.frames_of(msgs)
     n = len(frames)
-    have, lat, lon = (0, 0.0, 0.0) if loc is None else (1, loc[0], loc[1])
+    opts = emul_build.opts(loc, local_cpr=local_S, commb=commb_S, track=S)
     h = e.emul_new(17)
     assert h
     tr = to.Tracker(S)
@@ -57,7 +56,7 @@ def _run(e, msgs, loc, S, splits, local_S=0, each=False, commb_S=0):
         c = min(c, n - pos)
         if c <= 0:
             break
-        assert e.emul_decode(h, C.c_void_p(frames.ctypes.data + 80 * pos), c, have, lat, lon, local_S, commb_S, S,
+        assert e.emul_decode(h, C.c_void_p(frames.ctypes.data + 80 * pos), c, opts,
                              C.c_void_p(recs.ctypes.data + 144 * pos)) == 0
         tr.feed(frames[pos:pos + c], recs[pos:pos + c])
         if each:
@@ -69,8 +68,8 @@ def _run(e, msgs, loc, S, splits, local_S=0, each=False, commb_S=0):
     for now in (ts[n // 2], ts[-1] + S / 2):
         to.assert_rows_equal(_snapshot(e, h, now, S), tr.snapshot_array(now), ("now", now))
     e.emul_reset(h)
-    assert e.emul_snapshot(h, math.nan, S, WORDS, None, 0) == 0
-    assert e.emul_snapshot(h, ts[-1], S, WORDS, None, 0) == 0
+    assert e.emul_snapshot(h, math.nan, S, 0, WORDS, None, None, 0) == 0
+    assert e.emul_snapshot(h, ts[-1], S, 0, WORDS, None, None, 0) == 0
     e.emul_free(h)
     return final, recs
 
@@ -132,13 +131,7 @@ def test_one_address_with_long_runs_in_a_step(emul):
 def test_a_walk_without_the_expiry_test_is_caught(tmp_path, tmp_path_factory):
     """Mutation: a row never expires, so a record after a silence keeps the old row instead of starting a new one (or
     of being ignored)."""
-    for sub in ("gr_air_modes_b200/csrc", "include", "tests/simt"):
-        shutil.copytree(os.path.join(ROOT, sub), str(tmp_path / sub))
-    p = tmp_path / "gr_air_modes_b200/csrc/amb_decode_track.cuh"
-    src = p.read_text()
-    a = "const bool alive = live && !(t - seen > (double)max_age);"
-    assert src.count(a) == 1
-    p.write_text(src.replace(a, "const bool alive = live;"))
-    e = emul_build.decode_emul(tmp_path_factory, tmp_path / "tests/simt/decode_emul.cc")
+    e = emul_build.mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_track.cuh",
+                          "const bool alive = live && !(t - seen > (double)max_age);", "const bool alive = live;")
     with pytest.raises(AssertionError):
         _run(e, tc.burst_scene(), None, 3, [])
