@@ -1,7 +1,7 @@
 // Host side of libairmodes_b200.so: stream context, per-call orchestration and the C ABI declared in
 // include/airmodes_b200.h. No CPU implementation of the hot path lives here: every compute entry point
 // launches the kernels in amb_kernels.cu or fails. Citations are file:line under gr-air-modes.
-#include "amb_internal.h"
+#include "amb_chain.h"
 #include "amb_params.h"
 #include "amb_order_kernels.cuh"
 
@@ -56,7 +56,7 @@ struct amb_ctx {
     int chip_off[240];
     int kc = 0, guard = 0;
     float2* carry[3] = {nullptr, nullptr, nullptr};   // [2] stays all zero (sample history before the stream)
-    float2* tail[2] = {nullptr, nullptr}; int tail_cap = 0;
+    float2* tail[2] = {nullptr, nullptr};   // AMB_TAIL_CAP samples each
     float2* staging = nullptr; size_t staging_cap = 0;
     // host ingest pipeline (amb_process with host memory): ring of pinned + device chunk buffers, copy stream
     cudaStream_t stream_h = nullptr;
@@ -78,13 +78,8 @@ struct amb_ctx {
     // optional DC blocker (rx_path.py:39-41)
     int use_dcblock = 0, dc_D = 0, dc_nc = 0, dc_cur = 0;
     float2* dc_carry[2] = {nullptr, nullptr}; float2* dc_out = nullptr; float2* dc_ma0 = nullptr; size_t dc_cap = 0;
-    uint32_t* coarse[2] = {nullptr, nullptr}; uint32_t* fine[2] = {nullptr, nullptr}; uint32_t* span_count[2] = {nullptr, nullptr};
-    size_t rows_cap = 0; int spans_cap = 0;
-    int* cand_j = nullptr; uint32_t* cand_info = nullptr; float* cand_avg = nullptr; unsigned cand_cap = 0;
-    int* det_list = nullptr;
-    void* walk_scratch = nullptr;
-    amb_frame* frames = nullptr; unsigned frame_cap = 0; unsigned frames_ub = 0;
-    float* chips = nullptr; bool keep_chips = false;
+    AmbChainBufs bufs;                   // bitmaps, candidates, frames, chips, ap_filter state (amb_chain.h)
+    bool keep_chips = false;
     AmbCounters* ctr = nullptr; AmbWalkState* st = nullptr;
     // stream state
     uint64_t n_in = 0; long long r_done = 0; bool flushed = false;
@@ -105,14 +100,13 @@ struct amb_ctx {
     int ec = 0;                          // option "ec": error correction over up to K low-confidence bits (0 = off)
     int ec_any = 0;                      // option "ec_any": DF17 correction over up to M (1, 2) bits anywhere (0 = off)
     int ap_filter = 0;                   // option "ap_filter": address/parity check against the last S seconds (0 = off)
-    AmbApState ap{};                     // its device state (allocated at the first call with the option on)
     bool seeked = false;                 // positioned by amb_seek since the last reset (no "ap_filter" there)
     // time-sharded operation (amb_seek / amb_resolve): a call whose walk + slice stages are still to run
     int defer = 0;                       // option "defer_resolve"
     int def_kind = 0;                    // 0 nothing pending, 1 full (walk + slice), 2 sequential walk only, 3 state only
-    int def_set = 0; bool def_par = false; long long def_nsamp = 0;
+    int def_set = 0;
     bool def_resolved = false;           // resolved once already: amb_resolve again = re-resolution with another entry
-    AmbWalkArgs def_wa{}; AmbSliceArgs def_sl{};
+    AmbChainSpan def{};                  // what its walk + slice stages read
     std::string err;
 };
 
@@ -160,23 +154,13 @@ static int make_tmap(amb_ctx* ctx, CUtensorMap* m, const void* base, size_t n_sa
     return AMB_OK;
 }
 
-static void free_dev(amb_ctx* c)
+static int chain_fail(amb_ctx* c, const AmbChainErr& er) { return fail(c, AMB_ERR_CUDA, er.what, er.e); }
+
+// The options the call's sparse kernels run with
+static AmbChainOpts chain_opts(const amb_ctx* c)
 {
-    for (int k = 0; k < 3; k++) { cudaFree(c->carry[k]); c->carry[k] = nullptr; }
-    for (int k = 0; k < 2; k++) {
-        cudaFree(c->tail[k]); cudaFree(c->coarse[k]); cudaFree(c->fine[k]); cudaFree(c->span_count[k]);
-        c->tail[k] = nullptr; c->coarse[k] = c->fine[k] = c->span_count[k] = nullptr;
-    }
-    cudaFree(c->staging);
-    cudaFree(c->dc_carry[0]); cudaFree(c->dc_carry[1]); cudaFree(c->dc_out); cudaFree(c->dc_ma0);
-    c->dc_carry[0] = c->dc_carry[1] = c->dc_out = c->dc_ma0 = nullptr; c->dc_cap = 0;
-    cudaFree(c->cand_j); cudaFree(c->cand_info); cudaFree(c->cand_avg); cudaFree(c->walk_scratch); c->walk_scratch = nullptr;
-    cudaFree(c->det_list); c->det_list = nullptr;
-    cudaFree(c->frames); cudaFree(c->chips); cudaFree(c->ctr); cudaFree(c->st);
-    c->staging = nullptr;
-    c->cand_j = nullptr; c->cand_info = nullptr; c->cand_avg = nullptr;
-    c->frames = nullptr; c->chips = nullptr; c->ctr = nullptr; c->st = nullptr;
-    c->rows_cap = 0; c->spans_cap = 0; c->cand_cap = 0; c->frame_cap = 0; c->staging_cap = 0;
+    return AmbChainOpts{c->sm_count, c->resolver != 1, c->exact_dense, c->keep_chips, c->ec, c->ec_any, c->ap_filter,
+                        c->P.rate_int};
 }
 
 static int setup_rate(amb_ctx* ctx)
@@ -187,9 +171,8 @@ static int setup_rate(amb_ctx* ctx)
     ctx->P = P;
     memcpy(ctx->chip_off, off, sizeof off);
     CK(amb_upload_tables(off));
-    ctx->guard = P.maxlate + (int)ceilf(P.skip_f) + 4;
-    int need = ctx->guard + P.L + 2 * P.spc_i + 64;
-    ctx->kc = (need + AMB_STAGE - 1) / AMB_STAGE * AMB_STAGE;
+    ctx->guard = amb_chain_guard(P);
+    ctx->kc = amb_chain_carry(P);
     if (ctx->use_dcblock) {                              // filter.dc_blocker_cc(100*self._spc, False)  rx_path.py:40
         ctx->dc_D = 100 * P.spc_i;
         ctx->dc_nc = 2 * ctx->dc_D - 2;
@@ -198,7 +181,6 @@ static int setup_rate(amb_ctx* ctx)
             CK(cudaMalloc(&ctx->dc_carry[k], (size_t)ctx->dc_nc * sizeof(float2)));
         }
     }
-    ctx->tail_cap = 4 * AMB_STAGE;
     for (int k = 0; k < 3; k++) {
         cudaFree(ctx->carry[k]); ctx->carry[k] = nullptr;
         CK(cudaMalloc(&ctx->carry[k], (size_t)ctx->kc * sizeof(float2)));
@@ -207,8 +189,8 @@ static int setup_rate(amb_ctx* ctx)
     }
     for (int k = 0; k < 2; k++) {
         cudaFree(ctx->tail[k]); ctx->tail[k] = nullptr;
-        CK(cudaMalloc(&ctx->tail[k], (size_t)ctx->tail_cap * sizeof(float2)));
-        int rc2 = make_tmap(ctx, &ctx->tm_tail[k], ctx->tail[k], (size_t)ctx->tail_cap); if (rc2) return rc2;
+        CK(cudaMalloc(&ctx->tail[k], (size_t)AMB_TAIL_CAP * sizeof(float2)));
+        int rc2 = make_tmap(ctx, &ctx->tm_tail[k], ctx->tail[k], (size_t)AMB_TAIL_CAP); if (rc2) return rc2;
     }
     return AMB_OK;
 }
@@ -226,17 +208,14 @@ static int reset_stream(amb_ctx* ctx)
     }
     ctx->sf0.clear(); ctx->sf1.clear(); ctx->sf_total = 0; ctx->sf_rdone = 0;
     ctx->carry_in = 2; ctx->n_in = 0; ctx->r_done = 0; ctx->flushed = false; ctx->have_last = false;
-    ctx->frames_ub = 0;
     ctx->pending.clear();
     ctx->def_kind = 0; ctx->def_resolved = false;
     ctx->pend_n = 0;                                   // samples gathered but not dispatched belong to the old stream
     ctx->snap_tail = ctx->snap_head; ctx->polled = 0;
     ctx->time_tags.clear();
     ctx->seeked = false;
-    if (ctx->ap.last) {                // confirmed addresses belong to the stream; the option itself stays
-        CK(cudaMemsetAsync(ctx->ap.last, 0, sizeof(unsigned long long) << 24, ctx->stream_b));
-        CK(cudaMemsetAsync(ctx->ap.count, 0, AMB_AP_BUCKETS * sizeof(unsigned), ctx->stream_b));
-    }
+    AmbChainErr er;
+    if (amb_chain_reset(&ctx->bufs, ctx->stream_b, &er) < 0) return chain_fail(ctx, er);
     return AMB_OK;
 }
 
@@ -318,10 +297,13 @@ void amb_destroy(amb_ctx* ctx)
     cudaSetDevice(ctx->device);
     if (ctx->stream) sync_all(ctx);
     if (ctx->stream_h) { cudaStreamSynchronize(ctx->stream_h); }
-    free_dev(ctx);
+    for (int k = 0; k < 3; k++) cudaFree(ctx->carry[k]);
+    cudaFree(ctx->tail[0]); cudaFree(ctx->tail[1]); cudaFree(ctx->staging);
+    cudaFree(ctx->dc_carry[0]); cudaFree(ctx->dc_carry[1]); cudaFree(ctx->dc_out); cudaFree(ctx->dc_ma0);
+    cudaFree(ctx->ctr); cudaFree(ctx->st);
+    amb_chain_free(&ctx->bufs);
     ingest_free(ctx);
     cudaFree(ctx->ord_key); cudaFree(ctx->ord_val); cudaFree(ctx->tags_dev);
-    cudaFree(ctx->ap.last); cudaFree(ctx->ap.count); cudaFree(ctx->ap.off); cudaFree(ctx->ap.cursor); cudaFree(ctx->ap.ent);
     if (ctx->stream_h) cudaStreamDestroy(ctx->stream_h);
     if (ctx->ctr_snap) cudaFreeHost(ctx->ctr_snap);
     for (int k = 0; k < AMB_SNAPS; k++) if (ctx->snap_ev[k]) cudaEventDestroy(ctx->snap_ev[k]);
@@ -395,7 +377,7 @@ int amb_query_geometry(float rate, float threshold_db, int use_pmf, amb_geometry
     out->pmf_len = use_pmf ? P.spc_i : 1; out->floor_len = P.L;
     out->chip_offset_239 = off[239];
     out->shard_back = P.H + P.L + P.spc_i;                         // block history + floor window + PMF window
-    out->shard_fwd = P.maxlate + (int)ceilf(P.skip_f) + 4 - P.H;   // = the streaming guard, in sample coordinates
+    out->shard_fwd = amb_chain_guard(P) - P.H;                    // the streaming guard, in sample coordinates
     return AMB_OK;
 }
 
@@ -464,121 +446,6 @@ int amb_synchronize(amb_ctx* ctx)
     return AMB_OK;
 }
 
-// Candidate capacity for a call that evaluates `len` start positions. Up to 2^25 positions (24 bytes per candidate
-// over the five arrays = 800 MB) the list can hold every position, so not even a flood of candidates (all-pass
-// filter on denormal-power input, DESIGN.md) can overflow it; longer calls get len / 8, at least 2^25.
-static unsigned cand_capacity(long long len)
-{
-    const long long big = 1ll << 25;
-    const long long cap = len <= big ? len : std::max<long long>(len / 8, big);
-    return (unsigned)std::max<long long>(1 << 16, cap + 1024);
-}
-
-// Grow the per-call scratch (bitmaps, span counts, candidate arrays, frame buffer). Growth synchronises both
-// streams; in steady state nothing happens here.
-static int ensure_call_buffers(amb_ctx* ctx, size_t rows_need, int n_spans, unsigned cap_need, unsigned fr_ub)
-{
-    if (ctx->rows_cap < rows_need) {
-        CK(sync_all(ctx));
-        const size_t rc = rows_need + rows_need / 8;
-        for (int k = 0; k < 2; k++) {
-            cudaFree(ctx->fine[k]); cudaFree(ctx->coarse[k]); ctx->fine[k] = ctx->coarse[k] = nullptr;
-            CK(cudaMalloc(&ctx->fine[k], rc * 8 * sizeof(uint32_t)));
-            CK(cudaMalloc(&ctx->coarse[k], (rc / 32 + 2) * sizeof(uint32_t)));
-        }
-        ctx->rows_cap = rc;
-    }
-    if (ctx->spans_cap < n_spans) {
-        CK(sync_all(ctx));
-        for (int k = 0; k < 2; k++) {
-            cudaFree(ctx->span_count[k]); ctx->span_count[k] = nullptr;
-            CK(cudaMalloc(&ctx->span_count[k], (size_t)(n_spans + 64 + 128) * sizeof(uint32_t)));
-        }
-        ctx->spans_cap = n_spans + 64;
-    }
-    if (ctx->cand_cap < cap_need) {
-        CK(sync_all(ctx));
-        cudaFree(ctx->cand_j); cudaFree(ctx->cand_info); cudaFree(ctx->cand_avg); cudaFree(ctx->walk_scratch); cudaFree(ctx->det_list);
-        ctx->cand_j = nullptr; ctx->cand_info = nullptr; ctx->cand_avg = nullptr; ctx->walk_scratch = nullptr; ctx->det_list = nullptr;
-        CK(cudaMalloc(&ctx->det_list, (size_t)cap_need * sizeof(int)));
-        CK(cudaMalloc(&ctx->walk_scratch, amb_walk_scratch_bytes(cap_need, (long long)cap_need * 8 + 4096)));
-        CK(cudaMalloc(&ctx->cand_j, (size_t)cap_need * sizeof(int)));
-        CK(cudaMalloc(&ctx->cand_info, (size_t)cap_need * sizeof(uint32_t)));
-        CK(cudaMalloc(&ctx->cand_avg, (size_t)cap_need * sizeof(float)));
-        ctx->cand_cap = cap_need;
-    }
-    // a detection consumes >= skip0 samples (preamble_impl.cc:237): that bounds the frames of a call
-    if (ctx->frame_cap < ctx->frames_ub + fr_ub) {
-        CK(sync_all(ctx));
-        const unsigned ncap = (ctx->frames_ub + fr_ub) * 2 + 1024;
-        amb_frame* nf = nullptr; float* nc = nullptr;
-        CK(cudaMalloc(&nf, (size_t)ncap * sizeof(amb_frame)));
-        if (ctx->frames && ctx->frames_ub) CK(cudaMemcpy(nf, ctx->frames, (size_t)std::min(ctx->frames_ub, ctx->frame_cap) * sizeof(amb_frame), cudaMemcpyDeviceToDevice));
-        if (ctx->keep_chips) {
-            CK(cudaMalloc(&nc, (size_t)ncap * 240 * sizeof(float)));
-            if (ctx->chips && ctx->frames_ub) CK(cudaMemcpy(nc, ctx->chips, (size_t)std::min(ctx->frames_ub, ctx->frame_cap) * 240 * sizeof(float), cudaMemcpyDeviceToDevice));
-        }
-        cudaFree(ctx->frames); cudaFree(ctx->chips);
-        ctx->frames = nf; ctx->chips = nc; ctx->frame_cap = ncap;
-    }
-    if (ctx->keep_chips && !ctx->chips) CK(cudaMalloc(&ctx->chips, (size_t)ctx->frame_cap * 240 * sizeof(float)));
-    return AMB_OK;
-}
-
-// The slicer stage of every path: slice, then - with option "ec" or "ec_any" on - correct the frames it dropped for
-// their CRC, in place (one launch for both passes), then - with "ap_filter" on, fused paths only - check the address/parity
-// replies against the confirmed addresses (four launches). Everything that reads frames or the call's counters (polls,
-// drain, walk summaries, completion events) is enqueued after this on the same stream.
-static cudaError_t launch_ec_if_on(amb_ctx* ctx, amb_frame* frames, unsigned frame_cap, AmbCounters* ctr, int n, cudaStream_t s)
-{
-    if (!ctx->ec && !ctx->ec_any) return cudaSuccess;
-    ctx->stats.kernel_launches += 1;
-    return amb_launch_ec(frames, frame_cap, ctr, n, ctx->ec, ctx->ec_any, ctx->sm_count, s);
-}
-static cudaError_t launch_ap_if_on(amb_ctx* ctx, amb_frame* frames, unsigned frame_cap, AmbCounters* ctr, cudaStream_t s)
-{
-    if (!ctx->ap_filter) return cudaSuccess;
-    AmbApState& ap = ctx->ap;
-    cudaError_t e = cudaSuccess;
-    if (!ap.last) {                    // first call with the option on: 128 MiB table of 2^24 addresses, zeroed in order
-        unsigned long long* last = nullptr;
-        e = cudaMalloc(&last, sizeof(unsigned long long) << 24);
-        if (e == cudaSuccess) e = cudaMalloc(&ap.count, AMB_AP_BUCKETS * sizeof(unsigned));
-        if (e == cudaSuccess) e = cudaMalloc(&ap.off, AMB_AP_BUCKETS * sizeof(unsigned));
-        if (e == cudaSuccess) e = cudaMalloc(&ap.cursor, AMB_AP_BUCKETS * sizeof(unsigned));
-        if (e == cudaSuccess) e = cudaMemsetAsync(last, 0, sizeof(unsigned long long) << 24, s);
-        if (e == cudaSuccess) e = cudaMemsetAsync(ap.count, 0, AMB_AP_BUCKETS * sizeof(unsigned), s);
-        if (e != cudaSuccess) {        // all or nothing: the next call tries again
-            cudaFree(last); cudaFree(ap.count); cudaFree(ap.off); cudaFree(ap.cursor);
-            ap.count = ap.off = ap.cursor = nullptr;
-            return e;
-        }
-        ap.last = last;
-    }
-    if (ap.ent_cap < frame_cap) {      // grows with the frame buffer (which synchronised when it grew)
-        if ((e = cudaStreamSynchronize(s)) != cudaSuccess) return e;
-        cudaFree(ap.ent); ap.ent = nullptr; ap.ent_cap = 0;
-        if ((e = cudaMalloc(&ap.ent, (size_t)frame_cap * sizeof(AmbApEntry))) != cudaSuccess) return e;
-        ap.ent_cap = frame_cap;
-    }
-    const unsigned long long window = (unsigned long long)ctx->ap_filter * (unsigned long long)ctx->P.rate_int;
-    ctx->stats.kernel_launches += amb_launch_ap(frames, frame_cap, ctr, ap, window, ctx->sm_count, s, &e);
-    return e;
-}
-static cudaError_t slice_and_correct(amb_ctx* ctx, const AmbSliceArgs& sl, cudaStream_t s)
-{
-    cudaError_t e = amb_launch_slice(sl, ctx->sm_count, s);
-    if (e == cudaSuccess) e = launch_ec_if_on(ctx, sl.frames, sl.frame_cap, sl.ctr, 0, s);
-    if (e == cudaSuccess) e = launch_ap_if_on(ctx, sl.frames, sl.frame_cap, sl.ctr, s);
-    return e;
-}
-static cudaError_t slice_chips_and_correct(amb_ctx* ctx, const float* chips, int ndet, amb_frame* frames, cudaStream_t s)
-{
-    cudaError_t e = amb_launch_slice_chips(chips, ndet, frames, s);
-    if (e == cudaSuccess) e = launch_ec_if_on(ctx, frames, (unsigned)ndet, nullptr, ndet, s);
-    return e;
-}
-
 // One call of the chain over n_complex samples that are in DEVICE memory (or, mem_kind == AMB_MEM_HOST, in host
 // memory that goes through the one-piece staging buffer: the deferred / time-sharded mode only).
 static int process_core(amb_ctx* ctx, const float* iq, size_t n_complex, int mem_kind, int flush)
@@ -636,95 +503,65 @@ static int process_core(amb_ctx* ctx, const float* iq, size_t n_complex, int mem
         CK(cudaEventRecord(ctx->e_in, sa));
         CK(cudaStreamWaitEvent(sc, ctx->e_in, 0));
     }
-    const int n_new = (int)n_complex;
-    const int n_main = n_new & ~(AMB_STAGE - 1);
-    const int n_tv = n_new - n_main;
-    const int n_tail = (n_tv + 512 + AMB_STAGE - 1) / AMB_STAGE * AMB_STAGE;   // <= 3 tiles
-
+    const AmbSegs S = amb_chain_segs(ctx->carry[ctx->carry_in], kc, src, (int)n_complex, ctx->tail[set]);
+    const int n_tv = (int)n_complex - S.n_main;
     const int cin = ctx->carry_in;                         // carry this call reads
     const int cout = (cin == 0) ? 1 : 0;                   // carry this call writes (never the zero buffer [2])
-    AmbSegs S;
-    S.carry = ctx->carry[cin]; S.main_ = src; S.tail = ctx->tail[set];
-    S.n_carry = kc; S.n_main = n_main; S.n_tail = n_tail; S.n_valid = kc + n_new;
 
     const long long org = (long long)ctx->n_in - kc + P.H;        // reported index of j = 0
-    const long long n_after = (long long)ctx->n_in + n_new;
+    const long long n_after = (long long)ctx->n_in + (long long)n_complex;
     long long j_lo = ctx->r_done - org;
     long long j_hi, r_safe = 0, ntot = 0;
     if (flush) { ntot = n_after + P.H; j_hi = S.n_valid; }
     else { r_safe = n_after + P.H - ctx->guard; if (r_safe < ctx->r_done) r_safe = ctx->r_done; j_hi = r_safe - org; }
     ctx->last_org = org; ctx->have_last = true;
 
-    AmbWalkArgs wa{};
-    wa.P = P; wa.org = org; wa.ntot = ntot; wa.r_safe = r_safe; wa.flush = flush ? 1 : 0;
-    wa.ctr = ctx->ctr; wa.st = ctx->st; wa.sm_count = ctx->sm_count;
+    AmbChainCall call{};
+    call.P = P; call.S = S; call.org = org; call.ntot = ntot; call.r_safe = r_safe; call.flush = flush ? 1 : 0;
+    call.ctr = ctx->ctr; call.st = ctx->st; call.n_samples = (long long)S.n_carry + S.n_main + S.n_tail;
+    const AmbChainOpts opts = chain_opts(ctx);
+    AmbChainErr er;
 
     if (j_hi > j_lo) {
         AmbScanArgs a{};
-        a.P = P; a.S = S; a.j_lo = (int)j_lo; a.j_hi = (int)j_hi;
-        a.row_lo = (int)(j_lo / AMB_ROW) & ~(AMB_SPAN_ROWS_ALIGN - 1);
-        a.row_hi = (int)((j_hi + AMB_ROW - 1) / AMB_ROW);
-        const int rows = a.row_hi - a.row_lo;
-        const int target = (ctx->scan_ctas > 0 ? ctx->scan_ctas : ctx->sm_count * 4) * 4;    // one warp per span, 4 warps per CTA
-        int rps = (rows + target - 1) / target;
-        rps = (rps + AMB_SPAN_ROWS_ALIGN - 1) / AMB_SPAN_ROWS_ALIGN * AMB_SPAN_ROWS_ALIGN;
-        if (rps < AMB_SPAN_ROWS_ALIGN) rps = AMB_SPAN_ROWS_ALIGN;
-        a.rows_per_span = rps;
-        a.n_spans = (rows + rps - 1) / rps;
-        // ---- buffers (growth synchronises both streams; steady state does not)
-        const unsigned fr_ub = (unsigned)((j_hi - j_lo) / std::max(P.skip0, 1) + 2);
-        { int rc2 = ensure_call_buffers(ctx, (size_t)a.row_hi + 64, a.n_spans,
-                                        cand_capacity(j_hi - j_lo), fr_ub); if (rc2) return rc2; }
-        ctx->frames_ub += fr_ub;
-        a.coarse = ctx->coarse[set]; a.fine = ctx->fine[set]; a.span_count = ctx->span_count[set];
-        a.group_count = ctx->span_count[set] + ctx->spans_cap;     // 128 words behind the span counts
+        a.P = P; a.S = S;
+        amb_chain_geometry(&a, j_lo, j_hi, false, ctx->sm_count, ctx->scan_ctas);
+        // ---- buffers (growth synchronises every stream; steady state does not)
+        const unsigned fr_ub = amb_chain_frame_bound(P, j_hi - j_lo);
+        if (amb_chain_prepare(&ctx->bufs, &a, set, amb_chain_cand_capacity(j_hi - j_lo), fr_ub, ctx->keep_chips,
+                              [ctx] { return sync_all(ctx); }, &er) < 0) return chain_fail(ctx, er);
+        ctx->bufs.frames_ub += fr_ub;
         a.tm_carry = ctx->tm_carry[cin]; a.tm_tail = ctx->tm_tail[set];
-        if (n_main) { int rc2 = make_tmap(ctx, &a.tm_main, src, (size_t)n_main); if (rc2) return rc2; }
+        if (S.n_main) { int rc2 = make_tmap(ctx, &a.tm_main, src, (size_t)S.n_main); if (rc2) return rc2; }
         else a.tm_main = ctx->tm_tail[set];
 
         // ---- stream A: stage the tail + reset the group counts (in front of the scan: a hop over to stream C and
         // back would leave the scan stream idle), then stream over the IQ. Stream C's carry kernel reads the tail.
-        CK(amb_launch_prologue(ctx->tail[set], ctx->tail_cap, src + n_main, n_tv, a.group_count, 128, sa));
+        CK(amb_launch_prologue(ctx->tail[set], AMB_TAIL_CAP, src + S.n_main, n_tv, a.group_count, 128, sa));
+        ctx->stats.kernel_launches += 1;
         CK(cudaEventRecord(ctx->e_in, sa));
         CK(cudaStreamWaitEvent(sc, ctx->e_in, 0));
         if (ctx->aux_valid[set ^ 1]) CK(cudaStreamWaitEvent(sa, ctx->e_aux[set ^ 1], 0));   // carry written by the previous call
         const unsigned slot = (ctx->ring_n & 63u) * 2;
         if (ctx->timing) { CK(cudaEventRecord(ctx->ev[0], sa)); CK(cudaEventRecord(ctx->ring[slot], sa)); }
         CK(amb_launch_scan(a, ctx->sm_count, sa));
+        ctx->stats.kernel_launches += 1;
         if (ctx->timing) { CK(cudaEventRecord(ctx->ev[1], sa)); CK(cudaEventRecord(ctx->ring[slot + 1], sa)); ctx->ring_n++; }
         CK(cudaEventRecord(ctx->e_scan[set], sa));
 
-        // ---- stream B: everything sparse; runs under the NEXT call's scan
+        // ---- stream B: everything sparse; runs under the NEXT call's scan. A time-sharded span stops before the
+        // walk: its loop state arrives later (amb_resolve).
         CK(cudaStreamWaitEvent(sb, ctx->e_scan[set], 0));
-        const bool par = ctx->resolver != 1;
-        CK(amb_launch_compact(a, ctx->cand_j, ctx->cand_cap, ctx->ctr, par ? ctx->walk_scratch : nullptr,
-                              (long long)S.n_carry + S.n_main + S.n_tail, sb));
-        AmbExactArgs ea{};
-        ea.P = P; ea.S = S; ea.cand_j = ctx->cand_j; ea.cand_info = ctx->cand_info; ea.cand_avg = ctx->cand_avg; ea.ctr = ctx->ctr;
-        ea.dense_threshold = ctx->exact_dense;
-        CK(amb_launch_exact(ea, ctx->sm_count, sb));
-        ctx->stats.kernel_launches += 1;      // the exact stage is two launches (sparse / dense regime)
-        wa.cand_j = ctx->cand_j; wa.cand_info = ctx->cand_info; wa.det_list = ctx->det_list;
-        AmbSliceArgs sl{};
-        sl.P = P; sl.S = S; sl.cand_j = ctx->cand_j; sl.cand_info = ctx->cand_info; sl.cand_avg = ctx->cand_avg;
-        sl.det_list = ctx->det_list;
-        sl.ctr = ctx->ctr; sl.frames = ctx->frames; sl.frame_cap = ctx->frame_cap;
-        sl.chips_out = ctx->keep_chips ? ctx->chips : nullptr; sl.org = org;
-        if (ctx->defer) {       // time-sharded span: the loop state arrives later (amb_resolve)
-            ctx->def_kind = 1; ctx->def_resolved = false; ctx->def_set = set; ctx->def_par = par; ctx->def_wa = wa; ctx->def_sl = sl;
-            ctx->def_nsamp = (long long)S.n_carry + S.n_main + S.n_tail;
-            ctx->stats.kernel_launches += 4;
-        } else {
-            if (!par) { CK(amb_launch_walk_seq(wa, sb)); ctx->stats.kernel_launches += 1; }
-            else { CK(amb_launch_walk_par(wa, ctx->walk_scratch, ctx->cand_cap, (long long)S.n_carry + S.n_main + S.n_tail, sb)); ctx->stats.kernel_launches += 3; }
-            CK(slice_and_correct(ctx, sl, sb));
-            ctx->stats.kernel_launches += 5;
-        }
+        const int k = amb_chain_launch(a, call, &ctx->bufs, opts, ctx->defer != 0, sb, &ctx->def, &er);
+        if (k < 0) return chain_fail(ctx, er);
+        ctx->stats.kernel_launches += (uint64_t)k;
+        if (ctx->defer) { ctx->def_kind = 1; ctx->def_resolved = false; ctx->def_set = set; }
         ctx->ev_valid = ctx->timing;
     } else {
         // nothing can be decided yet (tiny call): keep it simple and serial
         if (ctx->done_valid[set ^ 1]) CK(cudaStreamWaitEvent(sa, ctx->e_done[set ^ 1], 0));
-        CK(amb_launch_prologue(ctx->tail[set], ctx->tail_cap, src + n_main, n_tv, nullptr, 0, sa));
+        CK(amb_launch_prologue(ctx->tail[set], AMB_TAIL_CAP, src + S.n_main, n_tv, nullptr, 0, sa));
+        ctx->stats.kernel_launches += 1;
         CK(cudaEventRecord(ctx->e_in, sa));
         CK(cudaStreamWaitEvent(sc, ctx->e_in, 0));
         if (ctx->aux_valid[set ^ 1]) CK(cudaStreamWaitEvent(sa, ctx->e_aux[set ^ 1], 0));
@@ -732,17 +569,16 @@ static int process_core(amb_ctx* ctx, const float* iq, size_t n_complex, int mem
         CK(cudaStreamWaitEvent(sb, ctx->e_scan[set], 0));
         if (ctx->defer) { ctx->def_kind = flush ? 2 : 3; ctx->def_resolved = false; ctx->def_set = set; }
         if (flush) {   // the resolver still has to close the stream
-            if (!ctx->cand_j) {
-                CK(cudaMalloc(&ctx->cand_j, 64 * sizeof(int)));
-                CK(cudaMalloc(&ctx->cand_info, 64 * sizeof(uint32_t)));
-                CK(cudaMalloc(&ctx->cand_avg, 64 * sizeof(float)));
-                CK(cudaMalloc(&ctx->det_list, 64 * sizeof(int)));
-                ctx->cand_cap = 64;
-            }
-            wa.cand_j = ctx->cand_j; wa.cand_info = ctx->cand_info; wa.det_list = ctx->det_list;
+            if (amb_chain_prepare_empty(&ctx->bufs, &er) < 0) return chain_fail(ctx, er);
+            AmbChainSpan& sp = ctx->def;
+            sp.wa = amb_chain_walk_args(call, ctx->bufs, ctx->sm_count);
+            sp.par = false; sp.walk_only = true;
             CK(cudaMemsetAsync(&ctx->ctr->ncand, 0, sizeof(unsigned), sb));
-            if (ctx->defer) ctx->def_wa = wa;
-            else { CK(amb_launch_walk_seq(wa, sb)); ctx->stats.kernel_launches += 1; }
+            if (!ctx->defer) {
+                const int k = amb_chain_resolve(sp, &ctx->bufs, opts, sb, &er);
+                if (k < 0) return chain_fail(ctx, er);
+                ctx->stats.kernel_launches += (uint64_t)k;
+            }
         }
         ctx->ev_valid = false;
     }
@@ -765,7 +601,7 @@ static int process_core(amb_ctx* ctx, const float* iq, size_t n_complex, int mem
     CK(amb_launch_carry(S, ctx->carry[cout], kc, sc));
     CK(cudaEventRecord(ctx->e_aux[set], sc));
     ctx->aux_valid[set] = true;
-    ctx->stats.kernel_launches += 2;
+    ctx->stats.kernel_launches += 1;
     ctx->carry_in = cout;
     ctx->n_in = (uint64_t)n_after;
     if (flush) ctx->flushed = true;
@@ -1031,7 +867,33 @@ int amb_seek(amb_ctx* ctx, uint64_t first_sample, uint64_t first_decision, const
     const long long pos = entry ? (long long)entry->pos : (long long)first_decision;
     const long long p = entry ? (long long)entry->p : (long long)first_decision;
     CK(amb_launch_set_state(ctx->st, pos, p, ctx->stream_b));          // after reset_stream's memset on stream B
+    ctx->stats.kernel_launches += 1;
     ctx->seeked = true;
+    return AMB_OK;
+}
+
+// The deferred call's walk + slice stages on stream B (amb_resolve, amb_resolve_device), from the entry state in
+// entry_dev (device memory, read when the kernel runs) or entry (NULL: where the previous span left the resolver).
+static int resolve_deferred(amb_ctx* ctx, const amb_walk_state* entry, const int64_t* entry_dev)
+{
+    cudaStream_t sb = ctx->stream_b;
+    if (ctx->def_resolved && ctx->def_kind == 1) {     // forget the earlier (speculative) resolution of this span
+        CK(amb_launch_walk_reset(ctx->def.wa, ctx->def.par ? ctx->bufs.walk_scratch : nullptr, ctx->def.n_samples, sb));
+        ctx->stats.kernel_launches += 1;
+    }
+    if (entry_dev) CK(amb_launch_set_state_dev(ctx->st, reinterpret_cast<const long long*>(entry_dev), sb));
+    else if (entry) CK(amb_launch_set_state(ctx->st, (long long)entry->pos, (long long)entry->p, sb));
+    if (entry_dev || entry) ctx->stats.kernel_launches += 1;
+    if (ctx->def_kind != 3) {
+        AmbChainErr er;
+        const int k = amb_chain_resolve(ctx->def, &ctx->bufs, chain_opts(ctx), sb, &er);
+        if (k < 0) return chain_fail(ctx, er);
+        ctx->stats.kernel_launches += (uint64_t)k;
+    }
+    CK(cudaEventRecord(ctx->e_done[ctx->def_set], sb));
+    if (ctx->timing) CK(cudaEventRecord(ctx->ev[3], sb));
+    if (!ctx->overlap) CK(cudaStreamWaitEvent(ctx->stream, ctx->e_done[ctx->def_set], 0));
+    ctx->def_resolved = true;
     return AMB_OK;
 }
 
@@ -1041,26 +903,7 @@ int amb_resolve(amb_ctx* ctx, const amb_walk_state* entry)
     if (!ctx->def_kind) return fail(ctx, AMB_ERR_STATE, "no deferred call to resolve");
     if (ctx->def_resolved && !entry) return fail(ctx, AMB_ERR_INVALID, "re-resolution needs an entry state");
     CK(cudaSetDevice(ctx->device));
-    cudaStream_t sb = ctx->stream_b;
-    if (ctx->def_resolved && ctx->def_kind == 1) {     // forget the earlier (speculative) resolution of this span
-        CK(amb_launch_walk_reset(ctx->def_wa, ctx->def_par ? ctx->walk_scratch : nullptr, ctx->def_nsamp, sb));
-        ctx->stats.kernel_launches += 1;
-    }
-    if (entry) CK(amb_launch_set_state(ctx->st, (long long)entry->pos, (long long)entry->p, sb));
-    if (ctx->def_kind == 1) {
-        if (!ctx->def_par) { CK(amb_launch_walk_seq(ctx->def_wa, sb)); ctx->stats.kernel_launches += 1; }
-        else { CK(amb_launch_walk_par(ctx->def_wa, ctx->walk_scratch, ctx->cand_cap, ctx->def_nsamp, sb)); ctx->stats.kernel_launches += 3; }
-        CK(slice_and_correct(ctx, ctx->def_sl, sb));
-        ctx->stats.kernel_launches += 1;
-    } else if (ctx->def_kind == 2) {
-        CK(amb_launch_walk_seq(ctx->def_wa, sb));
-        ctx->stats.kernel_launches += 1;
-    }
-    CK(cudaEventRecord(ctx->e_done[ctx->def_set], sb));
-    if (ctx->timing) CK(cudaEventRecord(ctx->ev[3], sb));
-    if (!ctx->overlap) CK(cudaStreamWaitEvent(ctx->stream, ctx->e_done[ctx->def_set], 0));
-    ctx->def_resolved = true;
-    return AMB_OK;
+    return resolve_deferred(ctx, entry, nullptr);
 }
 
 int amb_get_walk_state(amb_ctx* ctx, amb_walk_state* out)
@@ -1081,7 +924,7 @@ int amb_get_walk_summary(amb_ctx* ctx, amb_walk_summary* out)
     if (!ctx->def_kind || !ctx->def_resolved) return fail(ctx, AMB_ERR_STATE, "no resolved deferred span");
     CK(cudaSetDevice(ctx->device));
     const bool have = ctx->def_kind == 1;
-    if (have) { CK(amb_launch_walk_summary(ctx->def_wa, ctx->stream_b)); ctx->stats.kernel_launches += 1; }
+    if (have) { CK(amb_launch_walk_summary(ctx->def.wa, ctx->stream_b)); ctx->stats.kernel_launches += 1; }
     CK(cudaStreamSynchronize(ctx->stream_b));
     AmbWalkState st; AmbCounters h;
     CK(cudaMemcpy(&st, ctx->st, sizeof st, cudaMemcpyDeviceToHost));
@@ -1102,8 +945,8 @@ int amb_walk_summary_async(amb_ctx* ctx, int64_t* dev_out6)
     if (!ctx->def_kind || !ctx->def_resolved) return fail(ctx, AMB_ERR_STATE, "no resolved deferred span");
     CK(cudaSetDevice(ctx->device));
     const bool have = ctx->def_kind == 1;
-    if (have) { CK(amb_launch_walk_summary(ctx->def_wa, ctx->stream_b)); ctx->stats.kernel_launches += 1; }
-    AmbWalkArgs wa = ctx->def_wa; wa.st = ctx->st; wa.ctr = ctx->ctr;
+    if (have) { CK(amb_launch_walk_summary(ctx->def.wa, ctx->stream_b)); ctx->stats.kernel_launches += 1; }
+    AmbWalkArgs wa = ctx->def.wa; wa.st = ctx->st; wa.ctr = ctx->ctr;
     CK(amb_launch_pack_summary(wa, ctx->P.i_exact, have ? 1 : 0, reinterpret_cast<long long*>(dev_out6), ctx->stream_b));
     CK(cudaEventRecord(ctx->e_done[ctx->def_set], ctx->stream_b));
     ctx->stats.kernel_launches += 1;
@@ -1132,29 +975,9 @@ int amb_resolve_device(amb_ctx* ctx, const int64_t* entry_dev, void* after_strea
     if (!ctx || !entry_dev) return AMB_ERR_INVALID;
     if (!ctx->def_kind) return fail(ctx, AMB_ERR_STATE, "no deferred call to resolve");
     CK(cudaSetDevice(ctx->device));
-    cudaStream_t sb = ctx->stream_b;
     CK(cudaEventRecord(ctx->e_in, after_stream ? (cudaStream_t)after_stream : ctx->stream));
-    CK(cudaStreamWaitEvent(sb, ctx->e_in, 0));
-    if (ctx->def_resolved && ctx->def_kind == 1) {
-        CK(amb_launch_walk_reset(ctx->def_wa, ctx->def_par ? ctx->walk_scratch : nullptr, ctx->def_nsamp, sb));
-        ctx->stats.kernel_launches += 1;
-    }
-    CK(amb_launch_set_state_dev(ctx->st, reinterpret_cast<const long long*>(entry_dev), sb));
-    if (ctx->def_kind == 1) {
-        if (!ctx->def_par) { CK(amb_launch_walk_seq(ctx->def_wa, sb)); ctx->stats.kernel_launches += 1; }
-        else { CK(amb_launch_walk_par(ctx->def_wa, ctx->walk_scratch, ctx->cand_cap, ctx->def_nsamp, sb)); ctx->stats.kernel_launches += 3; }
-        CK(slice_and_correct(ctx, ctx->def_sl, sb));
-        ctx->stats.kernel_launches += 1;
-    } else if (ctx->def_kind == 2) {
-        CK(amb_launch_walk_seq(ctx->def_wa, sb));
-        ctx->stats.kernel_launches += 1;
-    }
-    CK(cudaEventRecord(ctx->e_done[ctx->def_set], sb));
-    if (ctx->timing) CK(cudaEventRecord(ctx->ev[3], sb));
-    if (!ctx->overlap) CK(cudaStreamWaitEvent(ctx->stream, ctx->e_done[ctx->def_set], 0));
-    ctx->stats.kernel_launches += 1;
-    ctx->def_resolved = true;
-    return AMB_OK;
+    CK(cudaStreamWaitEvent(ctx->stream_b, ctx->e_in, 0));
+    return resolve_deferred(ctx, nullptr, entry_dev);
 }
 
 /* Make a stream wait for everything enqueued so far (no host synchronisation): amb_join = the caller-visible stream,
@@ -1197,7 +1020,7 @@ static int fetch_frames(amb_ctx* ctx, unsigned upto)
     const size_t base = ctx->pending.size();
     const unsigned cnt = upto - ctx->polled;
     ctx->pending.resize(base + cnt);
-    CK(cudaMemcpy(ctx->pending.data() + base, ctx->frames + ctx->polled, (size_t)cnt * sizeof(amb_frame), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(ctx->pending.data() + base, ctx->bufs.frames + ctx->polled, (size_t)cnt * sizeof(amb_frame), cudaMemcpyDeviceToHost));
     std::sort(ctx->pending.begin() + base, ctx->pending.end(),
               [](const amb_frame& x, const amb_frame& y) { return x.sample_index < y.sample_index; });
     for (size_t k = base; k < ctx->pending.size(); k++) stamp(ctx, &ctx->pending[k]);
@@ -1230,7 +1053,7 @@ static int collect(amb_ctx* ctx)
     if (h.nframes) CK(cudaMemset(&ctx->ctr->nframes, 0, sizeof(unsigned)));
     ctx->polled = 0;
     ctx->snap_tail = ctx->snap_head;
-    ctx->frames_ub = 0;
+    ctx->bufs.frames_ub = 0;
     if (ctx->def_kind && ctx->def_resolved) { ctx->def_kind = 0; ctx->def_resolved = false; }   // frames read: span is final
     return AMB_OK;
 }
@@ -1309,7 +1132,7 @@ int amb_drain_device(amb_ctx* ctx, amb_frame* out_dev, int cap)
             CK(cudaMemcpy(ctx->tags_dev, t.data(), (size_t)ntags * sizeof(AmbTagDev), cudaMemcpyHostToDevice));
         }
         cudaError_t e = cudaSuccess;
-        const int launched = amb_launch_order(ctx->frames + ctx->polled, n, npad, ctx->order_tile, ctx->ord_key, ctx->ord_val, out_dev,
+        const int launched = amb_launch_order(ctx->bufs.frames + ctx->polled, n, npad, ctx->order_tile, ctx->ord_key, ctx->ord_val, out_dev,
                                               (unsigned long long)ctx->P.rate_int, ctx->t0_secs, ctx->t0_frac, ctx->tags_dev, ntags,
                                               ctx->stream_b, &e);
         if (e != cudaSuccess) return fail(ctx, AMB_ERR_CUDA, "amb_drain_device launch", e);
@@ -1319,7 +1142,7 @@ int amb_drain_device(amb_ctx* ctx, amb_frame* out_dev, int cap)
     if (h.nframes) CK(cudaMemset(&ctx->ctr->nframes, 0, sizeof(unsigned)));
     ctx->polled = 0;
     ctx->snap_tail = ctx->snap_head;
-    ctx->frames_ub = 0;
+    ctx->bufs.frames_ub = 0;
     if (ctx->def_kind && ctx->def_resolved) { ctx->def_kind = 0; ctx->def_resolved = false; }
     return (int)n;
 }
@@ -1414,14 +1237,14 @@ int amb_debug_candidates(amb_ctx* ctx, uint64_t* index, uint32_t* info, int max)
     if (!ctx) return AMB_ERR_INVALID;
     CK(cudaSetDevice(ctx->device));
     CK(sync_all(ctx));
-    if (!ctx->have_last || !ctx->cand_j) return 0;
+    if (!ctx->have_last || !ctx->bufs.cand_j) return 0;
     AmbCounters h;
     CK(cudaMemcpy(&h, ctx->ctr, sizeof h, cudaMemcpyDeviceToHost));
     const int n = (int)std::min<unsigned>(h.ncand, (unsigned)std::max(max, 0));
     if (n <= 0) return 0;
     std::vector<int> j(n);
-    CK(cudaMemcpy(j.data(), ctx->cand_j, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
-    if (info) CK(cudaMemcpy(info, ctx->cand_info, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(j.data(), ctx->bufs.cand_j, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
+    if (info) CK(cudaMemcpy(info, ctx->bufs.cand_info, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
     if (index) for (int k = 0; k < n; k++) index[k] = (uint64_t)(ctx->last_org + j[k]);
     return n;
 }
@@ -1549,7 +1372,12 @@ int amb_slicer_process(amb_ctx* ctx, const float* chips, int ndet, const uint64_
     CK(cudaMalloc(&f, (size_t)ndet * sizeof(amb_frame)));
     cudaError_t e = cudaMemsetAsync(f, 0, (size_t)ndet * sizeof(amb_frame), ctx->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d, chips, (size_t)ndet * 240 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = slice_chips_and_correct(ctx, d, ndet, f, ctx->stream);
+    if (e == cudaSuccess) e = amb_launch_slice_chips(d, ndet, f, ctx->stream);
+    if (e == cudaSuccess) {
+        AmbChainErr er;
+        const int k = amb_chain_ec(f, (unsigned)ndet, nullptr, ndet, chain_opts(ctx), ctx->stream, &er);
+        if (k < 0) e = er.e; else ctx->stats.kernel_launches += (uint64_t)k;
+    }
     if (e == cudaSuccess) e = cudaMemcpyAsync(out, f, (size_t)ndet * sizeof(amb_frame), cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
     cudaFree(d); cudaFree(f);
@@ -1596,43 +1424,23 @@ int amb_preamble_process(amb_ctx* ctx, const float* in0, const float* in1, size_
         // local reported coordinate j = r - b0; evaluate starts in [r_done, flush ? ntot : r_safe)
         const long long j_lo = ctx->sf_rdone - b0, j_hi = (flush ? ntot : r_safe) - b0;
         AmbScanArgs a{};
-        a.P = P; a.j_lo = (int)j_lo; a.j_hi = (int)std::max(j_hi, j_lo); a.row_lo = 0; a.row_hi = (int)((a.j_hi + AMB_ROW - 1) / AMB_ROW);
-        const int rows = a.row_hi;
-        const int target = ctx->sm_count * 16;
-        int rps = ((rows + target - 1) / target + AMB_SPAN_ROWS_ALIGN - 1) / AMB_SPAN_ROWS_ALIGN * AMB_SPAN_ROWS_ALIGN;
-        if (rps < AMB_SPAN_ROWS_ALIGN) rps = AMB_SPAN_ROWS_ALIGN;
-        a.rows_per_span = rps; a.n_spans = std::max(1, (rows + rps - 1) / rps);
-        ctx->frames_ub = 0;
-        const unsigned fr_ub = (unsigned)((long long)m / std::max(P.skip0, 1) + 2);
-        const bool keep = ctx->keep_chips; ctx->keep_chips = true;
-        rc = ensure_call_buffers(ctx, (size_t)a.row_hi + 64, a.n_spans, cand_capacity((long long)m + P.H), fr_ub);
-        ctx->keep_chips = keep;
-        if (rc != AMB_OK) break;
-        a.coarse = ctx->coarse[0]; a.fine = ctx->fine[0]; a.span_count = ctx->span_count[0];
-        a.group_count = ctx->span_count[0] + ctx->spans_cap;
-        e = cudaMemsetAsync(ctx->coarse[0], 0, ((size_t)a.row_hi / 32 + 2) * sizeof(uint32_t), s);
-        if (e == cudaSuccess) e = cudaMemsetAsync(ctx->span_count[0], 0, (size_t)(ctx->spans_cap + 128) * sizeof(uint32_t), s);
-        if (e == cudaSuccess) e = cudaMemsetAsync(ctx->ctr, 0, sizeof(AmbCounters), s);
-        if (e == cudaSuccess && first) e = cudaMemsetAsync(ctx->st, 0, sizeof(AmbWalkState), s);
-        if (e == cudaSuccess) e = amb_launch_stream_candidates(a, d0, d1, (long long)m, ctx->sm_count, s);
-        if (e == cudaSuccess) e = amb_launch_compact(a, ctx->cand_j, ctx->cand_cap, ctx->ctr, ctx->walk_scratch, (long long)m + P.H + 4096, s);
-        AmbExactArgs ea{};
-        ea.P = P; ea.cand_j = ctx->cand_j; ea.cand_info = ctx->cand_info; ea.cand_avg = ctx->cand_avg; ea.ctr = ctx->ctr;
-        ea.in0 = d0; ea.in1 = d1; ea.n_streams = (long long)m;
-        if (e == cudaSuccess) e = amb_launch_exact(ea, ctx->sm_count, s);
-        AmbWalkArgs wa{};
-        wa.P = P; wa.org = b0; wa.ntot = ntot; wa.r_safe = r_safe; wa.flush = flush ? 1 : 0; wa.ctr = ctx->ctr; wa.st = ctx->st; wa.sm_count = ctx->sm_count;
-        wa.cand_j = ctx->cand_j; wa.cand_info = ctx->cand_info; wa.det_list = ctx->det_list;
-        if (e == cudaSuccess) e = (ctx->resolver == 1) ? amb_launch_walk_seq(wa, s)
-                                                       : amb_launch_walk_par(wa, ctx->walk_scratch, ctx->cand_cap, (long long)m + P.H + 4096, s);
-        AmbSliceArgs sl{};
-        sl.P = P; sl.cand_j = ctx->cand_j; sl.cand_info = ctx->cand_info; sl.cand_avg = ctx->cand_avg; sl.ctr = ctx->ctr;
-        sl.det_list = ctx->det_list;
-        sl.frames = ctx->frames; sl.frame_cap = ctx->frame_cap; sl.chips_out = ctx->chips; sl.org = b0;
-        sl.in0 = d0; sl.in1 = d1; sl.n_streams = (long long)m;
-        if (e == cudaSuccess) e = slice_and_correct(ctx, sl, s);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        ctx->stats.kernel_launches += 8;
+        a.P = P;
+        amb_chain_geometry(&a, j_lo, std::max(j_hi, j_lo), true, ctx->sm_count, 0);
+        ctx->bufs.frames_ub = 0;
+        AmbChainErr er;
+        if (amb_chain_prepare(&ctx->bufs, &a, 0, amb_chain_cand_capacity((long long)m + P.H), amb_chain_frame_bound(P, (long long)m),
+                              true, [ctx] { return sync_all(ctx); }, &er) < 0) { rc = chain_fail(ctx, er); break; }
+        AmbChainCall call{};
+        call.P = P; call.in0 = d0; call.in1 = d1; call.n_streams = (long long)m;
+        call.org = b0; call.ntot = ntot; call.r_safe = r_safe; call.flush = flush ? 1 : 0;
+        call.ctr = ctx->ctr; call.st = ctx->st; call.n_samples = (long long)m + P.H + 4096;
+        AmbChainOpts opts = chain_opts(ctx);
+        opts.keep_chips = true;
+        AmbChainSpan sp;
+        int k = amb_chain_split_scan(a, ctx->bufs, d0, d1, (long long)m, ctx->ctr, first ? ctx->st : nullptr, ctx->sm_count, s, &er);
+        if (k >= 0) { const int k2 = amb_chain_launch(a, call, &ctx->bufs, opts, false, s, &sp, &er); k = k2 < 0 ? -1 : k + k2; }
+        e = k < 0 ? er.e : cudaStreamSynchronize(s);
+        if (k > 0) ctx->stats.kernel_launches += (uint64_t)k;
         if (e != cudaSuccess) { rc = fail(ctx, AMB_ERR_CUDA, "amb_preamble_process", e); break; }
         AmbCounters h;
         e = cudaMemcpy(&h, ctx->ctr, sizeof h, cudaMemcpyDeviceToHost);
@@ -1642,8 +1450,8 @@ int amb_preamble_process(amb_ctx* ctx, const float* in0, const float* in1, size_
         std::vector<amb_frame> fr(nd);
         std::vector<float> ch((size_t)nd * 240);
         if (nd) {
-            e = cudaMemcpy(fr.data(), ctx->frames, (size_t)nd * sizeof(amb_frame), cudaMemcpyDeviceToHost);
-            if (e == cudaSuccess) e = cudaMemcpy(ch.data(), ctx->chips, (size_t)nd * 240 * sizeof(float), cudaMemcpyDeviceToHost);
+            e = cudaMemcpy(fr.data(), ctx->bufs.frames, (size_t)nd * sizeof(amb_frame), cudaMemcpyDeviceToHost);
+            if (e == cudaSuccess) e = cudaMemcpy(ch.data(), ctx->bufs.chips, (size_t)nd * 240 * sizeof(float), cudaMemcpyDeviceToHost);
             if (e != cudaSuccess) { rc = fail(ctx, AMB_ERR_CUDA, "D2H", e); break; }
         }
         std::vector<unsigned> order(nd);
@@ -1655,7 +1463,7 @@ int amb_preamble_process(amb_ctx* ctx, const float* in0, const float* in1, size_
             memcpy(chips_out + (size_t)k * 240, ch.data() + (size_t)order[k] * 240, 240 * sizeof(float));
         }
         cudaMemset(&ctx->ctr->nframes, 0, sizeof(unsigned));
-        ctx->frames_ub = 0;
+        ctx->bufs.frames_ub = 0;
         // keep what a later call still has to look at: items from (r_safe - H) on
         if (flush) { ctx->sf0.clear(); ctx->sf1.clear(); ctx->sf_total = 0; ctx->sf_rdone = 0; }
         else {

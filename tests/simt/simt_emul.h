@@ -149,8 +149,11 @@ struct CUtensorMap { alignas(64) unsigned long long opaque[16]; };
 static unsigned char* simt_dyn_smem = nullptr;       // dynamic shared memory of the running block
 #define AMB_ID(...) __VA_ARGS__
 #define AMB_DYN_SMEM(type, name, align) type* name = reinterpret_cast<type*>(simt_dyn_smem)
+// every AMB_LAUNCH is counted: the library's kernel_launches statistic must equal simt_launch_count()'s growth
+static unsigned long long simt_launches = 0;
+extern "C" unsigned long long simt_launch_count() { return simt_launches; }
 #define AMB_LAUNCH(kernel, grid, block, smem, stream, ...) \
-    simt_launch_dyn((unsigned)(grid), (unsigned)(block), (size_t)(smem), [&] { AMB_ID kernel(__VA_ARGS__); })
+    (simt_launches++, simt_launch_dyn((unsigned)(grid), (unsigned)(block), (size_t)(smem), [&] { AMB_ID kernel(__VA_ARGS__); }))
 
 template <typename T> static inline T min(T a, T b) { return b < a ? b : a; }
 template <typename T> static inline T max(T a, T b) { return a < b ? b : a; }
