@@ -41,6 +41,9 @@ AXG_N = 6
 TRACK_EXT_MAX = 3600
 # SBS-1 feed (decoder options sbs1, sbs1_tz; include/airmodes_b200.h AMB_SBS1_TZ_*)
 SBS1_TZ_MIN, SBS1_TZ_MAX = -720, 840
+# coverage map (decoder option coverage; include/airmodes_b200.h AMB_COVERAGE_*)
+COVERAGE_ROWS, COVERAGE_BANDS = 72, 9
+COVERAGE_ALTITUDES = (0, 1000, 2000, 5000, 10000, 15000, 20000, 25000, 30000)
 ERR_OVERFLOW = -5                # AMB_ERR_OVERFLOW: the buffer is too small (amb_decoder_sbs1 reports the size needed)
 
 
@@ -222,6 +225,9 @@ SYMBOLS = [
     ("amb_decoder_aircraft_ext_device", C.c_int, [_vp, C.c_double, _vp, _vp, C.c_int]),
     ("amb_decoder_sbs1", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("amb_decoder_sbs1_device", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("amb_decoder_coverage", C.c_int, [_vp, _vp]),
+    ("amb_decoder_coverage_device", C.c_int, [_vp, _vp]),
+    ("amb_decoder_coverage_reset", C.c_int, [_vp]),
     ("amb_decoder_stats", C.c_int, [_vp, _u64p, _f32p]),
     ("amb_decoder_last_error", C.c_char_p, [_vp]),
     ("amb_frame_bits", C.c_uint64, [C.POINTER(Frame), C.c_int, C.c_int]),

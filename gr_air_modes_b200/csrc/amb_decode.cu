@@ -15,6 +15,9 @@
 // With option "local_cpr" on, six more (amb_decode_local.cuh): amb_local_keys, the four partition kernels of the pairing
 // stage on ICAO keys, amb_local_walk - the local decode of the position messages the global decode left without a fix,
 // with a direct-mapped table of reference positions in HBM (2^24 x 24 B) carried from batch to batch.
+// With option "coverage" on, one more right after those (amb_decode_coverage.cuh): amb_coverage_kernel - the greatest
+// range per 5-degree bearing sector and altitude band of az_map_model, folded into a 72 x 9 grid in HBM (5184 B) by
+// shared and global atomicMax on the bits of the ranges, carried from batch to batch; amb_decoder_coverage copies it out.
 // With option "commb" on, six more after those (amb_decode_commb.cuh): amb_commb_keys, the four partition kernels on
 // address keys, amb_commb_walk - Comm-B register inference of the DF20/21 replies the parser does not handle, with a
 // direct-mapped table of ADS-B velocities in HBM (2^24 x 24 B) carried from batch to batch.
@@ -236,6 +239,11 @@ int amb_decoder_set_option(amb_decoder* d, const char* name, int value)
         d->st.sbs1 = value;
         return AMB_OK;
     }
+    if (strcmp(name, "coverage") == 0) {
+        if (value != 0 && value != 1) return dfail(d, AMB_ERR_INVALID, "coverage: 0 (off) or 1 (on)");
+        d->st.coverage = value;
+        return AMB_OK;
+    }
     if (strcmp(name, "sbs1_tz") == 0) {
         if (value < AMB_SBS1_TZ_MIN || value > AMB_SBS1_TZ_MAX)
             return dfail(d, AMB_ERR_INVALID, "sbs1_tz: -720 .. 840 minutes");
@@ -416,6 +424,45 @@ int amb_decoder_sbs1(amb_decoder* d, char* out, size_t cap, size_t* n_bytes)
 int amb_decoder_sbs1_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes)
 {
     return sbs1_impl(d, out_dev, cap, n_bytes, true);
+}
+
+// the coverage grid into out (host or device memory); all zeros while the grid is not allocated yet
+static int coverage_impl(amb_decoder* d, double* out, bool out_on_device)
+{
+    const char* fn = out_on_device ? "amb_decoder_coverage_device" : "amb_decoder_coverage";
+    char what[96];
+    if (!d || !out) { snprintf(what, sizeof what, "%s: bad argument", fn); return dfail(d, AMB_ERR_INVALID, what); }
+    if (d->st.coverage <= 0) { snprintf(what, sizeof what, "%s: option coverage is off", fn); return dfail(d, AMB_ERR_STATE, what); }
+    const size_t bytes = AMB_COVERAGE_CELLS * sizeof(double);
+    static_assert(sizeof(double) == sizeof(unsigned long long), "coverage cell layout");
+    if (!d->st.cgrid && !out_on_device) { memset(out, 0, bytes); return AMB_OK; }
+    DCK(cudaSetDevice(d->device));
+    cudaStream_t s = d->stream;
+    if (!d->st.cgrid) DCK(cudaMemsetAsync(out, 0, bytes, s));
+    else DCK(cudaMemcpyAsync(out, d->st.cgrid, bytes, out_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s));
+    DCK(cudaStreamSynchronize(s));
+    return AMB_OK;
+}
+
+int amb_decoder_coverage(amb_decoder* d, double* out)
+{
+    return coverage_impl(d, out, false);
+}
+
+int amb_decoder_coverage_device(amb_decoder* d, double* out_dev)
+{
+    return coverage_impl(d, out_dev, true);
+}
+
+int amb_decoder_coverage_reset(amb_decoder* d)
+{
+    if (!d) return AMB_ERR_INVALID;
+    if (d->st.coverage <= 0) return dfail(d, AMB_ERR_STATE, "amb_decoder_coverage_reset: option coverage is off");
+    if (!d->st.cgrid) return AMB_OK;
+    DCK(cudaSetDevice(d->device));
+    DCK(cudaMemsetAsync(d->st.cgrid, 0, AMB_COVERAGE_CELLS * sizeof(unsigned long long), d->stream));
+    DCK(cudaStreamSynchronize(d->stream));
+    return AMB_OK;
 }
 
 int amb_decoder_stats(amb_decoder* d, uint64_t* kernel_launches, float* ms_last)

@@ -50,6 +50,7 @@ __global__ void __launch_bounds__(128) amb_resolve_kernel(amb_fields* __restrict
 #include "amb_decode_track.cuh"
 #include "amb_decode_track_ext.cuh"
 #include "amb_decode_sbs1.cuh"
+#include "amb_decode_coverage.cuh"
 
 // ---- state and launch sequence ------------------------------------------------------------------------------------
 // What the stages of one decode read and write besides the frames and the records, and the one owner of that memory:
@@ -85,13 +86,15 @@ struct AmbDecodeState {
     AmbSbs1Ctr* sctr = nullptr;          // the id counter and the base recorded at reset
     AmbSbs1Bufs sb;                      // the stage's per-call scratch and the packed lines, one entry per frame
     int scap = 0;                        // frames sb holds
+    int coverage = 0;                    // option "coverage": 1 = on, 0 = off
+    unsigned long long* cgrid = nullptr; // the coverage grid: the bits of AMB_COVERAGE_CELLS doubles, all >= +0.0
     int have_loc = 0; double lat = 0.0, lon = 0.0;      // receiver location
 };
 
 // What amb_decode_prepare, amb_decode_reset and amb_decode_launch return when a stage's memory or launch fails.
 enum { AMB_STAGE_FIELDS = -1, AMB_STAGE_PAIRING = -2, AMB_STAGE_RESOLVE = -3, AMB_STAGE_LOCAL = -4,
        AMB_STAGE_COMMB = -5, AMB_STAGE_TRACK = -6, AMB_STAGE_OPSTATUS = -7, AMB_STAGE_TRACK_EXT = -8,
-       AMB_STAGE_SBS1 = -9 };
+       AMB_STAGE_SBS1 = -9, AMB_STAGE_COVERAGE = -10 };
 
 // By -AMB_STAGE_* - 1: what a failed launch of the stage reports, and what a failure of its memory reports.
 static const struct { const char* launch; const char* memory; } amb_stage_names[] = {
@@ -104,6 +107,7 @@ static const struct { const char* launch; const char* memory; } amb_stage_names[
     {"op status", "op status table (384 MiB)"},
     {"aircraft table extension", "aircraft table extension (2.25 GiB)"},
     {"SBS-1 feed", "SBS-1 id table (128 MiB)"},
+    {"coverage map", "coverage grid (5184 B)"},
 };
 
 // cudaMalloc, then every byte set to `fill` unless it is < 0; *p is NULL after a failed cudaMalloc
@@ -127,7 +131,8 @@ static void amb_sbs1_bufs_free(AmbSbs1Bufs* b)
 // tables, which every decode needs): the per-frame records, from 4096 frames up, doubling; the address-keyed records
 // once a stage that partitions them is on; each stage's table, bitmap, clock and counter at its first decode with the
 // option on, filled as an empty one (the track extension only while track is on too); the SBS-1 scratch as the frame
-// capacity grows. Returns 0, or the AMB_STAGE_* code of the stage whose memory could not be had, with *err set.
+// capacity grows; the coverage grid at the first decode with the option on. Returns 0, or the AMB_STAGE_* code of the
+// stage whose memory could not be had, with *err set.
 static int amb_decode_prepare(AmbDecodeState* st, int n, cudaStream_t s, cudaError_t* err)
 {
     if (!st->table) AMB_STAGE_TRY(AMB_STAGE_PAIRING, amb_decode_alloc(&st->table, st->table_slots * sizeof(AmbCprSlot), 0xFF, s));
@@ -198,12 +203,15 @@ static int amb_decode_prepare(AmbDecodeState* st, int n, cudaStream_t s, cudaErr
             st->scap = st->cap;
         }
     }
+    if (st->coverage > 0 && !st->cgrid)                 // every cell +0.0
+        AMB_STAGE_TRY(AMB_STAGE_COVERAGE, amb_decode_alloc(&st->cgrid, AMB_COVERAGE_CELLS * sizeof(unsigned long long), 0, s));
     return 0;
 }
 
 // amb_decoder_reset on stream s, for whatever is allocated: every table empty again. The rows of the aircraft table
 // and its extension stay (a row whose bit is clear is never read), and so does the SBS-1 id table (ids up to G are
-// dead once base = G). Returns 0, or the AMB_STAGE_* code of the stage whose memory could not be cleared, with *err set.
+// dead once base = G); the coverage grid is cleared. Returns 0, or the AMB_STAGE_* code of the stage whose memory could
+// not be cleared, with *err set.
 static int amb_decode_reset(AmbDecodeState* st, cudaStream_t s, cudaError_t* err)
 {
     static const AmbTrackClock none = {NAN, 0u, 0u};
@@ -219,6 +227,8 @@ static int amb_decode_reset(AmbDecodeState* st, cudaStream_t s, cudaError_t* err
     if (st->sctr)
         AMB_STAGE_TRY(AMB_STAGE_SBS1, cudaMemcpyAsync(&st->sctr->base, &st->sctr->G, sizeof(unsigned long long),
                                                       cudaMemcpyDeviceToDevice, s));
+    if (st->cgrid)
+        AMB_STAGE_TRY(AMB_STAGE_COVERAGE, cudaMemsetAsync(st->cgrid, 0, AMB_COVERAGE_CELLS * sizeof(unsigned long long), s));
     return 0;
 }
 #undef AMB_STAGE_TRY
@@ -227,7 +237,7 @@ static int amb_decode_reset(AmbDecodeState* st, cudaStream_t s, cudaError_t* err
 static void amb_decode_free(AmbDecodeState* st)
 {
     void* const all[] = {st->table, st->nl_T, st->pos, st->pair, st->keys, st->ltable, st->ctable, st->otable, st->trows,
-                         st->tocc, st->tclk, st->snap_cnt, st->xrows, st->xocc, st->stable, st->sctr};
+                         st->tocc, st->tclk, st->snap_cnt, st->xrows, st->xocc, st->stable, st->sctr, st->cgrid};
     for (void* p : all) cudaFree(p);
     amb_v3_free(&st->v3);
     amb_sbs1_bufs_free(&st->sb);
@@ -235,9 +245,10 @@ static void amb_decode_free(AmbDecodeState* st)
 }
 
 // Enqueue one decode of the n frames into the n records on stream s, in this order: fields, pairing, resolve, then the
-// local CPR, Comm-B, op-status and track stages whose S is > 0, and the track extension when track and track_ext are
-// both > 0, then the SBS-1 feed when sbs1 is on. Returns how many kernels were launched (7, plus 6 per stage that is
-// on, plus 10 for the SBS-1 feed), or an AMB_STAGE_* code with *err set.
+// local CPR stage when its S is > 0, the coverage map when coverage is on (after the local stage, so that local fixes
+// reach it), the Comm-B, op-status and track stages whose S is > 0, and the track extension when track and track_ext
+// are both > 0, then the SBS-1 feed when sbs1 is on. Returns how many kernels were launched (7, plus 6 per stage that
+// is on, plus 1 for the coverage map and 10 for the SBS-1 feed), or an AMB_STAGE_* code with *err set.
 static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n, amb_fields* fields, cudaStream_t s,
                              cudaError_t* err)
 {
@@ -255,6 +266,10 @@ static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n,
                                         st->lat, st->lon, st->nl_T, s, err);
         if (kl < 0) return AMB_STAGE_LOCAL;
         k += kl;
+    }
+    if (st->coverage > 0) {
+        if (amb_coverage_launch(fields, n, st->cgrid, s, err) < 0) return AMB_STAGE_COVERAGE;
+        k += 1;
     }
     if (st->commb > 0) {
         const int kc = amb_commb_launch(&st->v3, frames, fields, st->pos, st->keys, n, st->ctable, st->commb, s, err);

@@ -49,6 +49,9 @@ AXG_OPS, AXG_TS, AXG_INTEG, AXG_B40, AXG_B50, AXG_B60 = (
 TRACK_EXT_MAX = _lib.TRACK_EXT_MAX
 # SBS-1 feed (decoder options sbs1 and sbs1_tz; include/airmodes_b200.h AMB_SBS1_TZ_*)
 SBS1_TZ_MIN, SBS1_TZ_MAX = _lib.SBS1_TZ_MIN, _lib.SBS1_TZ_MAX
+# coverage map (decoder option coverage; include/airmodes_b200.h AMB_COVERAGE_*): 72 bearing rows of 5 degrees, and the
+# upper edges in feet of the nine altitude bands (az_map.py:42)
+COVERAGE_ROWS, COVERAGE_BANDS, COVERAGE_ALTITUDES = _lib.COVERAGE_ROWS, _lib.COVERAGE_BANDS, _lib.COVERAGE_ALTITUDES
 
 FIELDS_DTYPE = np.dtype(Fields)
 FRAME_DTYPE = np.dtype(Frame)
@@ -118,11 +121,20 @@ def check_opstatus(seconds) -> int:
     return check_option("opstatus", seconds)
 
 
-def check_sbs1(on) -> int:
-    """Validate a setting of decoder option sbs1: False / True or 0 / 1. Raises ValueError otherwise."""
+def _check_switch(name: str, on) -> int:
     if isinstance(on, (bool, np.bool_)) or (isinstance(on, (int, np.integer)) and int(on) in (0, 1)):
         return int(on)
-    raise ValueError("sbs1: False / True (0 / 1), got %r" % (on,))
+    raise ValueError("%s: False / True (0 / 1), got %r" % (name, on))
+
+
+def check_sbs1(on) -> int:
+    """Validate a setting of decoder option sbs1: False / True or 0 / 1. Raises ValueError otherwise."""
+    return _check_switch("sbs1", on)
+
+
+def check_coverage(on) -> int:
+    """Validate a setting of decoder option coverage: False / True or 0 / 1. Raises ValueError otherwise."""
+    return _check_switch("coverage", on)
 
 
 def check_sbs1_tz(minutes) -> int:
@@ -235,6 +247,25 @@ _AC_COLUMNS = (("altitude", AC_HAS_ALT), ("squawk", AC_HAS_SQUAWK), ("ident", AC
                ("vertical", AC_HAS_VELOCITY), ("heading", AC_HAS_HEADING), ("eps", AC_HAS_EPS))
 
 
+def coverage_to_dict(grid, location) -> dict:
+    """A coverage grid (batch_decoder.coverage(): COVERAGE_ROWS x COVERAGE_BANDS ranges) -> plain dict for JSON:
+      location  the receiver's [lat, lon] the ranges were measured from
+      unit      "statute miles", the unit of the records' range (cpr.py:162)
+      sectors   per row i: "bearing" 5 i, and the bearings [from, to) it holds, from = 5 i - 2.5 (357.5 for row 0), to =
+                5 i + 2.5; a bearing b lands in row int(b + 2.5) // 5 % 72 with the sum in IEEE double, so a bearing
+                within rounding of an edge may land on the other side (include/airmodes_b200.h rule 3)
+      bands     per band j: "altitude" = COVERAGE_ALTITUDES[j] in feet; band j holds the greatest range of the positions
+                at or below that altitude, and the last band that of every position ("altitude" null)
+      ranges    the grid, ranges[row][band]; 0.0 where nothing was heard."""
+    grid = np.asarray(grid, dtype=np.float64).reshape(COVERAGE_ROWS, COVERAGE_BANDS)
+    sectors = [{"bearing": 5.0 * i, "from": 357.5 if i == 0 else 5.0 * i - 2.5, "to": 5.0 * i + 2.5}
+               for i in range(COVERAGE_ROWS)]
+    bands = [{"altitude": a if j < COVERAGE_BANDS - 1 else None} for j, a in enumerate(COVERAGE_ALTITUDES)]
+    return {"location": None if location is None else [float(location[0]), float(location[1])],
+            "unit": "statute miles", "sectors": sectors, "bands": bands, "altitudes": list(COVERAGE_ALTITUDES),
+            "ranges": grid.tolist()}
+
+
 def aircraft_to_dict(row) -> dict:
     """One AIRCRAFT_DTYPE row -> plain dict for JSON: ident as str, a column whose flag is clear as None, on_ground as
     bool, and rssi = 10 log10(max(1e-8, ref_level)) as the reference computes it from the slicer's level (parse.py:430)."""
@@ -309,14 +340,18 @@ class batch_decoder:
     sbs1 = True also writes, on the device, the SBS-1 (BaseStation) lines the reference's output_sbs1 would send for the
     decoded messages, with aircraft ids carried from call to call and the date and time of each frame's stamp shifted
     by sbs1_tz minutes; read the last decode's lines with sbs1_text() / sbs1_text_device() (DESIGN.md §8 "SBS-1
-    feed")."""
+    feed").
+    coverage = True also keeps, on the device, the reference's azimuth map model: the greatest range heard in every
+    5-degree bearing sector for each of nine altitude bands, from the positions with a range (a receiver location is
+    needed); read with coverage() / coverage_device(), clear with reset_coverage() (DESIGN.md §8 "Receiver
+    coverage")."""
 
     def __init__(self, my_location=None, device: int = 0, local_cpr: int = 0, track: int = 0, commb: int = 0,
-                 opstatus: int = 0, track_ext: int = 0, sbs1=False, sbs1_tz: int = 0):
+                 opstatus: int = 0, track_ext: int = 0, sbs1=False, sbs1_tz: int = 0, coverage=False):
         settings = {"local_cpr": check_option("local_cpr", local_cpr), "track": check_option("track", track),
                     "commb": check_option("commb", commb), "opstatus": check_option("opstatus", opstatus),
                     "track_ext": check_option("track_ext", track_ext)}
-        sbs1, sbs1_tz = check_sbs1(sbs1), check_sbs1_tz(sbs1_tz)
+        sbs1, sbs1_tz, coverage = check_sbs1(sbs1), check_sbs1_tz(sbs1_tz), check_coverage(coverage)
         self._lib = _lib.load()
         h = C.c_void_p()
         have, lat, lon = self._loc(my_location)
@@ -336,6 +371,9 @@ class batch_decoder:
             self.set_sbs1(True)
         if sbs1_tz:
             self.set_sbs1_tz(sbs1_tz)
+        self._coverage = 0
+        if coverage:
+            self.set_coverage(True)
 
     @staticmethod
     def _loc(loc):
@@ -353,8 +391,8 @@ class batch_decoder:
         self.my_location = new_location
 
     def reset(self):
-        """Forget every stored report, reference position, velocity, op status and aircraft; the option settings
-        stay."""
+        """Forget every stored report, reference position, velocity, op status and aircraft, and clear the coverage
+        grid; the option settings stay."""
         self._check(self._lib.amb_decoder_reset(self._h))
 
     def _set_option(self, name, seconds):
@@ -439,6 +477,41 @@ class batch_decoder:
             raise RuntimeError("sbs1_text_device: %d bytes needed, out_dev holds %d" % (n.value, out_dev.numel()))
         self._check(rc)
         return int(n.value)
+
+    def set_coverage(self, on):
+        """Option coverage on (True) or off (False); applies from the next decode. The grid is kept while it is off."""
+        on = check_coverage(on)
+        self._check(self._lib.amb_decoder_set_option(self._h, b"coverage", on))
+        self._coverage = on
+
+    def get_coverage(self) -> bool:
+        return bool(self._coverage)
+
+    def coverage(self) -> np.ndarray:
+        """The coverage grid: a (COVERAGE_ROWS, COVERAGE_BANDS) float64 array, [bearing row, altitude band], statute
+        miles; all zeros before the first decode with the option on. Needs the option coverage on."""
+        out = np.zeros((COVERAGE_ROWS, COVERAGE_BANDS), dtype=np.float64)
+        self._check(self._lib.amb_decoder_coverage(self._h, C.c_void_p(out.ctypes.data)))
+        return out
+
+    def coverage_device(self, out_dev=None):
+        """coverage() into device memory: a CUDA float64 tensor of shape (COVERAGE_ROWS, COVERAGE_BANDS) (out_dev when
+        one is given: contiguous, float64, that many elements). Nothing but the call crosses PCIe."""
+        import torch
+        if out_dev is None:
+            out_dev = torch.empty((COVERAGE_ROWS, COVERAGE_BANDS), dtype=torch.float64,
+                                  device=torch.device("cuda", self._device))
+        if out_dev.dtype != torch.float64 or not out_dev.is_cuda or not out_dev.is_contiguous() or \
+                out_dev.numel() != COVERAGE_ROWS * COVERAGE_BANDS:
+            raise ValueError("coverage_device: out_dev must be a contiguous CUDA float64 tensor of %d elements"
+                             % (COVERAGE_ROWS * COVERAGE_BANDS))
+        torch.cuda.current_stream(out_dev.device).synchronize()          # the decoder runs on its own stream
+        self._check(self._lib.amb_decoder_coverage_device(self._h, C.c_void_p(out_dev.data_ptr())))
+        return out_dev
+
+    def reset_coverage(self):
+        """Clear the coverage grid and nothing else (az_map_model.reset, az_map.py:77-82). Needs the option on."""
+        self._check(self._lib.amb_decoder_coverage_reset(self._h))
 
     @staticmethod
     def _now(now):

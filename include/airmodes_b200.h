@@ -610,6 +610,29 @@ typedef struct amb_aircraft_ext {
 #define AMB_SBS1_TZ_MIN (-720)
 #define AMB_SBS1_TZ_MAX 840
 
+/* Receiver coverage map (amb_decoder_set_option(d, "coverage", 1)): the model behind the reference's azimuth map
+ * (az_map_model, python/az_map.py:35-82, fed by az_map_output.output, az_map.py:187-202): the greatest range heard in
+ * each 5-degree bearing sector, separately for nine altitude bands. It folds in the records of this decoder in stream
+ * order, continuing across calls, since the last amb_decoder_reset or amb_decoder_coverage_reset:
+ *   1 counted   a record counts when its frame was queued, its status lacks AMB_FS_NO_HANDLER, df == 17, bds is 0x05 or
+ *               0x06 and it has AMB_FS_HAS_RANGE (the type17_dl messages az_map_output gets a range for). Without a
+ *               receiver location nothing counts. A local fix (option "local_cpr") counts like a global one.
+ *   2 altitude  BDS0,6 counts as 0 ft; BDS0,5 uses the record's altitude (decode_alt(alt, False); may be negative).
+ *   3 cell      row = ((int64)(bearing + 2.5)) / 5 % 72: the sum in IEEE double, truncated, then divided as an integer
+ *               (az_map.py:66 with npoints = 72), so the double just below 2.5 lands in row 1, and 357.5 and 360.0 in
+ *               row 0. col = the index of the first of AMB_COVERAGE_ALTITUDES >= altitude, or 8 when altitude >= 30000.
+ *   4 update    for every band j in col..8: if range > cell[row][j] then cell[row][j] = range. Cells start at +0.0, so
+ *               a range of 0 (or a NaN) changes nothing.
+ *   5 units     the records' range: statute miles (cpr.py:162). amb_decoder_set_location changes the ranges of later
+ *               records and leaves the grid as it is.
+ * The grid is AMB_COVERAGE_ROWS x AMB_COVERAGE_BANDS doubles (5184 bytes of device memory, allocated zeroed at the first
+ * decode with the option on); row i covers the bearings [5i - 2.5, 5i + 2.5) up to the rounding of rule 3. It is a
+ * maximum over a fixed grid, so it does not depend on how the stream is cut into calls. A decode with the option on
+ * launches one kernel more; with it off nothing changes. */
+#define AMB_COVERAGE_ROWS 72     /* 5-degree bearing sectors, row i centred on 5 i degrees */
+#define AMB_COVERAGE_BANDS 9     /* altitude bands, by their upper edge: */
+#define AMB_COVERAGE_ALTITUDES {0, 1000, 2000, 5000, 10000, 15000, 20000, 25000, 30000}   /* feet (az_map.py:42) */
+
 typedef struct amb_decoder amb_decoder;
 /* cpr_decoder(my_location) (cpr.py:184-190) + the parser; have_location = 0 is my_location = None. */
 AMB_API int amb_decoder_create(int device, int have_location, double lat, double lon, amb_decoder** out);
@@ -634,6 +657,7 @@ AMB_API int amb_decoder_create(int device, int have_location, double lat, double
  * cleared (by amb_decoder_reset). A decode with both on launches six kernels more; off changes nothing.
  * "sbs1": 0 (default, off) or 1, the SBS-1 feed (see AMB_SBS1_TZ_MIN); applies from the next call.
  * "sbs1_tz": AMB_SBS1_TZ_MIN .. AMB_SBS1_TZ_MAX minutes (default 0, UTC) added to the stamp in the SBS-1 date and time.
+ * "coverage": 0 (default, off) or 1, the receiver coverage map (see AMB_COVERAGE_ROWS); applies from the next call.
  * Unknown names and out-of-range values return AMB_ERR_INVALID. */
 AMB_API int amb_decoder_set_option(amb_decoder* d, const char* name, int value);
 /* Snapshot of the per-aircraft table at time `now`: every row with seen <= now and now - seen <= S, in ascending
@@ -656,11 +680,18 @@ AMB_API int amb_decoder_aircraft_ext_device(amb_decoder* d, double now, amb_airc
  * to device memory instead, so only the byte count crosses PCIe. */
 AMB_API int amb_decoder_sbs1(amb_decoder* d, char* out, size_t cap, size_t* n_bytes);
 AMB_API int amb_decoder_sbs1_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes);
+/* The coverage grid, AMB_COVERAGE_ROWS x AMB_COVERAGE_BANDS doubles, row-major (bearing row first, band second), into
+ * out (host memory); _device copies it to device memory. All zeros before the first decode with the option on.
+ * amb_decoder_coverage_reset clears the grid and nothing else (az_map_model.reset, az_map.py:77-82). All three return
+ * AMB_ERR_STATE when the option "coverage" is off. */
+AMB_API int amb_decoder_coverage(amb_decoder* d, double* out);
+AMB_API int amb_decoder_coverage_device(amb_decoder* d, double* out_dev);
+AMB_API int amb_decoder_coverage_reset(amb_decoder* d);
 AMB_API void amb_decoder_destroy(amb_decoder* d);
 AMB_API int amb_decoder_set_location(amb_decoder* d, int have_location, double lat, double lon);   /* cpr.py:192-193 */
 AMB_API int amb_decoder_reset(amb_decoder* d);                      /* forget every stored report, reference position,
                                                                        velocity, op status, aircraft and extension
-                                                                       group */
+                                                                       group, and clear the coverage grid */
 /* Decode n frames (host or device array, stream order = non-decreasing time). out: n records in host memory.
  * Frames with passed == 0 get AMB_FS_NOT_QUEUED and do not touch the CPR state. */
 AMB_API int amb_decode_frames(amb_decoder* d, const amb_frame* frames, int n, int mem_kind, amb_fields* out);

@@ -9,8 +9,11 @@ gr_complex), and the same two outlets for the slicer's messages: printed to stdo
 default instead: the text reports of python/msprint.py, decoded on the GPU (gr_air_modes_b200.decode: parse.py,
 altitude.py, cpr.py for whole batches). With -P [PORT] the SBS-1 (BaseStation) feed of apps/modes_rx -P is served on
 TCP port PORT (default 30003): the lines are formed on the GPU by the decoder (gr_air_modes_b200.decode, option sbs1)
-with the date and time of each message's stamp in the host's local time, and sent by gr_air_modes_b200.sbs1. KML and
-FlightGear outputs are the reference's own pure-Python consumers of the dl_data feed and are not re-implemented.
+with the date and time of each message's stamp in the host's local time, and sent by gr_air_modes_b200.sbs1. With
+-l LAT,LON --coverage PATH the receiver coverage map of apps/modes_gui's azimuth map (python/az_map.py, the model, not
+the widget) - the greatest range heard per 5-degree bearing sector and altitude band, in statute miles - is kept on the
+GPU by the decoder (option coverage) and written to PATH as JSON after every chunk. KML and FlightGear outputs are the
+reference's own pure-Python consumers of the dl_data feed and are not re-implemented.
 
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 [-T 7.0] [-d] [-t 5556] [-n] [--reports | -l 37.4,-122.1]
     python tools/modes_rx_b200.py -s 127.0.0.1:12345 -r 4e6 --udp-idle 2.0
@@ -20,6 +23,7 @@ FlightGear outputs are the reference's own pure-Python consumers of the dl_data 
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 --reports --commb 30
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 --reports --opstatus 60
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -l 37.4,-122.1 -P 30003
+    python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -l 37.4,-122.1 --coverage coverage.json
 
 Differences, all on the far side of rx_path:
 * live radios (-s uhd / osmocom) need GNU Radio: use gr_air_modes_b200.gr_adapter.rx_path inside modes_radio.
@@ -115,18 +119,23 @@ class print_queue:
         self.count += 1
 
 
-def write_aircraft(path, rows, ext=None):
-    """The aircraft table (AIRCRAFT_DTYPE rows) as a JSON list, one object per aircraft (decode.aircraft_to_dict, or
-    decode.aircraft_ext_to_dict with the extension rows `ext`), written to a temporary file beside `path` and renamed
-    over it, so that a reader never sees a half-written file."""
-    from gr_air_modes_b200 import decode
+def write_json(path, obj):
+    """obj as JSON, written to a temporary file beside `path` and renamed over it, so that a reader never sees a
+    half-written file."""
     tmp = "%s.tmp%d" % (path, os.getpid())
     with open(tmp, "w") as f:
-        if ext is None:
-            json.dump([decode.aircraft_to_dict(r) for r in rows], f)
-        else:
-            json.dump([decode.aircraft_ext_to_dict(r, x) for r, x in zip(rows, ext)], f)
+        json.dump(obj, f)
     os.replace(tmp, path)
+
+
+def write_aircraft(path, rows, ext=None):
+    """The aircraft table (AIRCRAFT_DTYPE rows) as a JSON list, one object per aircraft (decode.aircraft_to_dict, or
+    decode.aircraft_ext_to_dict with the extension rows `ext`), through write_json."""
+    from gr_air_modes_b200 import decode
+    if ext is None:
+        write_json(path, [decode.aircraft_to_dict(r) for r in rows])
+    else:
+        write_json(path, [decode.aircraft_ext_to_dict(r, x) for r, x in zip(rows, ext)])
 
 
 class report_queue:
@@ -135,16 +144,18 @@ class report_queue:
     (gr_air_modes_b200.decode), the line format from gr_air_modes_b200.report. out=None decodes without printing;
     aircraft=PATH writes the decoder's aircraft table (option track) to PATH after every batch, with the extension of
     every row when track_ext is on; sbs1=server (gr_air_modes_b200.sbs1.sbs1_server) sends the batch's SBS-1 lines to
-    it, with the date and time shifted by sbs1_tz minutes."""
+    it, with the date and time shifted by sbs1_tz minutes; coverage=PATH writes the decoder's coverage map (option
+    coverage) to PATH after every batch (decode.coverage_to_dict)."""
 
     def __init__(self, location, device, out=sys.stdout, local_cpr=0, track=0, aircraft=None, decoder=None, commb=0,
-                 opstatus=0, track_ext=0, sbs1=None, sbs1_tz=0):
+                 opstatus=0, track_ext=0, sbs1=None, sbs1_tz=0, coverage=None):
         from gr_air_modes_b200 import decode
         self._dec = decoder if decoder is not None else \
             decode.batch_decoder(location, device, local_cpr=local_cpr, track=track, commb=commb,
                                  opstatus=opstatus, track_ext=track_ext, sbs1=sbs1 is not None,
-                                 sbs1_tz=sbs1_tz)   # = cpr_decoder(my_position), apps/modes_rx:68
+                                 sbs1_tz=sbs1_tz, coverage=coverage is not None)   # = cpr_decoder(my_position), apps/modes_rx:68
         self._out, self._texts, self.count, self._aircraft = out, [], 0, aircraft
+        self._coverage, self._location = coverage, location
         self._ext = track_ext > 0
         self._sbs1 = sbs1
 
@@ -172,6 +183,9 @@ class report_queue:
             write_aircraft(self._aircraft, *self._dec.aircraft_ext())
         elif self._aircraft:
             write_aircraft(self._aircraft, self._dec.aircraft())
+        if self._coverage:
+            from gr_air_modes_b200 import decode
+            write_json(self._coverage, decode.coverage_to_dict(self._dec.coverage(), self._location))
 
     def close(self):
         self._dec.close()
@@ -240,7 +254,13 @@ def parse_args(argv=None):
     ap.add_argument("--sbs1-wait", type=float, default=0.0, metavar="S",
                     help="with -P: wait up to S seconds for the first SBS-1 client before reading the source (for "
                          "replaying a recording); 0 = start at once, as modes_rx")
+    ap.add_argument("--coverage", type=str, default=None, metavar="PATH",
+                    help="after every chunk, write the receiver coverage map to PATH as JSON: the greatest range "
+                         "(statute miles) heard per 5-degree bearing sector and altitude band, as modes_gui's azimuth "
+                         "map keeps it (needs -l; decodes the messages even without --reports)")
     args = ap.parse_args(argv)
+    if args.coverage and args.location is None:
+        ap.error("--coverage needs -l LAT,LON")
     if args.sbs1 is not None and not 0 < args.sbs1 < 65536:
         ap.error("--sbs1: a TCP port 1 .. 65535")
     if not 0 <= args.sbs1_wait <= 3600:
@@ -296,6 +316,8 @@ def main(argv=None):
         if args.sbs1_wait and not server.wait_for_client(args.sbs1_wait):
             print("# no SBS-1 client within %g s, starting anyway" % args.sbs1_wait, file=sys.stderr)
     feed = {"sbs1": server, "sbs1_tz": local_utc_offset_minutes()} if server is not None else {}
+    if args.coverage:
+        feed["coverage"] = args.coverage
     if not args.no_print:
         if args.reports or args.location is not None:
             reporter = report_queue(my_position, args.device, local_cpr=args.local_cpr, track=args.track, commb=args.commb,
@@ -304,7 +326,7 @@ def main(argv=None):
         else:
             printer = print_queue()
             sinks.append(printer)
-    if (args.aircraft or server is not None) and reporter is None:   # the table or the feed without printed reports
+    if (args.aircraft or server is not None or args.coverage) and reporter is None:   # no printed reports
         reporter = report_queue(my_position, args.device, out=None, local_cpr=args.local_cpr, track=args.track,
                                 aircraft=args.aircraft, **({"commb": args.commb, "opstatus": args.opstatus,
                                                             "track_ext": args.track_ext} if args.track_ext else {}),
