@@ -225,6 +225,8 @@ SYMBOLS = [
     ("amb_decoder_aircraft_ext_device", C.c_int, [_vp, C.c_double, _vp, _vp, C.c_int]),
     ("amb_decoder_sbs1", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("amb_decoder_sbs1_device", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("amb_decoder_reports", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("amb_decoder_reports_device", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("amb_decoder_coverage", C.c_int, [_vp, _vp]),
     ("amb_decoder_coverage_device", C.c_int, [_vp, _vp]),
     ("amb_decoder_coverage_reset", C.c_int, [_vp]),

@@ -35,6 +35,9 @@
 // kernels on address keys, amb_sbs1_walk, amb_sbs1_ids - the aircraft ids of sbs1.py, with a direct-mapped table of the
 // latest id per address in HBM (2^24 x 8 B) carried from batch to batch - and amb_sbs1_format, amb_sbs1_scan,
 // amb_sbs1_gather, which write the call's SBS-1 lines and pack them on the device; amb_decoder_sbs1 copies them out.
+// With option "reports" on, three more after those (amb_decode_reports.cuh): amb_reports_len, amb_sbs1_scan,
+// amb_reports_write - the call's text reports, the lines of report.py, packed on the device; amb_decoder_reports copies
+// them out.
 #include "amb_launch.h"
 #include "amb_decode_core.h"
 #include "amb_decode_kernels.cuh"
@@ -59,6 +62,7 @@ struct amb_decoder {
     amb_aircraft_ext* d_xsnap = nullptr; int xsnap_cap = 0;   // ... and their extensions
     int sbs1_nb = -1;                    // blocks of lines of the last decode (its byte total is st.sb.boff[sbs1_nb]);
                                          // -1: the last decode wrote no lines
+    int reports_nb = -1;                 // the same for the text reports (st.rb.boff[reports_nb])
     uint64_t launches = 0; float ms_last = 0.f;
     std::string err;
 };
@@ -239,6 +243,11 @@ int amb_decoder_set_option(amb_decoder* d, const char* name, int value)
         d->st.sbs1 = value;
         return AMB_OK;
     }
+    if (strcmp(name, "reports") == 0) {
+        if (value != 0 && value != 1) return dfail(d, AMB_ERR_INVALID, "reports: 0 (off) or 1 (on)");
+        d->st.reports = value;
+        return AMB_OK;
+    }
     if (strcmp(name, "coverage") == 0) {
         if (value != 0 && value != 1) return dfail(d, AMB_ERR_INVALID, "coverage: 0 (off) or 1 (on)");
         d->st.coverage = value;
@@ -281,9 +290,9 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
 {
     if (!d || n < 0 || (n > 0 && (!frames || !out)) || (mem_kind != AMB_MEM_HOST && mem_kind != AMB_MEM_DEVICE))
         return dfail(d, AMB_ERR_INVALID, "amb_decode_frames: bad argument");
-    if (n == 0) { d->sbs1_nb = -1; return AMB_OK; }
+    if (n == 0) { d->sbs1_nb = d->reports_nb = -1; return AMB_OK; }
     DCK(cudaSetDevice(d->device));
-    d->sbs1_nb = -1;
+    d->sbs1_nb = d->reports_nb = -1;
     int rc = prepare(d, n);
     if (rc != AMB_OK) return rc;
     cudaStream_t s = d->stream;
@@ -300,6 +309,7 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
     if (k < 0) return dfail(d, AMB_ERR_CUDA, amb_stage_names[-k - 1].launch, e);
     d->launches += (uint64_t)k;
     if (d->st.sbs1 > 0) d->sbs1_nb = (n + 127) / 128;
+    if (d->st.reports > 0) d->reports_nb = (n + 127) / 128;
     if (!out_on_device) {
         rc = staged_d2h(d, out, d->d_fields, (size_t)n * sizeof(amb_fields), s);
         if (rc != AMB_OK) return rc;
@@ -392,28 +402,37 @@ int amb_decoder_aircraft_ext_device(amb_decoder* d, double now, amb_aircraft* ou
     return snapshot_impl(d, now, out_dev, ext_dev, cap, true, true);
 }
 
-// the last decode's lines into out (host or device memory)
-static int sbs1_impl(amb_decoder* d, char* out, size_t cap, size_t* n_bytes, bool out_on_device)
+// the last decode's packed lines (nb blocks; total at boff[nb], text) into out (host or device memory); fn names the
+// call, option the option it needs
+static int text_impl(amb_decoder* d, bool on, int nb, const unsigned long long* boff, const char* text, const char* fn,
+                     const char* option, char* out, size_t cap, size_t* n_bytes, bool out_on_device)
 {
-    if (!d || !n_bytes || (cap > 0 && !out)) return dfail(d, AMB_ERR_INVALID, "amb_decoder_sbs1: bad argument");
+    char what[96];
+    if (!d || !n_bytes || (cap > 0 && !out)) { snprintf(what, sizeof what, "%s: bad argument", fn); return dfail(d, AMB_ERR_INVALID, what); }
     *n_bytes = 0;
-    if (d->st.sbs1 <= 0) return dfail(d, AMB_ERR_STATE, "amb_decoder_sbs1: option sbs1 is off");
-    if (d->sbs1_nb < 0) return AMB_OK;                   // no decode with the option on since it was set
+    if (!on) { snprintf(what, sizeof what, "%s: option %s is off", fn, option); return dfail(d, AMB_ERR_STATE, what); }
+    if (nb < 0) return AMB_OK;                          // no decode with the option on since it was set
     DCK(cudaSetDevice(d->device));
     cudaStream_t s = d->stream;
     unsigned long long total = 0;
-    DCK(cudaMemcpyAsync(&total, d->st.sb.boff + d->sbs1_nb, sizeof total, cudaMemcpyDeviceToHost, s));
+    DCK(cudaMemcpyAsync(&total, boff + nb, sizeof total, cudaMemcpyDeviceToHost, s));
     DCK(cudaStreamSynchronize(s));
     *n_bytes = (size_t)total;
-    if (total > cap) return dfail(d, AMB_ERR_OVERFLOW, "amb_decoder_sbs1: output buffer too small");
+    if (total > cap) { snprintf(what, sizeof what, "%s: output buffer too small", fn); return dfail(d, AMB_ERR_OVERFLOW, what); }
     if (total == 0) return AMB_OK;
-    if (out_on_device) DCK(cudaMemcpyAsync(out, d->st.sb.text, (size_t)total, cudaMemcpyDeviceToDevice, s));
+    if (out_on_device) DCK(cudaMemcpyAsync(out, text, (size_t)total, cudaMemcpyDeviceToDevice, s));
     else {
-        int rc = staged_d2h(d, out, d->st.sb.text, (size_t)total, s);
+        int rc = staged_d2h(d, out, text, (size_t)total, s);
         if (rc != AMB_OK) return rc;
     }
     DCK(cudaStreamSynchronize(s));
     return AMB_OK;
+}
+
+static int sbs1_impl(amb_decoder* d, char* out, size_t cap, size_t* n_bytes, bool out_on_device)
+{
+    return text_impl(d, d && d->st.sbs1 > 0, d ? d->sbs1_nb : -1, d ? d->st.sb.boff : nullptr, d ? d->st.sb.text : nullptr,
+                     "amb_decoder_sbs1", "sbs1", out, cap, n_bytes, out_on_device);
 }
 
 int amb_decoder_sbs1(amb_decoder* d, char* out, size_t cap, size_t* n_bytes)
@@ -424,6 +443,23 @@ int amb_decoder_sbs1(amb_decoder* d, char* out, size_t cap, size_t* n_bytes)
 int amb_decoder_sbs1_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes)
 {
     return sbs1_impl(d, out_dev, cap, n_bytes, true);
+}
+
+static int reports_impl(amb_decoder* d, char* out, size_t cap, size_t* n_bytes, bool out_on_device)
+{
+    return text_impl(d, d && d->st.reports > 0, d ? d->reports_nb : -1, d ? d->st.rb.boff : nullptr,
+                     d ? d->st.rb.text : nullptr, out_on_device ? "amb_decoder_reports_device" : "amb_decoder_reports",
+                     "reports", out, cap, n_bytes, out_on_device);
+}
+
+int amb_decoder_reports(amb_decoder* d, char* out, size_t cap, size_t* n_bytes)
+{
+    return reports_impl(d, out, cap, n_bytes, false);
+}
+
+int amb_decoder_reports_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes)
+{
+    return reports_impl(d, out_dev, cap, n_bytes, true);
 }
 
 // the coverage grid into out (host or device memory); all zeros while the grid is not allocated yet

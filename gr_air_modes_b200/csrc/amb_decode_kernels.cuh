@@ -51,6 +51,7 @@ __global__ void __launch_bounds__(128) amb_resolve_kernel(amb_fields* __restrict
 #include "amb_decode_track_ext.cuh"
 #include "amb_decode_sbs1.cuh"
 #include "amb_decode_coverage.cuh"
+#include "amb_decode_reports.cuh"
 
 // ---- state and launch sequence ------------------------------------------------------------------------------------
 // What the stages of one decode read and write besides the frames and the records, and the one owner of that memory:
@@ -88,13 +89,18 @@ struct AmbDecodeState {
     int scap = 0;                        // frames sb holds
     int coverage = 0;                    // option "coverage": 1 = on, 0 = off
     unsigned long long* cgrid = nullptr; // the coverage grid: the bits of AMB_COVERAGE_CELLS doubles, all >= +0.0
+    int reports = 0;                     // option "reports": 1 = on, 0 = off
+    unsigned* rfirst = nullptr;          // 1 until the first queued frame since creation or reset has been formatted
+    AmbReportBufs rb;                    // the stage's per-call scratch and the packed lines
+    int rcap = 0;                        // frames rb holds
     int have_loc = 0; double lat = 0.0, lon = 0.0;      // receiver location
 };
 
 // What amb_decode_prepare, amb_decode_reset and amb_decode_launch return when a stage's memory or launch fails.
 enum { AMB_STAGE_FIELDS = -1, AMB_STAGE_PAIRING = -2, AMB_STAGE_RESOLVE = -3, AMB_STAGE_LOCAL = -4,
        AMB_STAGE_COMMB = -5, AMB_STAGE_TRACK = -6, AMB_STAGE_OPSTATUS = -7, AMB_STAGE_TRACK_EXT = -8,
-       AMB_STAGE_SBS1 = -9, AMB_STAGE_COVERAGE = -10 };
+       AMB_STAGE_SBS1 = -9, AMB_STAGE_COVERAGE = -10,
+       AMB_STAGE_REPORTS = -11 };
 
 // By -AMB_STAGE_* - 1: what a failed launch of the stage reports, and what a failure of its memory reports.
 static const struct { const char* launch; const char* memory; } amb_stage_names[] = {
@@ -108,6 +114,7 @@ static const struct { const char* launch; const char* memory; } amb_stage_names[
     {"aircraft table extension", "aircraft table extension (2.25 GiB)"},
     {"SBS-1 feed", "SBS-1 id table (128 MiB)"},
     {"coverage map", "coverage grid (5184 B)"},
+    {"text reports", "text report buffers (478 B per frame)"},
 };
 
 // cudaMalloc, then every byte set to `fill` unless it is < 0; *p is NULL after a failed cudaMalloc
@@ -125,13 +132,21 @@ static void amb_sbs1_bufs_free(AmbSbs1Bufs* b)
     *b = AmbSbs1Bufs();
 }
 
+static void amb_report_bufs_free(AmbReportBufs* b)
+{
+    void* const all[] = {b->len, b->bsum, b->boff, b->text};
+    for (void* p : all) cudaFree(p);
+    *b = AmbReportBufs();
+}
+
 #define AMB_STAGE_TRY(stage, call) do { if ((*err = (call)) != cudaSuccess) return (stage); } while (0)
 
 // Allocate on stream s what the stages that are on need for a decode of n frames (n = 0: only the pairing and NL
 // tables, which every decode needs): the per-frame records, from 4096 frames up, doubling; the address-keyed records
 // once a stage that partitions them is on; each stage's table, bitmap, clock and counter at its first decode with the
 // option on, filled as an empty one (the track extension only while track is on too); the SBS-1 scratch as the frame
-// capacity grows; the coverage grid at the first decode with the option on. Returns 0, or the AMB_STAGE_* code of the
+// capacity grows; the coverage grid at the first decode with the option on; the text reports' first-message flag (set)
+// at the first decode with the option on, and their buffers as the frame capacity grows. Returns 0, or the AMB_STAGE_* code of the
 // stage whose memory could not be had, with *err set.
 static int amb_decode_prepare(AmbDecodeState* st, int n, cudaStream_t s, cudaError_t* err)
 {
@@ -205,13 +220,31 @@ static int amb_decode_prepare(AmbDecodeState* st, int n, cudaStream_t s, cudaErr
     }
     if (st->coverage > 0 && !st->cgrid)                 // every cell +0.0
         AMB_STAGE_TRY(AMB_STAGE_COVERAGE, amb_decode_alloc(&st->cgrid, AMB_COVERAGE_CELLS * sizeof(unsigned long long), 0, s));
+    if (st->reports > 0) {
+        if (!st->rfirst) {
+            static const unsigned one = 1u;
+            AMB_STAGE_TRY(AMB_STAGE_REPORTS, amb_decode_alloc(&st->rfirst, sizeof one, -1, s));
+            AMB_STAGE_TRY(AMB_STAGE_REPORTS, cudaMemcpyAsync(st->rfirst, &one, sizeof one, cudaMemcpyHostToDevice, s));
+        }
+        if (st->rcap < st->cap) {
+            amb_report_bufs_free(&st->rb);
+            st->rcap = 0;
+            const size_t c = (size_t)st->cap, nb = (c + 127) / 128;
+            AmbReportBufs& b = st->rb;
+            AMB_STAGE_TRY(AMB_STAGE_REPORTS, amb_decode_alloc(&b.len, c * sizeof(uint32_t), -1, s));
+            AMB_STAGE_TRY(AMB_STAGE_REPORTS, amb_decode_alloc(&b.bsum, nb * sizeof(uint32_t), -1, s));
+            AMB_STAGE_TRY(AMB_STAGE_REPORTS, amb_decode_alloc(&b.boff, (nb + 1) * sizeof(unsigned long long), -1, s));
+            AMB_STAGE_TRY(AMB_STAGE_REPORTS, amb_decode_alloc(&b.text, c * AMB_REP_MAX_LINE, -1, s));
+            st->rcap = st->cap;
+        }
+    }
     return 0;
 }
 
 // amb_decoder_reset on stream s, for whatever is allocated: every table empty again. The rows of the aircraft table
 // and its extension stay (a row whose bit is clear is never read), and so does the SBS-1 id table (ids up to G are
-// dead once base = G); the coverage grid is cleared. Returns 0, or the AMB_STAGE_* code of the stage whose memory could
-// not be cleared, with *err set.
+// dead once base = G); the coverage grid is cleared; the text reports' first-message flag is set again. Returns 0, or
+// the AMB_STAGE_* code of the stage whose memory could not be cleared, with *err set.
 static int amb_decode_reset(AmbDecodeState* st, cudaStream_t s, cudaError_t* err)
 {
     static const AmbTrackClock none = {NAN, 0u, 0u};
@@ -229,6 +262,10 @@ static int amb_decode_reset(AmbDecodeState* st, cudaStream_t s, cudaError_t* err
                                                       cudaMemcpyDeviceToDevice, s));
     if (st->cgrid)
         AMB_STAGE_TRY(AMB_STAGE_COVERAGE, cudaMemsetAsync(st->cgrid, 0, AMB_COVERAGE_CELLS * sizeof(unsigned long long), s));
+    if (st->rfirst) {
+        static const unsigned one = 1u;
+        AMB_STAGE_TRY(AMB_STAGE_REPORTS, cudaMemcpyAsync(st->rfirst, &one, sizeof one, cudaMemcpyHostToDevice, s));
+    }
     return 0;
 }
 #undef AMB_STAGE_TRY
@@ -237,18 +274,21 @@ static int amb_decode_reset(AmbDecodeState* st, cudaStream_t s, cudaError_t* err
 static void amb_decode_free(AmbDecodeState* st)
 {
     void* const all[] = {st->table, st->nl_T, st->pos, st->pair, st->keys, st->ltable, st->ctable, st->otable, st->trows,
-                         st->tocc, st->tclk, st->snap_cnt, st->xrows, st->xocc, st->stable, st->sctr, st->cgrid};
+                         st->tocc, st->tclk, st->snap_cnt, st->xrows, st->xocc, st->stable, st->sctr, st->cgrid,
+                         st->rfirst};
     for (void* p : all) cudaFree(p);
     amb_v3_free(&st->v3);
     amb_sbs1_bufs_free(&st->sb);
+    amb_report_bufs_free(&st->rb);
     *st = AmbDecodeState();
 }
 
 // Enqueue one decode of the n frames into the n records on stream s, in this order: fields, pairing, resolve, then the
 // local CPR stage when its S is > 0, the coverage map when coverage is on (after the local stage, so that local fixes
 // reach it), the Comm-B, op-status and track stages whose S is > 0, and the track extension when track and track_ext
-// are both > 0, then the SBS-1 feed when sbs1 is on. Returns how many kernels were launched (7, plus 6 per stage that
-// is on, plus 1 for the coverage map and 10 for the SBS-1 feed), or an AMB_STAGE_* code with *err set.
+// are both > 0, then the SBS-1 feed when sbs1 is on, then the text reports when reports is on. Returns how many kernels
+// were launched (7, plus 6 per stage that is on, plus 1 for the coverage map, 10 for the SBS-1 feed and 3 for the text
+// reports), or an AMB_STAGE_* code with *err set.
 static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n, amb_fields* fields, cudaStream_t s,
                              cudaError_t* err)
 {
@@ -297,6 +337,11 @@ static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n,
                                        s, err);
         if (ks < 0) return AMB_STAGE_SBS1;
         k += ks;
+    }
+    if (st->reports > 0) {
+        const int kr = amb_reports_launch(frames, fields, n, st->rfirst, &st->rb, s, err);
+        if (kr < 0) return AMB_STAGE_REPORTS;
+        k += kr;
     }
     return k;
 }

@@ -73,9 +73,29 @@ AMB_HD char* amb_sbs1_hex6(char* p, uint32_t v)         // %06X of a 24-bit valu
 
 AMB_HD uint64_t amb_sbs1_bits(double x) { uint64_t b; memcpy(&b, &x, 8); return b; }
 
-// '%.<prec>f' % x (prec 1..5) as Python writes it: the exact binary value rounded half to even, the sign of -0.0 and of
-// a value that rounds to zero kept, nan / inf / -inf. Returns nullptr for |x| >= 2^63 (never a field of a line).
-AMB_HD char* amb_sbs1_fixed(char* p, double x, int prec)
+AMB_HD char* amb_fmt_u128(char* p, unsigned __int128 v)  // %i of a non-negative int below 2^128
+{
+    if (!(v >> 64)) return amb_sbs1_u64(p, (uint64_t)v);
+    uint32_t w[4] = {(uint32_t)(v >> 96), (uint32_t)(v >> 64), (uint32_t)(v >> 32), (uint32_t)v};
+    char t[39]; int n = 0;
+    for (bool more = true; more;) {                     // divide the 32-bit limbs by 10, most significant first
+        uint64_t r = 0;
+        more = false;
+        for (int i = 0; i < 4; i++) {
+            const uint64_t x = (r << 32) | w[i];
+            w[i] = (uint32_t)(x / 10); r = x % 10;
+            more = more || w[i];
+        }
+        t[n++] = (char)('0' + r);
+    }
+    while (n) *p++ = t[--n];
+    return p;
+}
+
+// '%.<prec>f' % x (prec 0..8) as Python writes it: the exact binary value rounded half to even (for prec 0 the last
+// digit is the integer part's, and no point is written), the sign of -0.0 and of a value that rounds to zero kept,
+// nan / inf / -inf. Returns nullptr for |x| >= 2^lim (lim 53..66), which the caller never formats.
+AMB_HD char* amb_fmt_fixed(char* p, double x, int prec, int lim)
 {
     const uint64_t b = amb_sbs1_bits(x);
     const int ex = (int)((b >> 52) & 0x7FF);
@@ -89,27 +109,33 @@ AMB_HD char* amb_sbs1_fixed(char* p, double x, int prec)
     if (ex) { m |= 1ull << 52; sh = 1075 - ex; } else sh = 1074;
     uint64_t P = 1;
     for (int i = 0; i < prec; i++) P *= 10;
-    uint64_t ip, fd;                                    // integer part, decimals
+    unsigned __int128 ip;                               // integer part
+    uint64_t fd;                                        // decimals
     if (sh <= 0) {
-        if (-sh > 10) return nullptr;                   // m << -sh would reach 2^63
-        ip = m << -sh; fd = 0;
+        if (-sh > lim - 53) return nullptr;             // m << -sh would reach 2^lim
+        ip = (unsigned __int128)m << -sh; fd = 0;
     } else {
         ip = sh < 64 ? m >> sh : 0;
         const uint64_t f = sh < 64 ? m & ((1ull << sh) - 1) : m;    // the fraction is f / 2^sh
-        if (sh >= 128) fd = 0;                          // f * P < 2^71 < 2^(sh - 1): below half a unit of the last digit
+        if (sh >= 128) fd = 0;                          // f * P < 2^80 < 2^(sh - 1): below half a unit of the last digit
         else {
             const unsigned __int128 num = (unsigned __int128)f * P;
             uint64_t q = (uint64_t)(num >> sh);
             const unsigned __int128 rem = num - ((unsigned __int128)q << sh), half = (unsigned __int128)1 << (sh - 1);
-            if (rem > half || (rem == half && (q & 1))) q++;
+            if (!prec) { if (rem > half || (rem == half && (ip & 1))) ip++; }   // the last digit is the integer part's
+            else if (rem > half || (rem == half && (q & 1))) q++;
             if (q == P) { q = 0; ip++; }
             fd = q;
         }
     }
-    p = amb_sbs1_u64(p, ip);
+    p = amb_fmt_u128(p, ip);
+    if (!prec) return p;
     *p++ = '.';
     return amb_sbs1_dec(p, (unsigned)fd, prec);
 }
+
+// '%.<prec>f' % x (prec 1..5) of a line's field; nullptr for |x| >= 2^63 (never a field of a line).
+AMB_HD char* amb_sbs1_fixed(char* p, double x, int prec) { return amb_fmt_fixed(p, x, prec, 63); }
 
 // '%i' % x of a float: int(x), truncated toward zero (-0.0 and -0.5 print 0). nullptr where Python raises (nan, inf)
 // or |x| >= 2^63.

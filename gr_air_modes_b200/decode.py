@@ -137,6 +137,11 @@ def check_coverage(on) -> int:
     return _check_switch("coverage", on)
 
 
+def check_reports(on) -> int:
+    """Validate a setting of decoder option reports: False / True or 0 / 1. Raises ValueError otherwise."""
+    return _check_switch("reports", on)
+
+
 def check_sbs1_tz(minutes) -> int:
     """Validate a setting of decoder option sbs1_tz: an int in SBS1_TZ_MIN .. SBS1_TZ_MAX minutes. Raises ValueError
     otherwise."""
@@ -344,14 +349,20 @@ class batch_decoder:
     coverage = True also keeps, on the device, the reference's azimuth map model: the greatest range heard in every
     5-degree bearing sector for each of nine altitude bands, from the positions with a range (a receiver location is
     needed); read with coverage() / coverage_device(), clear with reset_coverage() (DESIGN.md §8 "Receiver
-    coverage")."""
+    coverage").
+    reports = True also writes, on the device, the text reports the reference's stdout printer (msprint.py, what
+    modes_rx prints by default) prints for the decoded messages: report.format_report of each frame's slicer text and
+    its record, the stream's first queued message at the slicer's precision 6; read the last decode's lines with
+    report_text() / report_text_device() (DESIGN.md §8 "Text reports")."""
 
     def __init__(self, my_location=None, device: int = 0, local_cpr: int = 0, track: int = 0, commb: int = 0,
-                 opstatus: int = 0, track_ext: int = 0, sbs1=False, sbs1_tz: int = 0, coverage=False):
+                 opstatus: int = 0, track_ext: int = 0, sbs1=False, sbs1_tz: int = 0, coverage=False,
+                 reports=False):
         settings = {"local_cpr": check_option("local_cpr", local_cpr), "track": check_option("track", track),
                     "commb": check_option("commb", commb), "opstatus": check_option("opstatus", opstatus),
                     "track_ext": check_option("track_ext", track_ext)}
         sbs1, sbs1_tz, coverage = check_sbs1(sbs1), check_sbs1_tz(sbs1_tz), check_coverage(coverage)
+        reports = check_reports(reports)
         self._lib = _lib.load()
         h = C.c_void_p()
         have, lat, lon = self._loc(my_location)
@@ -374,6 +385,9 @@ class batch_decoder:
         self._coverage = 0
         if coverage:
             self.set_coverage(True)
+        self._reports = 0
+        if reports:
+            self.set_reports(True)
 
     @staticmethod
     def _loc(loc):
@@ -453,30 +467,54 @@ class batch_decoder:
     def get_sbs1_tz(self) -> int:
         return self._sbs1_tz
 
-    def sbs1_text(self) -> bytes:
-        """The SBS-1 lines of the last decode, concatenated ("\\r\\n" after each). Needs the option sbs1 on."""
+    def _text(self, fetch) -> bytes:
         n = C.c_size_t()
-        rc = self._lib.amb_decoder_sbs1(self._h, None, 0, C.byref(n))
+        rc = fetch(self._h, None, 0, C.byref(n))
         if rc == _lib.ERR_OVERFLOW:
             buf = C.create_string_buffer(n.value)
-            self._check(self._lib.amb_decoder_sbs1(self._h, buf, n.value, C.byref(n)))
+            self._check(fetch(self._h, buf, n.value, C.byref(n)))
             return buf.raw[: n.value]
         self._check(rc)
         return b""
 
+    def _text_device(self, fetch, name, out_dev) -> int:
+        import torch
+        if out_dev.dtype != torch.uint8 or not out_dev.is_cuda or not out_dev.is_contiguous():
+            raise ValueError("%s: out_dev must be a contiguous CUDA uint8 tensor" % name)
+        n = C.c_size_t()
+        torch.cuda.current_stream(out_dev.device).synchronize()          # the decoder runs on its own stream
+        rc = fetch(self._h, C.c_void_p(out_dev.data_ptr()), int(out_dev.numel()), C.byref(n))
+        if rc == _lib.ERR_OVERFLOW:
+            raise RuntimeError("%s: %d bytes needed, out_dev holds %d" % (name, n.value, out_dev.numel()))
+        self._check(rc)
+        return int(n.value)
+
+    def sbs1_text(self) -> bytes:
+        """The SBS-1 lines of the last decode, concatenated ("\\r\\n" after each). Needs the option sbs1 on."""
+        return self._text(self._lib.amb_decoder_sbs1)
+
     def sbs1_text_device(self, out_dev) -> int:
         """sbs1_text() into out_dev, a CUDA uint8 tensor; returns the byte count. Only the count crosses PCIe. Raises
         RuntimeError (with the size needed) when out_dev is too small."""
-        import torch
-        if out_dev.dtype != torch.uint8 or not out_dev.is_cuda or not out_dev.is_contiguous():
-            raise ValueError("sbs1_text_device: out_dev must be a contiguous CUDA uint8 tensor")
-        n = C.c_size_t()
-        torch.cuda.current_stream(out_dev.device).synchronize()          # the decoder runs on its own stream
-        rc = self._lib.amb_decoder_sbs1_device(self._h, C.c_void_p(out_dev.data_ptr()), int(out_dev.numel()), C.byref(n))
-        if rc == _lib.ERR_OVERFLOW:
-            raise RuntimeError("sbs1_text_device: %d bytes needed, out_dev holds %d" % (n.value, out_dev.numel()))
-        self._check(rc)
-        return int(n.value)
+        return self._text_device(self._lib.amb_decoder_sbs1_device, "sbs1_text_device", out_dev)
+
+    def set_reports(self, on):
+        """Option reports on (True) or off (False); applies from the next decode."""
+        on = check_reports(on)
+        self._check(self._lib.amb_decoder_set_option(self._h, b"reports", on))
+        self._reports = on
+
+    def get_reports(self) -> bool:
+        return bool(self._reports)
+
+    def report_text(self) -> bytes:
+        """The text reports of the last decode, concatenated ("\\n" after each line). Needs the option reports on."""
+        return self._text(self._lib.amb_decoder_reports)
+
+    def report_text_device(self, out_dev) -> int:
+        """report_text() into out_dev, a CUDA uint8 tensor; returns the byte count. Only the count crosses PCIe. Raises
+        RuntimeError (with the size needed) when out_dev is too small."""
+        return self._text_device(self._lib.amb_decoder_reports_device, "report_text_device", out_dev)
 
     def set_coverage(self, on):
         """Option coverage on (True) or off (False); applies from the next decode. The grid is kept while it is off."""

@@ -633,6 +633,36 @@ typedef struct amb_aircraft_ext {
 #define AMB_COVERAGE_BANDS 9     /* altitude bands, by their upper edge: */
 #define AMB_COVERAGE_ALTITUDES {0, 1000, 2000, 5000, 10000, 15000, 20000, 25000, 30000}   /* feet (az_map.py:42) */
 
+/* Text reports (amb_decoder_set_option(d, "reports", 1)): every decode also writes the lines that the reference's stdout
+ * printer (air_modes.output_print, python/msprint.py; what apps/modes_rx prints by default) would print for its records.
+ * For every frame, in stream order, the line is exactly report.format_report(text, record) + "\n" of
+ * gr_air_modes_b200/report.py, where text = amb_format_message(frame, first); where format_report returns None nothing
+ * is written. The lines of one call are concatenated in record order. Consequences:
+ *   1 printed   frames that were not queued print nothing; AMB_FS_NO_HANDLER prints nothing unless option "commb" gave a
+ *               DF20/21 record a register (DECODED / RESOLVED) or option "opstatus" decoded a TC 31 / TC 29 squitter,
+ *               which print their own lines; DF0 with AMB_FS_METRIC_ALT or ri in {1, 5, 6, 7, 8}, DF4 with
+ *               AMB_FS_METRIC_ALT, DF4/5 with fs 0, 6 or 7, DF16, BDS0,8 whose cat is out of its ftc's row, BDS0,5 / 0,6
+ *               without AMB_FS_HAS_POS (a local fix of option "local_cpr" counts), TCAS tti 2 without a threat
+ *               altitude and DF20 without an altitude print nothing. The stage runs after every other stage.
+ *   2 prefix    "(%i %.8f) " from the message text, not the raw frame: level' = the double nearest to "%.*g" of the
+ *               frame's float32 ref_level (precision 6 for the first message, 10 after), rssi = 10 * log10(max(1e-8,
+ *               level')) truncated; frac' = the double nearest to "%.10g" of frac, secs' = secs + int(frac'),
+ *               frac' -= int(frac'), and "%.8f" of float(secs') + frac'. So the lines are the same whether the frames
+ *               came from rx_path or were parsed back from its messages.
+ *   3 first     the first queued frame the stage formats after amb_decoder_create or the last amb_decoder_reset takes
+ *               precision 6: the stream's first message when the decoder sees the stream from its start. Turning the
+ *               option on mid-stream counts from there; turning it off and on again does not restart the count.
+ *   4 numbers   as Python's % writes them: %.Nf (N = 0, 1, 2, 3, 6, 8) the exact binary value rounded half to even (the
+ *               stamp exact up to secs = 2^64 - 1), %i of a float truncated, %x / %.6x / %04x lower-case hex. The
+ *               derived values are report.py / decode.py's fp64 expressions in the same order, without contraction. A
+ *               NaN level prints -80; a +inf level, a frac that is not finite or |frac| >= 2^64, and a body number
+ *               %.Nf / %i cannot hold below 2^63 write no line (Python raises, or prints what the receiver never
+ *               writes).
+ *   5 log10     where level' is a power of ten the rssi is 10 times its exponent; elsewhere 10 * log10(level') lies far
+ *               from an integer for every float32 level, so the device's log10 truncates as CPython's does.
+ * One flag word (the first message) and, per frame of capacity, 4 + 478 bytes plus 12 bytes per 128 frames, allocated
+ * at the first decode with the option on. A decode with the option on launches three kernels more; with it off
+ * nothing changes. */
 typedef struct amb_decoder amb_decoder;
 /* cpr_decoder(my_location) (cpr.py:184-190) + the parser; have_location = 0 is my_location = None. */
 AMB_API int amb_decoder_create(int device, int have_location, double lat, double lon, amb_decoder** out);
@@ -658,6 +688,7 @@ AMB_API int amb_decoder_create(int device, int have_location, double lat, double
  * "sbs1": 0 (default, off) or 1, the SBS-1 feed (see AMB_SBS1_TZ_MIN); applies from the next call.
  * "sbs1_tz": AMB_SBS1_TZ_MIN .. AMB_SBS1_TZ_MAX minutes (default 0, UTC) added to the stamp in the SBS-1 date and time.
  * "coverage": 0 (default, off) or 1, the receiver coverage map (see AMB_COVERAGE_ROWS); applies from the next call.
+ * "reports": 0 (default, off) or 1, the text reports (see amb_decoder_reports); applies from the next call.
  * Unknown names and out-of-range values return AMB_ERR_INVALID. */
 AMB_API int amb_decoder_set_option(amb_decoder* d, const char* name, int value);
 /* Snapshot of the per-aircraft table at time `now`: every row with seen <= now and now - seen <= S, in ascending
@@ -680,6 +711,12 @@ AMB_API int amb_decoder_aircraft_ext_device(amb_decoder* d, double now, amb_airc
  * to device memory instead, so only the byte count crosses PCIe. */
 AMB_API int amb_decoder_sbs1(amb_decoder* d, char* out, size_t cap, size_t* n_bytes);
 AMB_API int amb_decoder_sbs1_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes);
+/* The text reports of the last decode, concatenated ("\n" after each line), into out (cap bytes; no terminator);
+ * *n_bytes = their length. AMB_ERR_STATE when the option "reports" is off; a buffer of fewer than *n_bytes bytes returns
+ * AMB_ERR_OVERFLOW with nothing written (out may then be NULL with cap 0). One 8-byte copy to the host, then the text;
+ * _device copies the text to device memory instead, so only the byte count crosses PCIe. */
+AMB_API int amb_decoder_reports(amb_decoder* d, char* out, size_t cap, size_t* n_bytes);
+AMB_API int amb_decoder_reports_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes);
 /* The coverage grid, AMB_COVERAGE_ROWS x AMB_COVERAGE_BANDS doubles, row-major (bearing row first, band second), into
  * out (host memory); _device copies it to device memory. All zeros before the first decode with the option on.
  * amb_decoder_coverage_reset clears the grid and nothing else (az_map_model.reset, az_map.py:77-82). All three return

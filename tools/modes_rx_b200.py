@@ -140,12 +140,13 @@ def write_aircraft(path, rows, ext=None):
 
 class report_queue:
     """What apps/modes_rx prints by default: air_modes.output_print(cpr_dec, publisher) (apps/modes_rx:77-78,
-    python/msprint.py) - one text report per parsed message. The numbers come from the GPU batch decoder
-    (gr_air_modes_b200.decode), the line format from gr_air_modes_b200.report. out=None decodes without printing;
+    python/msprint.py) - one text report per parsed message. The GPU batch decoder (gr_air_modes_b200.decode) forms
+    the lines on the device (option reports: gr_air_modes_b200.report's lines). out=None decodes without printing;
     aircraft=PATH writes the decoder's aircraft table (option track) to PATH after every batch, with the extension of
     every row when track_ext is on; sbs1=server (gr_air_modes_b200.sbs1.sbs1_server) sends the batch's SBS-1 lines to
     it, with the date and time shifted by sbs1_tz minutes; coverage=PATH writes the decoder's coverage map (option
-    coverage) to PATH after every batch (decode.coverage_to_dict)."""
+    coverage) to PATH after every batch (decode.coverage_to_dict). A decoder given as `decoder` is used as it is, except
+    that option reports is turned on when out is not None."""
 
     def __init__(self, location, device, out=sys.stdout, local_cpr=0, track=0, aircraft=None, decoder=None, commb=0,
                  opstatus=0, track_ext=0, sbs1=None, sbs1_tz=0, coverage=None):
@@ -153,7 +154,10 @@ class report_queue:
         self._dec = decoder if decoder is not None else \
             decode.batch_decoder(location, device, local_cpr=local_cpr, track=track, commb=commb,
                                  opstatus=opstatus, track_ext=track_ext, sbs1=sbs1 is not None,
-                                 sbs1_tz=sbs1_tz, coverage=coverage is not None)   # = cpr_decoder(my_position), apps/modes_rx:68
+                                 sbs1_tz=sbs1_tz, coverage=coverage is not None,
+                                 reports=out is not None)   # = cpr_decoder(my_position), apps/modes_rx:68
+        if decoder is not None and out is not None:
+            decoder.set_reports(True)                   # flush() prints the decoder's text reports
         self._out, self._texts, self.count, self._aircraft = out, [], 0, aircraft
         self._coverage, self._location = coverage, location
         self._ext = track_ext > 0
@@ -167,15 +171,14 @@ class report_queue:
 
     def flush(self):
         """Decode and print everything queued since the last call (one GPU batch)."""
-        from gr_air_modes_b200 import report
         if self._texts:
-            recs = self._dec.decode_messages(self._texts)
+            self._dec.decode_messages(self._texts)
             if self._sbs1 is not None:
                 self._sbs1.send(self._dec.sbs1_text())
             if self._out is not None:
-                for line in report.report_lines(self._texts, recs):
-                    self._out.write(line + "\n")
-                    self.count += 1
+                text = self._dec.report_text()
+                self._out.write(text.decode("latin-1"))
+                self.count += text.count(b"\n")
             self._texts = []
         if self._out is not None:
             self._out.flush()
