@@ -44,6 +44,7 @@ SBS1_TZ_MIN, SBS1_TZ_MAX = -720, 840
 # coverage map (decoder option coverage; include/airmodes_b200.h AMB_COVERAGE_*)
 COVERAGE_ROWS, COVERAGE_BANDS = 72, 9
 COVERAGE_ALTITUDES = (0, 1000, 2000, 5000, 10000, 15000, 20000, 25000, 30000)
+ERR_INVALID = -1                 # AMB_ERR_INVALID
 ERR_OVERFLOW = -5                # AMB_ERR_OVERFLOW: the buffer is too small (amb_decoder_sbs1 reports the size needed)
 
 
@@ -163,10 +164,33 @@ class AircraftExt(C.Structure):
                 ("pad_", C.c_uint8 * 10)]
 
 
+class MlatFix(C.Structure):
+    """struct amb_mlat_fix (112 bytes): one multilateration fix (include/airmodes_b200.h amb_mlat)."""
+    _fields_ = [("data", C.c_uint8 * 14), ("nbits", C.c_uint8), ("df", C.c_uint8), ("addr", C.c_uint32),
+                ("status", C.c_uint8), ("n", C.c_uint8), ("steps", C.c_uint8), ("ref", C.c_uint8),
+                ("stations", C.c_uint32), ("altitude", C.c_int32), ("secs", C.c_uint64), ("frac", C.c_double),
+                ("lat", C.c_double), ("lon", C.c_double), ("height", C.c_double), ("x", C.c_double), ("y", C.c_double),
+                ("z", C.c_double), ("rms", C.c_double), ("dop", C.c_double)]
+
+
+class MlatCounts(C.Structure):
+    """struct amb_mlat_counts (80 bytes): amb_mlat_stats."""
+    _fields_ = [("eligible", C.c_uint64), ("carried", C.c_uint64), ("solved", C.c_uint64),
+                ("no_convergence", C.c_uint64), ("degenerate", C.c_uint64), ("too_few", C.c_uint64),
+                ("duplicate", C.c_uint64), ("span", C.c_uint64), ("kernel_launches", C.c_uint64),
+                ("ms_last", C.c_float), ("pad_", C.c_uint32)]
+
+
+# amb_mlat_fix.status (include/airmodes_b200.h AMB_MLAT_*)
+MLAT_SOLVED, MLAT_NO_CONVERGENCE, MLAT_DEGENERATE = 1, 2, 3
+MLAT_MIN_STATIONS, MLAT_MAX_STATIONS = 3, 32
+
 assert C.sizeof(Frame) == 80
 assert C.sizeof(Fields) == 144
 assert C.sizeof(Aircraft) == 128
 assert C.sizeof(AircraftExt) == 144
+assert C.sizeof(MlatFix) == 112
+assert C.sizeof(MlatCounts) == 80
 
 # every symbol include/airmodes_b200.h declares: (name, restype, argtypes)
 _vp, _f32p, _u64p = C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_uint64)
@@ -232,6 +256,19 @@ SYMBOLS = [
     ("amb_decoder_coverage_reset", C.c_int, [_vp]),
     ("amb_decoder_stats", C.c_int, [_vp, _u64p, _f32p]),
     ("amb_decoder_last_error", C.c_char_p, [_vp]),
+    ("amb_mlat_create", C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double),
+                                  C.POINTER(C.c_double), C.POINTER(_vp)]),
+    ("amb_mlat_destroy", None, [_vp]),
+    ("amb_mlat_set_option", C.c_int, [_vp, C.c_char_p, C.c_double]),
+    ("amb_mlat_get_option", C.c_int, [_vp, C.c_char_p, C.POINTER(C.c_double)]),
+    ("amb_mlat_set_offset", C.c_int, [_vp, C.c_int, C.c_double]),
+    ("amb_mlat_reset", C.c_int, [_vp]),
+    ("amb_mlat_process", C.c_int, [_vp, C.POINTER(_vp), C.POINTER(C.c_int), C.c_uint64, C.c_double, C.c_int, _vp,
+                                   C.c_int, C.POINTER(C.c_int)]),
+    ("amb_mlat_process_device", C.c_int, [_vp, C.POINTER(_vp), C.POINTER(C.c_int), C.c_uint64, C.c_double, C.c_int,
+                                          _vp, C.c_int, C.POINTER(C.c_int)]),
+    ("amb_mlat_stats", C.c_int, [_vp, C.POINTER(MlatCounts)]),
+    ("amb_mlat_last_error", C.c_char_p, [_vp]),
     ("amb_frame_bits", C.c_uint64, [C.POINTER(Frame), C.c_int, C.c_int]),
     ("amb_strerror", C.c_char_p, [C.c_int]),
     ("amb_last_error", C.c_char_p, [_vp]),

@@ -38,9 +38,11 @@
 // With option "reports" on, three more after those (amb_decode_reports.cuh): amb_reports_len, amb_sbs1_scan,
 // amb_reports_write - the call's text reports, the lines of report.py, packed on the device; amb_decoder_reports copies
 // them out.
+// The multilateration object amb_mlat (amb_mlat.cuh) lives here too: its C ABI is at the end of this file.
 #include "amb_launch.h"
 #include "amb_decode_core.h"
 #include "amb_decode_kernels.cuh"
+#include "amb_mlat.cuh"
 
 #include <stdio.h>
 #include <string.h>
@@ -516,5 +518,272 @@ uint64_t amb_frame_bits(const amb_frame* f, int start, int num)
     if (!f || start < 1 || num < 1 || num > 64) return 0;
     return amb_bits(amb_msg_from_frame(*f), start, num);
 }
+
+}  // extern "C"
+
+// ---- multilateration (amb_mlat.cuh) ---------------------------------------------------------------------------------
+struct amb_mlat {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    AmbMlatState st;
+    amb_mlat_counts totals = {};
+    std::string err;
+};
+
+static thread_local std::string g_mlat_create_err;
+
+static int mfail(amb_mlat* m, int code, const char* what, cudaError_t e = cudaSuccess)
+{
+    if (m) {
+        char buf[256];
+        if (e != cudaSuccess) snprintf(buf, sizeof buf, "%s: %s", what, cudaGetErrorString(e));
+        else snprintf(buf, sizeof buf, "%s", what);
+        m->err = buf;
+    }
+    return code;
+}
+#define MCK(call)                                                                  \
+    do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return mfail(m, AMB_ERR_CUDA, #call, e_); } while (0)
+
+// llh2ecef (mlat.py:77-86) of a station, and the terms of the start point overhead it
+static AmbMlatStation mlat_station(double lat_deg, double lon_deg, double height)
+{
+    AmbMlatStation o;
+    const double lat = lat_deg * (M_PI / 180.0), lon = lon_deg * (M_PI / 180.0);
+    o.sl = sin(lat); o.cl = cos(lat); o.so = sin(lon); o.co = cos(lon);
+    o.n = AMB_MLAT_WGS_A / sqrt(1 - AMB_MLAT_WGS_E2 * (o.sl * o.sl));
+    o.s[0] = (o.n + height) * o.cl * o.co; o.s[1] = (o.n + height) * o.cl * o.so;
+    o.s[2] = (o.n * (1 - AMB_MLAT_WGS_E2) + height) * o.sl;
+    return o;
+}
+
+extern "C" {
+
+int amb_mlat_create(int device, int K, const double* lat, const double* lon, const double* height, amb_mlat** out)
+{
+    static_assert(sizeof(amb_mlat_fix) == 112, "amb_mlat_fix layout");
+    static_assert(sizeof(amb_mlat_counts) == 80, "amb_mlat_counts layout");
+    static_assert(sizeof(AmbMlatItem) == 48, "item layout");
+    if (!out) return AMB_ERR_INVALID;
+    *out = nullptr;
+    if (K < AMB_MLAT_MIN_STATIONS || K > AMB_MLAT_MAX_STATIONS || !lat || !lon || !height) {
+        g_mlat_create_err = "amb_mlat_create: K must be 3 .. 32, with lat, lon and height for each station";
+        return AMB_ERR_INVALID;
+    }
+    for (int k = 0; k < K; k++)
+        if (!(fabs(lat[k]) <= 90.0) || !(fabs(lon[k]) <= 360.0) || !(fabs(height[k]) < 1e6)) {
+            g_mlat_create_err = "amb_mlat_create: a station position is out of range";
+            return AMB_ERR_INVALID;
+        }
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) return AMB_ERR_NO_DEVICE;
+    cudaDeviceProp prop;
+    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return AMB_ERR_NO_DEVICE;
+    if (prop.major != 9 || prop.minor != 0) return AMB_ERR_NO_DEVICE;   // sm_90a cubin only; there is no CPU path
+    amb_mlat* m = new (std::nothrow) amb_mlat();
+    if (!m) return AMB_ERR_INVALID;
+    m->device = device;
+    m->st.K = K;
+    AmbMlatStation sta[AMB_MLAT_MAX_STATIONS];
+    double dmax = 0.0;
+    for (int k = 0; k < K; k++) sta[k] = mlat_station(lat[k], lon[k], height[k]);
+    for (int i = 0; i < K; i++)
+        for (int j = i + 1; j < K; j++) {
+            const double d = amb_mlat_norm3(sta[i].s[0] - sta[j].s[0], sta[i].s[1] - sta[j].s[1], sta[i].s[2] - sta[j].s[2]);
+            dmax = d > dmax ? d : dmax;
+        }
+    m->st.W = dmax / AMB_MLAT_C + 2e-6;
+    int rc = AMB_OK;
+    do {
+        if (cudaSetDevice(device) != cudaSuccess) { rc = AMB_ERR_NO_DEVICE; break; }
+        if (cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) != cudaSuccess ||
+            cudaEventCreate(&m->e0) != cudaSuccess || cudaEventCreate(&m->e1) != cudaSuccess) { rc = AMB_ERR_CUDA; break; }
+        if (cudaMalloc(&m->st.sta, (size_t)K * sizeof(AmbMlatStation)) != cudaSuccess ||
+            cudaMemcpy(m->st.sta, sta, (size_t)K * sizeof(AmbMlatStation), cudaMemcpyHostToDevice) != cudaSuccess) {
+            rc = AMB_ERR_CUDA; break;
+        }
+    } while (0);
+    if (rc != AMB_OK) { g_mlat_create_err = "CUDA resource creation failed"; amb_mlat_destroy(m); return rc; }
+    g_mlat_create_err.clear();
+    *out = m;
+    return AMB_OK;
+}
+
+void amb_mlat_destroy(amb_mlat* m)
+{
+    if (!m) return;
+    cudaSetDevice(m->device);
+    if (m->stream) cudaStreamSynchronize(m->stream);
+    amb_mlat_free(&m->st);
+    if (m->e0) cudaEventDestroy(m->e0);
+    if (m->e1) cudaEventDestroy(m->e1);
+    if (m->stream) cudaStreamDestroy(m->stream);
+    delete m;
+}
+
+int amb_mlat_set_option(amb_mlat* m, const char* name, double value)
+{
+    if (!m || !name) return AMB_ERR_INVALID;
+    if (strcmp(name, "window_us") == 0) {
+        if (!(value > 0.0) || !(value <= 1e6)) return mfail(m, AMB_ERR_INVALID, "window_us: > 0 .. 1e6 microseconds");
+        m->st.W = value / 1e6;
+        return AMB_OK;
+    }
+    return mfail(m, AMB_ERR_INVALID, "amb_mlat_set_option: unknown option");
+}
+
+int amb_mlat_get_option(amb_mlat* m, const char* name, double* value)
+{
+    if (!m || !name || !value) return AMB_ERR_INVALID;
+    if (strcmp(name, "window_us") == 0) { *value = m->st.W * 1e6; return AMB_OK; }
+    return mfail(m, AMB_ERR_INVALID, "amb_mlat_get_option: unknown option");
+}
+
+int amb_mlat_set_offset(amb_mlat* m, int k, double seconds)
+{
+    if (!m) return AMB_ERR_INVALID;
+    if (k < 0 || k >= m->st.K) return mfail(m, AMB_ERR_INVALID, "amb_mlat_set_offset: no such station");
+    if (!(fabs(seconds) <= 1.0)) return mfail(m, AMB_ERR_INVALID, "amb_mlat_set_offset: |seconds| <= 1");
+    m->st.off[k] = seconds;
+    return AMB_OK;
+}
+
+int amb_mlat_reset(amb_mlat* m)
+{
+    if (!m) return AMB_ERR_INVALID;
+    m->st.C = 0;
+    m->totals.carried = 0;
+    return AMB_OK;
+}
+
+static int mlat_impl(amb_mlat* m, const amb_frame* const* frames, const int* counts, uint64_t end_secs, double end_frac,
+                     int flush, amb_mlat_fix* out, int cap, int* n_out, bool on_device)
+{
+    const char* fn = on_device ? "amb_mlat_process_device" : "amb_mlat_process";
+    char what[128];
+    if (!m || !frames || !counts || !n_out || cap < 0 || (cap > 0 && !out) || (!flush && !(end_frac - end_frac == 0.0))) {
+        snprintf(what, sizeof what, "%s: bad argument", fn);
+        return mfail(m, AMB_ERR_INVALID, what);
+    }
+    *n_out = 0;
+    AmbMlatState* s = &m->st;
+    AmbMlatCall c;
+    memset(&c, 0, sizeof c);
+    c.K = s->K;
+    long long P = 0, total = 0;
+    for (int k = 0; k < s->K; k++) {
+        if (counts[k] < 0 || (counts[k] > 0 && !frames[k])) { snprintf(what, sizeof what, "%s: bad frames of station %d", fn, k); return mfail(m, AMB_ERR_INVALID, what); }
+        c.count[k] = counts[k]; c.base[k] = (int)P; c.off[k] = s->off[k];
+        P += (counts[k] + AMB_MLAT_BLOCK - 1) / AMB_MLAT_BLOCK * AMB_MLAT_BLOCK;
+        total += counts[k];
+    }
+    if (P + s->C > (1ll << 30)) { snprintf(what, sizeof what, "%s: more than 2^30 frames in one call", fn); return mfail(m, AMB_ERR_INVALID, what); }
+    c.base[s->K] = (int)P;
+    const int nb = (int)(P / AMB_MLAT_BLOCK);
+    MCK(cudaSetDevice(m->device));
+    cudaStream_t st = m->stream;
+    cudaError_t e = cudaSuccess;
+    // the scan buffers serve the raw blocks and, after the count, the N <= C + total items: sized for both now, because
+    // the count's offsets in boff[0] are read again after it
+    const long long nbn_max = (s->C + total + AMB_MLAT_BLOCK - 1) / AMB_MLAT_BLOCK;
+    if (amb_mlat_prepare_raw(s, nbn_max > nb ? (int)nbn_max : nb, &e) < 0)
+        return mfail(m, AMB_ERR_CUDA, "amb_mlat: scratch memory", e);
+    MCK(cudaEventRecord(m->e0, st));
+    if (on_device) {
+        for (int k = 0; k < s->K; k++) c.f[k] = frames[k];
+    } else if (total) {
+        if (s->raw_cap < (size_t)total) {
+            if (s->raw) cudaFree(s->raw);
+            s->raw = nullptr; s->raw_cap = 0;
+            MCK(cudaMalloc(&s->raw, (size_t)total * sizeof(amb_frame)));
+            s->raw_cap = (size_t)total;
+        }
+        size_t at = 0;
+        for (int k = 0; k < s->K; k++) {
+            if (counts[k]) MCK(cudaMemcpyAsync(s->raw + at, frames[k], (size_t)counts[k] * sizeof(amb_frame), cudaMemcpyHostToDevice, st));
+            c.f[k] = s->raw + at;
+            at += (size_t)counts[k];
+        }
+    }
+    uint64_t launches = 0;
+    unsigned long long E = 0;
+    if (nb) {
+        launches += (uint64_t)amb_mlat_launch_count(c, nb, s, st, &e);
+        if (e != cudaSuccess) return mfail(m, AMB_ERR_CUDA, "amb_mlat: count", e);
+        MCK(cudaMemcpyAsync(&E, s->boff[0] + nb, sizeof E, cudaMemcpyDeviceToHost, st));
+        MCK(cudaStreamSynchronize(st));
+    }
+    const int N = s->C + (int)E;
+    int G = 0, Cn = 0;
+    unsigned long long ctr[AMB_MC_N] = {};
+    if (N > 0) {
+        int npad = 1;
+        while (npad < N) npad <<= 1;
+        if (amb_mlat_prepare_items(s, N, npad, &e) < 0) return mfail(m, AMB_ERR_CUDA, "amb_mlat: scratch memory", e);
+        launches += (uint64_t)amb_mlat_launch_group(c, nb, N, npad, 2048u, end_secs, end_frac, flush, s, st, &e);
+        if (e != cudaSuccess) return mfail(m, AMB_ERR_CUDA, "amb_mlat: grouping", e);
+        const int nbn = (N + AMB_MLAT_BLOCK - 1) / AMB_MLAT_BLOCK;
+        unsigned long long g = 0, cn = 0;
+        MCK(cudaMemcpyAsync(&g, s->boff[0] + nbn, sizeof g, cudaMemcpyDeviceToHost, st));
+        MCK(cudaMemcpyAsync(&cn, s->boff[1] + nbn, sizeof cn, cudaMemcpyDeviceToHost, st));
+        MCK(cudaMemcpyAsync(ctr, s->ctr, sizeof ctr, cudaMemcpyDeviceToHost, st));
+        MCK(cudaStreamSynchronize(st));
+        if (ctr[AMB_MC_UNORDERED]) {
+            snprintf(what, sizeof what, "%s: a station's frames are not in time order", fn);
+            return mfail(m, AMB_ERR_INVALID, what);
+        }
+        G = (int)g; Cn = (int)cn;
+        if (G > cap) {
+            *n_out = G;
+            snprintf(what, sizeof what, "%s: output buffer too small", fn);
+            return mfail(m, AMB_ERR_OVERFLOW, what);
+        }
+        if (!on_device && s->fix_cap < G) {
+            if (s->fix) cudaFree(s->fix);
+            s->fix = nullptr; s->fix_cap = 0;
+            MCK(cudaMalloc(&s->fix, (size_t)G * sizeof(amb_mlat_fix)));
+            s->fix_cap = G;
+        }
+        launches += (uint64_t)amb_mlat_launch_solve(N, G, on_device ? out : s->fix, s, st, &e);
+        if (e != cudaSuccess) return mfail(m, AMB_ERR_CUDA, "amb_mlat: solve", e);
+        if (!on_device && G) MCK(cudaMemcpyAsync(out, s->fix, (size_t)G * sizeof(amb_mlat_fix), cudaMemcpyDeviceToHost, st));
+        MCK(cudaMemcpyAsync(ctr, s->ctr, sizeof ctr, cudaMemcpyDeviceToHost, st));
+    }
+    MCK(cudaEventRecord(m->e1, st));
+    MCK(cudaStreamSynchronize(st));
+    // commit
+    s->C = Cn;
+    *n_out = G;
+    amb_mlat_counts& t = m->totals;
+    t.eligible += E; t.carried = (uint64_t)Cn;
+    t.solved += ctr[AMB_MC_SOLVED]; t.no_convergence += ctr[AMB_MC_NO_CONV]; t.degenerate += ctr[AMB_MC_DEGENERATE];
+    t.too_few += ctr[AMB_MC_TOO_FEW]; t.duplicate += ctr[AMB_MC_DUPLICATE]; t.span += ctr[AMB_MC_SPAN];
+    t.kernel_launches += launches;
+    float ms = 0.f;
+    if (cudaEventElapsedTime(&ms, m->e0, m->e1) == cudaSuccess) t.ms_last = ms;
+    return AMB_OK;
+}
+
+int amb_mlat_process(amb_mlat* m, const amb_frame* const* frames, const int* counts, uint64_t end_secs, double end_frac,
+                     int flush, amb_mlat_fix* out, int cap, int* n_out)
+{
+    return mlat_impl(m, frames, counts, end_secs, end_frac, flush, out, cap, n_out, false);
+}
+
+int amb_mlat_process_device(amb_mlat* m, const amb_frame* const* frames_dev, const int* counts, uint64_t end_secs,
+                            double end_frac, int flush, amb_mlat_fix* out_dev, int cap, int* n_out)
+{
+    return mlat_impl(m, frames_dev, counts, end_secs, end_frac, flush, out_dev, cap, n_out, true);
+}
+
+int amb_mlat_stats(amb_mlat* m, amb_mlat_counts* out)
+{
+    if (!m || !out) return AMB_ERR_INVALID;
+    *out = m->totals;
+    return AMB_OK;
+}
+
+const char* amb_mlat_last_error(const amb_mlat* m) { return m ? m->err.c_str() : g_mlat_create_err.c_str(); }
 
 }  // extern "C"

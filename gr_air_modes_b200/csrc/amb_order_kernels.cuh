@@ -94,18 +94,15 @@ __global__ void __launch_bounds__(128) amb_order_gather_kernel(const amb_frame* 
     out[i] = f;
 }
 
-// Enqueue keys -> network -> gather on stream s. key/val hold npad = next power of two >= n entries. Returns the number of
-// kernels launched (for the launch counter).
-static int amb_launch_order(const amb_frame* frames, unsigned n, unsigned npad, unsigned tile, unsigned long long* key, unsigned* val,
-                            amb_frame* out, unsigned long long rate, unsigned long long t0_secs, double t0_frac,
-                            const AmbTagDev* tags, int ntags, cudaStream_t s, cudaError_t* err)
+// The network alone on key/val (npad entries, a power of two), ascending by key, on stream s. Returns the number of
+// kernels launched. Not static: the multilateration stage of the decoder's translation unit sorts with it too.
+int amb_launch_bitonic(unsigned long long* key, unsigned* val, unsigned npad, unsigned tile, cudaStream_t s)
 {
     int launches = 0;
     if (tile > npad) tile = npad;
     const unsigned tiles = npad / tile;
     const size_t smem = (size_t)tile * (sizeof(unsigned long long) + sizeof(unsigned));
     const unsigned lthreads = tile / 2 < 512 ? (tile / 2 < 32 ? 32 : tile / 2) : 512;
-    AMB_LAUNCH((amb_order_keys_kernel), (npad + 255) / 256, 256, 0, s, frames, n, npad, key, val); launches++;
     if (npad > 1) {
         AMB_LAUNCH((amb_order_local_kernel), tiles, lthreads, smem, s, key, val, npad, tile, 2u, tile); launches++;
         for (unsigned k = tile << 1; k <= npad && k; k <<= 1) {
@@ -115,6 +112,18 @@ static int amb_launch_order(const amb_frame* frames, unsigned n, unsigned npad, 
             AMB_LAUNCH((amb_order_local_kernel), tiles, lthreads, smem, s, key, val, npad, tile, k, k); launches++;
         }
     }
+    return launches;
+}
+
+// Enqueue keys -> network -> gather on stream s. key/val hold npad = next power of two >= n entries. Returns the number of
+// kernels launched (for the launch counter).
+static int amb_launch_order(const amb_frame* frames, unsigned n, unsigned npad, unsigned tile, unsigned long long* key, unsigned* val,
+                            amb_frame* out, unsigned long long rate, unsigned long long t0_secs, double t0_frac,
+                            const AmbTagDev* tags, int ntags, cudaStream_t s, cudaError_t* err)
+{
+    int launches = 0;
+    AMB_LAUNCH((amb_order_keys_kernel), (npad + 255) / 256, 256, 0, s, frames, n, npad, key, val); launches++;
+    launches += amb_launch_bitonic(key, val, npad, tile, s);
     AMB_LAUNCH((amb_order_gather_kernel), (n + 127) / 128, 128, 0, s, frames, val, n, out, rate, t0_secs, t0_frac, tags, ntags); launches++;
     *err = cudaGetLastError();
     return launches;

@@ -423,3 +423,72 @@ def make_fleet_scene_device(rate: float, n: int, n_aircraft: int, n_bursts: int,
         ok = (idx >= 0) & (idx < n)
         iq2.index_add_(0, idx[ok], vals[ok])
     return iq, (frames, nbytes, starts, who)
+
+
+# ---- several synchronized receivers (multilateration) -------------------------------------------------------------
+def ac13(feet: int) -> int:
+    """The 13-bit AC field of `feet` (a multiple of 25 from -1000 ft) in the 25-ft Q-bit coding."""
+    n = (feet + 1000) // 25
+    return ((n >> 5) << 7) | (((n >> 4) & 1) << 5) | 0x10 | (n & 0x0F)
+
+
+def me_alt12(feet: int) -> int:
+    """The 12-bit ME altitude of `feet` (25-ft Q-bit coding)."""
+    n = (feet + 1000) // 25
+    return ((n >> 4) << 5) | 0x10 | (n & 0x0F)
+
+
+def mlat_frame(kind: int, addr: int, feet: int, rng: np.random.Generator) -> bytes:
+    """DF4 / DF20 altitude reply (AP = CRC ^ address) or DF17 TC 11 airborne position with the ME altitude `feet`."""
+    if kind == 17:
+        me = (11 << 51) | (me_alt12(feet) << 36) | int(rng.integers(0, 1 << 35))
+        body = bytes([(17 << 3) | 5]) + addr.to_bytes(3, "big") + me.to_bytes(7, "big")
+        return body + crc24(body).to_bytes(3, "big")
+    head = (kind << 27) | (int(rng.integers(0, 2)) << 24) | ac13(feet)       # FS 0/1, DR 0, UM 0
+    body = head.to_bytes(4, "big")
+    if kind == 20:
+        body += bytes(7)                                                     # MB: no register
+    return body + (crc24(body) ^ addr).to_bytes(3, "big")
+
+
+def make_mlat_scenes(rate: float, n: int, stations, aircraft, n_tx: int, seed: int, *, t0=(1_700_000_000, 0.25),
+                     noise_sigma: float = 0.01, snr_db: float = 25.0, kinds=(4, 20, 17)):
+    """K Scenes of the same n_tx transmissions as K synchronized receivers hear them.
+
+    stations: [(lat, lon, height_m)]; aircraft: [(addr, lat, lon, height_m)] (the altitude code is the height in feet
+    rounded to 25 ft). The receivers' sample 0 is at t0 = (secs, frac); transmission j leaves at T_j (spread over the
+    recording at least 400 us apart) and starts at (T_j - t0 + |p - s_k| / c) * rate in scene k, each scene with its
+    own noise. Returns (scenes, truth): truth[j] = dict(frame, kind, addr, feet, ecef, T) with T in seconds after t0."""
+    from .mlat import SPEED_OF_LIGHT, llh2ecef
+    rng = np.random.Generator(np.random.PCG64(seed))
+    spc = rate / 2e6
+    S = [np.array(llh2ecef(*s)) for s in stations]
+    span = 240 * spc + 8
+    guard = 4e-3 * rate                                                      # the longest baseline delay, with room
+    slots = int((n - 2 * guard) // (400e-6 * rate))
+    pick = np.sort(rng.choice(slots, size=min(n_tx, slots), replace=False))
+    truth = []
+    for j in pick:
+        addr, lat, lon, h = aircraft[int(rng.integers(0, len(aircraft)))]
+        feet = int(round(h / 0.3048 / 25.0)) * 25
+        kind = int(kinds[int(rng.integers(0, len(kinds)))])
+        p = np.array(llh2ecef(lat, lon, h))
+        T = (guard + j * 400e-6 * rate + rng.uniform(0, 100e-6 * rate)) / rate
+        truth.append({"frame": mlat_frame(kind, addr, feet, rng), "kind": kind, "addr": addr, "feet": feet, "ecef": p,
+                      "T": T})
+    scenes = []
+    amp = float(np.sqrt(2.0 * noise_sigma ** 2 * 10 ** (snr_db / 10)))
+    for k, s in enumerate(S):
+        iq = (rng.standard_normal((n, 2), dtype=np.float32) * np.float32(noise_sigma))
+        c = iq.view(np.complex64).reshape(n)
+        bursts = []
+        for tr in truth:
+            start = (tr["T"] + float(np.linalg.norm(tr["ecef"] - s)) / SPEED_OF_LIGHT) * rate
+            if start + span >= n:
+                continue
+            b = Burst(float(start), tr["frame"], amp, float(rng.uniform(0, 2 * np.pi)))
+            n0, w = burst_waveform(b, spc)
+            c[n0:n0 + w.size] += w
+            bursts.append(b)
+        scenes.append(Scene(rate, n, iq.reshape(2 * n), bursts))
+    return scenes, truth

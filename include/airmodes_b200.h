@@ -741,6 +741,93 @@ AMB_API const char* amb_decoder_last_error(const amb_decoder* d);   /* d == NULL
  * amb_fields does not carry. */
 AMB_API uint64_t amb_frame_bits(const amb_frame* f, int start, int num);
 
+/* ---- multilateration (amb_mlat): K synchronized receivers' frames grouped by transmission, each group solved --------
+ * The model behind the reference's mlat.py / mlat_client.py, with a formulation that solves physical stamps (the
+ * reference's mlat_iter leaves out the reference station's own range, DESIGN.md 8 "Multilateration"). The rules:
+ *   stations   K = AMB_MLAT_MIN_STATIONS .. AMB_MLAT_MAX_STATIONS, each at lat, lon (degrees) and height (m above the
+ *              WGS84 ellipsoid; no geoid correction). Station k's ECEF s_k is llh2ecef of mlat.py:77-86.
+ *   offset     per station, seconds (default 0), subtracted from frac: t = (secs, frac - off_k). It absorbs cable and
+ *              front-end delays and the index bias of stations at different rates.
+ *   eligible   passed != 0 and either DF 0, 4, 16 or 20 whose AC13 field (message bits 20..32, decode_alt with
+ *              bit13 = 1) decodes to feet - not metric, not code 0 - with the address amb_frame.crc; or DF17 TC 9..18
+ *              whose 12-bit ME altitude (bit13 = 0) decodes the same way, with the address AA. Nothing else (the solve
+ *              needs the altitude). h = feet * 0.3048 m, used as height above the ellipsoid as mlat.py does.
+ *   time diff  d(a, b) = (double)(int64)(secs_a - secs_b) + (frac_a - frac_b), never a difference of secs + frac sums.
+ *              t orders by the sign of d, ties by station index.
+ *   run        the eligible frames of all stations (the carried ones included) sorted by (payload, t, station); a run
+ *              is a maximal sequence of identical payloads (nbits and bytes) whose consecutive frames are at most W
+ *              apart (d <= W). W = option "window_us" / 1e6 s; default: the largest station-to-station distance / c
+ *              plus 2 us.
+ *   complete   the call's end stamp promises that every station has delivered every frame with t <= end. A run is
+ *              complete when d(end, t_last) >= W or the call has flush set. The frames of incomplete runs are carried
+ *              on the device into the next call; the others are dropped after the call. amb_mlat_reset clears the carry.
+ *   accepted   a complete run with no station twice (else DUPLICATE), at least 3 frames (else TOO_FEW) and
+ *              d(t_last, t_first) <= W (else SPAN) is a group; the others are only counted.
+ *   solve      per group, fp64 without contraction. c = 299792458 / 1.0003, a = 6378137, b = 6356752.314245,
+ *              e2 = 0.0066943799901975848. Reference station r = the earliest t (ties: lower index); rows follow
+ *              ascending station index. x starts at llh2ecef(lat_r, lon_r, h). Rows: for i != r
+ *              |x - s_i| - |x - s_r| - c d(t_i, t_r) with gradient (x - s_i)/|x - s_i| - (x - s_r)/|x - s_r|, and the
+ *              altitude row |x| - |llh2ecef(lat(x), lon(x), h)| (Bowring's ecef2llh, mlat.py:58-86) with gradient
+ *              x/|x|: n = number of stations rows. Each Gauss-Newton step solves J dx = -f by Householder QR
+ *              (DESIGN.md 8 writes out the operations). |dx| <= 1e-3 m: SOLVED; 25 steps without: NO_CONVERGENCE; a
+ *              diagonal |R_jj| < 1e-9 max |R_jj| (or all zero): DEGENERATE.
+ *   fix        one amb_mlat_fix per group, ordered by the reference station's t (ties: lower reference station). rms
+ *              and dop = sqrt(trace((J^T J)^-1)) are evaluated at the last x (dop NaN when that J is degenerate).
+ * The grouping does not depend on how the streams are cut into calls, as long as every call's end keeps its promise. */
+#define AMB_MLAT_MIN_STATIONS 3
+#define AMB_MLAT_MAX_STATIONS 32
+#define AMB_MLAT_SOLVED 1
+#define AMB_MLAT_NO_CONVERGENCE 2
+#define AMB_MLAT_DEGENERATE 3
+typedef struct amb_mlat amb_mlat;
+/* 112 bytes */
+typedef struct amb_mlat_fix {
+    uint8_t data[14];      /* the payload (nbits / 8 bytes; the rest zero) */
+    uint8_t nbits, df;
+    uint32_t addr;         /* AA of DF17, the address/parity overlay (amb_frame.crc) of DF0/4/16/20 */
+    uint8_t status;        /* AMB_MLAT_* */
+    uint8_t n;             /* stations in the group = rows of the solve */
+    uint8_t steps;         /* Gauss-Newton steps taken */
+    uint8_t ref;           /* the reference station r */
+    uint32_t stations;     /* bit k: station k heard it */
+    int32_t altitude;      /* feet */
+    uint64_t secs;         /* emission time t_r - |x - s_r| / c: secs, and frac normalised to [0, 1) */
+    double frac;
+    double lat, lon, height;   /* ecef2llh of x: degrees, degrees, m above the ellipsoid */
+    double x, y, z;            /* ECEF, m */
+    double rms;                /* sqrt(sum f^2 / n) at x, m */
+    double dop;                /* sqrt(trace((J^T J)^-1)) at x */
+} amb_mlat_fix;
+typedef struct amb_mlat_counts {
+    uint64_t eligible;         /* eligible frames taken in */
+    uint64_t carried;          /* frames carried into the next call now */
+    uint64_t solved, no_convergence, degenerate;     /* groups by outcome */
+    uint64_t too_few, duplicate, span;               /* complete runs rejected, by reason */
+    uint64_t kernel_launches;
+    float ms_last;             /* device time of the last call */
+    uint32_t pad_;
+} amb_mlat_counts;   /* 80 bytes */
+/* K stations; lat[k], lon[k] in degrees, height[k] in m above the ellipsoid. */
+AMB_API int amb_mlat_create(int device, int K, const double* lat, const double* lon, const double* height, amb_mlat** out);
+AMB_API void amb_mlat_destroy(amb_mlat* m);
+/* "window_us": W in microseconds, > 0 (a double: W = value / 1e6 s); applies from the next call. */
+AMB_API int amb_mlat_set_option(amb_mlat* m, const char* name, double value);
+AMB_API int amb_mlat_get_option(amb_mlat* m, const char* name, double* value);
+AMB_API int amb_mlat_set_offset(amb_mlat* m, int k, double seconds);   /* applies to the frames of later calls */
+AMB_API int amb_mlat_reset(amb_mlat* m);                             /* drop the carried frames */
+/* One call: frames[k] holds counts[k] frames of station k in stream order (non-decreasing t), host memory for
+ * amb_mlat_process, device memory for amb_mlat_process_device; out holds cap fixes in the same kind of memory.
+ * (end_secs, end_frac): see "complete" above; flush = 1 completes every run (end is then not read).
+ * Returns AMB_OK with *n_out fixes written. When more than cap fixes are due, returns AMB_ERR_OVERFLOW with *n_out = the
+ * number due and changes nothing - carry, counters and kernel_launches stay as they were: call again with a larger
+ * buffer. A station whose frames are out of time order returns AMB_ERR_INVALID and changes nothing either. Synchronises the stage's own stream: device frames must be complete when called. */
+AMB_API int amb_mlat_process(amb_mlat* m, const amb_frame* const* frames, const int* counts, uint64_t end_secs,
+                             double end_frac, int flush, amb_mlat_fix* out, int cap, int* n_out);
+AMB_API int amb_mlat_process_device(amb_mlat* m, const amb_frame* const* frames_dev, const int* counts, uint64_t end_secs,
+                                    double end_frac, int flush, amb_mlat_fix* out_dev, int cap, int* n_out);
+AMB_API int amb_mlat_stats(amb_mlat* m, amb_mlat_counts* out);
+AMB_API const char* amb_mlat_last_error(const amb_mlat* m);          /* m == NULL: the last failed amb_mlat_create */
+
 AMB_API const char* amb_strerror(int code);
 AMB_API const char* amb_last_error(const amb_ctx* ctx);
 AMB_API const char* amb_version(void);
