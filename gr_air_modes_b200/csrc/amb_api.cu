@@ -115,19 +115,6 @@ static void ingest_free(amb_ctx* c);
 static int ingest_dispatch_pending(amb_ctx* ctx, int flush);
 }
 
-static int fail(amb_ctx* c, int code, const char* what, cudaError_t e = cudaSuccess)
-{
-    if (c) {
-        char buf[256];
-        if (e != cudaSuccess) snprintf(buf, sizeof buf, "%s: %s", what, cudaGetErrorString(e));
-        else snprintf(buf, sizeof buf, "%s", what);
-        c->err = buf;
-    }
-    return code;
-}
-#define CK(call)                                                                  \
-    do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return fail(ctx, AMB_ERR_CUDA, #call, e_); } while (0)
-
 static cudaError_t sync_all(amb_ctx* c)
 {
     cudaError_t e = cudaStreamSynchronize(c->stream);
@@ -170,7 +157,7 @@ static int setup_rate(amb_ctx* ctx)
     if (rc != AMB_OK) return fail(ctx, rc, "unsupported rate (need 2e6 <= rate <= 20e6 and int(rate/2e6) consistent)");
     ctx->P = P;
     memcpy(ctx->chip_off, off, sizeof off);
-    CK(amb_upload_tables(off));
+    CK(ctx, amb_upload_tables(off));
     ctx->guard = amb_chain_guard(P);
     ctx->kc = amb_chain_carry(P);
     if (ctx->use_dcblock) {                              // filter.dc_blocker_cc(100*self._spc, False)  rx_path.py:40
@@ -178,18 +165,18 @@ static int setup_rate(amb_ctx* ctx)
         ctx->dc_nc = 2 * ctx->dc_D - 2;
         for (int k = 0; k < 2; k++) {
             cudaFree(ctx->dc_carry[k]); ctx->dc_carry[k] = nullptr;
-            CK(cudaMalloc(&ctx->dc_carry[k], (size_t)ctx->dc_nc * sizeof(float2)));
+            CK(ctx, cudaMalloc(&ctx->dc_carry[k], (size_t)ctx->dc_nc * sizeof(float2)));
         }
     }
     for (int k = 0; k < 3; k++) {
         cudaFree(ctx->carry[k]); ctx->carry[k] = nullptr;
-        CK(cudaMalloc(&ctx->carry[k], (size_t)ctx->kc * sizeof(float2)));
-        CK(cudaMemset(ctx->carry[k], 0, (size_t)ctx->kc * sizeof(float2)));
+        CK(ctx, cudaMalloc(&ctx->carry[k], (size_t)ctx->kc * sizeof(float2)));
+        CK(ctx, cudaMemset(ctx->carry[k], 0, (size_t)ctx->kc * sizeof(float2)));
         int rc2 = make_tmap(ctx, &ctx->tm_carry[k], ctx->carry[k], (size_t)ctx->kc); if (rc2) return rc2;
     }
     for (int k = 0; k < 2; k++) {
         cudaFree(ctx->tail[k]); ctx->tail[k] = nullptr;
-        CK(cudaMalloc(&ctx->tail[k], (size_t)AMB_TAIL_CAP * sizeof(float2)));
+        CK(ctx, cudaMalloc(&ctx->tail[k], (size_t)AMB_TAIL_CAP * sizeof(float2)));
         int rc2 = make_tmap(ctx, &ctx->tm_tail[k], ctx->tail[k], (size_t)AMB_TAIL_CAP); if (rc2) return rc2;
     }
     return AMB_OK;
@@ -199,11 +186,11 @@ static int reset_stream(amb_ctx* ctx)
 {
     // counters and resolver state belong to stream B (in order after the previous call's tail kernels);
     // the sample history restarts from the all-zero carry buffer, so nothing has to be cleared on stream A
-    CK(cudaMemsetAsync(ctx->ctr, 0, sizeof(AmbCounters), ctx->stream_b));
-    CK(cudaMemsetAsync(ctx->st, 0, sizeof(AmbWalkState), ctx->stream_b));
+    CK(ctx, cudaMemsetAsync(ctx->ctr, 0, sizeof(AmbCounters), ctx->stream_b));
+    CK(ctx, cudaMemsetAsync(ctx->st, 0, sizeof(AmbWalkState), ctx->stream_b));
     if (ctx->use_dcblock) {   // raw-sample history of the DC blocker restarts from zeros (only stream A touches it)
-        CK(cudaMemsetAsync(ctx->dc_carry[0], 0, (size_t)ctx->dc_nc * sizeof(float2), ctx->stream));
-        CK(cudaMemsetAsync(ctx->dc_carry[1], 0, (size_t)ctx->dc_nc * sizeof(float2), ctx->stream));
+        CK(ctx, cudaMemsetAsync(ctx->dc_carry[0], 0, (size_t)ctx->dc_nc * sizeof(float2), ctx->stream));
+        CK(ctx, cudaMemsetAsync(ctx->dc_carry[1], 0, (size_t)ctx->dc_nc * sizeof(float2), ctx->stream));
         ctx->dc_cur = 0;
     }
     ctx->sf0.clear(); ctx->sf1.clear(); ctx->sf_total = 0; ctx->sf_rdone = 0;
@@ -245,11 +232,8 @@ int amb_create(int device, float rate, float threshold_db, int use_pmf, int use_
 {
     if (!out) return AMB_ERR_INVALID;
     *out = nullptr;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) return AMB_ERR_NO_DEVICE;
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return AMB_ERR_NO_DEVICE;
-    if (prop.major != 9 || prop.minor != 0) return AMB_ERR_NO_DEVICE;  // sm_90a cubin only
+    if (amb_check_device(device, &prop) != AMB_OK) return AMB_ERR_NO_DEVICE;
     amb_ctx* ctx = new amb_ctx();
     ctx->device = device; ctx->sm_count = prop.multiProcessorCount;
     ctx->rate_arg = rate; ctx->thr_db = threshold_db; ctx->use_pmf = use_pmf ? 1 : 0;
@@ -325,15 +309,15 @@ void amb_destroy(amb_ctx* ctx)
 int amb_reset(amb_ctx* ctx)
 {
     if (!ctx) return AMB_ERR_INVALID;
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     return reset_stream(ctx);
 }
 
 int amb_set_rate(amb_ctx* ctx, float channel_rate)
 {
     if (!ctx) return AMB_ERR_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    CK(sync_all(ctx));
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, sync_all(ctx));
     const float old = ctx->rate_arg;
     ctx->rate_arg = channel_rate;
     int rc = setup_rate(ctx);
@@ -384,7 +368,7 @@ int amb_query_geometry(float rate, float threshold_db, int use_pmf, amb_geometry
 int amb_set_stream(amb_ctx* ctx, void* cuda_stream)
 {
     if (!ctx) return AMB_ERR_INVALID;
-    CK(sync_all(ctx));
+    CK(ctx, sync_all(ctx));
     if (ctx->own_stream) { cudaStreamDestroy(ctx->stream); ctx->own_stream = false; }
     ctx->stream = (cudaStream_t)cuda_stream;
     return AMB_OK;
@@ -419,10 +403,10 @@ int amb_set_option(amb_ctx* ctx, const char* name, int value)
     if (!strcmp(name, "copy_threads")) { if (value < 0 || value > 64) return AMB_ERR_INVALID; ctx->copy_threads = value; return AMB_OK; }
     if (!strcmp(name, "ingest_chunk")) {                   // samples per chunk of the host ingest ring (multiple of 512)
         if (value < 4096 || (value & 511)) return AMB_ERR_INVALID;
-        CK(cudaSetDevice(ctx->device));
+        CK(ctx, cudaSetDevice(ctx->device));
         if (ctx->pend_n) { int rc = ingest_dispatch_pending(ctx, 0); if (rc) return rc; }
-        CK(sync_all(ctx));
-        if (ctx->stream_h) CK(cudaStreamSynchronize(ctx->stream_h));
+        CK(ctx, sync_all(ctx));
+        if (ctx->stream_h) CK(ctx, cudaStreamSynchronize(ctx->stream_h));
         ingest_free(ctx);
         ctx->ing_chunk = (size_t)value;
         if (ctx->coalesce > ctx->ing_chunk) ctx->coalesce = ctx->ing_chunk;
@@ -440,9 +424,9 @@ int amb_set_option(amb_ctx* ctx, const char* name, int value)
 int amb_synchronize(amb_ctx* ctx)
 {
     if (!ctx) return AMB_ERR_INVALID;
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     if (ctx->pend_n) { int rc = ingest_dispatch_pending(ctx, 0); if (rc) return rc; }
-    CK(sync_all(ctx));
+    CK(ctx, sync_all(ctx));
     return AMB_OK;
 }
 
@@ -456,52 +440,52 @@ static int process_core(amb_ctx* ctx, const float* iq, size_t n_complex, int mem
     const AmbParams& P = ctx->P;
     const int kc = ctx->kc;
     const int set = (int)(ctx->call_idx & 1u);             // double-buffered per-call scratch
-    if (ctx->timing) CK(cudaEventRecord(ctx->ev[2], sa));
+    if (ctx->timing) CK(ctx, cudaEventRecord(ctx->ev[2], sa));
     // stream C stages the tail and the next carry. It starts where the caller's stream is now (the input is
     // ready there) and after call k-2's sparse kernels, the last users of this set's buffers.
-    CK(cudaEventRecord(ctx->e_in, sa));
-    CK(cudaStreamWaitEvent(sc, ctx->e_in, 0));
-    if (ctx->done_valid[set]) { CK(cudaStreamWaitEvent(sc, ctx->e_done[set], 0)); CK(cudaStreamWaitEvent(sa, ctx->e_done[set], 0)); }
+    CK(ctx, cudaEventRecord(ctx->e_in, sa));
+    CK(ctx, cudaStreamWaitEvent(sc, ctx->e_in, 0));
+    if (ctx->done_valid[set]) { CK(ctx, cudaStreamWaitEvent(sc, ctx->e_done[set], 0)); CK(ctx, cudaStreamWaitEvent(sa, ctx->e_done[set], 0)); }
 
     // ---- input placement: device pointers are used in place, host data goes through a staging buffer
     const float2* src = reinterpret_cast<const float2*>(iq);
     if (mem_kind == AMB_MEM_HOST || ((uintptr_t)iq & 15u)) {
         if (ctx->staging_cap < n_complex) {
-            CK(sync_all(ctx));
+            CK(ctx, sync_all(ctx));
             cudaFree(ctx->staging); ctx->staging = nullptr;
             size_t ncap = n_complex + 1024;
-            CK(cudaMalloc(&ctx->staging, ncap * sizeof(float2)));
+            CK(ctx, cudaMalloc(&ctx->staging, ncap * sizeof(float2)));
             ctx->staging_cap = ncap;
         }
         // the previous call's exact/slice kernels and its carry kernel may still read the staging buffer
-        if (ctx->done_valid[set ^ 1]) CK(cudaStreamWaitEvent(sa, ctx->e_done[set ^ 1], 0));
-        if (ctx->aux_valid[set ^ 1]) CK(cudaStreamWaitEvent(sa, ctx->e_aux[set ^ 1], 0));
+        if (ctx->done_valid[set ^ 1]) CK(ctx, cudaStreamWaitEvent(sa, ctx->e_done[set ^ 1], 0));
+        if (ctx->aux_valid[set ^ 1]) CK(ctx, cudaStreamWaitEvent(sa, ctx->e_aux[set ^ 1], 0));
         if (n_complex)
-            CK(cudaMemcpyAsync(ctx->staging, iq, n_complex * sizeof(float2),
+            CK(ctx, cudaMemcpyAsync(ctx->staging, iq, n_complex * sizeof(float2),
                                mem_kind == AMB_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, sa));
         src = ctx->staging;
-        CK(cudaEventRecord(ctx->e_in, sa));
-        CK(cudaStreamWaitEvent(sc, ctx->e_in, 0));
+        CK(ctx, cudaEventRecord(ctx->e_in, sa));
+        CK(ctx, cudaStreamWaitEvent(sc, ctx->e_in, 0));
     }
     if (ctx->use_dcblock) {
         // ---- DC blocker: x -> out[n] = x[n-D+1] - MA(MA(x))[n] into a ctx-owned buffer that then plays the input
         if (ctx->dc_cap < n_complex + (size_t)ctx->dc_D) {
-            CK(sync_all(ctx));
+            CK(ctx, sync_all(ctx));
             cudaFree(ctx->dc_out); ctx->dc_out = nullptr;
             const size_t ncap = n_complex + (size_t)ctx->dc_D + 1024;
-            CK(cudaMalloc(&ctx->dc_out, ncap * sizeof(float2)));
+            CK(ctx, cudaMalloc(&ctx->dc_out, ncap * sizeof(float2)));
             ctx->dc_cap = ncap;
         }
         // the previous call's exact/slice kernels and its carry kernel still read dc_out
-        if (ctx->done_valid[set ^ 1]) CK(cudaStreamWaitEvent(sa, ctx->e_done[set ^ 1], 0));
-        if (ctx->aux_valid[set ^ 1]) CK(cudaStreamWaitEvent(sa, ctx->e_aux[set ^ 1], 0));
-        CK(amb_launch_dcblock(ctx->dc_carry[ctx->dc_cur], ctx->dc_nc, src, (long long)n_complex, ctx->dc_D,
+        if (ctx->done_valid[set ^ 1]) CK(ctx, cudaStreamWaitEvent(sa, ctx->e_done[set ^ 1], 0));
+        if (ctx->aux_valid[set ^ 1]) CK(ctx, cudaStreamWaitEvent(sa, ctx->e_aux[set ^ 1], 0));
+        CK(ctx, amb_launch_dcblock(ctx->dc_carry[ctx->dc_cur], ctx->dc_nc, src, (long long)n_complex, ctx->dc_D,
                               ctx->dc_ma0, ctx->dc_out, ctx->dc_carry[ctx->dc_cur ^ 1], sa));
         ctx->dc_cur ^= 1;
         ctx->stats.kernel_launches += n_complex ? 2 : 1;
         src = ctx->dc_out;
-        CK(cudaEventRecord(ctx->e_in, sa));
-        CK(cudaStreamWaitEvent(sc, ctx->e_in, 0));
+        CK(ctx, cudaEventRecord(ctx->e_in, sa));
+        CK(ctx, cudaStreamWaitEvent(sc, ctx->e_in, 0));
     }
     const AmbSegs S = amb_chain_segs(ctx->carry[ctx->carry_in], kc, src, (int)n_complex, ctx->tail[set]);
     const int n_tv = (int)n_complex - S.n_main;
@@ -537,21 +521,21 @@ static int process_core(amb_ctx* ctx, const float* iq, size_t n_complex, int mem
 
         // ---- stream A: stage the tail + reset the group counts (in front of the scan: a hop over to stream C and
         // back would leave the scan stream idle), then stream over the IQ. Stream C's carry kernel reads the tail.
-        CK(amb_launch_prologue(ctx->tail[set], AMB_TAIL_CAP, src + S.n_main, n_tv, a.group_count, 128, sa));
+        CK(ctx, amb_launch_prologue(ctx->tail[set], AMB_TAIL_CAP, src + S.n_main, n_tv, a.group_count, 128, sa));
         ctx->stats.kernel_launches += 1;
-        CK(cudaEventRecord(ctx->e_in, sa));
-        CK(cudaStreamWaitEvent(sc, ctx->e_in, 0));
-        if (ctx->aux_valid[set ^ 1]) CK(cudaStreamWaitEvent(sa, ctx->e_aux[set ^ 1], 0));   // carry written by the previous call
+        CK(ctx, cudaEventRecord(ctx->e_in, sa));
+        CK(ctx, cudaStreamWaitEvent(sc, ctx->e_in, 0));
+        if (ctx->aux_valid[set ^ 1]) CK(ctx, cudaStreamWaitEvent(sa, ctx->e_aux[set ^ 1], 0));   // carry written by the previous call
         const unsigned slot = (ctx->ring_n & 63u) * 2;
-        if (ctx->timing) { CK(cudaEventRecord(ctx->ev[0], sa)); CK(cudaEventRecord(ctx->ring[slot], sa)); }
-        CK(amb_launch_scan(a, ctx->sm_count, sa));
+        if (ctx->timing) { CK(ctx, cudaEventRecord(ctx->ev[0], sa)); CK(ctx, cudaEventRecord(ctx->ring[slot], sa)); }
+        CK(ctx, amb_launch_scan(a, ctx->sm_count, sa));
         ctx->stats.kernel_launches += 1;
-        if (ctx->timing) { CK(cudaEventRecord(ctx->ev[1], sa)); CK(cudaEventRecord(ctx->ring[slot + 1], sa)); ctx->ring_n++; }
-        CK(cudaEventRecord(ctx->e_scan[set], sa));
+        if (ctx->timing) { CK(ctx, cudaEventRecord(ctx->ev[1], sa)); CK(ctx, cudaEventRecord(ctx->ring[slot + 1], sa)); ctx->ring_n++; }
+        CK(ctx, cudaEventRecord(ctx->e_scan[set], sa));
 
         // ---- stream B: everything sparse; runs under the NEXT call's scan. A time-sharded span stops before the
         // walk: its loop state arrives later (amb_resolve).
-        CK(cudaStreamWaitEvent(sb, ctx->e_scan[set], 0));
+        CK(ctx, cudaStreamWaitEvent(sb, ctx->e_scan[set], 0));
         const int k = amb_chain_launch(a, call, &ctx->bufs, opts, ctx->defer != 0, sb, &ctx->def, &er);
         if (k < 0) return chain_fail(ctx, er);
         ctx->stats.kernel_launches += (uint64_t)k;
@@ -559,21 +543,21 @@ static int process_core(amb_ctx* ctx, const float* iq, size_t n_complex, int mem
         ctx->ev_valid = ctx->timing;
     } else {
         // nothing can be decided yet (tiny call): keep it simple and serial
-        if (ctx->done_valid[set ^ 1]) CK(cudaStreamWaitEvent(sa, ctx->e_done[set ^ 1], 0));
-        CK(amb_launch_prologue(ctx->tail[set], AMB_TAIL_CAP, src + S.n_main, n_tv, nullptr, 0, sa));
+        if (ctx->done_valid[set ^ 1]) CK(ctx, cudaStreamWaitEvent(sa, ctx->e_done[set ^ 1], 0));
+        CK(ctx, amb_launch_prologue(ctx->tail[set], AMB_TAIL_CAP, src + S.n_main, n_tv, nullptr, 0, sa));
         ctx->stats.kernel_launches += 1;
-        CK(cudaEventRecord(ctx->e_in, sa));
-        CK(cudaStreamWaitEvent(sc, ctx->e_in, 0));
-        if (ctx->aux_valid[set ^ 1]) CK(cudaStreamWaitEvent(sa, ctx->e_aux[set ^ 1], 0));
-        CK(cudaEventRecord(ctx->e_scan[set], sa));
-        CK(cudaStreamWaitEvent(sb, ctx->e_scan[set], 0));
+        CK(ctx, cudaEventRecord(ctx->e_in, sa));
+        CK(ctx, cudaStreamWaitEvent(sc, ctx->e_in, 0));
+        if (ctx->aux_valid[set ^ 1]) CK(ctx, cudaStreamWaitEvent(sa, ctx->e_aux[set ^ 1], 0));
+        CK(ctx, cudaEventRecord(ctx->e_scan[set], sa));
+        CK(ctx, cudaStreamWaitEvent(sb, ctx->e_scan[set], 0));
         if (ctx->defer) { ctx->def_kind = flush ? 2 : 3; ctx->def_resolved = false; ctx->def_set = set; }
         if (flush) {   // the resolver still has to close the stream
             if (amb_chain_prepare_empty(&ctx->bufs, &er) < 0) return chain_fail(ctx, er);
             AmbChainSpan& sp = ctx->def;
             sp.wa = amb_chain_walk_args(call, ctx->bufs, ctx->sm_count);
             sp.par = false; sp.walk_only = true;
-            CK(cudaMemsetAsync(&ctx->ctr->ncand, 0, sizeof(unsigned), sb));
+            CK(ctx, cudaMemsetAsync(&ctx->ctr->ncand, 0, sizeof(unsigned), sb));
             if (!ctx->defer) {
                 const int k = amb_chain_resolve(sp, &ctx->bufs, opts, sb, &er);
                 if (k < 0) return chain_fail(ctx, er);
@@ -585,21 +569,21 @@ static int process_core(amb_ctx* ctx, const float* iq, size_t n_complex, int mem
     if (!ctx->defer && ctx->ctr_snap && ctx->snap_head - ctx->snap_tail < AMB_SNAPS) {
         // where the frame counter stands once this call is through: read without blocking by amb_poll_ready
         const unsigned k = (unsigned)(ctx->snap_head % AMB_SNAPS);
-        CK(cudaMemcpyAsync(&ctx->ctr_snap[k], ctx->ctr, sizeof(AmbCounters), cudaMemcpyDeviceToHost, sb));
-        CK(cudaEventRecord(ctx->snap_ev[k], sb));
+        CK(ctx, cudaMemcpyAsync(&ctx->ctr_snap[k], ctx->ctr, sizeof(AmbCounters), cudaMemcpyDeviceToHost, sb));
+        CK(ctx, cudaEventRecord(ctx->snap_ev[k], sb));
         ctx->snap_head++;
     }
-    CK(cudaEventRecord(ctx->e_done[set], sb));
+    CK(ctx, cudaEventRecord(ctx->e_done[set], sb));
     ctx->done_valid[set] = true;
     if (ctx->timing) {
-        CK(cudaEventRecord(ctx->ev[3], sb));
-        if (ctx->ev_valid) CK(cudaEventRecord(ctx->ring_done[(ctx->ring_n - 1) & 63u], sb));
+        CK(ctx, cudaEventRecord(ctx->ev[3], sb));
+        if (ctx->ev_valid) CK(ctx, cudaEventRecord(ctx->ring_done[(ctx->ring_n - 1) & 63u], sb));
     }
     // ---- carry the tail of the stream into the next call (stream C, concurrently with this call's scan).
     // The buffer written here is the one the PREVIOUS call's scan and sparse kernels read as their carry.
-    if (ctx->done_valid[set ^ 1]) CK(cudaStreamWaitEvent(sc, ctx->e_done[set ^ 1], 0));
-    CK(amb_launch_carry(S, ctx->carry[cout], kc, sc));
-    CK(cudaEventRecord(ctx->e_aux[set], sc));
+    if (ctx->done_valid[set ^ 1]) CK(ctx, cudaStreamWaitEvent(sc, ctx->e_done[set ^ 1], 0));
+    CK(ctx, amb_launch_carry(S, ctx->carry[cout], kc, sc));
+    CK(ctx, cudaEventRecord(ctx->e_aux[set], sc));
     ctx->aux_valid[set] = true;
     ctx->stats.kernel_launches += 1;
     ctx->carry_in = cout;
@@ -608,8 +592,8 @@ static int process_core(amb_ctx* ctx, const float* iq, size_t n_complex, int mem
     else if (j_hi > j_lo) ctx->r_done = r_safe;
     ctx->call_idx++;
     if (!ctx->overlap) {                                                    // strict stream-ordered behaviour on stream A
-        CK(cudaStreamWaitEvent(sa, ctx->e_done[set], 0));
-        CK(cudaStreamWaitEvent(sa, ctx->e_aux[set], 0));
+        CK(ctx, cudaStreamWaitEvent(sa, ctx->e_done[set], 0));
+        CK(ctx, cudaStreamWaitEvent(sa, ctx->e_aux[set], 0));
     }
     return AMB_OK;
 }
@@ -690,17 +674,17 @@ void amb_parallel_memcpy(void* dst, const void* src, size_t n) { copy_pool(0)->c
 
 static int ingest_setup(amb_ctx* ctx, bool need_raw)
 {
-    if (!ctx->stream_h) CK(cudaStreamCreateWithFlags(&ctx->stream_h, cudaStreamNonBlocking));
+    if (!ctx->stream_h) CK(ctx, cudaStreamCreateWithFlags(&ctx->stream_h, cudaStreamNonBlocking));
     for (int k = 0; k < AMB_ING_SLOTS; k++) {
         AmbIngestSlot& sl = ctx->ing[k];
         if (!sl.dev) {
-            CK(cudaMalloc(&sl.dev, ctx->ing_chunk * sizeof(float2)));
-            CK(cudaMallocHost(&sl.pin, ctx->ing_chunk * sizeof(float2)));
-            CK(cudaEventCreateWithFlags(&sl.e_h2d, cudaEventDisableTiming));
-            CK(cudaEventCreateWithFlags(&sl.e_free_b, cudaEventDisableTiming));
-            CK(cudaEventCreateWithFlags(&sl.e_free_c, cudaEventDisableTiming));
+            CK(ctx, cudaMalloc(&sl.dev, ctx->ing_chunk * sizeof(float2)));
+            CK(ctx, cudaMallocHost(&sl.pin, ctx->ing_chunk * sizeof(float2)));
+            CK(ctx, cudaEventCreateWithFlags(&sl.e_h2d, cudaEventDisableTiming));
+            CK(ctx, cudaEventCreateWithFlags(&sl.e_free_b, cudaEventDisableTiming));
+            CK(ctx, cudaEventCreateWithFlags(&sl.e_free_c, cudaEventDisableTiming));
         }
-        if (need_raw && !sl.dev_raw) CK(cudaMalloc(&sl.dev_raw, ctx->ing_chunk * 4));
+        if (need_raw && !sl.dev_raw) CK(ctx, cudaMalloc(&sl.dev_raw, ctx->ing_chunk * 4));
     }
     return AMB_OK;
 }
@@ -726,26 +710,26 @@ static int ingest_dispatch(amb_ctx* ctx, const void* src, size_t m, bool sc16, b
     AmbIngestSlot& sl = ctx->ing[s_idx];
     cudaStream_t sh = ctx->stream_h;
     if (sl.used) {        // the chunk that lived here before: its sparse kernels and its carry kernel must be through
-        CK(cudaStreamWaitEvent(sh, sl.e_free_b, 0));
-        CK(cudaStreamWaitEvent(sh, sl.e_free_c, 0));
+        CK(ctx, cudaStreamWaitEvent(sh, sl.e_free_b, 0));
+        CK(ctx, cudaStreamWaitEvent(sh, sl.e_free_c, 0));
     }
     if (m) {
         const cudaMemcpyKind kind = src_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
         if (sc16) {
-            CK(cudaMemcpyAsync(sl.dev_raw, src, m * 4, kind, sh));
-            CK(amb_launch_widen_sc16(sl.dev_raw, sl.dev, (long long)m, ctx->sm_count, sh));
+            CK(ctx, cudaMemcpyAsync(sl.dev_raw, src, m * 4, kind, sh));
+            CK(ctx, amb_launch_widen_sc16(sl.dev_raw, sl.dev, (long long)m, ctx->sm_count, sh));
             ctx->stats.kernel_launches += 1;
         } else {
-            CK(cudaMemcpyAsync(sl.dev, src, m * sizeof(float2), kind, sh));
+            CK(ctx, cudaMemcpyAsync(sl.dev, src, m * sizeof(float2), kind, sh));
         }
     }
-    CK(cudaEventRecord(sl.e_h2d, sh));
+    CK(ctx, cudaEventRecord(sl.e_h2d, sh));
     sl.h2d_pending = true;
-    CK(cudaStreamWaitEvent(ctx->stream, sl.e_h2d, 0));
+    CK(ctx, cudaStreamWaitEvent(ctx->stream, sl.e_h2d, 0));
     int rc = process_core(ctx, reinterpret_cast<const float*>(sl.dev), m, AMB_MEM_DEVICE, flush);
     if (rc != AMB_OK) return rc;
-    CK(cudaEventRecord(sl.e_free_b, ctx->stream_b));
-    CK(cudaEventRecord(sl.e_free_c, ctx->stream_c));
+    CK(ctx, cudaEventRecord(sl.e_free_b, ctx->stream_b));
+    CK(ctx, cudaEventRecord(sl.e_free_c, ctx->stream_c));
     sl.used = true;
     ctx->ing_next++;
     return AMB_OK;
@@ -755,7 +739,7 @@ static int ingest_dispatch(amb_ctx* ctx, const void* src, size_t m, bool sc16, b
 static int ingest_pinned_slot(amb_ctx* ctx, char** out)
 {
     AmbIngestSlot& sl = ctx->ing[ctx->ing_next % AMB_ING_SLOTS];
-    if (sl.h2d_pending) { CK(cudaEventSynchronize(sl.e_h2d)); sl.h2d_pending = false; }
+    if (sl.h2d_pending) { CK(ctx, cudaEventSynchronize(sl.e_h2d)); sl.h2d_pending = false; }
     *out = static_cast<char*>(sl.pin);
     return AMB_OK;
 }
@@ -813,7 +797,7 @@ static int ingest(amb_ctx* ctx, const void* data, size_t n, int mem_kind, int fl
     if (flush && !flushed) { int rc = ingest_dispatch_pending(ctx, 1); if (rc) return rc; }   // also closes an empty stream
     // host memory is consumed when the call returns: the copies out of a pinned caller buffer are asynchronous, so wait
     // for the last of them (the kernels behind it stay asynchronous)
-    if (last_direct) CK(cudaEventSynchronize(last_direct));
+    if (last_direct) CK(ctx, cudaEventSynchronize(last_direct));
     return AMB_OK;
 }
 
@@ -824,7 +808,7 @@ int amb_process(amb_ctx* ctx, const float* iq, size_t n_complex, int mem_kind, i
     if (ctx->flushed) return fail(ctx, AMB_ERR_STATE, "stream already flushed; amb_reset first");
     if (ctx->def_kind && !ctx->def_resolved)
         return fail(ctx, AMB_ERR_STATE, "amb_resolve pending (deferred mode allows one call per span)");
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     if (ctx->defer) {     // time-sharded span: one pass, input stays where it is (or goes through the one-piece staging buffer)
         if (mem_kind != AMB_MEM_HOST && mem_kind != AMB_MEM_DEVICE)
             return fail(ctx, AMB_ERR_UNSUPPORTED, "16-bit input is not available in deferred (time-sharded) mode");
@@ -851,7 +835,7 @@ int amb_process(amb_ctx* ctx, const float* iq, size_t n_complex, int mem_kind, i
 int amb_seek(amb_ctx* ctx, uint64_t first_sample, uint64_t first_decision, const amb_walk_state* entry)
 {
     if (!ctx) return AMB_ERR_INVALID;
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     const AmbParams& P = ctx->P;
     if (first_sample) {
         if (ctx->use_dcblock) return fail(ctx, AMB_ERR_UNSUPPORTED, "amb_seek into a stream is not available with the DC blocker");
@@ -866,7 +850,7 @@ int amb_seek(amb_ctx* ctx, uint64_t first_sample, uint64_t first_decision, const
     ctx->r_done = (long long)first_decision;
     const long long pos = entry ? (long long)entry->pos : (long long)first_decision;
     const long long p = entry ? (long long)entry->p : (long long)first_decision;
-    CK(amb_launch_set_state(ctx->st, pos, p, ctx->stream_b));          // after reset_stream's memset on stream B
+    CK(ctx, amb_launch_set_state(ctx->st, pos, p, ctx->stream_b));          // after reset_stream's memset on stream B
     ctx->stats.kernel_launches += 1;
     ctx->seeked = true;
     return AMB_OK;
@@ -878,11 +862,11 @@ static int resolve_deferred(amb_ctx* ctx, const amb_walk_state* entry, const int
 {
     cudaStream_t sb = ctx->stream_b;
     if (ctx->def_resolved && ctx->def_kind == 1) {     // forget the earlier (speculative) resolution of this span
-        CK(amb_launch_walk_reset(ctx->def.wa, ctx->def.par ? ctx->bufs.walk_scratch : nullptr, ctx->def.n_samples, sb));
+        CK(ctx, amb_launch_walk_reset(ctx->def.wa, ctx->def.par ? ctx->bufs.walk_scratch : nullptr, ctx->def.n_samples, sb));
         ctx->stats.kernel_launches += 1;
     }
-    if (entry_dev) CK(amb_launch_set_state_dev(ctx->st, reinterpret_cast<const long long*>(entry_dev), sb));
-    else if (entry) CK(amb_launch_set_state(ctx->st, (long long)entry->pos, (long long)entry->p, sb));
+    if (entry_dev) CK(ctx, amb_launch_set_state_dev(ctx->st, reinterpret_cast<const long long*>(entry_dev), sb));
+    else if (entry) CK(ctx, amb_launch_set_state(ctx->st, (long long)entry->pos, (long long)entry->p, sb));
     if (entry_dev || entry) ctx->stats.kernel_launches += 1;
     if (ctx->def_kind != 3) {
         AmbChainErr er;
@@ -890,9 +874,9 @@ static int resolve_deferred(amb_ctx* ctx, const amb_walk_state* entry, const int
         if (k < 0) return chain_fail(ctx, er);
         ctx->stats.kernel_launches += (uint64_t)k;
     }
-    CK(cudaEventRecord(ctx->e_done[ctx->def_set], sb));
-    if (ctx->timing) CK(cudaEventRecord(ctx->ev[3], sb));
-    if (!ctx->overlap) CK(cudaStreamWaitEvent(ctx->stream, ctx->e_done[ctx->def_set], 0));
+    CK(ctx, cudaEventRecord(ctx->e_done[ctx->def_set], sb));
+    if (ctx->timing) CK(ctx, cudaEventRecord(ctx->ev[3], sb));
+    if (!ctx->overlap) CK(ctx, cudaStreamWaitEvent(ctx->stream, ctx->e_done[ctx->def_set], 0));
     ctx->def_resolved = true;
     return AMB_OK;
 }
@@ -902,7 +886,7 @@ int amb_resolve(amb_ctx* ctx, const amb_walk_state* entry)
     if (!ctx) return AMB_ERR_INVALID;
     if (!ctx->def_kind) return fail(ctx, AMB_ERR_STATE, "no deferred call to resolve");
     if (ctx->def_resolved && !entry) return fail(ctx, AMB_ERR_INVALID, "re-resolution needs an entry state");
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     return resolve_deferred(ctx, entry, nullptr);
 }
 
@@ -910,10 +894,10 @@ int amb_get_walk_state(amb_ctx* ctx, amb_walk_state* out)
 {
     if (!ctx || !out) return AMB_ERR_INVALID;
     if (ctx->def_kind && !ctx->def_resolved) return fail(ctx, AMB_ERR_STATE, "amb_resolve pending");
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaStreamSynchronize(ctx->stream_b));
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, cudaStreamSynchronize(ctx->stream_b));
     AmbWalkState st;
-    CK(cudaMemcpy(&st, ctx->st, sizeof st, cudaMemcpyDeviceToHost));
+    CK(ctx, cudaMemcpy(&st, ctx->st, sizeof st, cudaMemcpyDeviceToHost));
     out->pos = st.pos; out->p = st.p;
     return AMB_OK;
 }
@@ -922,13 +906,13 @@ int amb_get_walk_summary(amb_ctx* ctx, amb_walk_summary* out)
 {
     if (!ctx || !out) return AMB_ERR_INVALID;
     if (!ctx->def_kind || !ctx->def_resolved) return fail(ctx, AMB_ERR_STATE, "no resolved deferred span");
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     const bool have = ctx->def_kind == 1;
-    if (have) { CK(amb_launch_walk_summary(ctx->def.wa, ctx->stream_b)); ctx->stats.kernel_launches += 1; }
-    CK(cudaStreamSynchronize(ctx->stream_b));
+    if (have) { CK(ctx, amb_launch_walk_summary(ctx->def.wa, ctx->stream_b)); ctx->stats.kernel_launches += 1; }
+    CK(ctx, cudaStreamSynchronize(ctx->stream_b));
     AmbWalkState st; AmbCounters h;
-    CK(cudaMemcpy(&st, ctx->st, sizeof st, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(&h, ctx->ctr, sizeof h, cudaMemcpyDeviceToHost));
+    CK(ctx, cudaMemcpy(&st, ctx->st, sizeof st, cudaMemcpyDeviceToHost));
+    CK(ctx, cudaMemcpy(&h, ctx->ctr, sizeof h, cudaMemcpyDeviceToHost));
     out->pos = st.pos; out->p = st.p;
     out->first_real = (have && st.first_real != ~0ull) ? (int64_t)st.first_real : -1;
     out->first_packet = (have && st.first_packet != ~0ull) ? (int64_t)st.first_packet : -1;
@@ -943,12 +927,12 @@ int amb_walk_summary_async(amb_ctx* ctx, int64_t* dev_out6)
 {
     if (!ctx || !dev_out6) return AMB_ERR_INVALID;
     if (!ctx->def_kind || !ctx->def_resolved) return fail(ctx, AMB_ERR_STATE, "no resolved deferred span");
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     const bool have = ctx->def_kind == 1;
-    if (have) { CK(amb_launch_walk_summary(ctx->def.wa, ctx->stream_b)); ctx->stats.kernel_launches += 1; }
+    if (have) { CK(ctx, amb_launch_walk_summary(ctx->def.wa, ctx->stream_b)); ctx->stats.kernel_launches += 1; }
     AmbWalkArgs wa = ctx->def.wa; wa.st = ctx->st; wa.ctr = ctx->ctr;
-    CK(amb_launch_pack_summary(wa, ctx->P.i_exact, have ? 1 : 0, reinterpret_cast<long long*>(dev_out6), ctx->stream_b));
-    CK(cudaEventRecord(ctx->e_done[ctx->def_set], ctx->stream_b));
+    CK(ctx, amb_launch_pack_summary(wa, ctx->P.i_exact, have ? 1 : 0, reinterpret_cast<long long*>(dev_out6), ctx->stream_b));
+    CK(ctx, cudaEventRecord(ctx->e_done[ctx->def_set], ctx->stream_b));
     ctx->stats.kernel_launches += 1;
     return AMB_OK;
 }
@@ -960,9 +944,9 @@ int amb_walk_summary_async(amb_ctx* ctx, int64_t* dev_out6)
 int amb_compose_entries_async(amb_ctx* ctx, const int64_t* gathered_dev, int n_spans, int64_t* out_dev, void* cuda_stream)
 {
     if (!ctx || !gathered_dev || !out_dev || n_spans < 1 || n_spans > 4096) return AMB_ERR_INVALID;
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
-    CK(amb_launch_compose(reinterpret_cast<const long long*>(gathered_dev), n_spans, reinterpret_cast<long long*>(out_dev), st));
+    CK(ctx, amb_launch_compose(reinterpret_cast<const long long*>(gathered_dev), n_spans, reinterpret_cast<long long*>(out_dev), st));
     ctx->stats.kernel_launches += 1;
     return AMB_OK;
 }
@@ -974,9 +958,9 @@ int amb_resolve_device(amb_ctx* ctx, const int64_t* entry_dev, void* after_strea
 {
     if (!ctx || !entry_dev) return AMB_ERR_INVALID;
     if (!ctx->def_kind) return fail(ctx, AMB_ERR_STATE, "no deferred call to resolve");
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaEventRecord(ctx->e_in, after_stream ? (cudaStream_t)after_stream : ctx->stream));
-    CK(cudaStreamWaitEvent(ctx->stream_b, ctx->e_in, 0));
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, cudaEventRecord(ctx->e_in, after_stream ? (cudaStream_t)after_stream : ctx->stream));
+    CK(ctx, cudaStreamWaitEvent(ctx->stream_b, ctx->e_in, 0));
     return resolve_deferred(ctx, nullptr, entry_dev);
 }
 
@@ -986,12 +970,12 @@ int amb_resolve_device(amb_ctx* ctx, const int64_t* entry_dev, void* after_strea
 int amb_join_stream(amb_ctx* ctx, void* cuda_stream)
 {
     if (!ctx) return AMB_ERR_INVALID;
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     if (ctx->pend_n) { int rc = ingest_dispatch_pending(ctx, 0); if (rc) return rc; }
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : ctx->stream;
     for (int k = 0; k < 2; k++) {
-        if (ctx->done_valid[k]) CK(cudaStreamWaitEvent(st, ctx->e_done[k], 0));
-        if (ctx->aux_valid[k]) CK(cudaStreamWaitEvent(st, ctx->e_aux[k], 0));
+        if (ctx->done_valid[k]) CK(ctx, cudaStreamWaitEvent(st, ctx->e_done[k], 0));
+        if (ctx->aux_valid[k]) CK(ctx, cudaStreamWaitEvent(st, ctx->e_aux[k], 0));
     }
     return AMB_OK;
 }
@@ -1020,7 +1004,7 @@ static int fetch_frames(amb_ctx* ctx, unsigned upto)
     const size_t base = ctx->pending.size();
     const unsigned cnt = upto - ctx->polled;
     ctx->pending.resize(base + cnt);
-    CK(cudaMemcpy(ctx->pending.data() + base, ctx->bufs.frames + ctx->polled, (size_t)cnt * sizeof(amb_frame), cudaMemcpyDeviceToHost));
+    CK(ctx, cudaMemcpy(ctx->pending.data() + base, ctx->bufs.frames + ctx->polled, (size_t)cnt * sizeof(amb_frame), cudaMemcpyDeviceToHost));
     std::sort(ctx->pending.begin() + base, ctx->pending.end(),
               [](const amb_frame& x, const amb_frame& y) { return x.sample_index < y.sample_index; });
     for (size_t k = base; k < ctx->pending.size(); k++) stamp(ctx, &ctx->pending[k]);
@@ -1031,10 +1015,10 @@ static int fetch_frames(amb_ctx* ctx, unsigned upto)
 // Everything enqueued so far is through; counters of the last call read back.
 static int collect_sync(amb_ctx* ctx, AmbCounters* h)
 {
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     if (ctx->pend_n) { int rc = ingest_dispatch_pending(ctx, 0); if (rc) return rc; }
-    CK(sync_all(ctx));
-    CK(cudaMemcpy(h, ctx->ctr, sizeof *h, cudaMemcpyDeviceToHost));
+    CK(ctx, sync_all(ctx));
+    CK(ctx, cudaMemcpy(h, ctx->ctr, sizeof *h, cudaMemcpyDeviceToHost));
     ctx->stats.candidates = h->ncand;
     ctx->stats.candidates_real = h->nreal_call;
     ctx->stats.detections = h->ndet_call;
@@ -1050,7 +1034,7 @@ static int collect(amb_ctx* ctx)
     AmbCounters h;
     { int rc = collect_sync(ctx, &h); if (rc) return rc; }
     { int rc = fetch_frames(ctx, h.nframes); if (rc) return rc; }
-    if (h.nframes) CK(cudaMemset(&ctx->ctr->nframes, 0, sizeof(unsigned)));
+    if (h.nframes) CK(ctx, cudaMemset(&ctx->ctr->nframes, 0, sizeof(unsigned)));
     ctx->polled = 0;
     ctx->snap_tail = ctx->snap_head;
     ctx->bufs.frames_ub = 0;
@@ -1081,7 +1065,7 @@ int amb_poll_frames(amb_ctx* ctx, amb_frame* out, int max)
 int amb_poll_ready(amb_ctx* ctx, amb_frame* out, int max)
 {
     if (!ctx || (!out && max > 0)) return AMB_ERR_INVALID;
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     bool have = false; AmbCounters last{};
     while (ctx->snap_tail < ctx->snap_head) {
         const unsigned k = (unsigned)(ctx->snap_tail % AMB_SNAPS);
@@ -1116,20 +1100,20 @@ int amb_drain_device(amb_ctx* ctx, amb_frame* out_dev, int cap)
         unsigned npad = 1; while (npad < n) npad <<= 1;
         if (ctx->ord_cap < npad) {
             cudaFree(ctx->ord_key); cudaFree(ctx->ord_val); ctx->ord_key = nullptr; ctx->ord_val = nullptr; ctx->ord_cap = 0;
-            CK(cudaMalloc(&ctx->ord_key, (size_t)npad * sizeof(unsigned long long)));
-            CK(cudaMalloc(&ctx->ord_val, (size_t)npad * sizeof(unsigned)));
+            CK(ctx, cudaMalloc(&ctx->ord_key, (size_t)npad * sizeof(unsigned long long)));
+            CK(ctx, cudaMalloc(&ctx->ord_val, (size_t)npad * sizeof(unsigned)));
             ctx->ord_cap = npad;
         }
         const int ntags = (int)ctx->time_tags.size();
         if (ntags) {
             if (ctx->tags_dev_cap < ntags) {
                 cudaFree(ctx->tags_dev); ctx->tags_dev = nullptr; ctx->tags_dev_cap = 0;
-                CK(cudaMalloc(&ctx->tags_dev, (size_t)ntags * 2 * sizeof(AmbTagDev)));
+                CK(ctx, cudaMalloc(&ctx->tags_dev, (size_t)ntags * 2 * sizeof(AmbTagDev)));
                 ctx->tags_dev_cap = ntags * 2;
             }
             std::vector<AmbTagDev> t((size_t)ntags);
             for (int k = 0; k < ntags; k++) t[(size_t)k] = {ctx->time_tags[(size_t)k].offset, ctx->time_tags[(size_t)k].secs, ctx->time_tags[(size_t)k].frac};
-            CK(cudaMemcpy(ctx->tags_dev, t.data(), (size_t)ntags * sizeof(AmbTagDev), cudaMemcpyHostToDevice));
+            CK(ctx, cudaMemcpy(ctx->tags_dev, t.data(), (size_t)ntags * sizeof(AmbTagDev), cudaMemcpyHostToDevice));
         }
         cudaError_t e = cudaSuccess;
         const int launched = amb_launch_order(ctx->bufs.frames + ctx->polled, n, npad, ctx->order_tile, ctx->ord_key, ctx->ord_val, out_dev,
@@ -1137,9 +1121,9 @@ int amb_drain_device(amb_ctx* ctx, amb_frame* out_dev, int cap)
                                               ctx->stream_b, &e);
         if (e != cudaSuccess) return fail(ctx, AMB_ERR_CUDA, "amb_drain_device launch", e);
         ctx->stats.kernel_launches += (uint64_t)launched;
-        CK(cudaStreamSynchronize(ctx->stream_b));
+        CK(ctx, cudaStreamSynchronize(ctx->stream_b));
     }
-    if (h.nframes) CK(cudaMemset(&ctx->ctr->nframes, 0, sizeof(unsigned)));
+    if (h.nframes) CK(ctx, cudaMemset(&ctx->ctr->nframes, 0, sizeof(unsigned)));
     ctx->polled = 0;
     ctx->snap_tail = ctx->snap_head;
     ctx->bufs.frames_ub = 0;
@@ -1161,22 +1145,22 @@ int amb_add_time_tag(amb_ctx* ctx, uint64_t offset, uint64_t secs, double frac)
 int amb_wait_stream(amb_ctx* ctx, void* cuda_stream)
 {
     if (!ctx) return AMB_ERR_INVALID;
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     if ((cudaStream_t)cuda_stream == ctx->stream) return AMB_OK;
-    CK(cudaEventRecord(ctx->e_in, (cudaStream_t)cuda_stream));
-    CK(cudaStreamWaitEvent(ctx->stream, ctx->e_in, 0));
+    CK(ctx, cudaEventRecord(ctx->e_in, (cudaStream_t)cuda_stream));
+    CK(ctx, cudaStreamWaitEvent(ctx->stream, ctx->e_in, 0));
     return AMB_OK;
 }
 
 int amb_get_stats(amb_ctx* ctx, amb_stats* out)
 {
     if (!ctx || !out) return AMB_ERR_INVALID;
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     if (ctx->pend_n) { int rc = ingest_dispatch_pending(ctx, 0); if (rc) return rc; }
-    CK(sync_all(ctx));
+    CK(ctx, sync_all(ctx));
     AmbCounters h; AmbWalkState st;
-    CK(cudaMemcpy(&h, ctx->ctr, sizeof h, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(&st, ctx->st, sizeof st, cudaMemcpyDeviceToHost));
+    CK(ctx, cudaMemcpy(&h, ctx->ctr, sizeof h, cudaMemcpyDeviceToHost));
+    CK(ctx, cudaMemcpy(&st, ctx->st, sizeof st, cudaMemcpyDeviceToHost));
     ctx->stats.samples_in = ctx->n_in;
     ctx->stats.candidates = h.ncand;
     ctx->stats.candidates_real = h.nreal_call;
@@ -1196,15 +1180,15 @@ int amb_get_stats(amb_ctx* ctx, amb_stats* out)
 int amb_get_scan_times(amb_ctx* ctx, float* ms_out, int max)
 {
     if (!ctx || (!ms_out && max > 0)) return AMB_ERR_INVALID;
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     if (ctx->pend_n) { int rc = ingest_dispatch_pending(ctx, 0); if (rc) return rc; }
-    CK(sync_all(ctx));
+    CK(ctx, sync_all(ctx));
     const unsigned have = ctx->ring_n < 64u ? ctx->ring_n : 64u;
     const unsigned n = have < (unsigned)(max > 0 ? max : 0) ? have : (unsigned)(max > 0 ? max : 0);
     for (unsigned k = 0; k < n; k++) {
         const unsigned call = ctx->ring_n - n + k;
         float ms = 0.f;
-        CK(cudaEventElapsedTime(&ms, ctx->ring[(call & 63u) * 2], ctx->ring[(call & 63u) * 2 + 1]));
+        CK(ctx, cudaEventElapsedTime(&ms, ctx->ring[(call & 63u) * 2], ctx->ring[(call & 63u) * 2 + 1]));
         ms_out[k] = ms;
     }
     return (int)n;
@@ -1215,9 +1199,9 @@ int amb_get_scan_times(amb_ctx* ctx, float* ms_out, int max)
 int amb_get_timeline(amb_ctx* ctx, float* ms_out, int max_calls)
 {
     if (!ctx || (!ms_out && max_calls > 0)) return AMB_ERR_INVALID;
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     if (ctx->pend_n) { int rc = ingest_dispatch_pending(ctx, 0); if (rc) return rc; }
-    CK(sync_all(ctx));
+    CK(ctx, sync_all(ctx));
     const unsigned have = ctx->ring_n < 63u ? ctx->ring_n : 63u;
     const unsigned n = have < (unsigned)(max_calls > 0 ? max_calls : 0) ? have : (unsigned)(max_calls > 0 ? max_calls : 0);
     for (unsigned k = 0; k < n; k++) {
@@ -1225,7 +1209,7 @@ int amb_get_timeline(amb_ctx* ctx, float* ms_out, int max_calls)
         float gap = 0.f, sc = 0.f, tail = 0.f;
         if (call > 0 && ctx->ring_n - (call - 1) <= 64u)
             if (cudaEventElapsedTime(&gap, ctx->ring[((call - 1) & 63u) * 2 + 1], ctx->ring[(call & 63u) * 2]) != cudaSuccess) { gap = 0.f; cudaGetLastError(); }
-        CK(cudaEventElapsedTime(&sc, ctx->ring[(call & 63u) * 2], ctx->ring[(call & 63u) * 2 + 1]));
+        CK(ctx, cudaEventElapsedTime(&sc, ctx->ring[(call & 63u) * 2], ctx->ring[(call & 63u) * 2 + 1]));
         if (cudaEventElapsedTime(&tail, ctx->ring[(call & 63u) * 2 + 1], ctx->ring_done[call & 63u]) != cudaSuccess) { tail = 0.f; cudaGetLastError(); }
         ms_out[3 * k] = gap; ms_out[3 * k + 1] = sc; ms_out[3 * k + 2] = tail;
     }
@@ -1235,16 +1219,16 @@ int amb_get_timeline(amb_ctx* ctx, float* ms_out, int max_calls)
 int amb_debug_candidates(amb_ctx* ctx, uint64_t* index, uint32_t* info, int max)
 {
     if (!ctx) return AMB_ERR_INVALID;
-    CK(cudaSetDevice(ctx->device));
-    CK(sync_all(ctx));
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, sync_all(ctx));
     if (!ctx->have_last || !ctx->bufs.cand_j) return 0;
     AmbCounters h;
-    CK(cudaMemcpy(&h, ctx->ctr, sizeof h, cudaMemcpyDeviceToHost));
+    CK(ctx, cudaMemcpy(&h, ctx->ctr, sizeof h, cudaMemcpyDeviceToHost));
     const int n = (int)std::min<unsigned>(h.ncand, (unsigned)std::max(max, 0));
     if (n <= 0) return 0;
     std::vector<int> j(n);
-    CK(cudaMemcpy(j.data(), ctx->bufs.cand_j, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
-    if (info) CK(cudaMemcpy(info, ctx->bufs.cand_info, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    CK(ctx, cudaMemcpy(j.data(), ctx->bufs.cand_j, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
+    if (info) CK(ctx, cudaMemcpy(info, ctx->bufs.cand_info, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
     if (index) for (int k = 0; k < n; k++) index[k] = (uint64_t)(ctx->last_org + j[k]);
     return n;
 }
@@ -1308,10 +1292,10 @@ int amb_device_crc(amb_ctx* ctx, const uint8_t* data, int n, int length, uint32_
 {
     if (!ctx || !data || !out || n < 0 || length < 1 || length > 11) return AMB_ERR_INVALID;
     if (n == 0) return AMB_OK;
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     uint8_t* d = nullptr; uint32_t* o = nullptr;
-    CK(cudaMalloc(&d, (size_t)n * length));
-    CK(cudaMalloc(&o, (size_t)n * sizeof(uint32_t)));
+    CK(ctx, cudaMalloc(&d, (size_t)n * length));
+    CK(ctx, cudaMalloc(&o, (size_t)n * sizeof(uint32_t)));
     cudaError_t e = cudaMemcpyAsync(d, data, (size_t)n * length, cudaMemcpyHostToDevice, ctx->stream);
     if (e == cudaSuccess) e = amb_launch_crc(d, n, length, o, ctx->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(out, o, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
@@ -1329,7 +1313,7 @@ int amb_dump_stage(amb_ctx* ctx, int stage, const float* iq, size_t n_complex, f
     if (ctx->use_dcblock && stage != AMB_STAGE_DC)
         return fail(ctx, AMB_ERR_UNSUPPORTED, "m2/bb/avg dumps take the demodulator's input; dump AMB_STAGE_DC and feed it to a context without the DC blocker");
     if (n_complex == 0) return AMB_OK;
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
     if (stage == AMB_STAGE_DC) {     // the whole buffer as one stream: zero history (GNU Radio's delay lines start at zero)
         const int D = 100 * ctx->P.spc_i, nc = 2 * D - 2;                       // rx_path.py:40
@@ -1349,7 +1333,7 @@ int amb_dump_stage(amb_ctx* ctx, int stage, const float* iq, size_t n_complex, f
         return AMB_OK;
     }
     float2* d = nullptr; float* t = nullptr; float* o = nullptr;
-    CK(cudaMalloc(&d, n_complex * sizeof(float2)));
+    CK(ctx, cudaMalloc(&d, n_complex * sizeof(float2)));
     cudaError_t e = cudaMalloc(&t, n_complex * sizeof(float));
     if (e == cudaSuccess) e = cudaMalloc(&o, n_complex * sizeof(float));
     if (e == cudaSuccess) e = cudaMemcpyAsync(d, iq, n_complex * sizeof(float2), cudaMemcpyHostToDevice, s);
@@ -1366,10 +1350,10 @@ int amb_slicer_process(amb_ctx* ctx, const float* chips, int ndet, const uint64_
 {
     if (!ctx || ndet < 0 || (ndet && (!chips || !out))) return AMB_ERR_INVALID;
     if (ndet == 0) return 0;
-    CK(cudaSetDevice(ctx->device));
+    CK(ctx, cudaSetDevice(ctx->device));
     float* d = nullptr; amb_frame* f = nullptr;
-    CK(cudaMalloc(&d, (size_t)ndet * 240 * sizeof(float)));
-    CK(cudaMalloc(&f, (size_t)ndet * sizeof(amb_frame)));
+    CK(ctx, cudaMalloc(&d, (size_t)ndet * 240 * sizeof(float)));
+    CK(ctx, cudaMalloc(&f, (size_t)ndet * sizeof(amb_frame)));
     cudaError_t e = cudaMemsetAsync(f, 0, (size_t)ndet * sizeof(amb_frame), ctx->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d, chips, (size_t)ndet * 240 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream);
     if (e == cudaSuccess) e = amb_launch_slice_chips(d, ndet, f, ctx->stream);
@@ -1396,8 +1380,8 @@ int amb_preamble_process(amb_ctx* ctx, const float* in0, const float* in1, size_
 {
     if (!ctx || (n && (!in0 || !in1)) || max_det < 0 || (max_det && (!chips_out || !index_out))) return AMB_ERR_INVALID;
     if (n > 0x40000000ull) return fail(ctx, AMB_ERR_INVALID, "at most 2^30 items per call");
-    CK(cudaSetDevice(ctx->device));
-    CK(sync_all(ctx));
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, sync_all(ctx));
     const AmbParams& P = ctx->P;
     cudaStream_t s = ctx->stream;
     // combined = undecided tail of the previous calls ++ new items; item index of combined[0] is b0
@@ -1408,8 +1392,8 @@ int amb_preamble_process(amb_ctx* ctx, const float* in0, const float* in1, size_
     const long long ntot = total + P.H;                              // items incl. history (reported coordinates)
     const long long r_safe = std::max<long long>(ctx->sf_rdone, total + P.H - ctx->guard);
     float* d0 = nullptr; float* d1 = nullptr;
-    CK(cudaMalloc(&d0, (m + 1) * sizeof(float)));
-    CK(cudaMalloc(&d1, (m + 1) * sizeof(float)));
+    CK(ctx, cudaMalloc(&d0, (m + 1) * sizeof(float)));
+    CK(ctx, cudaMalloc(&d1, (m + 1) * sizeof(float)));
     int rc = AMB_OK;
     do {
         cudaError_t e = cudaSuccess;

@@ -1,10 +1,11 @@
 // Batch field decode (SURVEY.md 8 row f4): kernels + C ABI of amb_decoder (include/airmodes_b200.h).
 // The per-message arithmetic is in amb_decode_core.h, the kernels, amb_decode_launch - the one launch sequence of a
-// decode - and the stages' memory (amb_decode_prepare / amb_decode_reset / amb_decode_free) in amb_decode_kernels.cuh
-// and the stage headers it includes (launch-free headers, so that tests/simt can run the same kernel source, sequence
-// and memory rules under a host emulator); this file keeps the frames, records and snapshot rows on their way between
-// the caller and the stages, copies the frames in and the records out. Compiled with -fmad=false: latitude/longitude follow cpr.py
-// operation by operation in IEEE double, nothing may be contracted. Citations are file:line under gr-air-modes/python.
+// decode - the stages' memory (amb_decode_prepare / amb_decode_reset / amb_decode_free), the option table and the
+// read-outs of the results in amb_decode_kernels.cuh and the stage headers it includes (launch-free headers, so that
+// tests/simt can run the same kernel source, sequence, memory, option and read-out rules under a host emulator); this
+// file keeps the frames, records and snapshot rows on their way between the caller and the stages, copies the frames
+// in and the records out. Compiled with -fmad=false: latitude/longitude follow cpr.py operation by operation in IEEE
+// double, nothing may be contracted. Citations are file:line under gr-air-modes/python.
 //
 // Seven launches per decode, in stream order:
 //   amb_fields_kernel   one thread per frame: bit fields, altitude, squawk, ident, velocity; emits the CPR report
@@ -62,27 +63,11 @@ struct amb_decoder {
     void* pin[2] = {nullptr, nullptr}; cudaEvent_t pin_ev[2] = {nullptr, nullptr}; size_t pin_bytes = 0;
     amb_aircraft* d_snap = nullptr; int snap_cap = 0;   // snapshot rows on their way to host memory
     amb_aircraft_ext* d_xsnap = nullptr; int xsnap_cap = 0;   // ... and their extensions
-    int sbs1_nb = -1;                    // blocks of lines of the last decode (its byte total is st.sb.boff[sbs1_nb]);
-                                         // -1: the last decode wrote no lines
-    int reports_nb = -1;                 // the same for the text reports (st.rb.boff[reports_nb])
     uint64_t launches = 0; float ms_last = 0.f;
     std::string err;
 };
 
 static thread_local std::string g_create_err;          // why the last amb_decoder_create on this thread failed
-
-static int dfail(amb_decoder* d, int code, const char* what, cudaError_t e = cudaSuccess)
-{
-    if (d) {
-        char buf[256];
-        if (e != cudaSuccess) snprintf(buf, sizeof buf, "%s: %s", what, cudaGetErrorString(e));
-        else snprintf(buf, sizeof buf, "%s", what);
-        d->err = buf;
-    }
-    return code;
-}
-#define DCK(call)                                                                  \
-    do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return dfail(d, AMB_ERR_CUDA, #call, e_); } while (0)
 
 // ---- host ---------------------------------------------------------------------------------------------------------
 extern "C" void amb_parallel_memcpy(void* dst, const void* src, size_t n);      // amb_api.cu (the ingest copy threads)
@@ -92,8 +77,8 @@ static int alloc_pinned(amb_decoder* d)
 {
     if (d->pin[0]) return AMB_OK;
     for (int k = 0; k < 2; k++) {
-        DCK(cudaMallocHost(&d->pin[k], AMB_DEC_PIECE));
-        DCK(cudaEventCreateWithFlags(&d->pin_ev[k], cudaEventDisableTiming));
+        CK(d, cudaMallocHost(&d->pin[k], AMB_DEC_PIECE));
+        CK(d, cudaEventCreateWithFlags(&d->pin_ev[k], cudaEventDisableTiming));
     }
     d->pin_bytes = AMB_DEC_PIECE;
     return AMB_OK;
@@ -106,10 +91,10 @@ static int staged_h2d(amb_decoder* d, void* dst, const void* src, size_t bytes, 
     size_t off = 0; int k = 0;
     while (off < bytes) {
         const size_t m = bytes - off < AMB_DEC_PIECE ? bytes - off : AMB_DEC_PIECE;
-        DCK(cudaEventSynchronize(d->pin_ev[k]));
+        CK(d, cudaEventSynchronize(d->pin_ev[k]));
         amb_parallel_memcpy(d->pin[k], static_cast<const char*>(src) + off, m);
-        DCK(cudaMemcpyAsync(static_cast<char*>(dst) + off, d->pin[k], m, cudaMemcpyHostToDevice, s));
-        DCK(cudaEventRecord(d->pin_ev[k], s));
+        CK(d, cudaMemcpyAsync(static_cast<char*>(dst) + off, d->pin[k], m, cudaMemcpyHostToDevice, s));
+        CK(d, cudaEventRecord(d->pin_ev[k], s));
         off += m; k ^= 1;
     }
     return AMB_OK;
@@ -123,12 +108,12 @@ static int staged_d2h(amb_decoder* d, void* dst, const void* src, size_t bytes, 
     for (size_t i = 0; i <= np; i++) {
         if (i < np) {
             const size_t off = i * AMB_DEC_PIECE, m = bytes - off < AMB_DEC_PIECE ? bytes - off : AMB_DEC_PIECE;
-            DCK(cudaMemcpyAsync(d->pin[i & 1], static_cast<const char*>(src) + off, m, cudaMemcpyDeviceToHost, s));
-            DCK(cudaEventRecord(d->pin_ev[i & 1], s));
+            CK(d, cudaMemcpyAsync(d->pin[i & 1], static_cast<const char*>(src) + off, m, cudaMemcpyDeviceToHost, s));
+            CK(d, cudaEventRecord(d->pin_ev[i & 1], s));
         }
         if (i >= 1) {
             const size_t off = (i - 1) * AMB_DEC_PIECE, m = bytes - off < AMB_DEC_PIECE ? bytes - off : AMB_DEC_PIECE;
-            DCK(cudaEventSynchronize(d->pin_ev[(i - 1) & 1]));
+            CK(d, cudaEventSynchronize(d->pin_ev[(i - 1) & 1]));
             amb_parallel_memcpy(static_cast<char*>(dst) + off, d->pin[(i - 1) & 1], m);
         }
     }
@@ -147,11 +132,11 @@ static int prepare(amb_decoder* d, int n)
 {
     cudaError_t e = cudaSuccess;
     const int k = amb_decode_prepare(&d->st, n, d->stream, &e);
-    if (k < 0) return dfail(d, AMB_ERR_CUDA, amb_stage_names[-k - 1].memory, e);
+    if (k < 0) return fail(d, AMB_ERR_CUDA, amb_stage_names[-k - 1].memory, e);
     if (d->cap < d->st.cap) {
         free_bufs(d);
-        DCK(cudaMalloc(&d->d_frames, (size_t)d->st.cap * sizeof(amb_frame)));
-        DCK(cudaMalloc(&d->d_fields, (size_t)d->st.cap * sizeof(amb_fields)));
+        CK(d, cudaMalloc(&d->d_frames, (size_t)d->st.cap * sizeof(amb_frame)));
+        CK(d, cudaMalloc(&d->d_fields, (size_t)d->st.cap * sizeof(amb_fields)));
         d->cap = d->st.cap;
     }
     return AMB_OK;
@@ -173,15 +158,12 @@ int amb_decoder_create(int device, int have_location, double lat, double lon, am
                   "amb_aircraft_ext layout");
     if (!out) return AMB_ERR_INVALID;
     *out = nullptr;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) return AMB_ERR_NO_DEVICE;
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return AMB_ERR_NO_DEVICE;
-    if (prop.major != 9 || prop.minor != 0) return AMB_ERR_NO_DEVICE;   // sm_90a cubin only; there is no CPU path
+    if (amb_check_device(device, &prop) != AMB_OK) return AMB_ERR_NO_DEVICE;
     amb_decoder* d = new (std::nothrow) amb_decoder();
     if (!d) return AMB_ERR_INVALID;
     d->device = device;
-    d->st.have_loc = have_location ? 1 : 0; d->st.lat = lat; d->st.lon = lon;
+    amb_decode_set_location(&d->st, have_location, lat, lon);
     int rc = AMB_OK;
     do {
         if (cudaSetDevice(device) != cudaSuccess) { rc = AMB_ERR_NO_DEVICE; break; }
@@ -215,63 +197,26 @@ void amb_decoder_destroy(amb_decoder* d)
 int amb_decoder_set_location(amb_decoder* d, int have_location, double lat, double lon)
 {
     if (!d) return AMB_ERR_INVALID;
-    d->st.have_loc = have_location ? 1 : 0; d->st.lat = lat; d->st.lon = lon;
+    amb_decode_set_location(&d->st, have_location, lat, lon);
     return AMB_OK;
 }
 
 int amb_decoder_reset(amb_decoder* d)
 {
     if (!d) return AMB_ERR_INVALID;
-    DCK(cudaSetDevice(d->device));
+    CK(d, cudaSetDevice(d->device));
     cudaError_t e = cudaSuccess;
     const int k = amb_decode_reset(&d->st, d->stream, &e);
-    if (k < 0) return dfail(d, AMB_ERR_CUDA, amb_stage_names[-k - 1].memory, e);
-    DCK(cudaStreamSynchronize(d->stream));
+    if (k < 0) return fail(d, AMB_ERR_CUDA, amb_stage_names[-k - 1].memory, e);
+    CK(d, cudaStreamSynchronize(d->stream));
     return AMB_OK;
 }
 
 int amb_decoder_set_option(amb_decoder* d, const char* name, int value)
 {
-    static const struct { const char* name; int max; int AmbDecodeState::*seconds; } options[] = {
-        {"local_cpr", AMB_LOCAL_CPR_MAX, &AmbDecodeState::local_cpr},
-        {"commb", AMB_COMMB_MAX, &AmbDecodeState::commb},
-        {"track", AMB_TRACK_MAX, &AmbDecodeState::track},
-        {"opstatus", AMB_OPSTATUS_MAX, &AmbDecodeState::opstatus},
-        {"track_ext", AMB_TRACK_EXT_MAX, &AmbDecodeState::track_ext},
-    };
     if (!d || !name) return AMB_ERR_INVALID;
-    if (strcmp(name, "sbs1") == 0) {
-        if (value != 0 && value != 1) return dfail(d, AMB_ERR_INVALID, "sbs1: 0 (off) or 1 (on)");
-        d->st.sbs1 = value;
-        return AMB_OK;
-    }
-    if (strcmp(name, "reports") == 0) {
-        if (value != 0 && value != 1) return dfail(d, AMB_ERR_INVALID, "reports: 0 (off) or 1 (on)");
-        d->st.reports = value;
-        return AMB_OK;
-    }
-    if (strcmp(name, "coverage") == 0) {
-        if (value != 0 && value != 1) return dfail(d, AMB_ERR_INVALID, "coverage: 0 (off) or 1 (on)");
-        d->st.coverage = value;
-        return AMB_OK;
-    }
-    if (strcmp(name, "sbs1_tz") == 0) {
-        if (value < AMB_SBS1_TZ_MIN || value > AMB_SBS1_TZ_MAX)
-            return dfail(d, AMB_ERR_INVALID, "sbs1_tz: -720 .. 840 minutes");
-        d->st.sbs1_tz = value;
-        return AMB_OK;
-    }
-    for (const auto& o : options) {
-        if (strcmp(name, o.name) != 0) continue;
-        if (value < 0 || value > o.max) {
-            char what[64];
-            snprintf(what, sizeof what, "%s: 0 (off) .. %d seconds", o.name, o.max);
-            return dfail(d, AMB_ERR_INVALID, what);
-        }
-        d->st.*o.seconds = value;
-        return AMB_OK;
-    }
-    return dfail(d, AMB_ERR_INVALID, "amb_decoder_set_option: unknown option");
+    const char* refused = amb_decode_set_option(&d->st, name, value);
+    return refused ? fail(d, AMB_ERR_INVALID, refused) : AMB_OK;
 }
 
 static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_kind, amb_fields* out, bool out_on_device);
@@ -291,15 +236,15 @@ int amb_decode_frames_device(amb_decoder* d, const amb_frame* frames_dev, int n,
 static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_kind, amb_fields* out, bool out_on_device)
 {
     if (!d || n < 0 || (n > 0 && (!frames || !out)) || (mem_kind != AMB_MEM_HOST && mem_kind != AMB_MEM_DEVICE))
-        return dfail(d, AMB_ERR_INVALID, "amb_decode_frames: bad argument");
-    if (n == 0) { d->sbs1_nb = d->reports_nb = -1; return AMB_OK; }
-    DCK(cudaSetDevice(d->device));
-    d->sbs1_nb = d->reports_nb = -1;
+        return fail(d, AMB_ERR_INVALID, "amb_decode_frames: bad argument");
+    d->st.sbs1_nb = d->st.reports_nb = -1;              // until amb_decode_launch has launched every stage
+    if (n == 0) return AMB_OK;
+    CK(d, cudaSetDevice(d->device));
     int rc = prepare(d, n);
     if (rc != AMB_OK) return rc;
     cudaStream_t s = d->stream;
     amb_fields* const fields = out_on_device ? out : d->d_fields;
-    DCK(cudaEventRecord(d->e0, s));
+    CK(d, cudaEventRecord(d->e0, s));
     const amb_frame* src = frames;
     if (mem_kind == AMB_MEM_HOST) {
         rc = staged_h2d(d, d->d_frames, frames, (size_t)n * sizeof(amb_frame), s);
@@ -308,16 +253,14 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
     }
     cudaError_t e = cudaSuccess;
     const int k = amb_decode_launch(&d->st, src, n, fields, s, &e);
-    if (k < 0) return dfail(d, AMB_ERR_CUDA, amb_stage_names[-k - 1].launch, e);
+    if (k < 0) return fail(d, AMB_ERR_CUDA, amb_stage_names[-k - 1].launch, e);
     d->launches += (uint64_t)k;
-    if (d->st.sbs1 > 0) d->sbs1_nb = (n + 127) / 128;
-    if (d->st.reports > 0) d->reports_nb = (n + 127) / 128;
     if (!out_on_device) {
         rc = staged_d2h(d, out, d->d_fields, (size_t)n * sizeof(amb_fields), s);
         if (rc != AMB_OK) return rc;
     }
-    DCK(cudaEventRecord(d->e1, s));
-    DCK(cudaStreamSynchronize(s));
+    CK(d, cudaEventRecord(d->e1, s));
+    CK(d, cudaStreamSynchronize(s));
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, d->e0, d->e1) == cudaSuccess) d->ms_last = ms;
     return AMB_OK;
@@ -331,57 +274,48 @@ static int snapshot_impl(amb_decoder* d, double now, amb_aircraft* out, amb_airc
     char what[96];
     if (!d || max < 0 || (with_ext && out && !ext)) {
         snprintf(what, sizeof what, "%s: bad argument", fn);
-        return dfail(d, AMB_ERR_INVALID, what);
+        return fail(d, AMB_ERR_INVALID, what);
     }
-    if (d->st.track <= 0) { snprintf(what, sizeof what, "%s: option track is off", fn); return dfail(d, AMB_ERR_STATE, what); }
-    if (with_ext && d->st.track_ext <= 0) return dfail(d, AMB_ERR_STATE, "amb_decoder_aircraft_ext: option track_ext is off");
+    if (d->st.track <= 0) { snprintf(what, sizeof what, "%s: option track is off", fn); return fail(d, AMB_ERR_STATE, what); }
+    if (with_ext && d->st.track_ext <= 0) return fail(d, AMB_ERR_STATE, "amb_decoder_aircraft_ext: option track_ext is off");
     if (!d->st.tocc) return 0;                           // nothing decoded with the option on yet
-    DCK(cudaSetDevice(d->device));
+    CK(d, cudaSetDevice(d->device));
     cudaStream_t s = d->stream;
-    const unsigned nb = AMB_TRACK_WORDS / AMB_SNAP_WORDS;
-    uint32_t* off = d->st.snap_cnt + nb;
     cudaError_t e = cudaSuccess;
-    if (amb_snap_count_launch(d->st.tocc, d->st.trows, d->st.tclk, now, d->st.track, AMB_TRACK_WORDS, d->st.snap_cnt, off,
-                              s, &e) < 0)
-        return dfail(d, AMB_ERR_CUDA, "aircraft snapshot", e);
+    const int total = amb_decode_snapshot_count(&d->st, now, AMB_TRACK_WORDS, s, &e);
+    if (total < 0) return fail(d, AMB_ERR_CUDA, "aircraft snapshot", e);
     d->launches += 2;
-    uint32_t total = 0;
-    DCK(cudaMemcpyAsync(&total, off + nb, sizeof total, cudaMemcpyDeviceToHost, s));
-    DCK(cudaStreamSynchronize(s));
-    if (!out) return (int)total;
-    if (total > (uint32_t)max) { snprintf(what, sizeof what, "%s: output buffer too small", fn); return dfail(d, AMB_ERR_OVERFLOW, what); }
+    if (!out) return total;
+    if (total > max) { snprintf(what, sizeof what, "%s: output buffer too small", fn); return fail(d, AMB_ERR_OVERFLOW, what); }
     if (total == 0) return 0;
     amb_aircraft* dst = out;
     amb_aircraft_ext* xdst = ext;
     if (!out_on_device) {
-        if (d->snap_cap < (int)total) {
+        if (d->snap_cap < total) {
             if (d->d_snap) cudaFree(d->d_snap);
             d->d_snap = nullptr; d->snap_cap = 0;
-            DCK(cudaMalloc(&d->d_snap, (size_t)total * sizeof(amb_aircraft)));
-            d->snap_cap = (int)total;
+            CK(d, cudaMalloc(&d->d_snap, (size_t)total * sizeof(amb_aircraft)));
+            d->snap_cap = total;
         }
-        if (with_ext && d->xsnap_cap < (int)total) {
+        if (with_ext && d->xsnap_cap < total) {
             if (d->d_xsnap) cudaFree(d->d_xsnap);
             d->d_xsnap = nullptr; d->xsnap_cap = 0;
-            DCK(cudaMalloc(&d->d_xsnap, (size_t)total * sizeof(amb_aircraft_ext)));
-            d->xsnap_cap = (int)total;
+            CK(d, cudaMalloc(&d->d_xsnap, (size_t)total * sizeof(amb_aircraft_ext)));
+            d->xsnap_cap = total;
         }
         dst = d->d_snap;
         xdst = d->d_xsnap;
     }
-    const int k = with_ext ? amb_snap_gather_ext_launch(d->st.tocc, d->st.trows, d->st.tclk, now, d->st.track, AMB_TRACK_WORDS,
-                                                   off, dst, d->st.xocc, d->st.xrows, d->st.track_ext, xdst, s, &e)
-                      : amb_snap_gather_launch(d->st.tocc, d->st.trows, d->st.tclk, now, d->st.track, AMB_TRACK_WORDS, off,
-                                               dst, s, &e);
-    if (k < 0) return dfail(d, AMB_ERR_CUDA, "aircraft snapshot", e);
+    if (amb_decode_snapshot_gather(&d->st, now, AMB_TRACK_WORDS, dst, with_ext ? xdst : nullptr, s, &e) < 0)
+        return fail(d, AMB_ERR_CUDA, "aircraft snapshot", e);
     d->launches += 1;
     if (!out_on_device) {
         int rc = staged_d2h(d, out, d->d_snap, (size_t)total * sizeof(amb_aircraft), s);
         if (rc == AMB_OK && with_ext) rc = staged_d2h(d, ext, d->d_xsnap, (size_t)total * sizeof(amb_aircraft_ext), s);
         if (rc != AMB_OK) return rc;
     }
-    DCK(cudaStreamSynchronize(s));
-    return (int)total;
+    CK(d, cudaStreamSynchronize(s));
+    return total;
 }
 
 int amb_decoder_aircraft(amb_decoder* d, double now, amb_aircraft* out, int max)
@@ -404,81 +338,64 @@ int amb_decoder_aircraft_ext_device(amb_decoder* d, double now, amb_aircraft* ou
     return snapshot_impl(d, now, out_dev, ext_dev, cap, true, true);
 }
 
-// the last decode's packed lines (nb blocks; total at boff[nb], text) into out (host or device memory); fn names the
-// call, option the option it needs
-static int text_impl(amb_decoder* d, bool on, int nb, const unsigned long long* boff, const char* text, const char* fn,
-                     const char* option, char* out, size_t cap, size_t* n_bytes, bool out_on_device)
+// amb_decoder_sbs1(_device), and amb_decoder_reports(_device) when `reports`: the last decode's lines into out (host or
+// device memory)
+static int text_impl(amb_decoder* d, bool reports, char* out, size_t cap, size_t* n_bytes, bool out_on_device)
 {
+    const char* fn = !reports ? "amb_decoder_sbs1" : out_on_device ? "amb_decoder_reports_device" : "amb_decoder_reports";
     char what[96];
-    if (!d || !n_bytes || (cap > 0 && !out)) { snprintf(what, sizeof what, "%s: bad argument", fn); return dfail(d, AMB_ERR_INVALID, what); }
+    if (!d || !n_bytes || (cap > 0 && !out)) { snprintf(what, sizeof what, "%s: bad argument", fn); return fail(d, AMB_ERR_INVALID, what); }
     *n_bytes = 0;
-    if (!on) { snprintf(what, sizeof what, "%s: option %s is off", fn, option); return dfail(d, AMB_ERR_STATE, what); }
-    if (nb < 0) return AMB_OK;                          // no decode with the option on since it was set
-    DCK(cudaSetDevice(d->device));
+    if ((reports ? d->st.reports : d->st.sbs1) <= 0) {
+        snprintf(what, sizeof what, "%s: option %s is off", fn, reports ? "reports" : "sbs1");
+        return fail(d, AMB_ERR_STATE, what);
+    }
+    CK(d, cudaSetDevice(d->device));
     cudaStream_t s = d->stream;
+    const char* text = nullptr;
     unsigned long long total = 0;
-    DCK(cudaMemcpyAsync(&total, boff + nb, sizeof total, cudaMemcpyDeviceToHost, s));
-    DCK(cudaStreamSynchronize(s));
+    CK(d, amb_decode_text(&d->st, reports, s, &text, &total));
     *n_bytes = (size_t)total;
-    if (total > cap) { snprintf(what, sizeof what, "%s: output buffer too small", fn); return dfail(d, AMB_ERR_OVERFLOW, what); }
+    if (total > cap) { snprintf(what, sizeof what, "%s: output buffer too small", fn); return fail(d, AMB_ERR_OVERFLOW, what); }
     if (total == 0) return AMB_OK;
-    if (out_on_device) DCK(cudaMemcpyAsync(out, text, (size_t)total, cudaMemcpyDeviceToDevice, s));
+    if (out_on_device) CK(d, cudaMemcpyAsync(out, text, (size_t)total, cudaMemcpyDeviceToDevice, s));
     else {
         int rc = staged_d2h(d, out, text, (size_t)total, s);
         if (rc != AMB_OK) return rc;
     }
-    DCK(cudaStreamSynchronize(s));
+    CK(d, cudaStreamSynchronize(s));
     return AMB_OK;
-}
-
-static int sbs1_impl(amb_decoder* d, char* out, size_t cap, size_t* n_bytes, bool out_on_device)
-{
-    return text_impl(d, d && d->st.sbs1 > 0, d ? d->sbs1_nb : -1, d ? d->st.sb.boff : nullptr, d ? d->st.sb.text : nullptr,
-                     "amb_decoder_sbs1", "sbs1", out, cap, n_bytes, out_on_device);
 }
 
 int amb_decoder_sbs1(amb_decoder* d, char* out, size_t cap, size_t* n_bytes)
 {
-    return sbs1_impl(d, out, cap, n_bytes, false);
+    return text_impl(d, false, out, cap, n_bytes, false);
 }
 
 int amb_decoder_sbs1_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes)
 {
-    return sbs1_impl(d, out_dev, cap, n_bytes, true);
-}
-
-static int reports_impl(amb_decoder* d, char* out, size_t cap, size_t* n_bytes, bool out_on_device)
-{
-    return text_impl(d, d && d->st.reports > 0, d ? d->reports_nb : -1, d ? d->st.rb.boff : nullptr,
-                     d ? d->st.rb.text : nullptr, out_on_device ? "amb_decoder_reports_device" : "amb_decoder_reports",
-                     "reports", out, cap, n_bytes, out_on_device);
+    return text_impl(d, false, out_dev, cap, n_bytes, true);
 }
 
 int amb_decoder_reports(amb_decoder* d, char* out, size_t cap, size_t* n_bytes)
 {
-    return reports_impl(d, out, cap, n_bytes, false);
+    return text_impl(d, true, out, cap, n_bytes, false);
 }
 
 int amb_decoder_reports_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes)
 {
-    return reports_impl(d, out_dev, cap, n_bytes, true);
+    return text_impl(d, true, out_dev, cap, n_bytes, true);
 }
 
-// the coverage grid into out (host or device memory); all zeros while the grid is not allocated yet
+// the coverage grid into out (host or device memory)
 static int coverage_impl(amb_decoder* d, double* out, bool out_on_device)
 {
     const char* fn = out_on_device ? "amb_decoder_coverage_device" : "amb_decoder_coverage";
     char what[96];
-    if (!d || !out) { snprintf(what, sizeof what, "%s: bad argument", fn); return dfail(d, AMB_ERR_INVALID, what); }
-    if (d->st.coverage <= 0) { snprintf(what, sizeof what, "%s: option coverage is off", fn); return dfail(d, AMB_ERR_STATE, what); }
-    const size_t bytes = AMB_COVERAGE_CELLS * sizeof(double);
-    static_assert(sizeof(double) == sizeof(unsigned long long), "coverage cell layout");
-    if (!d->st.cgrid && !out_on_device) { memset(out, 0, bytes); return AMB_OK; }
-    DCK(cudaSetDevice(d->device));
-    cudaStream_t s = d->stream;
-    if (!d->st.cgrid) DCK(cudaMemsetAsync(out, 0, bytes, s));
-    else DCK(cudaMemcpyAsync(out, d->st.cgrid, bytes, out_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, s));
-    DCK(cudaStreamSynchronize(s));
+    if (!d || !out) { snprintf(what, sizeof what, "%s: bad argument", fn); return fail(d, AMB_ERR_INVALID, what); }
+    if (d->st.coverage <= 0) { snprintf(what, sizeof what, "%s: option coverage is off", fn); return fail(d, AMB_ERR_STATE, what); }
+    CK(d, cudaSetDevice(d->device));
+    CK(d, amb_decode_coverage(&d->st, out, out_on_device, d->stream));
     return AMB_OK;
 }
 
@@ -495,11 +412,11 @@ int amb_decoder_coverage_device(amb_decoder* d, double* out_dev)
 int amb_decoder_coverage_reset(amb_decoder* d)
 {
     if (!d) return AMB_ERR_INVALID;
-    if (d->st.coverage <= 0) return dfail(d, AMB_ERR_STATE, "amb_decoder_coverage_reset: option coverage is off");
+    if (d->st.coverage <= 0) return fail(d, AMB_ERR_STATE, "amb_decoder_coverage_reset: option coverage is off");
     if (!d->st.cgrid) return AMB_OK;
-    DCK(cudaSetDevice(d->device));
-    DCK(cudaMemsetAsync(d->st.cgrid, 0, AMB_COVERAGE_CELLS * sizeof(unsigned long long), d->stream));
-    DCK(cudaStreamSynchronize(d->stream));
+    CK(d, cudaSetDevice(d->device));
+    CK(d, cudaMemsetAsync(d->st.cgrid, 0, AMB_COVERAGE_CELLS * sizeof(unsigned long long), d->stream));
+    CK(d, cudaStreamSynchronize(d->stream));
     return AMB_OK;
 }
 
@@ -533,19 +450,6 @@ struct amb_mlat {
 
 static thread_local std::string g_mlat_create_err;
 
-static int mfail(amb_mlat* m, int code, const char* what, cudaError_t e = cudaSuccess)
-{
-    if (m) {
-        char buf[256];
-        if (e != cudaSuccess) snprintf(buf, sizeof buf, "%s: %s", what, cudaGetErrorString(e));
-        else snprintf(buf, sizeof buf, "%s", what);
-        m->err = buf;
-    }
-    return code;
-}
-#define MCK(call)                                                                  \
-    do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return mfail(m, AMB_ERR_CUDA, #call, e_); } while (0)
-
 // llh2ecef (mlat.py:77-86) of a station, and the terms of the start point overhead it
 static AmbMlatStation mlat_station(double lat_deg, double lon_deg, double height)
 {
@@ -576,11 +480,8 @@ int amb_mlat_create(int device, int K, const double* lat, const double* lon, con
             g_mlat_create_err = "amb_mlat_create: a station position is out of range";
             return AMB_ERR_INVALID;
         }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) return AMB_ERR_NO_DEVICE;
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return AMB_ERR_NO_DEVICE;
-    if (prop.major != 9 || prop.minor != 0) return AMB_ERR_NO_DEVICE;   // sm_90a cubin only; there is no CPU path
+    if (amb_check_device(device, &prop) != AMB_OK) return AMB_ERR_NO_DEVICE;
     amb_mlat* m = new (std::nothrow) amb_mlat();
     if (!m) return AMB_ERR_INVALID;
     m->device = device;
@@ -626,25 +527,25 @@ int amb_mlat_set_option(amb_mlat* m, const char* name, double value)
 {
     if (!m || !name) return AMB_ERR_INVALID;
     if (strcmp(name, "window_us") == 0) {
-        if (!(value > 0.0) || !(value <= 1e6)) return mfail(m, AMB_ERR_INVALID, "window_us: > 0 .. 1e6 microseconds");
+        if (!(value > 0.0) || !(value <= 1e6)) return fail(m, AMB_ERR_INVALID, "window_us: > 0 .. 1e6 microseconds");
         m->st.W = value / 1e6;
         return AMB_OK;
     }
-    return mfail(m, AMB_ERR_INVALID, "amb_mlat_set_option: unknown option");
+    return fail(m, AMB_ERR_INVALID, "amb_mlat_set_option: unknown option");
 }
 
 int amb_mlat_get_option(amb_mlat* m, const char* name, double* value)
 {
     if (!m || !name || !value) return AMB_ERR_INVALID;
     if (strcmp(name, "window_us") == 0) { *value = m->st.W * 1e6; return AMB_OK; }
-    return mfail(m, AMB_ERR_INVALID, "amb_mlat_get_option: unknown option");
+    return fail(m, AMB_ERR_INVALID, "amb_mlat_get_option: unknown option");
 }
 
 int amb_mlat_set_offset(amb_mlat* m, int k, double seconds)
 {
     if (!m) return AMB_ERR_INVALID;
-    if (k < 0 || k >= m->st.K) return mfail(m, AMB_ERR_INVALID, "amb_mlat_set_offset: no such station");
-    if (!(fabs(seconds) <= 1.0)) return mfail(m, AMB_ERR_INVALID, "amb_mlat_set_offset: |seconds| <= 1");
+    if (k < 0 || k >= m->st.K) return fail(m, AMB_ERR_INVALID, "amb_mlat_set_offset: no such station");
+    if (!(fabs(seconds) <= 1.0)) return fail(m, AMB_ERR_INVALID, "amb_mlat_set_offset: |seconds| <= 1");
     m->st.off[k] = seconds;
     return AMB_OK;
 }
@@ -664,7 +565,7 @@ static int mlat_impl(amb_mlat* m, const amb_frame* const* frames, const int* cou
     char what[128];
     if (!m || !frames || !counts || !n_out || cap < 0 || (cap > 0 && !out) || (!flush && !(end_frac - end_frac == 0.0))) {
         snprintf(what, sizeof what, "%s: bad argument", fn);
-        return mfail(m, AMB_ERR_INVALID, what);
+        return fail(m, AMB_ERR_INVALID, what);
     }
     *n_out = 0;
     AmbMlatState* s = &m->st;
@@ -673,35 +574,35 @@ static int mlat_impl(amb_mlat* m, const amb_frame* const* frames, const int* cou
     c.K = s->K;
     long long P = 0, total = 0;
     for (int k = 0; k < s->K; k++) {
-        if (counts[k] < 0 || (counts[k] > 0 && !frames[k])) { snprintf(what, sizeof what, "%s: bad frames of station %d", fn, k); return mfail(m, AMB_ERR_INVALID, what); }
+        if (counts[k] < 0 || (counts[k] > 0 && !frames[k])) { snprintf(what, sizeof what, "%s: bad frames of station %d", fn, k); return fail(m, AMB_ERR_INVALID, what); }
         c.count[k] = counts[k]; c.base[k] = (int)P; c.off[k] = s->off[k];
         P += (counts[k] + AMB_MLAT_BLOCK - 1) / AMB_MLAT_BLOCK * AMB_MLAT_BLOCK;
         total += counts[k];
     }
-    if (P + s->C > (1ll << 30)) { snprintf(what, sizeof what, "%s: more than 2^30 frames in one call", fn); return mfail(m, AMB_ERR_INVALID, what); }
+    if (P + s->C > (1ll << 30)) { snprintf(what, sizeof what, "%s: more than 2^30 frames in one call", fn); return fail(m, AMB_ERR_INVALID, what); }
     c.base[s->K] = (int)P;
     const int nb = (int)(P / AMB_MLAT_BLOCK);
-    MCK(cudaSetDevice(m->device));
+    CK(m, cudaSetDevice(m->device));
     cudaStream_t st = m->stream;
     cudaError_t e = cudaSuccess;
     // the scan buffers serve the raw blocks and, after the count, the N <= C + total items: sized for both now, because
     // the count's offsets in boff[0] are read again after it
     const long long nbn_max = (s->C + total + AMB_MLAT_BLOCK - 1) / AMB_MLAT_BLOCK;
     if (amb_mlat_prepare_raw(s, nbn_max > nb ? (int)nbn_max : nb, &e) < 0)
-        return mfail(m, AMB_ERR_CUDA, "amb_mlat: scratch memory", e);
-    MCK(cudaEventRecord(m->e0, st));
+        return fail(m, AMB_ERR_CUDA, "amb_mlat: scratch memory", e);
+    CK(m, cudaEventRecord(m->e0, st));
     if (on_device) {
         for (int k = 0; k < s->K; k++) c.f[k] = frames[k];
     } else if (total) {
         if (s->raw_cap < (size_t)total) {
             if (s->raw) cudaFree(s->raw);
             s->raw = nullptr; s->raw_cap = 0;
-            MCK(cudaMalloc(&s->raw, (size_t)total * sizeof(amb_frame)));
+            CK(m, cudaMalloc(&s->raw, (size_t)total * sizeof(amb_frame)));
             s->raw_cap = (size_t)total;
         }
         size_t at = 0;
         for (int k = 0; k < s->K; k++) {
-            if (counts[k]) MCK(cudaMemcpyAsync(s->raw + at, frames[k], (size_t)counts[k] * sizeof(amb_frame), cudaMemcpyHostToDevice, st));
+            if (counts[k]) CK(m, cudaMemcpyAsync(s->raw + at, frames[k], (size_t)counts[k] * sizeof(amb_frame), cudaMemcpyHostToDevice, st));
             c.f[k] = s->raw + at;
             at += (size_t)counts[k];
         }
@@ -710,9 +611,9 @@ static int mlat_impl(amb_mlat* m, const amb_frame* const* frames, const int* cou
     unsigned long long E = 0;
     if (nb) {
         launches += (uint64_t)amb_mlat_launch_count(c, nb, s, st, &e);
-        if (e != cudaSuccess) return mfail(m, AMB_ERR_CUDA, "amb_mlat: count", e);
-        MCK(cudaMemcpyAsync(&E, s->boff[0] + nb, sizeof E, cudaMemcpyDeviceToHost, st));
-        MCK(cudaStreamSynchronize(st));
+        if (e != cudaSuccess) return fail(m, AMB_ERR_CUDA, "amb_mlat: count", e);
+        CK(m, cudaMemcpyAsync(&E, s->boff[0] + nb, sizeof E, cudaMemcpyDeviceToHost, st));
+        CK(m, cudaStreamSynchronize(st));
     }
     const int N = s->C + (int)E;
     int G = 0, Cn = 0;
@@ -720,38 +621,38 @@ static int mlat_impl(amb_mlat* m, const amb_frame* const* frames, const int* cou
     if (N > 0) {
         int npad = 1;
         while (npad < N) npad <<= 1;
-        if (amb_mlat_prepare_items(s, N, npad, &e) < 0) return mfail(m, AMB_ERR_CUDA, "amb_mlat: scratch memory", e);
+        if (amb_mlat_prepare_items(s, N, npad, &e) < 0) return fail(m, AMB_ERR_CUDA, "amb_mlat: scratch memory", e);
         launches += (uint64_t)amb_mlat_launch_group(c, nb, N, npad, 2048u, end_secs, end_frac, flush, s, st, &e);
-        if (e != cudaSuccess) return mfail(m, AMB_ERR_CUDA, "amb_mlat: grouping", e);
+        if (e != cudaSuccess) return fail(m, AMB_ERR_CUDA, "amb_mlat: grouping", e);
         const int nbn = (N + AMB_MLAT_BLOCK - 1) / AMB_MLAT_BLOCK;
         unsigned long long g = 0, cn = 0;
-        MCK(cudaMemcpyAsync(&g, s->boff[0] + nbn, sizeof g, cudaMemcpyDeviceToHost, st));
-        MCK(cudaMemcpyAsync(&cn, s->boff[1] + nbn, sizeof cn, cudaMemcpyDeviceToHost, st));
-        MCK(cudaMemcpyAsync(ctr, s->ctr, sizeof ctr, cudaMemcpyDeviceToHost, st));
-        MCK(cudaStreamSynchronize(st));
+        CK(m, cudaMemcpyAsync(&g, s->boff[0] + nbn, sizeof g, cudaMemcpyDeviceToHost, st));
+        CK(m, cudaMemcpyAsync(&cn, s->boff[1] + nbn, sizeof cn, cudaMemcpyDeviceToHost, st));
+        CK(m, cudaMemcpyAsync(ctr, s->ctr, sizeof ctr, cudaMemcpyDeviceToHost, st));
+        CK(m, cudaStreamSynchronize(st));
         if (ctr[AMB_MC_UNORDERED]) {
             snprintf(what, sizeof what, "%s: a station's frames are not in time order", fn);
-            return mfail(m, AMB_ERR_INVALID, what);
+            return fail(m, AMB_ERR_INVALID, what);
         }
         G = (int)g; Cn = (int)cn;
         if (G > cap) {
             *n_out = G;
             snprintf(what, sizeof what, "%s: output buffer too small", fn);
-            return mfail(m, AMB_ERR_OVERFLOW, what);
+            return fail(m, AMB_ERR_OVERFLOW, what);
         }
         if (!on_device && s->fix_cap < G) {
             if (s->fix) cudaFree(s->fix);
             s->fix = nullptr; s->fix_cap = 0;
-            MCK(cudaMalloc(&s->fix, (size_t)G * sizeof(amb_mlat_fix)));
+            CK(m, cudaMalloc(&s->fix, (size_t)G * sizeof(amb_mlat_fix)));
             s->fix_cap = G;
         }
         launches += (uint64_t)amb_mlat_launch_solve(N, G, on_device ? out : s->fix, s, st, &e);
-        if (e != cudaSuccess) return mfail(m, AMB_ERR_CUDA, "amb_mlat: solve", e);
-        if (!on_device && G) MCK(cudaMemcpyAsync(out, s->fix, (size_t)G * sizeof(amb_mlat_fix), cudaMemcpyDeviceToHost, st));
-        MCK(cudaMemcpyAsync(ctr, s->ctr, sizeof ctr, cudaMemcpyDeviceToHost, st));
+        if (e != cudaSuccess) return fail(m, AMB_ERR_CUDA, "amb_mlat: solve", e);
+        if (!on_device && G) CK(m, cudaMemcpyAsync(out, s->fix, (size_t)G * sizeof(amb_mlat_fix), cudaMemcpyDeviceToHost, st));
+        CK(m, cudaMemcpyAsync(ctr, s->ctr, sizeof ctr, cudaMemcpyDeviceToHost, st));
     }
-    MCK(cudaEventRecord(m->e1, st));
-    MCK(cudaStreamSynchronize(st));
+    CK(m, cudaEventRecord(m->e1, st));
+    CK(m, cudaStreamSynchronize(st));
     // commit
     s->C = Cn;
     *n_out = G;

@@ -2,12 +2,15 @@
 // pairing stage between them in amb_decode_v3.cuh, the optional stages in the headers included below; then the state
 // every stage reads and writes, its lifecycle (amb_decode_prepare, amb_decode_reset, amb_decode_free) and the one launch
 // sequence of a decode (amb_decode_launch). The staging of frames and records and the C ABI are in amb_decode.cu, the
-// per-message arithmetic in amb_decode_core.h. Kept in headers without any <<< >>> launch, and with the state's memory
-// handled through cudaMalloc / cudaMemsetAsync / cudaMemcpyAsync / cudaFree only, so that tests/simt/ can compile the
-// very same kernel source and state handling for the host under a small SIMT emulator (CPU-side check of the
-// warp-level logic; the GPU tests remain the parity gate).
+// per-message arithmetic in amb_decode_core.h. Beside the state: its option table (amb_decode_set_option); last, the
+// read-outs of the stages' results (amb_decode_text, amb_decode_snapshot_*, amb_decode_coverage). Kept in headers
+// without any <<< >>> launch, and with the state's memory handled through cudaMalloc / cudaMemsetAsync /
+// cudaMemcpyAsync / cudaFree only, so that tests/simt/ can compile the very same kernel source and state handling for
+// the host under a small SIMT emulator (CPU-side check of the warp-level logic; the GPU tests remain the parity gate).
 #pragma once
 #include "amb_decode_core.h"
+
+#include <string.h>
 
 #define AMB_TABLE_SLOTS (1ull << 26)     // (24-bit ICAO, surface, even/odd)
 
@@ -93,8 +96,43 @@ struct AmbDecodeState {
     unsigned* rfirst = nullptr;          // 1 until the first queued frame since creation or reset has been formatted
     AmbReportBufs rb;                    // the stage's per-call scratch and the packed lines
     int rcap = 0;                        // frames rb holds
+    int sbs1_nb = -1;                    // blocks of lines of the last decode (its byte total is sb.boff[sbs1_nb]);
+                                         // -1: the last decode wrote no lines
+    int reports_nb = -1;                 // the same for the text reports (rb.boff[reports_nb])
     int have_loc = 0; double lat = 0.0, lon = 0.0;      // receiver location
 };
+
+// The options of amb_decoder_set_option: the member each one sets, the values it takes and what any other value reports.
+static const struct {
+    const char* name; int AmbDecodeState::*member; int lo, hi; const char* range;
+} amb_decode_options[] = {
+    {"local_cpr", &AmbDecodeState::local_cpr, 0, AMB_LOCAL_CPR_MAX, "local_cpr: 0 (off) .. 600 seconds"},
+    {"commb", &AmbDecodeState::commb, 0, AMB_COMMB_MAX, "commb: 0 (off) .. 600 seconds"},
+    {"track", &AmbDecodeState::track, 0, AMB_TRACK_MAX, "track: 0 (off) .. 3600 seconds"},
+    {"opstatus", &AmbDecodeState::opstatus, 0, AMB_OPSTATUS_MAX, "opstatus: 0 (off) .. 600 seconds"},
+    {"track_ext", &AmbDecodeState::track_ext, 0, AMB_TRACK_EXT_MAX, "track_ext: 0 (off) .. 3600 seconds"},
+    {"sbs1", &AmbDecodeState::sbs1, 0, 1, "sbs1: 0 (off) or 1 (on)"},
+    {"sbs1_tz", &AmbDecodeState::sbs1_tz, AMB_SBS1_TZ_MIN, AMB_SBS1_TZ_MAX, "sbs1_tz: -720 .. 840 minutes"},
+    {"coverage", &AmbDecodeState::coverage, 0, 1, "coverage: 0 (off) or 1 (on)"},
+    {"reports", &AmbDecodeState::reports, 0, 1, "reports: 0 (off) or 1 (on)"},
+};
+
+// Set option `name` of st to `value`, from the next decode on. Returns NULL, or why the setting is refused.
+static const char* amb_decode_set_option(AmbDecodeState* st, const char* name, int value)
+{
+    for (const auto& o : amb_decode_options) {
+        if (strcmp(name, o.name) != 0) continue;
+        if (value < o.lo || value > o.hi) return o.range;
+        st->*o.member = value;
+        return nullptr;
+    }
+    return "amb_decoder_set_option: unknown option";
+}
+
+static void amb_decode_set_location(AmbDecodeState* st, int have_location, double lat, double lon)
+{
+    st->have_loc = have_location ? 1 : 0; st->lat = lat; st->lon = lon;
+}
 
 // What amb_decode_prepare, amb_decode_reset and amb_decode_launch return when a stage's memory or launch fails.
 enum { AMB_STAGE_FIELDS = -1, AMB_STAGE_PAIRING = -2, AMB_STAGE_RESOLVE = -3, AMB_STAGE_LOCAL = -4,
@@ -288,11 +326,14 @@ static void amb_decode_free(AmbDecodeState* st)
 // reach it), the Comm-B, op-status and track stages whose S is > 0, and the track extension when track and track_ext
 // are both > 0, then the SBS-1 feed when sbs1 is on, then the text reports when reports is on. Returns how many kernels
 // were launched (7, plus 6 per stage that is on, plus 1 for the coverage map, 10 for the SBS-1 feed and 3 for the text
-// reports), or an AMB_STAGE_* code with *err set.
+// reports), or an AMB_STAGE_* code with *err set. Only a decode that launches every stage leaves lines of the SBS-1
+// feed and the text reports, whichever is on, for amb_decode_text: sbs1_nb and reports_nb are -1 otherwise, and a
+// caller that ends a decode before this call (n = 0, a failure) sets them to -1 itself.
 static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n, amb_fields* fields, cudaStream_t s,
                              cudaError_t* err)
 {
     const int nb = (n + 127) / 128;
+    st->sbs1_nb = st->reports_nb = -1;
     AMB_LAUNCH((amb_fields_kernel), nb, 128, 0, s, frames, n, fields, st->pos, st->pair);
     if ((*err = cudaGetLastError()) != cudaSuccess) return AMB_STAGE_FIELDS;
     const int kp = amb_v3_launch(&st->v3, st->pos, n, st->table, st->pair, s, err);
@@ -343,5 +384,61 @@ static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n,
         if (kr < 0) return AMB_STAGE_REPORTS;
         k += kr;
     }
+    if (st->sbs1 > 0) st->sbs1_nb = nb;
+    if (st->reports > 0) st->reports_nb = nb;
     return k;
+}
+
+// ---- read-outs ----------------------------------------------------------------------------------------------------
+// The lines of the last decode, the text reports' (reports) or the SBS-1 feed's, on stream s: *text their packed bytes
+// in the state's memory and *bytes their count, or NULL and 0 when the last decode wrote none.
+static cudaError_t amb_decode_text(const AmbDecodeState* st, bool reports, cudaStream_t s, const char** text,
+                                   unsigned long long* bytes)
+{
+    const int nb = reports ? st->reports_nb : st->sbs1_nb;
+    *text = nullptr; *bytes = 0;
+    if (nb < 0) return cudaSuccess;
+    *text = reports ? st->rb.text : st->sb.text;
+    const cudaError_t e = cudaMemcpyAsync(bytes, (reports ? st->rb.boff : st->sb.boff) + nb, sizeof *bytes,
+                                          cudaMemcpyDeviceToHost, s);
+    return e != cudaSuccess ? e : cudaStreamSynchronize(s);
+}
+
+// The aircraft table at `now` over the first `words` words of its bitmap (a multiple of AMB_SNAP_WORDS; the decoder
+// scans all AMB_TRACK_WORDS), on stream s, once the track stage has allocated it. amb_decode_snapshot_count counts the
+// rows shown and returns their total (2 launches); amb_decode_snapshot_gather then writes them to out, and their
+// extensions to ext unless it is NULL (1 launch). Both return -1 with *err set when a launch or a copy fails.
+static int amb_decode_snapshot_count(const AmbDecodeState* st, double now, unsigned words, cudaStream_t s, cudaError_t* err)
+{
+    const unsigned nb = words / AMB_SNAP_WORDS;
+    uint32_t* const off = st->snap_cnt + nb;
+    uint32_t total = 0;
+    if (amb_snap_count_launch(st->tocc, st->trows, st->tclk, now, st->track, words, st->snap_cnt, off, s, err) < 0 ||
+        (*err = cudaMemcpyAsync(&total, off + nb, sizeof total, cudaMemcpyDeviceToHost, s)) != cudaSuccess ||
+        (*err = cudaStreamSynchronize(s)) != cudaSuccess)
+        return -1;
+    return (int)total;
+}
+
+static int amb_decode_snapshot_gather(const AmbDecodeState* st, double now, unsigned words, amb_aircraft* out,
+                                      amb_aircraft_ext* ext, cudaStream_t s, cudaError_t* err)
+{
+    const uint32_t* off = st->snap_cnt + words / AMB_SNAP_WORDS;
+    const int k = ext ? amb_snap_gather_ext_launch(st->tocc, st->trows, st->tclk, now, st->track, words, off, out, st->xocc,
+                                                   st->xrows, st->track_ext, ext, s, err)
+                      : amb_snap_gather_launch(st->tocc, st->trows, st->tclk, now, st->track, words, off, out, s, err);
+    return k < 0 ? -1 : k;
+}
+
+// The coverage grid into out (AMB_COVERAGE_CELLS doubles, in device memory when out_on_device, else in host memory) on
+// stream s: all zeros while the grid is not allocated yet.
+static cudaError_t amb_decode_coverage(const AmbDecodeState* st, double* out, bool out_on_device, cudaStream_t s)
+{
+    static_assert(sizeof(double) == sizeof(unsigned long long), "coverage cell layout");
+    const size_t bytes = AMB_COVERAGE_CELLS * sizeof(double);
+    if (!st->cgrid && !out_on_device) { memset(out, 0, bytes); return cudaSuccess; }
+    const cudaError_t e = st->cgrid ? cudaMemcpyAsync(out, st->cgrid, bytes, out_on_device ? cudaMemcpyDeviceToDevice
+                                                                                            : cudaMemcpyDeviceToHost, s)
+                                    : cudaMemsetAsync(out, 0, bytes, s);
+    return e != cudaSuccess ? e : cudaStreamSynchronize(s);
 }

@@ -13,6 +13,7 @@ arithmetic runs in libairmodes_b200.so on the GPU; there is no CPU implementatio
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import math
 
 import numpy as np
@@ -86,72 +87,43 @@ def local_outcome(records):
     return np.asarray(records["pad_"], dtype=np.uint64) & np.uint64(0xFF)
 
 
-# the decoder options (amb_decoder_set_option) and their maxima in seconds
-OPTION_MAX = {"local_cpr": LOCAL_CPR_MAX, "track": TRACK_MAX, "commb": COMMB_MAX, "opstatus": OPSTATUS_MAX,
-              "track_ext": TRACK_EXT_MAX}
+# The decoder options (amb_decoder_set_option): name -> (kind, lowest, highest value). A "switch" is off or on; the
+# other kinds take integers in the unit they name, "seconds" from 0 (off).
+OPTIONS = {"local_cpr": ("seconds", 0, LOCAL_CPR_MAX), "track": ("seconds", 0, TRACK_MAX),
+           "commb": ("seconds", 0, COMMB_MAX), "opstatus": ("seconds", 0, OPSTATUS_MAX),
+           "track_ext": ("seconds", 0, TRACK_EXT_MAX), "sbs1": ("switch", 0, 1),
+           "sbs1_tz": ("minutes", SBS1_TZ_MIN, SBS1_TZ_MAX), "coverage": ("switch", 0, 1), "reports": ("switch", 0, 1)}
+# the maxima of the options in seconds
+OPTION_MAX = {name: top for name, (kind, _, top) in OPTIONS.items() if kind == "seconds"}
 
 
-def check_option(name: str, seconds) -> int:
-    """Validate a setting of decoder option `name`: an int in 0 (off) .. OPTION_MAX[name] seconds. Raises ValueError
-    otherwise."""
-    top = OPTION_MAX[name]
+def check_option(name: str, value) -> int:
+    """Validate a setting of decoder option `name` (OPTIONS): a switch takes False / True or 0 / 1, the other kinds an
+    int in their range. Returns it as an int; raises ValueError otherwise."""
+    kind, low, top = OPTIONS[name]
+    if kind == "switch":
+        if isinstance(value, (bool, np.bool_)) or (isinstance(value, (int, np.integer)) and int(value) in (0, 1)):
+            return int(value)
+        raise ValueError("%s: False / True (0 / 1), got %r" % (name, value))
     try:
-        ok = not isinstance(seconds, bool) and int(seconds) == seconds and 0 <= int(seconds) <= top
+        ok = not isinstance(value, bool) and int(value) == value and low <= int(value) <= top
     except (TypeError, ValueError):
         ok = False
     if not ok:
-        raise ValueError("%s: an integer number of seconds in 0 (off) .. %d, got %r" % (name, top, seconds))
-    return int(seconds)
+        span = "0 (off) .. %d" % top if kind == "seconds" else "%d .. %d" % (low, top)
+        raise ValueError("%s: an integer number of %s in %s, got %r" % (name, kind, span, value))
+    return int(value)
 
 
 # check_option bound to one option, under the names the module has always exported
-def check_local_cpr(seconds) -> int:
-    return check_option("local_cpr", seconds)
-
-
-def check_commb(seconds) -> int:
-    return check_option("commb", seconds)
-
-
-def check_track(seconds) -> int:
-    return check_option("track", seconds)
-
-
-def check_opstatus(seconds) -> int:
-    return check_option("opstatus", seconds)
-
-
-def _check_switch(name: str, on) -> int:
-    if isinstance(on, (bool, np.bool_)) or (isinstance(on, (int, np.integer)) and int(on) in (0, 1)):
-        return int(on)
-    raise ValueError("%s: False / True (0 / 1), got %r" % (name, on))
-
-
-def check_sbs1(on) -> int:
-    """Validate a setting of decoder option sbs1: False / True or 0 / 1. Raises ValueError otherwise."""
-    return _check_switch("sbs1", on)
-
-
-def check_coverage(on) -> int:
-    """Validate a setting of decoder option coverage: False / True or 0 / 1. Raises ValueError otherwise."""
-    return _check_switch("coverage", on)
-
-
-def check_reports(on) -> int:
-    """Validate a setting of decoder option reports: False / True or 0 / 1. Raises ValueError otherwise."""
-    return _check_switch("reports", on)
-
-
-def check_sbs1_tz(minutes) -> int:
-    """Validate a setting of decoder option sbs1_tz: an int in SBS1_TZ_MIN .. SBS1_TZ_MAX minutes. Raises ValueError
-    otherwise."""
-    try:
-        ok = not isinstance(minutes, bool) and int(minutes) == minutes and SBS1_TZ_MIN <= int(minutes) <= SBS1_TZ_MAX
-    except (TypeError, ValueError):
-        ok = False
-    if not ok:
-        raise ValueError("sbs1_tz: an integer number of minutes in %d .. %d, got %r" % (SBS1_TZ_MIN, SBS1_TZ_MAX, minutes))
-    return int(minutes)
+check_local_cpr = functools.partial(check_option, "local_cpr")
+check_commb = functools.partial(check_option, "commb")
+check_track = functools.partial(check_option, "track")
+check_opstatus = functools.partial(check_option, "opstatus")
+check_sbs1 = functools.partial(check_option, "sbs1")
+check_sbs1_tz = functools.partial(check_option, "sbs1_tz")
+check_coverage = functools.partial(check_option, "coverage")
+check_reports = functools.partial(check_option, "reports")
 
 
 def commb_outcome(records):
@@ -358,11 +330,9 @@ class batch_decoder:
     def __init__(self, my_location=None, device: int = 0, local_cpr: int = 0, track: int = 0, commb: int = 0,
                  opstatus: int = 0, track_ext: int = 0, sbs1=False, sbs1_tz: int = 0, coverage=False,
                  reports=False):
-        settings = {"local_cpr": check_option("local_cpr", local_cpr), "track": check_option("track", track),
-                    "commb": check_option("commb", commb), "opstatus": check_option("opstatus", opstatus),
-                    "track_ext": check_option("track_ext", track_ext)}
-        sbs1, sbs1_tz, coverage = check_sbs1(sbs1), check_sbs1_tz(sbs1_tz), check_coverage(coverage)
-        reports = check_reports(reports)
+        values = dict(local_cpr=local_cpr, track=track, commb=commb, opstatus=opstatus, track_ext=track_ext, sbs1=sbs1,
+                      sbs1_tz=sbs1_tz, coverage=coverage, reports=reports)
+        settings = {name: check_option(name, values[name]) for name in OPTIONS}
         self._lib = _lib.load()
         h = C.c_void_p()
         have, lat, lon = self._loc(my_location)
@@ -373,21 +343,10 @@ class batch_decoder:
         self._h = h
         self._device = int(device)
         self.my_location = my_location
-        self._options = dict.fromkeys(OPTION_MAX, 0)
-        for name, seconds in settings.items():
-            if seconds:
-                self._set_option(name, seconds)
-        self._sbs1, self._sbs1_tz = 0, 0
-        if sbs1:
-            self.set_sbs1(True)
-        if sbs1_tz:
-            self.set_sbs1_tz(sbs1_tz)
-        self._coverage = 0
-        if coverage:
-            self.set_coverage(True)
-        self._reports = 0
-        if reports:
-            self.set_reports(True)
+        self._options = dict.fromkeys(OPTIONS, 0)
+        for name, value in settings.items():
+            if value:
+                self._set_option(name, value)
 
     @staticmethod
     def _loc(loc):
@@ -409,10 +368,10 @@ class batch_decoder:
         grid; the option settings stay."""
         self._check(self._lib.amb_decoder_reset(self._h))
 
-    def _set_option(self, name, seconds):
-        seconds = check_option(name, seconds)
-        self._check(self._lib.amb_decoder_set_option(self._h, name.encode(), seconds))
-        self._options[name] = seconds
+    def _set_option(self, name, value):
+        value = check_option(name, value)
+        self._check(self._lib.amb_decoder_set_option(self._h, name.encode(), value))
+        self._options[name] = value
 
     def set_local_cpr(self, seconds: int):
         """Option local_cpr = S seconds (0 = off); applies from the next decode."""
@@ -451,21 +410,17 @@ class batch_decoder:
 
     def set_sbs1(self, on):
         """Option sbs1 on (True) or off (False); applies from the next decode."""
-        on = check_sbs1(on)
-        self._check(self._lib.amb_decoder_set_option(self._h, b"sbs1", on))
-        self._sbs1 = on
+        self._set_option("sbs1", on)
 
     def get_sbs1(self) -> bool:
-        return bool(self._sbs1)
+        return bool(self._options["sbs1"])
 
     def set_sbs1_tz(self, minutes: int):
         """Option sbs1_tz = minutes added to UTC in the SBS-1 date and time (0 = UTC); applies from the next decode."""
-        minutes = check_sbs1_tz(minutes)
-        self._check(self._lib.amb_decoder_set_option(self._h, b"sbs1_tz", minutes))
-        self._sbs1_tz = minutes
+        self._set_option("sbs1_tz", minutes)
 
     def get_sbs1_tz(self) -> int:
-        return self._sbs1_tz
+        return self._options["sbs1_tz"]
 
     def _text(self, fetch) -> bytes:
         n = C.c_size_t()
@@ -500,12 +455,10 @@ class batch_decoder:
 
     def set_reports(self, on):
         """Option reports on (True) or off (False); applies from the next decode."""
-        on = check_reports(on)
-        self._check(self._lib.amb_decoder_set_option(self._h, b"reports", on))
-        self._reports = on
+        self._set_option("reports", on)
 
     def get_reports(self) -> bool:
-        return bool(self._reports)
+        return bool(self._options["reports"])
 
     def report_text(self) -> bytes:
         """The text reports of the last decode, concatenated ("\\n" after each line). Needs the option reports on."""
@@ -518,12 +471,10 @@ class batch_decoder:
 
     def set_coverage(self, on):
         """Option coverage on (True) or off (False); applies from the next decode. The grid is kept while it is off."""
-        on = check_coverage(on)
-        self._check(self._lib.amb_decoder_set_option(self._h, b"coverage", on))
-        self._coverage = on
+        self._set_option("coverage", on)
 
     def get_coverage(self) -> bool:
-        return bool(self._coverage)
+        return bool(self._options["coverage"])
 
     def coverage(self) -> np.ndarray:
         """The coverage grid: a (COVERAGE_ROWS, COVERAGE_BANDS) float64 array, [bearing row, altitude band], statute

@@ -30,17 +30,15 @@ def build(tmp_path_factory, src) -> str:
     return _built[src]
 
 
-class EmulOpts(C.Structure):
-    """The options of one emulated decode (struct EmulOpts of tests/simt/decode_emul.cc): the receiver location and
-    every stage's S, 0 = off."""
-    _fields_ = [("have_loc", C.c_int), ("lat", C.c_double), ("lon", C.c_double), ("local_cpr", C.c_int),
-                ("commb", C.c_int), ("opstatus", C.c_int), ("track", C.c_int), ("track_ext", C.c_int), ("sbs1", C.c_int),
-                ("sbs1_tz", C.c_int)]
-
-
-def opts(loc=None, **stages):
-    """EmulOpts with the receiver at loc = (lat, lon) (None: no location) and the given stages on, e.g. commb=30."""
-    return EmulOpts(0, 0.0, 0.0, **stages) if loc is None else EmulOpts(1, loc[0], loc[1], **stages)
+def opts(e, h, loc=None, **stages):
+    """Set every option of the harness's decoder `h` (e: the bound harness), as amb_decoder_set_location and
+    amb_decoder_set_option would: the receiver at loc = (lat, lon) (None: no location), the options named in `stages` to
+    their values (e.g. commb=30, coverage=1) and every other option of decode.OPTIONS to 0."""
+    from gr_air_modes_b200 import decode
+    assert set(stages) <= set(decode.OPTIONS), stages
+    e.emul_set_location(h, *((0, 0.0, 0.0) if loc is None else (1, loc[0], loc[1])))
+    for name in decode.OPTIONS:
+        assert e.emul_set_option(h, name.encode(), int(stages.get(name, 0))) == 0, name
 
 
 def decode_emul(tmp_path_factory, src=DECODE_EMUL):
@@ -50,10 +48,16 @@ def decode_emul(tmp_path_factory, src=DECODE_EMUL):
     e.emul_new.argtypes = [C.c_int]
     e.emul_free.argtypes = [C.c_void_p]
     e.emul_reset.argtypes = [C.c_void_p]
-    e.emul_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(EmulOpts), C.c_void_p]
-    e.emul_snapshot.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int, C.c_uint, C.c_void_p, C.c_void_p, C.c_int]
-    e.emul_sbs1_text.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    e.emul_set_option.argtypes = [C.c_void_p, C.c_char_p, C.c_int]
+    e.emul_set_location.argtypes = [C.c_void_p, C.c_int, C.c_double, C.c_double]
+    e.emul_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+    e.emul_snapshot.argtypes = [C.c_void_p, C.c_double, C.c_uint, C.c_void_p, C.c_void_p, C.c_int]
+    e.emul_text.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]
     e.emul_sbs1_ids.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+    e.emul_coverage.argtypes = [C.c_void_p, C.c_void_p]
+    e.emul_coverage_records.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+    e.emul_reports_state.argtypes = [C.c_void_p]
+    e.simt_launch_count.restype = C.c_ulonglong
     return e
 
 

@@ -1,20 +1,16 @@
 // TEST HARNESS (not a product path): runs the decoder's kernel source - gr_air_modes_b200/csrc/amb_decode_kernels.cuh
-// and the stage headers it includes - on the host under tests/simt/simt_emul.h, with the decoder's own state and launch
-// sequence: amb_decode_prepare allocates what the stages that are on need (host memory here), amb_decode_launch enqueues
-// fields, pairing, resolve and every stage that is on, and amb_decode_reset / amb_decode_free are what
-// amb_decoder_reset / amb_decoder_destroy run. The tests/test_*_simt.py modules build it with plain g++ and bind it
-// through tests/emul_build.py.
+// and the stage headers it includes - on the host under tests/simt/simt_emul.h, with the decoder's own state, options,
+// launch sequence and read-outs: amb_decode_set_option / amb_decode_set_location set what amb_decoder_set_option /
+// amb_decoder_set_location set, amb_decode_prepare allocates what the stages that are on need (host memory here),
+// amb_decode_launch enqueues fields, pairing, resolve and every stage that is on, amb_decode_text, amb_decode_snapshot_*
+// and amb_decode_coverage read the results out, and amb_decode_reset / amb_decode_free are what amb_decoder_reset /
+// amb_decoder_destroy run. The tests/test_*_simt.py modules build it with plain g++ and bind it through
+// tests/emul_build.py.
 #include "simt_emul.h"
 
 #include "../../gr_air_modes_b200/csrc/amb_decode_kernels.cuh"
 
 #include <algorithm>
-
-// The options of one decode, as amb_decoder_set_location and amb_decoder_set_option set them (emul_build.EmulOpts).
-struct EmulOpts {
-    int have_loc; double lat, lon;
-    int local_cpr, commb, opstatus, track, track_ext, sbs1, sbs1_tz;
-};
 
 struct Emul {
     AmbDecodeState st;                                  // kept across calls, like the decoder's
@@ -44,9 +40,20 @@ extern "C" void emul_reset(void* h)
     amb_decode_reset(&static_cast<Emul*>(h)->st, nullptr, &err);
 }
 
+// amb_decoder_set_option, from the next emul_decode on: returns 0, or -1 when the setting is refused
+extern "C" int emul_set_option(void* h, const char* name, int value)
+{
+    return amb_decode_set_option(&static_cast<Emul*>(h)->st, name, value) ? -1 : 0;
+}
+
+extern "C" void emul_set_location(void* h, int have_location, double lat, double lon)
+{
+    amb_decode_set_location(&static_cast<Emul*>(h)->st, have_location, lat, lon);
+}
+
 // amb_decode_frames: returns 0, -1 when a position squitter's address does not fit the test's tables, -2 when a stage
 // fails to launch, -3 when the stages' memory cannot be had
-extern "C" int emul_decode(void* h, const amb_frame* frames, int n, const EmulOpts* o, amb_fields* out)
+extern "C" int emul_decode(void* h, const amb_frame* frames, int n, amb_fields* out)
 {
     AmbDecodeState& st = static_cast<Emul*>(h)->st;
     if (n <= 0) return 0;
@@ -55,9 +62,6 @@ extern "C" int emul_decode(void* h, const amb_frame* frames, int n, const EmulOp
         amb_decode_fields(frames[k], &r, &p);
         if (p.key != AMB_NO_KEY && (((size_t)p.key << 1) | 1u) >= st.table_slots) return -1;   // test table too small
     }
-    st.have_loc = o->have_loc; st.lat = o->lat; st.lon = o->lon;
-    st.local_cpr = o->local_cpr; st.commb = o->commb; st.opstatus = o->opstatus; st.track = o->track;
-    st.track_ext = o->track_ext; st.sbs1 = o->sbs1; st.sbs1_tz = o->sbs1_tz;
     const bool had_rows = st.trows, had_xrows = st.xrows;
     cudaError_t err = cudaSuccess;
     if (amb_decode_prepare(&st, n, nullptr, &err) < 0) return -3;
@@ -77,36 +81,29 @@ extern "C" int emul_decode(void* h, const amb_frame* frames, int n, const EmulOp
 
 // amb_decoder_aircraft (ext == NULL) or amb_decoder_aircraft_ext over the first `words` bitmap words (a multiple of
 // AMB_SNAP_WORDS): out == NULL returns the count, too small a `max` -5.
-extern "C" int emul_snapshot(void* h, double now, int S, int S2, unsigned words, amb_aircraft* out, amb_aircraft_ext* ext,
-                             int max)
+extern "C" int emul_snapshot(void* h, double now, unsigned words, amb_aircraft* out, amb_aircraft_ext* ext, int max)
 {
     const AmbDecodeState& st = static_cast<Emul*>(h)->st;
     if (!st.tocc) return 0;                             // nothing decoded with the track stage on yet
-    const unsigned nb = words / AMB_SNAP_WORDS;
-    uint32_t* off = st.snap_cnt + nb;
     cudaError_t err = cudaSuccess;
-    if (amb_snap_count_launch(st.tocc, st.trows, st.tclk, now, S, words, st.snap_cnt, off, nullptr, &err) < 0) return -1;
-    const int total = (int)off[nb];
+    const int total = amb_decode_snapshot_count(&st, now, words, nullptr, &err);
+    if (total < 0) return -1;
     if (!out) return total;
     if (total > max) return -5;
     if (total == 0) return 0;
-    const int k = ext ? amb_snap_gather_ext_launch(st.tocc, st.trows, st.tclk, now, S, words, off, out, st.xocc, st.xrows,
-                                                   S2, ext, nullptr, &err)
-                      : amb_snap_gather_launch(st.tocc, st.trows, st.tclk, now, S, words, off, out, nullptr, &err);
-    return k < 0 ? -1 : total;
+    return amb_decode_snapshot_gather(&st, now, words, out, ext, nullptr, &err) < 0 ? -1 : total;
 }
 
-// amb_decoder_sbs1 after a decode of n frames with the option on: its packed lines into text; returns 0, or -5 when
-// they do not fit `cap` (*n_bytes = their length either way)
-extern "C" int emul_sbs1_text(void* h, int n, char* text, size_t cap, size_t* n_bytes)
+// amb_decoder_reports (reports = 1) or amb_decoder_sbs1 (0): the last decode's packed lines into text; returns 0, or -5
+// when they do not fit `cap` (*n_bytes = their length either way)
+extern "C" int emul_text(void* h, int reports, char* text, size_t cap, size_t* n_bytes)
 {
-    const AmbDecodeState& st = static_cast<Emul*>(h)->st;
-    *n_bytes = 0;
-    if (n <= 0) return 0;
-    const size_t total = (size_t)st.sb.boff[(n + 127) / 128];
-    *n_bytes = total;
+    const char* src = nullptr;
+    unsigned long long total = 0;
+    amb_decode_text(&static_cast<Emul*>(h)->st, reports != 0, nullptr, &src, &total);
+    *n_bytes = (size_t)total;
     if (total > cap) return -5;
-    memcpy(text, st.sb.text, total);
+    if (total) memcpy(text, src, total);
     return 0;
 }
 
@@ -118,4 +115,30 @@ extern "C" int emul_sbs1_ids(void* h, const amb_fields* recs, int n, unsigned lo
     for (int k = 0; k < n; k++)
         if (amb_sbs1_published(&recs[k])) ids[m++] = st.sb.gid[k] - st.sctr->base;
     return m;
+}
+
+// amb_decoder_coverage: the grid into out (AMB_COVERAGE_CELLS doubles); returns whether the grid is allocated
+extern "C" int emul_coverage(void* h, double* out)
+{
+    const AmbDecodeState& st = static_cast<Emul*>(h)->st;
+    amb_decode_coverage(&st, out, false, nullptr);
+    return st.cgrid != nullptr;
+}
+
+// the coverage stage alone (amb_coverage_launch) over n given records, into the decoder's grid (allocated by
+// amb_decode_prepare with the option on): for records whose range and bearing a test chooses; returns 0, or -2 / -3
+extern "C" int emul_coverage_records(void* h, const amb_fields* recs, int n)
+{
+    AmbDecodeState& st = static_cast<Emul*>(h)->st;
+    st.coverage = 1;
+    cudaError_t err = cudaSuccess;
+    if (amb_decode_prepare(&st, 0, nullptr, &err) < 0) return -3;
+    return amb_coverage_launch(recs, n, st.cgrid, nullptr, &err) < 0 ? -2 : 0;
+}
+
+// what the text-report stage holds: bit 0 its buffers, bit 1 its first-message flag, bit 2 the flag's value
+extern "C" int emul_reports_state(void* h)
+{
+    const AmbDecodeState& st = static_cast<Emul*>(h)->st;
+    return (st.rb.text ? 1 : 0) | (st.rfirst ? 2 : 0) | (st.rfirst && *st.rfirst ? 4 : 0);
 }

@@ -27,16 +27,16 @@ def _decode(e, frames, S, splits, local_S=0, track_S=0):
     """Records of the emulated decode cut at `splits` (S = 0: the option off)."""
     from gr_air_modes_b200 import decode
     n = len(frames)
-    opts = emul_build.opts(local_cpr=local_S, commb=S, track=track_S)
     h = e.emul_new(17)
     assert h
+    emul_build.opts(e, h, local_cpr=local_S, commb=S, track=track_S)
     recs = np.zeros(n, dtype=decode.FIELDS_DTYPE)
     pos = 0
     for c in list(splits) + [n]:
         c = min(c, n - pos)
         if c <= 0:
             break
-        assert e.emul_decode(h, C.c_void_p(frames.ctypes.data + 80 * pos), c, opts,
+        assert e.emul_decode(h, C.c_void_p(frames.ctypes.data + 80 * pos), c,
                              C.c_void_p(recs.ctypes.data + 144 * pos)) == 0
         pos += c
     e.emul_free(h)

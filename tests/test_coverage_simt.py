@@ -1,6 +1,6 @@
 """The coverage stage's KERNEL SOURCE (gr_air_modes_b200/csrc/amb_decode_coverage.cuh, enqueued by the decoder's own
 amb_decode_launch after the local CPR stage) on the host under the SIMT emulator (tests/simt/simt_emul.h), through the
-decoder harness tests/simt/decode_emul.cc (with the coverage accessors of tests/simt/decode_coverage_emul.cc), against the sequential checker (tests/coverage_oracle.py) fed with the
+decoder harness tests/simt/decode_emul.cc, against the sequential checker (tests/coverage_oracle.py) fed with the
 decoder's own records: the grid byte for byte after every call, for single messages, cuts at 31/32/33 and random sizes,
 with local_cpr on and off, across a reset; records chosen to fall all into one cell, onto every row edge and its
 neighbouring doubles, onto every band edge, and records that must not count. Four mutants must fail: a kernel that
@@ -8,7 +8,6 @@ updates only the record's own band, a row from rint, a row from a comparison aga
 grid."""
 import ctypes as C
 import os
-import shutil
 import sys
 
 import numpy as np
@@ -22,42 +21,20 @@ import track_cases as tc  # noqa: E402
 
 LOC = (47.9, 11.1)
 KERNEL = "gr_air_modes_b200/csrc/amb_decode_coverage.cuh"
-HARNESS = os.path.join("tests", "simt", "decode_coverage_emul.cc")
-
-
-def _bind(tmp_path_factory, src):
-    """The decoder harness built from `src` (tests/simt/decode_coverage_emul.cc or a patched copy) and bound: the
-    entry points of tests/emul_build.decode_emul plus the coverage accessors."""
-    e = emul_build.decode_emul(tmp_path_factory, src)
-    e.emul_set_coverage.argtypes = [C.c_void_p, C.c_int]
-    e.emul_coverage.argtypes = [C.c_void_p, C.c_void_p]
-    e.emul_coverage_records.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
-    return e
-
-
-def _mutant(tmp_path, tmp_path_factory, rel, old, new):
-    """The harness built from a copy of the sources under tmp_path in which the text `old`, which must occur exactly
-    once in the file `rel`, reads `new`."""
-    for sub in ("gr_air_modes_b200/csrc", "include", "tests/simt"):
-        shutil.copytree(os.path.join(emul_build.ROOT, sub), str(tmp_path / sub))
-    p = tmp_path / rel
-    src = p.read_text()
-    assert src.count(old) == 1, old
-    p.write_text(src.replace(old, new))
-    return _bind(tmp_path_factory, tmp_path / HARNESS)
 
 
 @pytest.fixture(scope="module")
 def emul(tmp_path_factory):
-    return _bind(tmp_path_factory, os.path.join(emul_build.ROOT, HARNESS))
+    return emul_build.decode_emul(tmp_path_factory)
 
 
-def _decode(e, h, frames, opts, coverage):
-    """emul_decode of `frames` with the options `opts` and option coverage = `coverage`; returns the records."""
+def _decode(e, h, frames, loc, coverage, **stages):
+    """emul_decode of `frames` with the receiver at `loc`, option coverage = `coverage` and the other options `stages`;
+    returns the records."""
     from gr_air_modes_b200 import decode
     recs = np.zeros(len(frames), dtype=decode.FIELDS_DTYPE)
-    e.emul_set_coverage(h, coverage)
-    assert e.emul_decode(h, C.c_void_p(frames.ctypes.data), len(frames), opts, C.c_void_p(recs.ctypes.data)) == 0
+    emul_build.opts(e, h, loc, coverage=coverage, **stages)
+    assert e.emul_decode(h, C.c_void_p(frames.ctypes.data), len(frames), C.c_void_p(recs.ctypes.data)) == 0
     return recs
 
 
@@ -76,7 +53,7 @@ def _run(e, calls, loc, local_S=0, resets=()):
         if i in resets:
             e.emul_reset(h)
             chk.reset()
-        recs = _decode(e, h, frames, emul_build.opts(loc, local_cpr=local_S), 1)
+        recs = _decode(e, h, frames, loc, 1, local_cpr=local_S)
         want = chk.feed(recs)
         assert _grid(e, h).tobytes() == want.tobytes(), i
     e.emul_free(h)
@@ -185,7 +162,7 @@ def test_off_allocates_nothing_and_changes_no_record(emul):
     out = []
     for cov in (0, 1):
         h = emul.emul_new(17)
-        recs = _decode(emul, h, frames, emul_build.opts(loc, local_cpr=10, track=20), cov)
+        recs = _decode(emul, h, frames, loc, cov, local_cpr=10, track=20)
         assert emul.emul_coverage(h, C.c_void_p(np.zeros(648).ctypes.data)) == cov
         emul.emul_free(h)
         out.append(recs.tobytes())
@@ -210,24 +187,25 @@ def test_the_harness_itself_passes(emul):
 
 
 def test_a_kernel_updating_only_its_own_band_is_caught(tmp_path, tmp_path_factory):
-    e = _mutant(tmp_path, tmp_path_factory, KERNEL, "for (int j = row0; j <= i; j++)", "for (int j = i; j <= i; j++)")
+    e = emul_build.mutant(tmp_path, tmp_path_factory, KERNEL, "for (int j = row0; j <= i; j++)",
+                          "for (int j = i; j <= i; j++)")
     assert _caught(e)
 
 
 def test_a_row_from_rint_is_caught(tmp_path, tmp_path_factory):
-    e = _mutant(tmp_path, tmp_path_factory, KERNEL, "const long long t = (long long)(r.bearing + 2.5);",
-               "const long long t = (long long)rint(r.bearing / 5.0) * 5;")
+    e = emul_build.mutant(tmp_path, tmp_path_factory, KERNEL, "const long long t = (long long)(r.bearing + 2.5);",
+                          "const long long t = (long long)rint(r.bearing / 5.0) * 5;")
     assert _caught(e)
 
 
 def test_a_row_from_a_comparison_against_2_5_is_caught(tmp_path, tmp_path_factory):
-    e = _mutant(tmp_path, tmp_path_factory, KERNEL, "const long long t = (long long)(r.bearing + 2.5);",
-               "const long long f5 = (long long)r.bearing - (long long)r.bearing % 5; "
-               "const long long t = f5 + (r.bearing - (double)f5 >= 2.5 ? 5 : 0);")
+    e = emul_build.mutant(tmp_path, tmp_path_factory, KERNEL, "const long long t = (long long)(r.bearing + 2.5);",
+                          "const long long f5 = (long long)r.bearing - (long long)r.bearing % 5; "
+                          "const long long t = f5 + (r.bearing - (double)f5 >= 2.5 ? 5 : 0);")
     assert _caught(e)
 
 
 def test_a_reset_that_leaves_the_grid_is_caught(tmp_path, tmp_path_factory):
-    e = _mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_kernels.cuh",
-               "    if (st->cgrid)\n", "    if (false)\n")
+    e = emul_build.mutant(tmp_path, tmp_path_factory, "gr_air_modes_b200/csrc/amb_decode_kernels.cuh",
+                          "    if (st->cgrid)\n", "    if (false)\n")
     assert _caught(e)

@@ -112,8 +112,8 @@ def test_commb_ties_under_the_emulated_decoder(tmp_path_factory):
     for S in (0, 30):
         h = e.emul_new(17)
         recs = np.zeros(len(frames), dtype=decode.FIELDS_DTYPE)
-        assert e.emul_decode(h, C.c_void_p(frames.ctypes.data), len(frames), emul_build.opts(commb=S),
-                             C.c_void_p(recs.ctypes.data)) == 0
+        emul_build.opts(e, h, commb=S)
+        assert e.emul_decode(h, C.c_void_p(frames.ctypes.data), len(frames), C.c_void_p(recs.ctypes.data)) == 0
         e.emul_free(h)
         out[S] = recs
     py, _ = cpython_velocities(msgs, out[0])

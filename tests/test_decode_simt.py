@@ -54,8 +54,8 @@ def _traffic(n, seed, n_aircraft):
 def _run(e, s, arr, n, splits, loc):
     from gr_air_modes_b200 import decode
     have, lat, lon = (0, 0.0, 0.0) if loc is None else (1, loc[0], loc[1])
-    opts = emul_build.opts(loc)
     he, hs = e.emul_new(17), s.shim_new()
+    emul_build.opts(e, he, loc)
     got = np.zeros(n, dtype=decode.FIELDS_DTYPE)
     want = np.zeros(n, dtype=decode.FIELDS_DTYPE)
     base = C.addressof(arr)
@@ -65,7 +65,7 @@ def _run(e, s, arr, n, splits, loc):
         if c <= 0:
             break
         fr = C.c_void_p(base + 80 * pos)
-        assert e.emul_decode(he, fr, c, opts, C.c_void_p(got.ctypes.data + 144 * pos)) == 0
+        assert e.emul_decode(he, fr, c, C.c_void_p(got.ctypes.data + 144 * pos)) == 0
         s.shim_step(hs, fr, c, have, lat, lon, C.c_void_p(want.ctypes.data + 144 * pos))
         pos += c
     e.emul_free(he)

@@ -32,8 +32,8 @@ def _run(e, s, msgs, loc, S, splits):
     from gr_air_modes_b200 import decode
     arr, n = decode.frames_from_messages(msgs)
     have, lat, lon = (0, 0.0, 0.0) if loc is None else (1, loc[0], loc[1])
-    opts = emul_build.opts(loc, local_cpr=S)
     he = e.emul_new(17)
+    emul_build.opts(e, he, loc, local_cpr=S)
     hs = s.shim_local_new() if s is not None else None
     got = np.zeros(n, dtype=decode.FIELDS_DTYPE)
     want = np.zeros(n, dtype=decode.FIELDS_DTYPE)
@@ -43,7 +43,7 @@ def _run(e, s, msgs, loc, S, splits):
         if c <= 0:
             break
         fr = C.c_void_p(base + 80 * pos)
-        assert e.emul_decode(he, fr, c, opts, C.c_void_p(got.ctypes.data + 144 * pos)) == 0
+        assert e.emul_decode(he, fr, c, C.c_void_p(got.ctypes.data + 144 * pos)) == 0
         if hs is not None:
             s.shim_local_step(hs, fr, c, have, lat, lon, S, C.c_void_p(want.ctypes.data + 144 * pos))
         pos += c

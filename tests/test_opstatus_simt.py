@@ -27,17 +27,17 @@ def _decode(e, frames, S, splits, others=(0, 0, 0)):
     """Records of the emulated decode cut at `splits` (S = 0: the option off); others = local_cpr, commb, track S."""
     from gr_air_modes_b200 import decode
     local_S, commb_S, track_S = others
-    opts = emul_build.opts(local_cpr=local_S, commb=commb_S, opstatus=S, track=track_S)
     n = len(frames)
     h = e.emul_new(17)
     assert h
+    emul_build.opts(e, h, local_cpr=local_S, commb=commb_S, opstatus=S, track=track_S)
     recs = np.zeros(n, dtype=decode.FIELDS_DTYPE)
     pos = 0
     for c in list(splits) + [n]:
         c = min(c, n - pos)
         if c <= 0:
             break
-        assert e.emul_decode(h, C.c_void_p(frames.ctypes.data + 80 * pos), c, opts,
+        assert e.emul_decode(h, C.c_void_p(frames.ctypes.data + 80 * pos), c,
                              C.c_void_p(recs.ctypes.data + 144 * pos)) == 0
         pos += c
     e.emul_free(h)

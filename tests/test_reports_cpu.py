@@ -259,11 +259,11 @@ def test_lines_of_the_comm_b_op_status_and_local_cpr_cases(shim, tmp_path_factor
     kinds, local_lines = set(), 0
     for name, fr, stages in scenes:
         stages = dict(stages)
-        o = emul_build.opts(stages.pop("loc", None), **stages)
         h = e.emul_new(17)
         try:
+            emul_build.opts(e, h, stages.pop("loc", None), **stages)
             recs = np.zeros(len(fr), dtype=decode.FIELDS_DTYPE)
-            assert e.emul_decode(h, C.c_void_p(fr.ctypes.data), len(fr), o, C.c_void_p(recs.ctypes.data)) == 0
+            assert e.emul_decode(h, C.c_void_p(fr.ctypes.data), len(fr), C.c_void_p(recs.ctypes.data)) == 0
         finally:
             e.emul_free(h)
         text, first = [], True

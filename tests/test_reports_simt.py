@@ -1,6 +1,6 @@
 """The text-report stage's KERNEL SOURCE (gr_air_modes_b200/csrc/amb_decode_reports.cuh, enqueued last by the decoder's
 own amb_decode_launch) on the host under the SIMT emulator (tests/simt/simt_emul.h), through the decoder harness
-tests/simt/decode_emul.cc with the accessors of tests/simt/decode_reports_emul.cc: the packed text of every call byte
+tests/simt/decode_emul.cc: the packed text of every call byte
 for byte against report.format_report of the slicer's text of each frame and the decoder's own record, for single
 messages, cuts at 31/32/33 and random splits, with the other stages on and off, the first-message flag across calls,
 after a reset and with the option turned on mid-stream, a call of nothing but the longest lines, and every scene of
@@ -22,22 +22,10 @@ import emul_build  # noqa: E402
 import reports_cases as rc  # noqa: E402
 from helpers import load_decode_golden  # noqa: E402
 
-HARNESS = os.path.join("tests", "simt", "decode_reports_emul.cc")
-
-
-def _bind(tmp_path_factory, src):
-    e = emul_build.decode_emul(tmp_path_factory, src)
-    e.emul_set_reports.argtypes = [C.c_void_p, C.c_int]
-    e.emul_report_text.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]
-    e.emul_reports_state.argtypes = [C.c_void_p]
-    e.emul_set_coverage.argtypes = [C.c_void_p, C.c_int]
-    e.simt_launch_count.restype = C.c_ulonglong
-    return e
-
 
 @pytest.fixture(scope="module")
 def emul(tmp_path_factory):
-    return _bind(tmp_path_factory, os.path.join(emul_build.ROOT, HARNESS))
+    return emul_build.decode_emul(tmp_path_factory)
 
 
 def _scenes():
@@ -83,32 +71,32 @@ def _tcas_frames(n):
     return np.frombuffer(bytes(arr), dtype=decode.FRAME_DTYPE, count=m).copy()
 
 
-def _run(e, h, frames, opts, reports=1):
-    """One emulated decode; returns (records, the call's text or None when the option is off)."""
+def _run(e, h, frames, loc=None, reports=1, **stages):
+    """One emulated decode with the receiver at `loc`, option reports = `reports` and the other options `stages`;
+    returns (records, the call's text or None when the option is off)."""
     from gr_air_modes_b200 import decode
     recs = np.zeros(len(frames), dtype=decode.FIELDS_DTYPE)
-    e.emul_set_reports(h, reports)
-    assert e.emul_decode(h, C.c_void_p(frames.ctypes.data), len(frames), opts, C.c_void_p(recs.ctypes.data)) == 0
+    emul_build.opts(e, h, loc, reports=reports, **stages)
+    assert e.emul_decode(h, C.c_void_p(frames.ctypes.data), len(frames), C.c_void_p(recs.ctypes.data)) == 0
     if not reports:
         return recs, None
     n = C.c_size_t()
     buf = C.create_string_buffer(len(frames) * 480 + 1)
-    assert e.emul_report_text(h, len(frames), buf, len(buf), C.byref(n)) == 0
+    assert e.emul_text(h, 1, buf, len(buf), C.byref(n)) == 0
     return recs, buf.raw[: n.value]
 
 
-def _check_stream(e, frames, loc, cuts, opts=None, log2=17):
+def _check_stream(e, frames, loc, cuts, log2=17, **stages):
     """The stream cut at `cuts`, one call per piece: each call's text equals the expected text of its frames and
     records, the first call's first queued frame at precision 6."""
     h = e.emul_new(log2)
     try:
-        o = opts if opts is not None else emul_build.opts(loc)
         first = True
         for a, b in zip([0] + list(cuts), list(cuts) + [len(frames)]):
             if a == b:
                 continue
             part = np.ascontiguousarray(frames[a:b])
-            recs, text = _run(e, h, part, o)
+            recs, text = _run(e, h, part, loc, **stages)
             want = rc.expected_text(part, recs, first)
             assert text == want, (a, b, text[:300], want[:300])
             first = first and not np.any((recs["status"] & 0x80) == 0)
@@ -146,7 +134,7 @@ def test_random_splits(emul):
 def test_with_other_stages_on(emul, stages):
     fr, loc = _scenes()[0]
     fr = _small(fr)[:500]
-    _check_stream(emul, fr, loc, [200], emul_build.opts(loc, **stages))
+    _check_stream(emul, fr, loc, [200], **stages)
 
 
 def test_stamps_and_first_level(emul):
@@ -157,33 +145,32 @@ def test_stamps_and_first_level(emul):
 def test_first_message_across_calls_reset_and_mid_stream(emul):
     from gr_air_modes_b200 import decode
     fr = _stamp_frames()[:30]
-    o = emul_build.opts(None)
     h = emul.emul_new(15)
     try:
         a, b, c = fr[:10].copy(), fr[10:20].copy(), fr[20:].copy()
         b["ref_level"][0] = c["ref_level"][0] = np.float32(9.999999)
         # unqueued frames before the first queued one leave the flag for it
         a["passed"][:3] = 0
-        recs, text = _run(emul, h, a, o)
+        recs, text = _run(emul, h, a)
         assert text == rc.expected_text(a, recs, True)
-        recs, text = _run(emul, h, b, o)
+        recs, text = _run(emul, h, b)
         assert text == rc.expected_text(b, recs, False) and text != rc.expected_text(b, recs, True)
         emul.emul_reset(h)
         assert emul.emul_reports_state(h) & 4
-        recs, text = _run(emul, h, b, o)
+        recs, text = _run(emul, h, b)
         assert text == rc.expected_text(b, recs, True)
         # off and on again: the count goes on
-        _run(emul, h, a, o, reports=0)
-        recs, text = _run(emul, h, c, o)
+        _run(emul, h, a, reports=0)
+        recs, text = _run(emul, h, c)
         assert text == rc.expected_text(c, recs, False)
     finally:
         emul.emul_free(h)
     # turned on mid-stream: its first call's first queued frame is the first
     h = emul.emul_new(15)
     try:
-        _run(emul, h, a, o, reports=0)
+        _run(emul, h, a, reports=0)
         assert emul.emul_reports_state(h) == 0                    # nothing allocated while off
-        recs, text = _run(emul, h, c, o)
+        recs, text = _run(emul, h, c)
         assert text == rc.expected_text(c, recs, True)
         assert decode.FS_NOT_QUEUED == 0x80
     finally:
@@ -195,7 +182,7 @@ def test_a_call_of_the_longest_lines(emul):
     fr = _tcas_frames(300)
     h = emul.emul_new(15)
     try:
-        recs, text = _run(emul, h, fr, emul_build.opts(None))
+        recs, text = _run(emul, h, fr)
         assert text == rc.expected_text(fr, recs, True)
         lines = text.split(b"\n")[:-1]
         assert len(lines) == 300 and min(map(len, lines)) > 400, len(lines[0])
@@ -208,21 +195,19 @@ def test_launch_count_and_no_allocation_while_off(emul):
     fr = _small(_scenes()[0][0])[:300]
     from gr_air_modes_b200 import decode
     recs = np.zeros(len(fr), dtype=decode.FIELDS_DTYPE)
-    for stages, coverage in ((dict(), 0), (dict(local_cpr=10, commb=30), 1), (dict(sbs1=1, track=60, opstatus=30), 1)):
-        o = emul_build.opts((37.4, -122.1), **stages)
+    for stages in (dict(), dict(local_cpr=10, commb=30, coverage=1), dict(sbs1=1, track=60, opstatus=30, coverage=1)):
         counts = []
         for on in (0, 1):
             h = emul.emul_new(17)
             try:
-                emul.emul_set_reports(h, on)
-                emul.emul_set_coverage(h, coverage)
+                emul_build.opts(emul, h, (37.4, -122.1), reports=on, **stages)
                 k0 = emul.simt_launch_count()
-                assert emul.emul_decode(h, C.c_void_p(fr.ctypes.data), len(fr), o, C.c_void_p(recs.ctypes.data)) == 0
+                assert emul.emul_decode(h, C.c_void_p(fr.ctypes.data), len(fr), C.c_void_p(recs.ctypes.data)) == 0
                 counts.append(emul.simt_launch_count() - k0)
                 assert (emul.emul_reports_state(h) != 0) == bool(on)
             finally:
                 emul.emul_free(h)
-        assert counts[1] == counts[0] + 3, (stages, coverage, counts)
+        assert counts[1] == counts[0] + 3, (stages, counts)
 
 
 def _check_option_scenes(e):
@@ -230,7 +215,6 @@ def _check_option_scenes(e):
     their texts hold."""
     kinds = set()
     for name, fr, stages in rc.text_option_scenes(small=True):
-        o = emul_build.opts(None, **stages)
         n = len(fr)
         for cuts in ([], sorted({n // 3, min(n, n // 3 + 33)} - {0, n})):
             h = e.emul_new(17)
@@ -238,7 +222,7 @@ def _check_option_scenes(e):
                 first = True
                 for a, b in zip([0] + cuts, cuts + [n]):
                     part = np.ascontiguousarray(fr[a:b])
-                    recs, text = _run(e, h, part, o)
+                    recs, text = _run(e, h, part, **stages)
                     assert text == rc.expected_text(part, recs, first), (name, a, b)
                     first = first and not np.any((recs["status"] & 0x80) == 0)
                     kinds |= rc.line_kinds(text)
@@ -274,15 +258,7 @@ MUTANTS = [
 
 @pytest.mark.parametrize("which", range(len(MUTANTS)))
 def test_mutants_fail(tmp_path, tmp_path_factory, which):
-    rel, old, new = MUTANTS[which]
-    for sub in ("gr_air_modes_b200/csrc", "include", "tests/simt"):
-        import shutil
-        shutil.copytree(os.path.join(emul_build.ROOT, sub), str(tmp_path / sub))
-    p = tmp_path / rel
-    src = p.read_text()
-    assert src.count(old) == 1, old
-    p.write_text(src.replace(old, new))
-    e = _bind(tmp_path_factory, tmp_path / HARNESS)
+    e = emul_build.mutant(tmp_path, tmp_path_factory, *MUTANTS[which])
     fr, loc = _scenes()[0]
     with pytest.raises(AssertionError):
         _check_stream(e, _stamp_frames(), None, [])

@@ -35,10 +35,10 @@ def _call(e, h, frames, opts, tz, chk):
     buf = C.create_string_buffer(max(1, n * 192))
     nb = C.c_size_t()
     local_S, commb_S, opstatus_S, track_S = opts
-    o = emul_build.opts(LOC, local_cpr=local_S, commb=commb_S, opstatus=opstatus_S, track=track_S,
-                        track_ext=20 if track_S else 0, sbs1=1, sbs1_tz=tz)
-    assert e.emul_decode(h, C.c_void_p(frames.ctypes.data), n, o, C.c_void_p(recs.ctypes.data)) == 0
-    assert e.emul_sbs1_text(h, n, buf, len(buf), C.byref(nb)) == 0
+    emul_build.opts(e, h, LOC, local_cpr=local_S, commb=commb_S, opstatus=opstatus_S, track=track_S,
+                    track_ext=20 if track_S else 0, sbs1=1, sbs1_tz=tz)
+    assert e.emul_decode(h, C.c_void_p(frames.ctypes.data), n, C.c_void_p(recs.ctypes.data)) == 0
+    assert e.emul_text(h, 0, buf, len(buf), C.byref(nb)) == 0
     want_ids = []
     want = chk.feed(frames, recs, want_ids)
     got = buf.raw[: nb.value]

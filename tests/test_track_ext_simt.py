@@ -37,25 +37,25 @@ def _words(frames):
     return (top // 32 // 1024 + 1) * 1024
 
 
-def _snapshot(e, h, now, S, S2, words):
+def _snapshot(e, h, now, words):
     from gr_air_modes_b200 import decode
     now = math.nan if now is None else now
-    n = e.emul_snapshot(h, now, S, S2, words, None, None, 0)
+    n = e.emul_snapshot(h, now, words, None, None, 0)
     assert n >= 0
     out = np.zeros(n, dtype=decode.AIRCRAFT_DTYPE)
     ext = np.zeros(n, dtype=decode.AIRCRAFT_EXT_DTYPE)
     if n:
-        assert e.emul_snapshot(h, now, S, S2, words, C.c_void_p(out.ctypes.data), C.c_void_p(ext.ctypes.data),
+        assert e.emul_snapshot(h, now, words, C.c_void_p(out.ctypes.data), C.c_void_p(ext.ctypes.data),
                                n - 1) == -5
         assert not ext.view(np.uint8).any()
-        assert e.emul_snapshot(h, now, S, S2, words, C.c_void_p(out.ctypes.data), C.c_void_p(ext.ctypes.data),
+        assert e.emul_snapshot(h, now, words, C.c_void_p(out.ctypes.data), C.c_void_p(ext.ctypes.data),
                                n) == n
     return out, ext
 
 
 def _decode(e, h, frames, local_S, S, S2, recs):
-    opts = emul_build.opts(local_cpr=local_S, commb=COMMB_S, opstatus=OPSTATUS_S, track=S, track_ext=S2)
-    assert e.emul_decode(h, C.c_void_p(frames.ctypes.data), len(frames), opts, C.c_void_p(recs.ctypes.data)) == 0
+    emul_build.opts(e, h, local_cpr=local_S, commb=COMMB_S, opstatus=OPSTATUS_S, track=S, track_ext=S2)
+    assert e.emul_decode(h, C.c_void_p(frames.ctypes.data), len(frames), C.c_void_p(recs.ctypes.data)) == 0
 
 
 def _run(e, msgs, S, S2, splits, local_S=0, each=False):
@@ -78,13 +78,13 @@ def _run(e, msgs, S, S2, splits, local_S=0, each=False):
         _decode(e, h, frames[pos:pos + c], local_S, S, S2, recs)
         chk.feed(frames[pos:pos + c], recs)
         if each:
-            xo.assert_snapshots_equal(_snapshot(e, h, None, S, S2, words), chk.snapshot_arrays(), ("batch at", pos))
+            xo.assert_snapshots_equal(_snapshot(e, h, None, words), chk.snapshot_arrays(), ("batch at", pos))
         pos += c
     ts = [float(s) + float(f) for s, f in zip(frames["secs"], frames["frac"])]
-    final = _snapshot(e, h, None, S, S2, words)
+    final = _snapshot(e, h, None, words)
     xo.assert_snapshots_equal(final, chk.snapshot_arrays(), "end")
     for now in (ts[n // 2], ts[-1] + S2 / 2):
-        xo.assert_snapshots_equal(_snapshot(e, h, now, S, S2, words), chk.snapshot_arrays(now), ("now", now))
+        xo.assert_snapshots_equal(_snapshot(e, h, now, words), chk.snapshot_arrays(now), ("now", now))
     e.emul_free(h)
     return final
 
@@ -141,7 +141,7 @@ def test_a_group_exactly_S2_old_is_shown_and_one_2_to_the_minus_40_older_is_not(
     h = emul.emul_new(17)
     recs = np.zeros(len(frames), dtype=decode.FIELDS_DTYPE)
     _decode(emul, h, frames, 0, 60, 30, recs)
-    rows, ext = _snapshot(emul, h, now, 60, 30, 1024)
+    rows, ext = _snapshot(emul, h, now, 1024)
     emul.emul_free(h)
     xo.assert_snapshots_equal((rows, ext), xo.replay(frames, recs, 60, 30, now), "age edge")
     assert len(rows) == 1
@@ -168,12 +168,12 @@ def _reset_run(e, S=60, S2=600):
         if reset:
             e.emul_reset(h)
             chk.reset()
-            assert e.emul_snapshot(h, math.nan, S, S2, 1024, None, None, 0) == 0
+            assert e.emul_snapshot(h, math.nan, 1024, None, None, 0) == 0
         recs = np.zeros(len(fr), dtype=decode.FIELDS_DTYPE)
         _decode(e, h, fr, 0, S, S2, recs)
         chk.feed(fr, recs)
     for now in (None, 1003.0, 1010.0):                      # at 1003 and 1010 stream A's groups would be in range
-        got = _snapshot(e, h, now, S, S2, 1024)
+        got = _snapshot(e, h, now, 1024)
         xo.assert_snapshots_equal(got, chk.snapshot_arrays(now), ("after reset", now))
         assert len(got[0]) == 2 and not np.any(got[1]["shown"].astype(int) & ~AXG_INTEG)
     e.emul_free(h)

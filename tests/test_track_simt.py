@@ -27,16 +27,15 @@ def emul(tmp_path_factory):
     return emul_build.decode_emul(tmp_path_factory)
 
 
-def _snapshot(e, h, now, S):
+def _snapshot(e, h, now):
     from gr_air_modes_b200 import decode
-    n = e.emul_snapshot(h, math.nan if now is None else now, S, 0, WORDS, None, None, 0)
+    n = e.emul_snapshot(h, math.nan if now is None else now, WORDS, None, None, 0)
     assert n >= 0
     out = np.zeros(n, dtype=decode.AIRCRAFT_DTYPE)
     if n:
-        assert e.emul_snapshot(h, math.nan if now is None else now, S, 0, WORDS, C.c_void_p(out.ctypes.data), None,
+        assert e.emul_snapshot(h, math.nan if now is None else now, WORDS, C.c_void_p(out.ctypes.data), None,
                                n - 1) == -5
-        assert e.emul_snapshot(h, math.nan if now is None else now, S, 0, WORDS, C.c_void_p(out.ctypes.data), None,
-                               n) == n
+        assert e.emul_snapshot(h, math.nan if now is None else now, WORDS, C.c_void_p(out.ctypes.data), None, n) == n
     return out
 
 
@@ -46,9 +45,9 @@ def _run(e, msgs, loc, S, splits, local_S=0, each=False, commb_S=0):
     from gr_air_modes_b200 import decode
     frames = tc.frames_of(msgs)
     n = len(frames)
-    opts = emul_build.opts(loc, local_cpr=local_S, commb=commb_S, track=S)
     h = e.emul_new(17)
     assert h
+    emul_build.opts(e, h, loc, local_cpr=local_S, commb=commb_S, track=S)
     tr = to.Tracker(S)
     recs = np.zeros(n, dtype=decode.FIELDS_DTYPE)
     pos = 0
@@ -56,20 +55,20 @@ def _run(e, msgs, loc, S, splits, local_S=0, each=False, commb_S=0):
         c = min(c, n - pos)
         if c <= 0:
             break
-        assert e.emul_decode(h, C.c_void_p(frames.ctypes.data + 80 * pos), c, opts,
+        assert e.emul_decode(h, C.c_void_p(frames.ctypes.data + 80 * pos), c,
                              C.c_void_p(recs.ctypes.data + 144 * pos)) == 0
         tr.feed(frames[pos:pos + c], recs[pos:pos + c])
         if each:
-            to.assert_rows_equal(_snapshot(e, h, None, S), tr.snapshot_array(), ("batch at", pos))
+            to.assert_rows_equal(_snapshot(e, h, None), tr.snapshot_array(), ("batch at", pos))
         pos += c
     ts = to.t_of(frames)
-    final = _snapshot(e, h, None, S)
+    final = _snapshot(e, h, None)
     to.assert_rows_equal(final, tr.snapshot_array(), "end")
     for now in (ts[n // 2], ts[-1] + S / 2):
-        to.assert_rows_equal(_snapshot(e, h, now, S), tr.snapshot_array(now), ("now", now))
+        to.assert_rows_equal(_snapshot(e, h, now), tr.snapshot_array(now), ("now", now))
     e.emul_reset(h)
-    assert e.emul_snapshot(h, math.nan, S, 0, WORDS, None, None, 0) == 0
-    assert e.emul_snapshot(h, ts[-1], S, 0, WORDS, None, None, 0) == 0
+    assert e.emul_snapshot(h, math.nan, WORDS, None, None, 0) == 0
+    assert e.emul_snapshot(h, ts[-1], WORDS, None, None, 0) == 0
     e.emul_free(h)
     return final, recs
 
