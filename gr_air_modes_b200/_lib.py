@@ -251,6 +251,10 @@ SYMBOLS = [
     ("amb_decoder_sbs1_device", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("amb_decoder_reports", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("amb_decoder_reports_device", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("amb_decoder_beast", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("amb_decoder_beast_device", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("amb_decoder_avr", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("amb_decoder_avr_device", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("amb_decoder_coverage", C.c_int, [_vp, _vp]),
     ("amb_decoder_coverage_device", C.c_int, [_vp, _vp]),
     ("amb_decoder_coverage_reset", C.c_int, [_vp]),

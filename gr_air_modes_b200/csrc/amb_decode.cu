@@ -39,6 +39,9 @@
 // With option "reports" on, three more after those (amb_decode_reports.cuh): amb_reports_len, amb_sbs1_scan,
 // amb_reports_write - the call's text reports, the lines of report.py, packed on the device; amb_decoder_reports copies
 // them out.
+// With option "beast" on, three more after those (amb_decode_beast.cuh): amb_feed_len, amb_sbs1_scan, amb_feed_write -
+// the call's Beast binary messages, packed on the device; amb_decoder_beast copies them out. With option "avr" on, the
+// same three kernels once more for the AVR raw lines; amb_decoder_avr copies them out.
 // The multilateration object amb_mlat (amb_mlat.cuh) lives here too: its C ABI is at the end of this file.
 #include "amb_launch.h"
 #include "amb_decode_core.h"
@@ -237,7 +240,8 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
 {
     if (!d || n < 0 || (n > 0 && (!frames || !out)) || (mem_kind != AMB_MEM_HOST && mem_kind != AMB_MEM_DEVICE))
         return fail(d, AMB_ERR_INVALID, "amb_decode_frames: bad argument");
-    d->st.sbs1_nb = d->st.reports_nb = -1;              // until amb_decode_launch has launched every stage
+    d->st.sbs1_nb = d->st.reports_nb = d->st.beast_nb = d->st.avr_nb = -1;   // until amb_decode_launch has launched
+                                                                             // every stage
     if (n == 0) return AMB_OK;
     CK(d, cudaSetDevice(d->device));
     int rc = prepare(d, n);
@@ -338,23 +342,30 @@ int amb_decoder_aircraft_ext_device(amb_decoder* d, double now, amb_aircraft* ou
     return snapshot_impl(d, now, out_dev, ext_dev, cap, true, true);
 }
 
-// amb_decoder_sbs1(_device), and amb_decoder_reports(_device) when `reports`: the last decode's lines into out (host or
-// device memory)
-static int text_impl(amb_decoder* d, bool reports, char* out, size_t cap, size_t* n_bytes, bool out_on_device)
+// amb_decoder_sbs1(_device), amb_decoder_reports(_device), amb_decoder_beast(_device) and amb_decoder_avr(_device), by
+// kind (AMB_TEXT_*): the last decode's output into out (host or device memory)
+static int text_impl(amb_decoder* d, int kind, char* out, size_t cap, size_t* n_bytes, bool out_on_device)
 {
-    const char* fn = !reports ? "amb_decoder_sbs1" : out_on_device ? "amb_decoder_reports_device" : "amb_decoder_reports";
+    static const struct { const char* option; const char* fn; const char* fn_device; } kinds[] = {
+        {"sbs1", "amb_decoder_sbs1", "amb_decoder_sbs1"},
+        {"reports", "amb_decoder_reports", "amb_decoder_reports_device"},
+        {"beast", "amb_decoder_beast", "amb_decoder_beast_device"},
+        {"avr", "amb_decoder_avr", "amb_decoder_avr_device"},
+    };
+    const int on[] = {d ? d->st.sbs1 : 0, d ? d->st.reports : 0, d ? d->st.beast : 0, d ? d->st.avr : 0};
+    const char* fn = out_on_device ? kinds[kind].fn_device : kinds[kind].fn;
     char what[96];
     if (!d || !n_bytes || (cap > 0 && !out)) { snprintf(what, sizeof what, "%s: bad argument", fn); return fail(d, AMB_ERR_INVALID, what); }
     *n_bytes = 0;
-    if ((reports ? d->st.reports : d->st.sbs1) <= 0) {
-        snprintf(what, sizeof what, "%s: option %s is off", fn, reports ? "reports" : "sbs1");
+    if (on[kind] <= 0) {
+        snprintf(what, sizeof what, "%s: option %s is off", fn, kinds[kind].option);
         return fail(d, AMB_ERR_STATE, what);
     }
     CK(d, cudaSetDevice(d->device));
     cudaStream_t s = d->stream;
     const char* text = nullptr;
     unsigned long long total = 0;
-    CK(d, amb_decode_text(&d->st, reports, s, &text, &total));
+    CK(d, amb_decode_text(&d->st, kind, s, &text, &total));
     *n_bytes = (size_t)total;
     if (total > cap) { snprintf(what, sizeof what, "%s: output buffer too small", fn); return fail(d, AMB_ERR_OVERFLOW, what); }
     if (total == 0) return AMB_OK;
@@ -369,22 +380,42 @@ static int text_impl(amb_decoder* d, bool reports, char* out, size_t cap, size_t
 
 int amb_decoder_sbs1(amb_decoder* d, char* out, size_t cap, size_t* n_bytes)
 {
-    return text_impl(d, false, out, cap, n_bytes, false);
+    return text_impl(d, AMB_TEXT_SBS1, out, cap, n_bytes, false);
 }
 
 int amb_decoder_sbs1_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes)
 {
-    return text_impl(d, false, out_dev, cap, n_bytes, true);
+    return text_impl(d, AMB_TEXT_SBS1, out_dev, cap, n_bytes, true);
 }
 
 int amb_decoder_reports(amb_decoder* d, char* out, size_t cap, size_t* n_bytes)
 {
-    return text_impl(d, true, out, cap, n_bytes, false);
+    return text_impl(d, AMB_TEXT_REPORTS, out, cap, n_bytes, false);
 }
 
 int amb_decoder_reports_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes)
 {
-    return text_impl(d, true, out_dev, cap, n_bytes, true);
+    return text_impl(d, AMB_TEXT_REPORTS, out_dev, cap, n_bytes, true);
+}
+
+int amb_decoder_beast(amb_decoder* d, char* out, size_t cap, size_t* n_bytes)
+{
+    return text_impl(d, AMB_TEXT_BEAST, out, cap, n_bytes, false);
+}
+
+int amb_decoder_beast_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes)
+{
+    return text_impl(d, AMB_TEXT_BEAST, out_dev, cap, n_bytes, true);
+}
+
+int amb_decoder_avr(amb_decoder* d, char* out, size_t cap, size_t* n_bytes)
+{
+    return text_impl(d, AMB_TEXT_AVR, out, cap, n_bytes, false);
+}
+
+int amb_decoder_avr_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes)
+{
+    return text_impl(d, AMB_TEXT_AVR, out_dev, cap, n_bytes, true);
 }
 
 // the coverage grid into out (host or device memory)

@@ -55,6 +55,7 @@ __global__ void __launch_bounds__(128) amb_resolve_kernel(amb_fields* __restrict
 #include "amb_decode_sbs1.cuh"
 #include "amb_decode_coverage.cuh"
 #include "amb_decode_reports.cuh"
+#include "amb_decode_beast.cuh"
 
 // ---- state and launch sequence ------------------------------------------------------------------------------------
 // What the stages of one decode read and write besides the frames and the records, and the one owner of that memory:
@@ -96,9 +97,16 @@ struct AmbDecodeState {
     unsigned* rfirst = nullptr;          // 1 until the first queued frame since creation or reset has been formatted
     AmbReportBufs rb;                    // the stage's per-call scratch and the packed lines
     int rcap = 0;                        // frames rb holds
+    int beast = 0;                       // option "beast": 1 = on, 0 = off
+    AmbReportBufs bb;                    // the Beast feed's per-call scratch and packed messages
+    int bcap = 0;                        // frames bb holds
+    int avr = 0;                         // option "avr": 1 = "*" lines, 2 = "@" lines with the timestamp, 0 = off
+    AmbReportBufs ab;                    // the AVR feed's per-call scratch and packed lines
+    int acap = 0;                        // frames ab holds
     int sbs1_nb = -1;                    // blocks of lines of the last decode (its byte total is sb.boff[sbs1_nb]);
                                          // -1: the last decode wrote no lines
     int reports_nb = -1;                 // the same for the text reports (rb.boff[reports_nb])
+    int beast_nb = -1, avr_nb = -1;      // the same for the Beast messages (bb.boff[beast_nb]) and AVR lines (ab.boff)
     int have_loc = 0; double lat = 0.0, lon = 0.0;      // receiver location
 };
 
@@ -115,6 +123,8 @@ static const struct {
     {"sbs1_tz", &AmbDecodeState::sbs1_tz, AMB_SBS1_TZ_MIN, AMB_SBS1_TZ_MAX, "sbs1_tz: -720 .. 840 minutes"},
     {"coverage", &AmbDecodeState::coverage, 0, 1, "coverage: 0 (off) or 1 (on)"},
     {"reports", &AmbDecodeState::reports, 0, 1, "reports: 0 (off) or 1 (on)"},
+    {"beast", &AmbDecodeState::beast, 0, 1, "beast: 0 (off) or 1 (on)"},
+    {"avr", &AmbDecodeState::avr, 0, 2, "avr: 0 (off), 1 (* lines) or 2 (@ lines with the timestamp)"},
 };
 
 // Set option `name` of st to `value`, from the next decode on. Returns NULL, or why the setting is refused.
@@ -138,7 +148,7 @@ static void amb_decode_set_location(AmbDecodeState* st, int have_location, doubl
 enum { AMB_STAGE_FIELDS = -1, AMB_STAGE_PAIRING = -2, AMB_STAGE_RESOLVE = -3, AMB_STAGE_LOCAL = -4,
        AMB_STAGE_COMMB = -5, AMB_STAGE_TRACK = -6, AMB_STAGE_OPSTATUS = -7, AMB_STAGE_TRACK_EXT = -8,
        AMB_STAGE_SBS1 = -9, AMB_STAGE_COVERAGE = -10,
-       AMB_STAGE_REPORTS = -11 };
+       AMB_STAGE_REPORTS = -11, AMB_STAGE_BEAST = -12, AMB_STAGE_AVR = -13 };
 
 // By -AMB_STAGE_* - 1: what a failed launch of the stage reports, and what a failure of its memory reports.
 static const struct { const char* launch; const char* memory; } amb_stage_names[] = {
@@ -153,6 +163,8 @@ static const struct { const char* launch; const char* memory; } amb_stage_names[
     {"SBS-1 feed", "SBS-1 id table (128 MiB)"},
     {"coverage map", "coverage grid (5184 B)"},
     {"text reports", "text report buffers (478 B per frame)"},
+    {"Beast feed", "Beast feed buffers (44 B per frame)"},
+    {"AVR feed", "AVR feed buffers (43 B per frame)"},
 };
 
 // cudaMalloc, then every byte set to `fill` unless it is < 0; *p is NULL after a failed cudaMalloc
@@ -177,6 +189,22 @@ static void amb_report_bufs_free(AmbReportBufs* b)
     *b = AmbReportBufs();
 }
 
+// (Re)allocate b for cap frames of at most `bytes` bytes of output each; *have = cap once it is all there.
+static cudaError_t amb_report_bufs_alloc(AmbReportBufs* b, int* have, int cap, size_t bytes, cudaStream_t s)
+{
+    amb_report_bufs_free(b);
+    *have = 0;
+    const size_t c = (size_t)cap, nb = (c + 127) / 128;
+    cudaError_t e;
+    if ((e = amb_decode_alloc(&b->len, c * sizeof(uint32_t), -1, s)) != cudaSuccess ||
+        (e = amb_decode_alloc(&b->bsum, nb * sizeof(uint32_t), -1, s)) != cudaSuccess ||
+        (e = amb_decode_alloc(&b->boff, (nb + 1) * sizeof(unsigned long long), -1, s)) != cudaSuccess ||
+        (e = amb_decode_alloc(&b->text, c * bytes, -1, s)) != cudaSuccess)
+        return e;
+    *have = cap;
+    return cudaSuccess;
+}
+
 #define AMB_STAGE_TRY(stage, call) do { if ((*err = (call)) != cudaSuccess) return (stage); } while (0)
 
 // Allocate on stream s what the stages that are on need for a decode of n frames (n = 0: only the pairing and NL
@@ -184,8 +212,8 @@ static void amb_report_bufs_free(AmbReportBufs* b)
 // once a stage that partitions them is on; each stage's table, bitmap, clock and counter at its first decode with the
 // option on, filled as an empty one (the track extension only while track is on too); the SBS-1 scratch as the frame
 // capacity grows; the coverage grid at the first decode with the option on; the text reports' first-message flag (set)
-// at the first decode with the option on, and their buffers as the frame capacity grows. Returns 0, or the AMB_STAGE_* code of the
-// stage whose memory could not be had, with *err set.
+// at the first decode with the option on, and their buffers as the frame capacity grows; the Beast and AVR feeds'
+// buffers likewise. Returns 0, or the AMB_STAGE_* code of the stage whose memory could not be had, with *err set.
 static int amb_decode_prepare(AmbDecodeState* st, int n, cudaStream_t s, cudaError_t* err)
 {
     if (!st->table) AMB_STAGE_TRY(AMB_STAGE_PAIRING, amb_decode_alloc(&st->table, st->table_slots * sizeof(AmbCprSlot), 0xFF, s));
@@ -264,18 +292,13 @@ static int amb_decode_prepare(AmbDecodeState* st, int n, cudaStream_t s, cudaErr
             AMB_STAGE_TRY(AMB_STAGE_REPORTS, amb_decode_alloc(&st->rfirst, sizeof one, -1, s));
             AMB_STAGE_TRY(AMB_STAGE_REPORTS, cudaMemcpyAsync(st->rfirst, &one, sizeof one, cudaMemcpyHostToDevice, s));
         }
-        if (st->rcap < st->cap) {
-            amb_report_bufs_free(&st->rb);
-            st->rcap = 0;
-            const size_t c = (size_t)st->cap, nb = (c + 127) / 128;
-            AmbReportBufs& b = st->rb;
-            AMB_STAGE_TRY(AMB_STAGE_REPORTS, amb_decode_alloc(&b.len, c * sizeof(uint32_t), -1, s));
-            AMB_STAGE_TRY(AMB_STAGE_REPORTS, amb_decode_alloc(&b.bsum, nb * sizeof(uint32_t), -1, s));
-            AMB_STAGE_TRY(AMB_STAGE_REPORTS, amb_decode_alloc(&b.boff, (nb + 1) * sizeof(unsigned long long), -1, s));
-            AMB_STAGE_TRY(AMB_STAGE_REPORTS, amb_decode_alloc(&b.text, c * AMB_REP_MAX_LINE, -1, s));
-            st->rcap = st->cap;
-        }
+        if (st->rcap < st->cap)
+            AMB_STAGE_TRY(AMB_STAGE_REPORTS, amb_report_bufs_alloc(&st->rb, &st->rcap, st->cap, AMB_REP_MAX_LINE, s));
     }
+    if (st->beast > 0 && st->bcap < st->cap)
+        AMB_STAGE_TRY(AMB_STAGE_BEAST, amb_report_bufs_alloc(&st->bb, &st->bcap, st->cap, AMB_BEAST_MAX_MSG, s));
+    if (st->avr > 0 && st->acap < st->cap)
+        AMB_STAGE_TRY(AMB_STAGE_AVR, amb_report_bufs_alloc(&st->ab, &st->acap, st->cap, AMB_AVR_MAX_LINE, s));
     return 0;
 }
 
@@ -318,22 +341,25 @@ static void amb_decode_free(AmbDecodeState* st)
     amb_v3_free(&st->v3);
     amb_sbs1_bufs_free(&st->sb);
     amb_report_bufs_free(&st->rb);
+    amb_report_bufs_free(&st->bb);
+    amb_report_bufs_free(&st->ab);
     *st = AmbDecodeState();
 }
 
 // Enqueue one decode of the n frames into the n records on stream s, in this order: fields, pairing, resolve, then the
 // local CPR stage when its S is > 0, the coverage map when coverage is on (after the local stage, so that local fixes
 // reach it), the Comm-B, op-status and track stages whose S is > 0, and the track extension when track and track_ext
-// are both > 0, then the SBS-1 feed when sbs1 is on, then the text reports when reports is on. Returns how many kernels
-// were launched (7, plus 6 per stage that is on, plus 1 for the coverage map, 10 for the SBS-1 feed and 3 for the text
-// reports), or an AMB_STAGE_* code with *err set. Only a decode that launches every stage leaves lines of the SBS-1
-// feed and the text reports, whichever is on, for amb_decode_text: sbs1_nb and reports_nb are -1 otherwise, and a
-// caller that ends a decode before this call (n = 0, a failure) sets them to -1 itself.
+// are both > 0, then the SBS-1 feed when sbs1 is on, then the text reports when reports is on, then the Beast feed
+// and the AVR feed when beast / avr is on. Returns how many kernels were launched (7, plus 6 per stage that is on, plus
+// 1 for the coverage map, 10 for the SBS-1 feed and 3 each for the text reports, the Beast and the AVR feed), or an
+// AMB_STAGE_* code with *err set. Only a decode that launches every stage leaves the output of the SBS-1 feed, the text
+// reports and the two raw feeds, whichever is on, for amb_decode_text: sbs1_nb, reports_nb, beast_nb and avr_nb are -1
+// otherwise, and a caller that ends a decode before this call (n = 0, a failure) sets them to -1 itself.
 static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n, amb_fields* fields, cudaStream_t s,
                              cudaError_t* err)
 {
     const int nb = (n + 127) / 128;
-    st->sbs1_nb = st->reports_nb = -1;
+    st->sbs1_nb = st->reports_nb = st->beast_nb = st->avr_nb = -1;
     AMB_LAUNCH((amb_fields_kernel), nb, 128, 0, s, frames, n, fields, st->pos, st->pair);
     if ((*err = cudaGetLastError()) != cudaSuccess) return AMB_STAGE_FIELDS;
     const int kp = amb_v3_launch(&st->v3, st->pos, n, st->table, st->pair, s, err);
@@ -384,23 +410,41 @@ static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n,
         if (kr < 0) return AMB_STAGE_REPORTS;
         k += kr;
     }
+    if (st->beast > 0) {
+        const int kb = amb_feed_launch<AMB_FEED_BEAST>(frames, fields, n, 0, &st->bb, s, err);
+        if (kb < 0) return AMB_STAGE_BEAST;
+        k += kb;
+    }
+    if (st->avr > 0) {
+        const int ka = amb_feed_launch<AMB_FEED_AVR>(frames, fields, n, st->avr, &st->ab, s, err);
+        if (ka < 0) return AMB_STAGE_AVR;
+        k += ka;
+    }
     if (st->sbs1 > 0) st->sbs1_nb = nb;
     if (st->reports > 0) st->reports_nb = nb;
+    if (st->beast > 0) st->beast_nb = nb;
+    if (st->avr > 0) st->avr_nb = nb;
     return k;
 }
 
 // ---- read-outs ----------------------------------------------------------------------------------------------------
-// The lines of the last decode, the text reports' (reports) or the SBS-1 feed's, on stream s: *text their packed bytes
-// in the state's memory and *bytes their count, or NULL and 0 when the last decode wrote none.
-static cudaError_t amb_decode_text(const AmbDecodeState* st, bool reports, cudaStream_t s, const char** text,
+// The outputs amb_decode_text reads out, by kind.
+enum { AMB_TEXT_SBS1 = 0, AMB_TEXT_REPORTS = 1, AMB_TEXT_BEAST = 2, AMB_TEXT_AVR = 3 };
+
+// The output of the last decode of one kind (AMB_TEXT_*: the SBS-1 lines, the text reports, the Beast messages or the
+// AVR lines), on stream s: *text its packed bytes in the state's memory and *bytes their count, or NULL and 0 when the
+// last decode wrote none.
+static cudaError_t amb_decode_text(const AmbDecodeState* st, int kind, cudaStream_t s, const char** text,
                                    unsigned long long* bytes)
 {
-    const int nb = reports ? st->reports_nb : st->sbs1_nb;
+    const int nbs[] = {st->sbs1_nb, st->reports_nb, st->beast_nb, st->avr_nb};
+    const char* texts[] = {st->sb.text, st->rb.text, st->bb.text, st->ab.text};
+    const unsigned long long* boffs[] = {st->sb.boff, st->rb.boff, st->bb.boff, st->ab.boff};
+    const int nb = nbs[kind];
     *text = nullptr; *bytes = 0;
     if (nb < 0) return cudaSuccess;
-    *text = reports ? st->rb.text : st->sb.text;
-    const cudaError_t e = cudaMemcpyAsync(bytes, (reports ? st->rb.boff : st->sb.boff) + nb, sizeof *bytes,
-                                          cudaMemcpyDeviceToHost, s);
+    *text = texts[kind];
+    const cudaError_t e = cudaMemcpyAsync(bytes, boffs[kind] + nb, sizeof *bytes, cudaMemcpyDeviceToHost, s);
     return e != cudaSuccess ? e : cudaStreamSynchronize(s);
 }
 

@@ -16,12 +16,13 @@
 #pragma once
 #include "amb_report_format.h"
 
-// The stage's per-call scratch (n frames).
+// The stage's per-call scratch (n frames); the Beast and AVR feeds (amb_decode_beast.cuh) keep theirs in the same form.
 struct AmbReportBufs {
     uint32_t* len = nullptr;             // per record: bytes of its line
     uint32_t* bsum = nullptr;            // per block of 128 records: bytes of its lines
     unsigned long long* boff = nullptr;  // per block: byte offset of its lines; [blocks] = the total
-    char* text = nullptr;                // the packed lines, AMB_REP_MAX_LINE bytes per frame of capacity
+    char* text = nullptr;                // the packed lines, AMB_REP_MAX_LINE bytes per frame of capacity (the feeds:
+                                         // AMB_BEAST_MAX_MSG / AMB_AVR_MAX_LINE)
 };
 
 // Whether record k is the call's first queued record, for a lane that read the first-message flag as `set`; called by

@@ -87,12 +87,14 @@ def local_outcome(records):
     return np.asarray(records["pad_"], dtype=np.uint64) & np.uint64(0xFF)
 
 
-# The decoder options (amb_decoder_set_option): name -> (kind, lowest, highest value). A "switch" is off or on; the
-# other kinds take integers in the unit they name, "seconds" from 0 (off).
+# The decoder options (amb_decoder_set_option): name -> (kind, lowest, highest value). A "switch" is off or on, a
+# "form" one of the integers lowest .. highest (0 = off); the other kinds take integers in the unit they name,
+# "seconds" from 0 (off).
 OPTIONS = {"local_cpr": ("seconds", 0, LOCAL_CPR_MAX), "track": ("seconds", 0, TRACK_MAX),
            "commb": ("seconds", 0, COMMB_MAX), "opstatus": ("seconds", 0, OPSTATUS_MAX),
            "track_ext": ("seconds", 0, TRACK_EXT_MAX), "sbs1": ("switch", 0, 1),
-           "sbs1_tz": ("minutes", SBS1_TZ_MIN, SBS1_TZ_MAX), "coverage": ("switch", 0, 1), "reports": ("switch", 0, 1)}
+           "sbs1_tz": ("minutes", SBS1_TZ_MIN, SBS1_TZ_MAX), "coverage": ("switch", 0, 1), "reports": ("switch", 0, 1),
+           "beast": ("switch", 0, 1), "avr": ("form", 0, 2)}
 # the maxima of the options in seconds
 OPTION_MAX = {name: top for name, (kind, _, top) in OPTIONS.items() if kind == "seconds"}
 
@@ -105,6 +107,10 @@ def check_option(name: str, value) -> int:
         if isinstance(value, (bool, np.bool_)) or (isinstance(value, (int, np.integer)) and int(value) in (0, 1)):
             return int(value)
         raise ValueError("%s: False / True (0 / 1), got %r" % (name, value))
+    if kind == "form":
+        if not isinstance(value, (bool, np.bool_)) and isinstance(value, (int, np.integer)) and low <= int(value) <= top:
+            return int(value)
+        raise ValueError("%s: one of %s, got %r" % (name, ", ".join(str(v) for v in range(low, top + 1)), value))
     try:
         ok = not isinstance(value, bool) and int(value) == value and low <= int(value) <= top
     except (TypeError, ValueError):
@@ -124,6 +130,8 @@ check_sbs1 = functools.partial(check_option, "sbs1")
 check_sbs1_tz = functools.partial(check_option, "sbs1_tz")
 check_coverage = functools.partial(check_option, "coverage")
 check_reports = functools.partial(check_option, "reports")
+check_beast = functools.partial(check_option, "beast")
+check_avr = functools.partial(check_option, "avr")
 
 
 def commb_outcome(records):
@@ -325,13 +333,18 @@ class batch_decoder:
     reports = True also writes, on the device, the text reports the reference's stdout printer (msprint.py, what
     modes_rx prints by default) prints for the decoded messages: report.format_report of each frame's slicer text and
     its record, the stream's first queued message at the slicer's precision 6; read the last decode's lines with
-    report_text() / report_text_device() (DESIGN.md §8 "Text reports")."""
+    report_text() / report_text_device() (DESIGN.md §8 "Text reports").
+    beast = True also writes, on the device, every queued frame as a Beast binary message (dump1090's port 30005: the
+    payload, a 48-bit 12 MHz timestamp from the frame's stamp and a signal byte); avr = 1 writes it as an AVR raw line
+    ("*<hex>;", port 30002), avr = 2 as one with the timestamp ("@<timestamp><hex>;"). Read the last decode's bytes
+    with beast_bytes() / beast_bytes_device() and avr_text() / avr_text_device() (DESIGN.md §8 "Beast and AVR
+    feeds")."""
 
     def __init__(self, my_location=None, device: int = 0, local_cpr: int = 0, track: int = 0, commb: int = 0,
                  opstatus: int = 0, track_ext: int = 0, sbs1=False, sbs1_tz: int = 0, coverage=False,
-                 reports=False):
+                 reports=False, beast=False, avr: int = 0):
         values = dict(local_cpr=local_cpr, track=track, commb=commb, opstatus=opstatus, track_ext=track_ext, sbs1=sbs1,
-                      sbs1_tz=sbs1_tz, coverage=coverage, reports=reports)
+                      sbs1_tz=sbs1_tz, coverage=coverage, reports=reports, beast=beast, avr=avr)
         settings = {name: check_option(name, values[name]) for name in OPTIONS}
         self._lib = _lib.load()
         h = C.c_void_p()
@@ -468,6 +481,38 @@ class batch_decoder:
         """report_text() into out_dev, a CUDA uint8 tensor; returns the byte count. Only the count crosses PCIe. Raises
         RuntimeError (with the size needed) when out_dev is too small."""
         return self._text_device(self._lib.amb_decoder_reports_device, "report_text_device", out_dev)
+
+    def set_beast(self, on):
+        """Option beast on (True) or off (False); applies from the next decode."""
+        self._set_option("beast", on)
+
+    def get_beast(self) -> bool:
+        return bool(self._options["beast"])
+
+    def beast_bytes(self) -> bytes:
+        """The Beast binary messages of the last decode, concatenated. Needs the option beast on."""
+        return self._text(self._lib.amb_decoder_beast)
+
+    def beast_bytes_device(self, out_dev) -> int:
+        """beast_bytes() into out_dev, a CUDA uint8 tensor; returns the byte count. Only the count crosses PCIe. Raises
+        RuntimeError (with the size needed) when out_dev is too small."""
+        return self._text_device(self._lib.amb_decoder_beast_device, "beast_bytes_device", out_dev)
+
+    def set_avr(self, form: int):
+        """Option avr = 1 ("*" lines), 2 ("@" lines with the timestamp) or 0 (off); applies from the next decode."""
+        self._set_option("avr", form)
+
+    def get_avr(self) -> int:
+        return self._options["avr"]
+
+    def avr_text(self) -> bytes:
+        """The AVR raw lines of the last decode, concatenated (";\\n" ends each). Needs the option avr on."""
+        return self._text(self._lib.amb_decoder_avr)
+
+    def avr_text_device(self, out_dev) -> int:
+        """avr_text() into out_dev, a CUDA uint8 tensor; returns the byte count. Only the count crosses PCIe. Raises
+        RuntimeError (with the size needed) when out_dev is too small."""
+        return self._text_device(self._lib.amb_decoder_avr_device, "avr_text_device", out_dev)
 
     def set_coverage(self, on):
         """Option coverage on (True) or off (False); applies from the next decode. The grid is kept while it is off."""

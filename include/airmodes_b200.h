@@ -663,6 +663,30 @@ typedef struct amb_aircraft_ext {
  * One flag word (the first message) and, per frame of capacity, 4 + 478 bytes plus 12 bytes per 128 frames, allocated
  * at the first decode with the option on. A decode with the option on launches three kernels more; with it off
  * nothing changes. */
+
+/* Beast binary and AVR raw feeds (amb_decoder_set_option(d, "beast", 1), amb_decoder_set_option(d, "avr", 1 or 2)):
+ * every decode also writes its frames in the two wire formats dump1090 and readsb exchange raw frames in (Beast on TCP
+ * port 30005, AVR on 30002), what mlat-client and the other consumers of a receiver's raw frames read.
+ *   1 frames     a frame is written when its record lacks AMB_FS_NOT_QUEUED (frame.passed != 0), whatever its df and
+ *                status, AMB_FS_NO_HANDLER and DF20/21 Comm-B included; a frame fixed by option "ec" or "ec_any" with
+ *                its corrected data. The payload is data[0 .. nbits / 8): 14 bytes when nbits is 112, else 7 (nbits is
+ *                56 or 112 for every frame the slicer passes). The messages of one call are concatenated in record
+ *                order; nothing carries from call to call, so any cut of a stream into calls gives the same bytes.
+ *   2 timestamp  T = (secs * 12000000 + (uint64)(int64)rint(frac * 12e6)) mod 2^48: a 48-bit count at 12 MHz from the
+ *                frame's stamp, not a wall clock, in uint64 wraparound arithmetic (exact mod 2^48). frac * 12e6 is one
+ *                fp64 multiply without contraction, rint rounds half to even. T = 0 when frac is not finite or
+ *                |frac * 12e6| >= 2^62. With no start time rx_path stamps a frame sample_index / rate, so T is a
+ *                free-running sample clock; with a shared rx_time start, synchronized receivers give the same T for the
+ *                same instant, as multilateration needs.
+ *   3 signal     S from v = (double)ref_level, a power (the mean of four preamble samples of the PMF'd |x|^2): 0 when v
+ *                is NaN or v <= 0, 255 when v >= 1, else max(1, (int)rint(255.0 * sqrt(v))); (S / 255)^2 is the power.
+ *   4 Beast      0x1a, the type byte '2' (0x32) for 7 payload bytes or '3' (0x33) for 14, T in 6 bytes big-endian, S,
+ *                the payload; every 0x1a after the type byte is written twice. At most 2 + 2 * 21 = 44 bytes.
+ *   5 AVR        avr = 1: "*", the payload in upper-case hex, ";\n". avr = 2: "@", T in 12 upper-case hex digits, the
+ *                payload's hex, ";\n". Fixed length for a payload length: 17 / 31 bytes (avr 1), 29 / 43 (avr 2).
+ * Per frame of capacity, 4 + 44 bytes (Beast) and 4 + 43 bytes (AVR) plus 12 bytes per 128 frames each, allocated at
+ * the first decode with the option on. A decode launches three kernels more per option that is on; with both off
+ * nothing changes. */
 typedef struct amb_decoder amb_decoder;
 /* cpr_decoder(my_location) (cpr.py:184-190) + the parser; have_location = 0 is my_location = None. */
 AMB_API int amb_decoder_create(int device, int have_location, double lat, double lon, amb_decoder** out);
@@ -689,6 +713,9 @@ AMB_API int amb_decoder_create(int device, int have_location, double lat, double
  * "sbs1_tz": AMB_SBS1_TZ_MIN .. AMB_SBS1_TZ_MAX minutes (default 0, UTC) added to the stamp in the SBS-1 date and time.
  * "coverage": 0 (default, off) or 1, the receiver coverage map (see AMB_COVERAGE_ROWS); applies from the next call.
  * "reports": 0 (default, off) or 1, the text reports (see amb_decoder_reports); applies from the next call.
+ * "beast": 0 (default, off) or 1, the Beast binary feed (see amb_decoder_beast); applies from the next call.
+ * "avr": 0 (default, off), 1 ("*" lines) or 2 ("@" lines with the timestamp), the AVR raw feed (see amb_decoder_avr);
+ * applies from the next call.
  * Unknown names and out-of-range values return AMB_ERR_INVALID. */
 AMB_API int amb_decoder_set_option(amb_decoder* d, const char* name, int value);
 /* Snapshot of the per-aircraft table at time `now`: every row with seen <= now and now - seen <= S, in ascending
@@ -717,6 +744,14 @@ AMB_API int amb_decoder_sbs1_device(amb_decoder* d, char* out_dev, size_t cap, s
  * _device copies the text to device memory instead, so only the byte count crosses PCIe. */
 AMB_API int amb_decoder_reports(amb_decoder* d, char* out, size_t cap, size_t* n_bytes);
 AMB_API int amb_decoder_reports_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes);
+/* The Beast messages (amb_decoder_beast) or AVR lines (amb_decoder_avr) of the last decode, concatenated, into out (cap
+ * bytes; no terminator); *n_bytes = their length. AMB_ERR_STATE when the option "beast" / "avr" is off; a buffer of
+ * fewer than *n_bytes bytes returns AMB_ERR_OVERFLOW with nothing written (out may then be NULL with cap 0). One 8-byte
+ * copy to the host, then the bytes; _device copies them to device memory instead, so only the byte count crosses PCIe. */
+AMB_API int amb_decoder_beast(amb_decoder* d, char* out, size_t cap, size_t* n_bytes);
+AMB_API int amb_decoder_beast_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes);
+AMB_API int amb_decoder_avr(amb_decoder* d, char* out, size_t cap, size_t* n_bytes);
+AMB_API int amb_decoder_avr_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes);
 /* The coverage grid, AMB_COVERAGE_ROWS x AMB_COVERAGE_BANDS doubles, row-major (bearing row first, band second), into
  * out (host memory); _device copies it to device memory. All zeros before the first decode with the option on.
  * amb_decoder_coverage_reset clears the grid and nothing else (az_map_model.reset, az_map.py:77-82). All three return

@@ -12,8 +12,12 @@ TCP port PORT (default 30003): the lines are formed on the GPU by the decoder (g
 with the date and time of each message's stamp in the host's local time, and sent by gr_air_modes_b200.sbs1. With
 -l LAT,LON --coverage PATH the receiver coverage map of apps/modes_gui's azimuth map (python/az_map.py, the model, not
 the widget) - the greatest range heard per 5-degree bearing sector and altitude band, in statute miles - is kept on the
-GPU by the decoder (option coverage) and written to PATH as JSON after every chunk. KML and FlightGear outputs are the
-reference's own pure-Python consumers of the dl_data feed and are not re-implemented.
+GPU by the decoder (option coverage) and written to PATH as JSON after every chunk. With --beast [PORT] the frames are
+served as the Beast binary feed of dump1090 and readsb (default port 30005, what mlat-client and the other consumers of
+a receiver's raw frames read), with --avr [PORT] as the AVR raw feed (default port 30002; --avr-mlat for the "@" lines
+with the timestamp): the bytes are formed on the GPU by the decoder (options beast and avr) from the receive chain's own
+frames, stamps and levels, and sent by gr_air_modes_b200.sbs1's server. KML and FlightGear outputs are the reference's
+own pure-Python consumers of the dl_data feed and are not re-implemented.
 
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 [-T 7.0] [-d] [-t 5556] [-n] [--reports | -l 37.4,-122.1]
     python tools/modes_rx_b200.py -s 127.0.0.1:12345 -r 4e6 --udp-idle 2.0
@@ -24,6 +28,7 @@ reference's own pure-Python consumers of the dl_data feed and are not re-impleme
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 --reports --opstatus 60
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -l 37.4,-122.1 -P 30003
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -l 37.4,-122.1 --coverage coverage.json
+    python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -n --beast 30005 --avr 30002 --avr-mlat
 
 Differences, all on the far side of rx_path:
 * live radios (-s uhd / osmocom) need GNU Radio: use gr_air_modes_b200.gr_adapter.rx_path inside modes_radio.
@@ -196,6 +201,33 @@ class report_queue:
             self._sbs1.close()
 
 
+class raw_feed:
+    """The Beast binary and AVR raw feeds: every chunk's frames as the receive chain drained them (rx_path.frames, with
+    their own stamps and levels, not parsed back from the message text) through a batch decoder with option beast and
+    / or avr, and its bytes sent to the clients of `beast` / `avr` (gr_air_modes_b200.sbs1.sbs1_server each, or None).
+    avr_form: 1 for "*" lines, 2 for "@" lines with the timestamp."""
+
+    def __init__(self, device, beast=None, avr=None, avr_form=1):
+        from gr_air_modes_b200 import decode
+        self._dec = decode.batch_decoder(None, device, beast=beast is not None, avr=avr_form if avr is not None else 0)
+        self._beast, self._avr = beast, avr
+
+    def flush(self, frames):
+        if not frames:
+            return
+        self._dec.decode(frames)
+        if self._beast is not None:
+            self._beast.send(self._dec.beast_bytes())
+        if self._avr is not None:
+            self._avr.send(self._dec.avr_text())
+
+    def close(self):
+        self._dec.close()
+        for server in (self._beast, self._avr):
+            if server is not None:
+                server.close()
+
+
 def local_utc_offset_minutes() -> int:
     """The host's current UTC offset in minutes, as datetime.now() writes local time in the reference's lines
     (sbs1.py:113-115), within the decoder's -720 .. 840."""
@@ -261,6 +293,15 @@ def parse_args(argv=None):
                     help="after every chunk, write the receiver coverage map to PATH as JSON: the greatest range "
                          "(statute miles) heard per 5-degree bearing sector and altitude band, as modes_gui's azimuth "
                          "map keeps it (needs -l; decodes the messages even without --reports)")
+    ap.add_argument("--beast", type=int, nargs="?", const=30005, default=None, metavar="PORT",
+                    help="serve the frames as the Beast binary feed (dump1090's) on TCP port PORT (default 30005)")
+    ap.add_argument("--avr", type=int, nargs="?", const=30002, default=None, metavar="PORT",
+                    help="serve the frames as the AVR raw feed (\"*<hex>;\" lines) on TCP port PORT (default 30002)")
+    ap.add_argument("--avr-mlat", action="store_true", default=False,
+                    help="with --avr: \"@<timestamp><hex>;\" lines, the 48-bit 12 MHz timestamp of each frame")
+    ap.add_argument("--feed-wait", type=float, default=0.0, metavar="S",
+                    help="with --beast / --avr: wait up to S seconds for the first client of each feed before reading "
+                         "the source (for replaying a recording); 0 = start at once")
     args = ap.parse_args(argv)
     if args.coverage and args.location is None:
         ap.error("--coverage needs -l LAT,LON")
@@ -270,6 +311,15 @@ def parse_args(argv=None):
         ap.error("--sbs1-wait: 0 .. 3600 seconds")
     if args.sbs1_wait and args.sbs1 is None:
         ap.error("--sbs1-wait needs -P")
+    for name, port in (("--beast", args.beast), ("--avr", args.avr)):
+        if port is not None and not 0 < port < 65536:
+            ap.error("%s: a TCP port 1 .. 65535" % name)
+    if args.avr_mlat and args.avr is None:
+        ap.error("--avr-mlat needs --avr")
+    if not 0 <= args.feed_wait <= 3600:
+        ap.error("--feed-wait: 0 .. 3600 seconds")
+    if args.feed_wait and args.beast is None and args.avr is None:
+        ap.error("--feed-wait needs --beast or --avr")
     if not 0 <= args.track <= 3600:
         ap.error("--track: 0 (off) .. 3600 seconds")
     if args.aircraft and args.track <= 0:
@@ -335,6 +385,14 @@ def main(argv=None):
                                                             "track_ext": args.track_ext} if args.track_ext else {}),
                                 **feed)
         sinks.append(reporter)
+    raw = None
+    if args.beast is not None or args.avr is not None:
+        from gr_air_modes_b200.sbs1 import sbs1_server
+        servers = [sbs1_server(p) if p is not None else None for p in (args.beast, args.avr)]
+        for name, srv in zip(("Beast", "AVR"), servers):
+            if srv is not None and args.feed_wait and not srv.wait_for_client(args.feed_wait):
+                print("# no %s client within %g s, starting anyway" % (name, args.feed_wait), file=sys.stderr)
+        raw = raw_feed(args.device, *servers, avr_form=2 if args.avr_mlat else 1)
     pub = None
     if args.tcp is not None:
         from gr_air_modes_b200.zmq_pub import zmq_queue
@@ -363,6 +421,8 @@ def main(argv=None):
             sys.stdout.flush()
         if reporter:
             reporter.flush()
+        if raw:
+            raw.flush(rx.frames)
     st = rx.stats()
     print("# %d samples in, %d messages" % (st.samples_in, total), file=sys.stderr)
     if pub:
@@ -371,6 +431,8 @@ def main(argv=None):
         pub.close()
     if reporter:
         reporter.close()
+    if raw:
+        raw.close()
     rx.close()
     return 0
 
