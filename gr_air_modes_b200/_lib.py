@@ -46,6 +46,9 @@ COVERAGE_ROWS, COVERAGE_BANDS = 72, 9
 COVERAGE_ALTITUDES = (0, 1000, 2000, 5000, 10000, 15000, 20000, 25000, 30000)
 ERR_INVALID = -1                 # AMB_ERR_INVALID
 ERR_OVERFLOW = -5                # AMB_ERR_OVERFLOW: the buffer is too small (amb_decoder_sbs1 reports the size needed)
+ERR_STATE = -8                   # AMB_ERR_STATE: not valid in this state (e.g. a call after flush without reset)
+BEAST_CARRY_MAX = 43             # AMB_BEAST_CARRY_MAX
+BEAST_PUSH_MAX = 0x7FFF0000      # AMB_BEAST_PUSH_MAX
 
 
 class Frame(C.Structure):
@@ -181,6 +184,13 @@ class MlatCounts(C.Structure):
                 ("ms_last", C.c_float), ("pad_", C.c_uint32)]
 
 
+class BeastCounts(C.Structure):
+    """struct amb_beast_counts (72 bytes): amb_beast_reader_stats."""
+    _fields_ = [("bytes_in", C.c_uint64), ("modes", C.c_uint64), ("modeac", C.c_uint64), ("other", C.c_uint64),
+                ("truncated", C.c_uint64), ("skipped", C.c_uint64), ("passed", C.c_uint64), ("carried", C.c_uint64),
+                ("kernel_launches", C.c_uint64)]
+
+
 # amb_mlat_fix.status (include/airmodes_b200.h AMB_MLAT_*)
 MLAT_SOLVED, MLAT_NO_CONVERGENCE, MLAT_DEGENERATE = 1, 2, 3
 MLAT_MIN_STATIONS, MLAT_MAX_STATIONS = 3, 32
@@ -191,6 +201,7 @@ assert C.sizeof(Aircraft) == 128
 assert C.sizeof(AircraftExt) == 144
 assert C.sizeof(MlatFix) == 112
 assert C.sizeof(MlatCounts) == 80
+assert C.sizeof(BeastCounts) == 72
 
 # every symbol include/airmodes_b200.h declares: (name, restype, argtypes)
 _vp, _f32p, _u64p = C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_uint64)
@@ -273,6 +284,14 @@ SYMBOLS = [
                                           _vp, C.c_int, C.POINTER(C.c_int)]),
     ("amb_mlat_stats", C.c_int, [_vp, C.POINTER(MlatCounts)]),
     ("amb_mlat_last_error", C.c_char_p, [_vp]),
+    ("amb_beast_reader_create", C.c_int, [C.c_int, C.POINTER(_vp)]),
+    ("amb_beast_reader_destroy", None, [_vp]),
+    ("amb_beast_reader_reset", C.c_int, [_vp]),
+    ("amb_beast_reader_push", C.c_int, [_vp, _vp, C.c_size_t, C.c_int, C.c_int]),
+    ("amb_beast_reader_frames", C.c_int, [_vp, _vp, C.c_int]),
+    ("amb_beast_reader_frames_device", C.c_int, [_vp, _vp, C.c_int]),
+    ("amb_beast_reader_stats", C.c_int, [_vp, C.POINTER(BeastCounts)]),
+    ("amb_beast_reader_last_error", C.c_char_p, [_vp]),
     ("amb_frame_bits", C.c_uint64, [C.POINTER(Frame), C.c_int, C.c_int]),
     ("amb_strerror", C.c_char_p, [C.c_int]),
     ("amb_last_error", C.c_char_p, [_vp]),

@@ -42,11 +42,13 @@
 // With option "beast" on, three more after those (amb_decode_beast.cuh): amb_feed_len, amb_sbs1_scan, amb_feed_write -
 // the call's Beast binary messages, packed on the device; amb_decoder_beast copies them out. With option "avr" on, the
 // same three kernels once more for the AVR raw lines; amb_decoder_avr copies them out.
-// The multilateration object amb_mlat (amb_mlat.cuh) lives here too: its C ABI is at the end of this file.
+// The multilateration object amb_mlat (amb_mlat.cuh) and the Beast input reader amb_beast_reader (amb_beast_in.cuh)
+// live here too: their C ABIs are at the end of this file.
 #include "amb_launch.h"
 #include "amb_decode_core.h"
 #include "amb_decode_kernels.cuh"
 #include "amb_mlat.cuh"
+#include "amb_beast_in.cuh"
 
 #include <stdio.h>
 #include <string.h>
@@ -717,5 +719,168 @@ int amb_mlat_stats(amb_mlat* m, amb_mlat_counts* out)
 }
 
 const char* amb_mlat_last_error(const amb_mlat* m) { return m ? m->err.c_str() : g_mlat_create_err.c_str(); }
+
+}  // extern "C"
+
+// ---- Beast binary input (amb_beast_in.cuh) --------------------------------------------------------------------------
+struct amb_beast_reader {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    AmbBinDev* dv = nullptr;             // carry, stream offsets and counters, on the device
+    int cur = 0;                         // which of dv->str the next call reads
+    int* tlast = nullptr; int* tprev = nullptr; uint32_t* tfr = nullptr; unsigned long long* toff = nullptr;
+    int tiles_cap = 0;
+    uint8_t* stage = nullptr; size_t stage_cap = 0;   // host bytes on the device
+    amb_frame* frames = nullptr; int frames_cap = 0;  // the frames of the last call
+    int nframes = 0;
+    bool flushed = false;
+    uint64_t bytes_in = 0, launches = 0;
+    std::string err;
+};
+
+static thread_local std::string g_beast_create_err;
+
+extern "C" {
+
+int amb_beast_reader_create(int device, amb_beast_reader** out)
+{
+    static_assert(sizeof(amb_beast_counts) == 72, "amb_beast_counts layout");
+    if (!out) return AMB_ERR_INVALID;
+    *out = nullptr;
+    cudaDeviceProp prop;
+    if (amb_check_device(device, &prop) != AMB_OK) {
+        g_beast_create_err = "amb_beast_reader_create: no sm_90 device";
+        return AMB_ERR_NO_DEVICE;
+    }
+    amb_beast_reader* r = new (std::nothrow) amb_beast_reader();
+    if (!r) return AMB_ERR_INVALID;
+    r->device = device;
+    if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreateWithFlags(&r->stream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaMalloc(&r->dv, sizeof(AmbBinDev)) != cudaSuccess || cudaMemset(r->dv, 0, sizeof(AmbBinDev)) != cudaSuccess) {
+        g_beast_create_err = "CUDA resource creation failed";
+        amb_beast_reader_destroy(r);
+        return AMB_ERR_CUDA;
+    }
+    g_beast_create_err.clear();
+    *out = r;
+    return AMB_OK;
+}
+
+void amb_beast_reader_destroy(amb_beast_reader* r)
+{
+    if (!r) return;
+    cudaSetDevice(r->device);
+    if (r->stream) cudaStreamSynchronize(r->stream);
+    cudaFree(r->dv); cudaFree(r->tlast); cudaFree(r->tprev); cudaFree(r->tfr); cudaFree(r->toff);
+    cudaFree(r->stage); cudaFree(r->frames);
+    if (r->stream) cudaStreamDestroy(r->stream);
+    delete r;
+}
+
+int amb_beast_reader_reset(amb_beast_reader* r)
+{
+    if (!r) return AMB_ERR_INVALID;
+    CK(r, cudaSetDevice(r->device));
+    CK(r, cudaMemsetAsync(r->dv, 0, sizeof(AmbBinDev), r->stream));
+    CK(r, cudaStreamSynchronize(r->stream));
+    r->cur = 0; r->nframes = 0; r->flushed = false; r->bytes_in = 0;
+    return AMB_OK;
+}
+
+int amb_beast_reader_push(amb_beast_reader* r, const void* bytes, size_t n, int mem_kind, int flush)
+{
+    if (!r) return AMB_ERR_INVALID;
+    if ((mem_kind != AMB_MEM_HOST && mem_kind != AMB_MEM_DEVICE) || (n && !bytes))
+        return fail(r, AMB_ERR_INVALID, "amb_beast_reader_push: bad argument");
+    if (n > AMB_BEAST_PUSH_MAX) return fail(r, AMB_ERR_INVALID, "amb_beast_reader_push: more than AMB_BEAST_PUSH_MAX bytes");
+    if (r->flushed)
+        return fail(r, AMB_ERR_STATE, "amb_beast_reader_push: the stream was flushed (amb_beast_reader_reset starts a new one)");
+    CK(r, cudaSetDevice(r->device));
+    cudaStream_t st = r->stream;
+    const int nt = amb_bin_tiles((int)n);
+    if (r->tiles_cap < nt) {
+        cudaFree(r->tlast); cudaFree(r->tprev); cudaFree(r->tfr); cudaFree(r->toff);
+        r->tlast = r->tprev = nullptr; r->tfr = nullptr; r->toff = nullptr; r->tiles_cap = 0;
+        CK(r, cudaMalloc(&r->tlast, (size_t)nt * sizeof(int)));
+        CK(r, cudaMalloc(&r->tprev, (size_t)nt * sizeof(int)));
+        CK(r, cudaMalloc(&r->tfr, (size_t)nt * sizeof(uint32_t)));
+        CK(r, cudaMalloc(&r->toff, (size_t)(nt + 1) * sizeof(unsigned long long)));
+        r->tiles_cap = nt;
+    }
+    // a complete Mode S message takes at least 16 bytes
+    const int fcap = (int)((n + AMB_BEAST_CARRY_MAX) / 16 + 1);
+    if (r->frames_cap < fcap) {
+        cudaFree(r->frames); r->frames = nullptr; r->frames_cap = 0; r->nframes = 0;
+        CK(r, cudaMalloc(&r->frames, (size_t)fcap * sizeof(amb_frame)));
+        r->frames_cap = fcap;
+    }
+    const uint8_t* in = static_cast<const uint8_t*>(bytes);
+    if (mem_kind == AMB_MEM_HOST && n) {
+        if (r->stage_cap < n) {
+            cudaFree(r->stage); r->stage = nullptr; r->stage_cap = 0;
+            CK(r, cudaMalloc(&r->stage, n));
+            r->stage_cap = n;
+        }
+        CK(r, cudaMemcpyAsync(r->stage, bytes, n, cudaMemcpyHostToDevice, st));
+        in = r->stage;
+    }
+    cudaError_t e = cudaSuccess;
+    const int k = amb_bin_launch(r->dv, r->cur, in, (int)n, flush ? 1 : 0, r->tlast, r->tprev, r->tfr, r->toff, r->frames,
+                                 st, &e);
+    if (k < 0) return fail(r, AMB_ERR_CUDA, "amb_beast_reader_push: launch", e);
+    unsigned long long nf = 0;
+    CK(r, cudaMemcpyAsync(&nf, r->toff + nt, sizeof nf, cudaMemcpyDeviceToHost, st));
+    CK(r, cudaStreamSynchronize(st));
+    r->cur ^= 1;
+    r->nframes = (int)nf;
+    r->bytes_in += n;
+    r->launches += (uint64_t)k;
+    if (flush) r->flushed = true;
+    return (int)nf;
+}
+
+static int beast_frames(amb_beast_reader* r, amb_frame* out, int cap, cudaMemcpyKind kind, const char* fn)
+{
+    if (!r || cap < 0) return AMB_ERR_INVALID;
+    if (!out) return r->nframes;
+    if (cap < r->nframes) {
+        char what[96];
+        snprintf(what, sizeof what, "%s: output buffer too small", fn);
+        return fail(r, AMB_ERR_OVERFLOW, what);
+    }
+    if (r->nframes) {
+        CK(r, cudaSetDevice(r->device));
+        CK(r, cudaMemcpyAsync(out, r->frames, (size_t)r->nframes * sizeof(amb_frame), kind, r->stream));
+        CK(r, cudaStreamSynchronize(r->stream));
+    }
+    return r->nframes;
+}
+
+int amb_beast_reader_frames(amb_beast_reader* r, amb_frame* out, int cap)
+{
+    return beast_frames(r, out, cap, cudaMemcpyDeviceToHost, "amb_beast_reader_frames");
+}
+
+int amb_beast_reader_frames_device(amb_beast_reader* r, amb_frame* out_dev, int cap)
+{
+    return beast_frames(r, out_dev, cap, cudaMemcpyDeviceToDevice, "amb_beast_reader_frames_device");
+}
+
+int amb_beast_reader_stats(amb_beast_reader* r, amb_beast_counts* out)
+{
+    if (!r || !out) return AMB_ERR_INVALID;
+    AmbBinDev h;
+    CK(r, cudaSetDevice(r->device));
+    CK(r, cudaMemcpyAsync(&h, r->dv, sizeof h, cudaMemcpyDeviceToHost, r->stream));
+    CK(r, cudaStreamSynchronize(r->stream));
+    out->bytes_in = r->bytes_in;
+    out->modes = h.modes; out->modeac = h.modeac; out->other = h.other; out->truncated = h.truncated;
+    out->skipped = h.skipped; out->passed = h.passed;
+    out->carried = (uint64_t)h.str[r->cur].clen;
+    out->kernel_launches = r->launches;
+    return AMB_OK;
+}
+
+const char* amb_beast_reader_last_error(const amb_beast_reader* r) { return r ? r->err.c_str() : g_beast_create_err.c_str(); }
 
 }  // extern "C"

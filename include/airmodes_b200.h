@@ -863,6 +863,64 @@ AMB_API int amb_mlat_process_device(amb_mlat* m, const amb_frame* const* frames_
 AMB_API int amb_mlat_stats(amb_mlat* m, amb_mlat_counts* out);
 AMB_API const char* amb_mlat_last_error(const amb_mlat* m);          /* m == NULL: the last failed amb_mlat_create */
 
+/* ---- Beast binary input (amb_beast_reader): another receiver's frames, parsed on the device -------------------------
+ * The byte stream dump1090 and readsb serve on TCP port 30005 (and amb_decoder_beast writes) turned into amb_frame
+ * records for amb_decode_frames_device or amb_mlat_process_device. The rules are defined on the byte stream since
+ * amb_beast_reader_create or the last amb_beast_reader_reset, not on how it was cut into calls:
+ *   1 tokens     left to right, 0x1a 0x1a is one data token (an escaped 0x1a); 0x1a t with t != 0x1a a sync token of
+ *                type t; any other byte a data token. The stream's start counts as preceded by a byte that is not 0x1a:
+ *                a byte starts a token exactly when the run of 0x1a bytes right before it has even length.
+ *   2 messages   a sync token of type '1' (Mode A/C), '2' (Mode S short) or '3' (Mode S long) takes the next 9, 14 or 21
+ *                data tokens as its body: T (6 bytes, big-endian), S, then 2, 7 or 14 payload bytes. When a sync token
+ *                comes first the message is truncated: dropped and counted, its data tokens with it. Data tokens after a
+ *                complete body and before the next sync token, before the first sync token, and after a sync token of
+ *                any other type ('4' included; counted as "other") are skipped and counted. Mode A/C messages are
+ *                counted and give no frame.
+ *   3 frames     every complete Mode S message gives one amb_frame, in stream order: data = the payload zero-padded to
+ *                14 bytes, nbits 56 or 112 from the type, df = data[0] >> 3, crc = the slicer's syndrome
+ *                amb_modes_check_crc(data, nbits / 8 - 3) ^ the last 3 payload bytes, secs = T / 12000000,
+ *                frac = (double)(T % 12000000) / 12e6 (one IEEE division), ref_level = (float)((double)(S * S) / 65025.0),
+ *                sample_index = the stream offset of the message's sync byte; numlowconf, lowconfbits, ec, ec_flips and
+ *                pad_ are 0. These invert rules 2 to 4 of amb_decoder_beast: T and S of a frame written by it read back
+ *                unchanged.
+ *   4 passed     1 unless the payload is all zero, or nbits is not 112 for DF 16, 17, 20, 21 and 56 for the others, or
+ *                crc != 0 for DF 11 or 17 (the reference slicer's drop rules that need no samples). Unpassed frames are
+ *                still written, as amb_drain_device writes them; the decoder marks them AMB_FS_NOT_QUEUED.
+ *   5 calls      any cut of a stream into calls, flush on the last, gives the same frames and counters as one call. What
+ *                cannot be decided yet (an incomplete last message, a final lone 0x1a: at most AMB_BEAST_CARRY_MAX bytes)
+ *                is carried on the device to the next call. At flush an incomplete message is truncated and a final lone
+ *                0x1a is dropped uncounted; later calls return AMB_ERR_STATE until amb_beast_reader_reset. */
+#define AMB_BEAST_CARRY_MAX 43
+#define AMB_BEAST_PUSH_MAX ((size_t)0x7FFF0000)   /* bytes in one call: every index of the call fits an int */
+typedef struct amb_beast_reader amb_beast_reader;
+typedef struct amb_beast_counts {
+    uint64_t bytes_in;         /* bytes given since create or reset */
+    uint64_t modes;            /* complete Mode S messages (= frames) */
+    uint64_t modeac;           /* complete Mode A/C messages */
+    uint64_t other;            /* sync tokens of any other type */
+    uint64_t truncated;        /* Mode S and Mode A/C messages cut by a sync token or by flush */
+    uint64_t skipped;          /* data tokens outside every message body */
+    uint64_t passed;           /* frames with passed = 1 */
+    uint64_t carried;          /* bytes carried into the next call now */
+    uint64_t kernel_launches;  /* since create: five per call */
+} amb_beast_counts;   /* 72 bytes */
+AMB_API int amb_beast_reader_create(int device, amb_beast_reader** out);
+AMB_API void amb_beast_reader_destroy(amb_beast_reader* r);
+/* Start a new stream: drop the carry, offsets and counters (but kernel_launches) restart at 0, flush is undone. */
+AMB_API int amb_beast_reader_reset(amb_beast_reader* r);
+/* The next n bytes of the stream: host memory (AMB_MEM_HOST, copied once to the device) or device memory
+ * (AMB_MEM_DEVICE, read in place; it must be complete when called). flush != 0 ends the stream. Returns this call's frame
+ * count; they stay readable until the next call or reset. n > AMB_BEAST_PUSH_MAX or another memory kind:
+ * AMB_ERR_INVALID. Five kernel launches whatever n is; only the frame count crosses PCIe. Synchronises the reader's
+ * own stream. */
+AMB_API int amb_beast_reader_push(amb_beast_reader* r, const void* bytes, size_t n, int mem_kind, int flush);
+/* The frames of the last push into out (host memory; _device: device memory), as amb_drain_device writes them:
+ * out == NULL returns their count; cap below it returns AMB_ERR_OVERFLOW and writes nothing; else returns the count. */
+AMB_API int amb_beast_reader_frames(amb_beast_reader* r, amb_frame* out, int cap);
+AMB_API int amb_beast_reader_frames_device(amb_beast_reader* r, amb_frame* out_dev, int cap);
+AMB_API int amb_beast_reader_stats(amb_beast_reader* r, amb_beast_counts* out);
+AMB_API const char* amb_beast_reader_last_error(const amb_beast_reader* r);   /* r == NULL: the last failed create */
+
 AMB_API const char* amb_strerror(int code);
 AMB_API const char* amb_last_error(const amb_ctx* ctx);
 AMB_API const char* amb_version(void);

@@ -19,6 +19,14 @@ with the timestamp): the bytes are formed on the GPU by the decoder (options bea
 frames, stamps and levels, and sent by gr_air_modes_b200.sbs1's server. KML and FlightGear outputs are the reference's
 own pure-Python consumers of the dl_data feed and are not re-implemented.
 
+With --input beast the frames come from another receiver instead of the IQ chain: -s FILE replays a recorded Beast
+binary byte stream, -s HOST:PORT connects over TCP to a Beast server (dump1090 or readsb on port 30005, or this tool's
+own --beast) and ends when the server closes. The bytes are parsed on the GPU (gr_air_modes_b200.beast) and every
+chunk's frames go where the receive chain's go: their message lines to stdout, -t, --reports / -l, -P, --track /
+--aircraft and --coverage, and the frames themselves to --beast / --avr. The stamps are the feed's 48-bit 12 MHz
+counter, not wall-clock time: SBS-1 dates on Beast input follow that counter. Options that only configure the receive
+chain (-d, -r, -T, --ec, --ec-any, --ap-filter, --resample) are errors with --input beast.
+
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 [-T 7.0] [-d] [-t 5556] [-n] [--reports | -l 37.4,-122.1]
     python tools/modes_rx_b200.py -s 127.0.0.1:12345 -r 4e6 --udp-idle 2.0
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 --track 60 --aircraft aircraft.json
@@ -29,6 +37,8 @@ own pure-Python consumers of the dl_data feed and are not re-implemented.
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -l 37.4,-122.1 -P 30003
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -l 37.4,-122.1 --coverage coverage.json
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -n --beast 30005 --avr 30002 --avr-mlat
+    python tools/modes_rx_b200.py --input beast -s 192.168.1.20:30005 --reports
+    python tools/modes_rx_b200.py --input beast -s feed.bin -l 37.4,-122.1 -P 30003
 
 Differences, all on the far side of rx_path:
 * live radios (-s uhd / osmocom) need GNU Radio: use gr_air_modes_b200.gr_adapter.rx_path inside modes_radio.
@@ -213,7 +223,7 @@ class raw_feed:
         self._beast, self._avr = beast, avr
 
     def flush(self, frames):
-        if not frames:
+        if len(frames) == 0:
             return
         self._dec.decode(frames)
         if self._beast is not None:
@@ -228,6 +238,64 @@ class raw_feed:
                 server.close()
 
 
+def beast_file_source(path, chunk):
+    """A recorded Beast byte stream: yields (bytes, last?), chunk bytes at a time."""
+    with open(path, "rb") as f:
+        data = f.read(chunk)
+        while True:
+            nxt = f.read(chunk)
+            yield data, not nxt
+            if not nxt:
+                return
+            data = nxt
+
+
+def beast_tcp_source(host, port, chunk):
+    """A Beast server's byte stream over TCP (dump1090 / readsb port 30005): yields (bytes, last?) as they arrive,
+    at most chunk bytes at a time; the stream ends when the server closes the connection."""
+    sock = socket.create_connection((host, port))
+    try:
+        while True:
+            d = sock.recv(min(chunk, 1 << 20))
+            yield d, not d
+            if not d:
+                return
+    finally:
+        sock.close()
+
+
+class beast_input:
+    """--input beast: the Beast bytes of another receiver parsed on the GPU (gr_air_modes_b200.beast.beast_reader) into
+    frames, and the message line of every passed frame (amb_format_messages, what the slicer queues) handed to `queue`
+    as rx_path hands its own."""
+
+    def __init__(self, queue, device):
+        from gr_air_modes_b200 import beast
+        self._reader = beast.beast_reader(device)
+        self._queue, self._first, self.messages = queue, True, 0
+
+    def process(self, data, last):
+        import ctypes as C
+        from gr_air_modes_b200 import _lib
+        fr = self._reader.process(data, flush=last)
+        if len(fr):
+            cap = 128 * len(fr) + 16
+            buf = C.create_string_buffer(cap)
+            k = _lib.check(_lib.load().amb_format_messages(C.c_void_p(fr.ctypes.data), len(fr), int(self._first), buf, cap))
+            if k:
+                for text in buf.value.decode("ascii").split("\n"):
+                    self._queue.handle(air_modes.message(text))
+                self._first = False
+                self.messages += k
+        return fr
+
+    def stats(self):
+        return self._reader.stats()
+
+    def close(self):
+        self._reader.close()
+
+
 def local_utc_offset_minutes() -> int:
     """The host's current UTC offset in minutes, as datetime.now() writes local time in the reference's lines
     (sbs1.py:113-115), within the decoder's -720 .. 840."""
@@ -238,11 +306,17 @@ def local_utc_offset_minutes() -> int:
 
 def parse_args(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
-    ap.add_argument("-s", "--source", required=True, help="<filename> (cfile) or <ip:port> (UDP of gr_complex)")   # radio.py:94-95
+    ap.add_argument("-s", "--source", required=True,
+                    help="<filename> (cfile) or <ip:port> (UDP of gr_complex); with --input beast a recorded Beast byte "
+                         "stream or <host:port> of a Beast TCP server")                                              # radio.py:94-95
+    ap.add_argument("--input", choices=("iq", "beast"), default="iq",
+                    help="iq (default): samples through the GPU receive chain; beast: another receiver's Beast binary "
+                         "frames (dump1090 / readsb port 30005), parsed on the GPU; their stamps are the feed's 12 MHz "
+                         "counter, so SBS-1 dates follow that counter, not the wall clock")
     ap.add_argument("-t", "--tcp", type=int, default=None, metavar="PORT",
                     help="publish messages as ZMQ dl_data on tcp://*:PORT")                                        # radio.py:96-97,80-82
-    ap.add_argument("-r", "--rate", type=float, default=4e6)                                                       # radio.py:112
-    ap.add_argument("-T", "--threshold", type=float, default=7.0)                                                  # radio.py:114
+    ap.add_argument("-r", "--rate", type=float, default=None, help="default 4e6")                                 # radio.py:112
+    ap.add_argument("-T", "--threshold", type=float, default=None, help="default 7.0")                            # radio.py:114
     ap.add_argument("-p", "--pmf", action="store_true", default=True, help="pulse matched filter (default on)")    # radio.py:116
     ap.add_argument("--no-pmf", dest="pmf", action="store_false")
     ap.add_argument("-d", "--dcblock", action="store_true", default=False)                                         # radio.py:118
@@ -254,7 +328,8 @@ def parse_args(argv=None):
     ap.add_argument("--resample", action="store_true", default=False,
                     help="rates below 4 Msps: resample to 4 Msps in front of the chain like radio.py:49-53 "
                          "(stand-in for GNU Radio's pfb.arb_resampler_ccf, tools/resample_standin.py)")
-    ap.add_argument("--chunk", type=int, default=1 << 24, help="complex samples per amb_process call")
+    ap.add_argument("--chunk", type=int, default=1 << 24,
+                    help="complex samples per amb_process call (with --input beast: bytes per call at most)")
     ap.add_argument("--udp-idle", type=float, default=2.0, help="end a UDP stream after this many idle seconds")
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--ec", type=int, default=0, metavar="K",
@@ -303,6 +378,15 @@ def parse_args(argv=None):
                     help="with --beast / --avr: wait up to S seconds for the first client of each feed before reading "
                          "the source (for replaying a recording); 0 = start at once")
     args = ap.parse_args(argv)
+    if args.input == "beast":
+        given = [name for name, on in (("-d", args.dcblock), ("-r", args.rate is not None), ("-T", args.threshold is not None),
+                                        ("--ec", args.ec), ("--ec-any", args.ec_any), ("--ap-filter", args.ap_filter),
+                                        ("--resample", args.resample)) if on]
+        if given:
+            ap.error("%s configure%s the receive chain, which --input beast does not run" %
+                     (", ".join(given), "s" if len(given) == 1 else ""))
+    args.rate = 4e6 if args.rate is None else args.rate
+    args.threshold = 7.0 if args.threshold is None else args.threshold
     if args.coverage and args.location is None:
         ap.error("--coverage needs -l LAT,LON")
     if args.sbs1 is not None and not 0 < args.sbs1 < 65536:
@@ -343,6 +427,8 @@ def parse_args(argv=None):
 def main(argv=None):
     args = parse_args(argv)
 
+    if args.input == "beast":
+        return main_beast(args)
     if args.source in ("uhd", "osmocom"):
         raise SystemExit("live radios need GNU Radio: use gr_air_modes_b200.gr_adapter.rx_path in modes_radio (INTEGRATION.md)")
     rate = int(args.rate)                                                                                          # radio.py:44
@@ -358,6 +444,69 @@ def main(argv=None):
     elif rate < 4e6:
         print("# rate %d < 4 Msps: the reference would resample to 4 Msps (radio.py:49-53, GNU Radio PFB, not "
               "reproduced; --resample runs a stand-in); running the chain at the native rate" % rate, file=sys.stderr)
+    sinks, printer, reporter, raw, pub = make_outputs(args)
+    rx = air_modes.rx_path(rx_rate, args.threshold, tee_queue(sinks), args.pmf, args.dcblock, device=args.device,
+                           ec=args.ec, ec_any=args.ec_any, ap_filter=args.ap_filter)   # radio.py:55-56
+
+    if ":" in args.source and not os.path.exists(args.source):
+        m = re.search(r"(.*)\:(\d{1,5})$", args.source)                                                           # radio.py:223-226
+        if not m:
+            raise SystemExit("Please input UDP source e.g. 192.168.10.1:12345")
+        print("Using UDP source %s:%s" % m.groups(), file=sys.stderr)
+        src = udp_source(open_udp(m.group(1), int(m.group(2)), args.udp_idle), args.chunk)
+    else:
+        print("Using file source %s" % args.source, file=sys.stderr)
+        src = file_source(args.source, args.chunk)
+    print("Rate is %i" % rate, file=sys.stderr)
+
+    total = 0
+    for block, last in src:
+        if resampler is not None:
+            block = resampler.push(block, last)
+        total += rx.process(block, flush=last)
+        if printer:
+            sys.stdout.flush()
+        if reporter:
+            reporter.flush()
+        if raw:
+            raw.flush(rx.frames)
+    st = rx.stats()
+    print("# %d samples in, %d messages" % (st.samples_in, total), file=sys.stderr)
+    close_outputs(reporter, raw, pub)
+    rx.close()
+    return 0
+
+
+def main_beast(args):
+    """--input beast: the outputs of main(), fed by another receiver's Beast frames instead of the receive chain."""
+    sinks, printer, reporter, raw, pub = make_outputs(args)
+    src_in = beast_input(tee_queue(sinks), args.device)
+    if ":" in args.source and not os.path.exists(args.source):
+        m = re.search(r"(.*)\:(\d{1,5})$", args.source)
+        if not m:
+            raise SystemExit("Please input a Beast server as host:port, e.g. 127.0.0.1:30005")
+        print("Using Beast TCP source %s:%s" % m.groups(), file=sys.stderr)
+        src = beast_tcp_source(m.group(1), int(m.group(2)), args.chunk)
+    else:
+        print("Using Beast file source %s" % args.source, file=sys.stderr)
+        src = beast_file_source(args.source, args.chunk)
+    for data, last in src:
+        frames = src_in.process(data, last)
+        if printer:
+            sys.stdout.flush()
+        if reporter:
+            reporter.flush()
+        if raw:
+            raw.flush(frames)
+    st = src_in.stats()
+    print("# %d bytes in, %d Mode S frames, %d messages" % (st["bytes_in"], st["modes"], src_in.messages), file=sys.stderr)
+    close_outputs(reporter, raw, pub)
+    src_in.close()
+    return 0
+
+
+def make_outputs(args):
+    """The sinks of the messages (printer, reporter, ZMQ publisher) and the raw feeds, as the options ask."""
     sinks = []
     printer = None
     reporter = None
@@ -398,33 +547,10 @@ def main(argv=None):
         from gr_air_modes_b200.zmq_pub import zmq_queue
         pub = zmq_queue(["tcp://*:%i" % args.tcp])
         sinks.append(pub)
-    rx = air_modes.rx_path(rx_rate, args.threshold, tee_queue(sinks), args.pmf, args.dcblock, device=args.device,
-                           ec=args.ec, ec_any=args.ec_any, ap_filter=args.ap_filter)   # radio.py:55-56
+    return sinks, printer, reporter, raw, pub
 
-    if ":" in args.source and not os.path.exists(args.source):
-        m = re.search(r"(.*)\:(\d{1,5})$", args.source)                                                           # radio.py:223-226
-        if not m:
-            raise SystemExit("Please input UDP source e.g. 192.168.10.1:12345")
-        print("Using UDP source %s:%s" % m.groups(), file=sys.stderr)
-        src = udp_source(open_udp(m.group(1), int(m.group(2)), args.udp_idle), args.chunk)
-    else:
-        print("Using file source %s" % args.source, file=sys.stderr)
-        src = file_source(args.source, args.chunk)
-    print("Rate is %i" % rate, file=sys.stderr)
 
-    total = 0
-    for block, last in src:
-        if resampler is not None:
-            block = resampler.push(block, last)
-        total += rx.process(block, flush=last)
-        if printer:
-            sys.stdout.flush()
-        if reporter:
-            reporter.flush()
-        if raw:
-            raw.flush(rx.frames)
-    st = rx.stats()
-    print("# %d samples in, %d messages" % (st.samples_in, total), file=sys.stderr)
+def close_outputs(reporter, raw, pub):
     if pub:
         import time
         time.sleep(0.2)                                                                                           # apps/modes_rx:88-91
@@ -433,8 +559,6 @@ def main(argv=None):
         reporter.close()
     if raw:
         raw.close()
-    rx.close()
-    return 0
 
 
 if __name__ == "__main__":
