@@ -266,6 +266,8 @@ SYMBOLS = [
     ("amb_decoder_beast_device", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("amb_decoder_avr", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("amb_decoder_avr_device", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("amb_decoder_flightgear", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("amb_decoder_flightgear_device", C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
     ("amb_decoder_coverage", C.c_int, [_vp, _vp]),
     ("amb_decoder_coverage_device", C.c_int, [_vp, _vp]),
     ("amb_decoder_coverage_reset", C.c_int, [_vp]),

@@ -42,6 +42,11 @@
 // With option "beast" on, three more after those (amb_decode_beast.cuh): amb_feed_len, amb_sbs1_scan, amb_feed_write -
 // the call's Beast binary messages, packed on the device; amb_decoder_beast copies them out. With option "avr" on, the
 // same three kernels once more for the AVR raw lines; amb_decoder_avr copies them out.
+// With option "flightgear" on, nine more after those (amb_decode_flightgear.cuh): amb_fg_keys, the four partition
+// kernels on address keys, amb_fg_walk - each position's latest callsign and velocity of its address, with a
+// direct-mapped table of them in HBM (2^24 x 32 B) carried from batch to batch - and amb_fg_count, amb_sbs1_scan,
+// amb_fg_write, which write the call's FlightGear position packets and pack them on the device;
+// amb_decoder_flightgear copies them out.
 // The multilateration object amb_mlat (amb_mlat.cuh) and the Beast input reader amb_beast_reader (amb_beast_in.cuh)
 // live here too: their C ABIs are at the end of this file.
 #include "amb_launch.h"
@@ -242,8 +247,8 @@ static int decode_impl(amb_decoder* d, const amb_frame* frames, int n, int mem_k
 {
     if (!d || n < 0 || (n > 0 && (!frames || !out)) || (mem_kind != AMB_MEM_HOST && mem_kind != AMB_MEM_DEVICE))
         return fail(d, AMB_ERR_INVALID, "amb_decode_frames: bad argument");
-    d->st.sbs1_nb = d->st.reports_nb = d->st.beast_nb = d->st.avr_nb = -1;   // until amb_decode_launch has launched
-                                                                             // every stage
+    // until amb_decode_launch has launched every stage
+    d->st.sbs1_nb = d->st.reports_nb = d->st.beast_nb = d->st.avr_nb = d->st.flightgear_nb = -1;
     if (n == 0) return AMB_OK;
     CK(d, cudaSetDevice(d->device));
     int rc = prepare(d, n);
@@ -344,8 +349,8 @@ int amb_decoder_aircraft_ext_device(amb_decoder* d, double now, amb_aircraft* ou
     return snapshot_impl(d, now, out_dev, ext_dev, cap, true, true);
 }
 
-// amb_decoder_sbs1(_device), amb_decoder_reports(_device), amb_decoder_beast(_device) and amb_decoder_avr(_device), by
-// kind (AMB_TEXT_*): the last decode's output into out (host or device memory)
+// amb_decoder_sbs1(_device), amb_decoder_reports(_device), amb_decoder_beast(_device), amb_decoder_avr(_device) and
+// amb_decoder_flightgear(_device), by kind (AMB_TEXT_*): the last decode's output into out (host or device memory)
 static int text_impl(amb_decoder* d, int kind, char* out, size_t cap, size_t* n_bytes, bool out_on_device)
 {
     static const struct { const char* option; const char* fn; const char* fn_device; } kinds[] = {
@@ -353,8 +358,10 @@ static int text_impl(amb_decoder* d, int kind, char* out, size_t cap, size_t* n_
         {"reports", "amb_decoder_reports", "amb_decoder_reports_device"},
         {"beast", "amb_decoder_beast", "amb_decoder_beast_device"},
         {"avr", "amb_decoder_avr", "amb_decoder_avr_device"},
+        {"flightgear", "amb_decoder_flightgear", "amb_decoder_flightgear_device"},
     };
-    const int on[] = {d ? d->st.sbs1 : 0, d ? d->st.reports : 0, d ? d->st.beast : 0, d ? d->st.avr : 0};
+    const int on[] = {d ? d->st.sbs1 : 0, d ? d->st.reports : 0, d ? d->st.beast : 0, d ? d->st.avr : 0,
+                      d ? d->st.flightgear : 0};
     const char* fn = out_on_device ? kinds[kind].fn_device : kinds[kind].fn;
     char what[96];
     if (!d || !n_bytes || (cap > 0 && !out)) { snprintf(what, sizeof what, "%s: bad argument", fn); return fail(d, AMB_ERR_INVALID, what); }
@@ -418,6 +425,16 @@ int amb_decoder_avr(amb_decoder* d, char* out, size_t cap, size_t* n_bytes)
 int amb_decoder_avr_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes)
 {
     return text_impl(d, AMB_TEXT_AVR, out_dev, cap, n_bytes, true);
+}
+
+int amb_decoder_flightgear(amb_decoder* d, char* out, size_t cap, size_t* n_bytes)
+{
+    return text_impl(d, AMB_TEXT_FLIGHTGEAR, out, cap, n_bytes, false);
+}
+
+int amb_decoder_flightgear_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes)
+{
+    return text_impl(d, AMB_TEXT_FLIGHTGEAR, out_dev, cap, n_bytes, true);
 }
 
 // the coverage grid into out (host or device memory)
@@ -487,11 +504,9 @@ static thread_local std::string g_mlat_create_err;
 static AmbMlatStation mlat_station(double lat_deg, double lon_deg, double height)
 {
     AmbMlatStation o;
-    const double lat = lat_deg * (M_PI / 180.0), lon = lon_deg * (M_PI / 180.0);
-    o.sl = sin(lat); o.cl = cos(lat); o.so = sin(lon); o.co = cos(lon);
-    o.n = AMB_MLAT_WGS_A / sqrt(1 - AMB_MLAT_WGS_E2 * (o.sl * o.sl));
-    o.s[0] = (o.n + height) * o.cl * o.co; o.s[1] = (o.n + height) * o.cl * o.so;
-    o.s[2] = (o.n * (1 - AMB_MLAT_WGS_E2) + height) * o.sl;
+    double t[5];
+    amb_llh2ecef(lat_deg, lon_deg, height, o.s, t);
+    o.n = t[0]; o.cl = t[1]; o.sl = t[2]; o.co = t[3]; o.so = t[4];
     return o;
 }
 

@@ -743,3 +743,22 @@ static inline void amb_build_nl_table(double* T)
         T[k] = hi;
     }
 }
+
+// ---- geodesy: llh2ecef (mlat.py:75-86), WGS84 without geoid correction ---------------------------------------------
+#define AMB_MLAT_WGS_A 6378137.0                 // mlat.py:52-54
+#define AMB_MLAT_WGS_B 6356752.314245
+#define AMB_MLAT_WGS_E2 0.0066943799901975848
+
+// ECEF of lat, lon (degrees) at alt (metres) into s[3], mlat.py's operations in its order. t (unless NULL) gets the
+// prime vertical radius n and cos / sin of lat and lon: t = {n, cl, sl, co, so}, which the multilateration's start
+// point reuses.
+AMB_HD void amb_llh2ecef(double lat_deg, double lon_deg, double alt, double* s, double* t)
+{
+    const double lat = lat_deg * (M_PI / 180.0), lon = lon_deg * (M_PI / 180.0);
+    const double sl = sin(lat), cl = cos(lat), so = sin(lon), co = cos(lon);
+    const double n = AMB_MLAT_WGS_A / sqrt(1 - AMB_MLAT_WGS_E2 * (sl * sl));
+    s[0] = (n + alt) * cl * co;
+    s[1] = (n + alt) * cl * so;
+    s[2] = (n * (1 - AMB_MLAT_WGS_E2) + alt) * sl;
+    if (t) { t[0] = n; t[1] = cl; t[2] = sl; t[3] = co; t[4] = so; }
+}

@@ -56,6 +56,7 @@ __global__ void __launch_bounds__(128) amb_resolve_kernel(amb_fields* __restrict
 #include "amb_decode_coverage.cuh"
 #include "amb_decode_reports.cuh"
 #include "amb_decode_beast.cuh"
+#include "amb_decode_flightgear.cuh"
 
 // ---- state and launch sequence ------------------------------------------------------------------------------------
 // What the stages of one decode read and write besides the frames and the records, and the one owner of that memory:
@@ -103,10 +104,16 @@ struct AmbDecodeState {
     int avr = 0;                         // option "avr": 1 = "*" lines, 2 = "@" lines with the timestamp, 0 = off
     AmbReportBufs ab;                    // the AVR feed's per-call scratch and packed lines
     int acap = 0;                        // frames ab holds
+    int flightgear = 0;                  // option "flightgear": 1 = on, 0 = off
+    AmbFgSlot* ftable = nullptr;         // latest callsign and velocity per address, AMB_FG_SLOTS
+    AmbFgSlot* fst = nullptr;            // one per frame: a position record's state as the walk leaves it
+    AmbReportBufs fb;                    // the FlightGear feed's per-call scratch and packed packets
+    int fcap = 0;                        // frames fst and fb hold
     int sbs1_nb = -1;                    // blocks of lines of the last decode (its byte total is sb.boff[sbs1_nb]);
                                          // -1: the last decode wrote no lines
     int reports_nb = -1;                 // the same for the text reports (rb.boff[reports_nb])
     int beast_nb = -1, avr_nb = -1;      // the same for the Beast messages (bb.boff[beast_nb]) and AVR lines (ab.boff)
+    int flightgear_nb = -1;              // the same for the FlightGear packets (fb.boff[flightgear_nb])
     int have_loc = 0; double lat = 0.0, lon = 0.0;      // receiver location
 };
 
@@ -125,6 +132,7 @@ static const struct {
     {"reports", &AmbDecodeState::reports, 0, 1, "reports: 0 (off) or 1 (on)"},
     {"beast", &AmbDecodeState::beast, 0, 1, "beast: 0 (off) or 1 (on)"},
     {"avr", &AmbDecodeState::avr, 0, 2, "avr: 0 (off), 1 (* lines) or 2 (@ lines with the timestamp)"},
+    {"flightgear", &AmbDecodeState::flightgear, 0, 1, "flightgear: 0 (off) or 1 (on)"},
 };
 
 // Set option `name` of st to `value`, from the next decode on. Returns NULL, or why the setting is refused.
@@ -148,7 +156,7 @@ static void amb_decode_set_location(AmbDecodeState* st, int have_location, doubl
 enum { AMB_STAGE_FIELDS = -1, AMB_STAGE_PAIRING = -2, AMB_STAGE_RESOLVE = -3, AMB_STAGE_LOCAL = -4,
        AMB_STAGE_COMMB = -5, AMB_STAGE_TRACK = -6, AMB_STAGE_OPSTATUS = -7, AMB_STAGE_TRACK_EXT = -8,
        AMB_STAGE_SBS1 = -9, AMB_STAGE_COVERAGE = -10,
-       AMB_STAGE_REPORTS = -11, AMB_STAGE_BEAST = -12, AMB_STAGE_AVR = -13 };
+       AMB_STAGE_REPORTS = -11, AMB_STAGE_BEAST = -12, AMB_STAGE_AVR = -13, AMB_STAGE_FLIGHTGEAR = -14 };
 
 // By -AMB_STAGE_* - 1: what a failed launch of the stage reports, and what a failure of its memory reports.
 static const struct { const char* launch; const char* memory; } amb_stage_names[] = {
@@ -165,6 +173,7 @@ static const struct { const char* launch; const char* memory; } amb_stage_names[
     {"text reports", "text report buffers (478 B per frame)"},
     {"Beast feed", "Beast feed buffers (44 B per frame)"},
     {"AVR feed", "AVR feed buffers (43 B per frame)"},
+    {"FlightGear feed", "FlightGear state table (512 MiB) and buffers (268 B per frame)"},
 };
 
 // cudaMalloc, then every byte set to `fill` unless it is < 0; *p is NULL after a failed cudaMalloc
@@ -213,7 +222,8 @@ static cudaError_t amb_report_bufs_alloc(AmbReportBufs* b, int* have, int cap, s
 // option on, filled as an empty one (the track extension only while track is on too); the SBS-1 scratch as the frame
 // capacity grows; the coverage grid at the first decode with the option on; the text reports' first-message flag (set)
 // at the first decode with the option on, and their buffers as the frame capacity grows; the Beast and AVR feeds'
-// buffers likewise. Returns 0, or the AMB_STAGE_* code of the stage whose memory could not be had, with *err set.
+// buffers likewise; the FlightGear feed's state table (empty) at the first decode with the option on, its per-frame
+// state and buffers as the frame capacity grows. Returns 0, or the AMB_STAGE_* code of the stage whose memory could not be had, with *err set.
 static int amb_decode_prepare(AmbDecodeState* st, int n, cudaStream_t s, cudaError_t* err)
 {
     if (!st->table) AMB_STAGE_TRY(AMB_STAGE_PAIRING, amb_decode_alloc(&st->table, st->table_slots * sizeof(AmbCprSlot), 0xFF, s));
@@ -232,7 +242,8 @@ static int amb_decode_prepare(AmbDecodeState* st, int n, cudaStream_t s, cudaErr
         AMB_STAGE_TRY(AMB_STAGE_FIELDS, amb_decode_alloc(&st->pair, (size_t)cap * sizeof(AmbPair), -1, s));
         st->cap = cap;
     }
-    if ((st->local_cpr > 0 || st->commb > 0 || st->opstatus > 0 || st->track > 0 || st->sbs1 > 0) && st->kcap < st->cap) {
+    if ((st->local_cpr > 0 || st->commb > 0 || st->opstatus > 0 || st->track > 0 || st->sbs1 > 0 ||
+         st->flightgear > 0) && st->kcap < st->cap) {
         cudaFree(st->keys);
         st->keys = nullptr; st->kcap = 0;
         AMB_STAGE_TRY(AMB_STAGE_FIELDS, amb_decode_alloc(&st->keys, (size_t)st->cap * sizeof(AmbPosRec), -1, s));
@@ -299,12 +310,23 @@ static int amb_decode_prepare(AmbDecodeState* st, int n, cudaStream_t s, cudaErr
         AMB_STAGE_TRY(AMB_STAGE_BEAST, amb_report_bufs_alloc(&st->bb, &st->bcap, st->cap, AMB_BEAST_MAX_MSG, s));
     if (st->avr > 0 && st->acap < st->cap)
         AMB_STAGE_TRY(AMB_STAGE_AVR, amb_report_bufs_alloc(&st->ab, &st->acap, st->cap, AMB_AVR_MAX_LINE, s));
+    if (st->flightgear > 0) {                           // every slot without a callsign or a velocity
+        if (!st->ftable)
+            AMB_STAGE_TRY(AMB_STAGE_FLIGHTGEAR, amb_decode_alloc(&st->ftable, (size_t)AMB_FG_SLOTS * sizeof(AmbFgSlot), 0, s));
+        if (st->fcap < st->cap) {
+            cudaFree(st->fst);
+            st->fst = nullptr; st->fcap = 0;
+            AMB_STAGE_TRY(AMB_STAGE_FLIGHTGEAR, amb_decode_alloc(&st->fst, (size_t)st->cap * sizeof(AmbFgSlot), -1, s));
+            AMB_STAGE_TRY(AMB_STAGE_FLIGHTGEAR, amb_report_bufs_alloc(&st->fb, &st->fcap, st->cap, AMB_FG_PACKET, s));
+        }
+    }
     return 0;
 }
 
 // amb_decoder_reset on stream s, for whatever is allocated: every table empty again. The rows of the aircraft table
 // and its extension stay (a row whose bit is clear is never read), and so does the SBS-1 id table (ids up to G are
-// dead once base = G); the coverage grid is cleared; the text reports' first-message flag is set again. Returns 0, or
+// dead once base = G); the coverage grid is cleared; the text reports' first-message flag is set again; the FlightGear
+// state table is cleared with a memset (no callsign, no velocity). Returns 0, or
 // the AMB_STAGE_* code of the stage whose memory could not be cleared, with *err set.
 static int amb_decode_reset(AmbDecodeState* st, cudaStream_t s, cudaError_t* err)
 {
@@ -327,6 +349,8 @@ static int amb_decode_reset(AmbDecodeState* st, cudaStream_t s, cudaError_t* err
         static const unsigned one = 1u;
         AMB_STAGE_TRY(AMB_STAGE_REPORTS, cudaMemcpyAsync(st->rfirst, &one, sizeof one, cudaMemcpyHostToDevice, s));
     }
+    if (st->ftable)
+        AMB_STAGE_TRY(AMB_STAGE_FLIGHTGEAR, cudaMemsetAsync(st->ftable, 0, (size_t)AMB_FG_SLOTS * sizeof(AmbFgSlot), s));
     return 0;
 }
 #undef AMB_STAGE_TRY
@@ -336,13 +360,14 @@ static void amb_decode_free(AmbDecodeState* st)
 {
     void* const all[] = {st->table, st->nl_T, st->pos, st->pair, st->keys, st->ltable, st->ctable, st->otable, st->trows,
                          st->tocc, st->tclk, st->snap_cnt, st->xrows, st->xocc, st->stable, st->sctr, st->cgrid,
-                         st->rfirst};
+                         st->rfirst, st->ftable, st->fst};
     for (void* p : all) cudaFree(p);
     amb_v3_free(&st->v3);
     amb_sbs1_bufs_free(&st->sb);
     amb_report_bufs_free(&st->rb);
     amb_report_bufs_free(&st->bb);
     amb_report_bufs_free(&st->ab);
+    amb_report_bufs_free(&st->fb);
     *st = AmbDecodeState();
 }
 
@@ -350,16 +375,17 @@ static void amb_decode_free(AmbDecodeState* st)
 // local CPR stage when its S is > 0, the coverage map when coverage is on (after the local stage, so that local fixes
 // reach it), the Comm-B, op-status and track stages whose S is > 0, and the track extension when track and track_ext
 // are both > 0, then the SBS-1 feed when sbs1 is on, then the text reports when reports is on, then the Beast feed
-// and the AVR feed when beast / avr is on. Returns how many kernels were launched (7, plus 6 per stage that is on, plus
-// 1 for the coverage map, 10 for the SBS-1 feed and 3 each for the text reports, the Beast and the AVR feed), or an
-// AMB_STAGE_* code with *err set. Only a decode that launches every stage leaves the output of the SBS-1 feed, the text
-// reports and the two raw feeds, whichever is on, for amb_decode_text: sbs1_nb, reports_nb, beast_nb and avr_nb are -1
+// and the AVR feed when beast / avr is on, then the FlightGear feed when flightgear is on. Returns how many kernels were
+// launched (7, plus 6 per stage that is on, plus 1 for the coverage map, 10 for the SBS-1 feed, 3 each for the text
+// reports, the Beast and the AVR feed and 9 for the FlightGear feed), or an AMB_STAGE_* code with *err set. Only a
+// decode that launches every stage leaves the output of the SBS-1 feed, the text reports, the two raw feeds and the
+// FlightGear feed, whichever is on, for amb_decode_text: sbs1_nb, reports_nb, beast_nb, avr_nb and flightgear_nb are -1
 // otherwise, and a caller that ends a decode before this call (n = 0, a failure) sets them to -1 itself.
 static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n, amb_fields* fields, cudaStream_t s,
                              cudaError_t* err)
 {
     const int nb = (n + 127) / 128;
-    st->sbs1_nb = st->reports_nb = st->beast_nb = st->avr_nb = -1;
+    st->sbs1_nb = st->reports_nb = st->beast_nb = st->avr_nb = st->flightgear_nb = -1;
     AMB_LAUNCH((amb_fields_kernel), nb, 128, 0, s, frames, n, fields, st->pos, st->pair);
     if ((*err = cudaGetLastError()) != cudaSuccess) return AMB_STAGE_FIELDS;
     const int kp = amb_v3_launch(&st->v3, st->pos, n, st->table, st->pair, s, err);
@@ -420,26 +446,32 @@ static int amb_decode_launch(AmbDecodeState* st, const amb_frame* frames, int n,
         if (ka < 0) return AMB_STAGE_AVR;
         k += ka;
     }
+    if (st->flightgear > 0) {
+        const int kf = amb_fg_launch(&st->v3, frames, fields, st->keys, n, st->ftable, st->fst, &st->fb, s, err);
+        if (kf < 0) return AMB_STAGE_FLIGHTGEAR;
+        k += kf;
+    }
     if (st->sbs1 > 0) st->sbs1_nb = nb;
     if (st->reports > 0) st->reports_nb = nb;
     if (st->beast > 0) st->beast_nb = nb;
     if (st->avr > 0) st->avr_nb = nb;
+    if (st->flightgear > 0) st->flightgear_nb = nb;
     return k;
 }
 
 // ---- read-outs ----------------------------------------------------------------------------------------------------
 // The outputs amb_decode_text reads out, by kind.
-enum { AMB_TEXT_SBS1 = 0, AMB_TEXT_REPORTS = 1, AMB_TEXT_BEAST = 2, AMB_TEXT_AVR = 3 };
+enum { AMB_TEXT_SBS1 = 0, AMB_TEXT_REPORTS = 1, AMB_TEXT_BEAST = 2, AMB_TEXT_AVR = 3, AMB_TEXT_FLIGHTGEAR = 4 };
 
-// The output of the last decode of one kind (AMB_TEXT_*: the SBS-1 lines, the text reports, the Beast messages or the
-// AVR lines), on stream s: *text its packed bytes in the state's memory and *bytes their count, or NULL and 0 when the
+// The output of the last decode of one kind (AMB_TEXT_*: the SBS-1 lines, the text reports, the Beast messages, the
+// AVR lines or the FlightGear packets), on stream s: *text its packed bytes in the state's memory and *bytes their count, or NULL and 0 when the
 // last decode wrote none.
 static cudaError_t amb_decode_text(const AmbDecodeState* st, int kind, cudaStream_t s, const char** text,
                                    unsigned long long* bytes)
 {
-    const int nbs[] = {st->sbs1_nb, st->reports_nb, st->beast_nb, st->avr_nb};
-    const char* texts[] = {st->sb.text, st->rb.text, st->bb.text, st->ab.text};
-    const unsigned long long* boffs[] = {st->sb.boff, st->rb.boff, st->bb.boff, st->ab.boff};
+    const int nbs[] = {st->sbs1_nb, st->reports_nb, st->beast_nb, st->avr_nb, st->flightgear_nb};
+    const char* texts[] = {st->sb.text, st->rb.text, st->bb.text, st->ab.text, st->fb.text};
+    const unsigned long long* boffs[] = {st->sb.boff, st->rb.boff, st->bb.boff, st->ab.boff, st->fb.boff};
     const int nb = nbs[kind];
     *text = nullptr; *bytes = 0;
     if (nb < 0) return cudaSuccess;

@@ -19,9 +19,6 @@
 #pragma once
 
 #define AMB_MLAT_C (299792458.0 / 1.0003)       // mlat.py:95
-#define AMB_MLAT_WGS_A 6378137.0                 // mlat.py:52-54
-#define AMB_MLAT_WGS_B 6356752.314245
-#define AMB_MLAT_WGS_E2 0.0066943799901975848
 #define AMB_MLAT_MAX_STEPS 25
 #define AMB_MLAT_STOP 1e-3                       // |dx| in m
 #define AMB_MLAT_RCOND 1e-9

@@ -94,7 +94,7 @@ OPTIONS = {"local_cpr": ("seconds", 0, LOCAL_CPR_MAX), "track": ("seconds", 0, T
            "commb": ("seconds", 0, COMMB_MAX), "opstatus": ("seconds", 0, OPSTATUS_MAX),
            "track_ext": ("seconds", 0, TRACK_EXT_MAX), "sbs1": ("switch", 0, 1),
            "sbs1_tz": ("minutes", SBS1_TZ_MIN, SBS1_TZ_MAX), "coverage": ("switch", 0, 1), "reports": ("switch", 0, 1),
-           "beast": ("switch", 0, 1), "avr": ("form", 0, 2)}
+           "beast": ("switch", 0, 1), "avr": ("form", 0, 2), "flightgear": ("switch", 0, 1)}
 # the maxima of the options in seconds
 OPTION_MAX = {name: top for name, (kind, _, top) in OPTIONS.items() if kind == "seconds"}
 
@@ -132,6 +132,7 @@ check_coverage = functools.partial(check_option, "coverage")
 check_reports = functools.partial(check_option, "reports")
 check_beast = functools.partial(check_option, "beast")
 check_avr = functools.partial(check_option, "avr")
+check_flightgear = functools.partial(check_option, "flightgear")
 
 
 def commb_outcome(records):
@@ -338,13 +339,18 @@ class batch_decoder:
     payload, a 48-bit 12 MHz timestamp from the frame's stamp and a signal byte); avr = 1 writes it as an AVR raw line
     ("*<hex>;", port 30002), avr = 2 as one with the timestamp ("@<timestamp><hex>;"). Read the last decode's bytes
     with beast_bytes() / beast_bytes_device() and avr_text() / avr_text_device() (DESIGN.md §8 "Beast and AVR
-    feeds")."""
+    feeds").
+    flightgear = True also writes, on the device, the FlightGear multiplayer position packets (232 bytes each, one UDP
+    datagram apiece) the reference's output_flightgear would send: one per position of an aircraft whose callsign and
+    velocity have been heard since the last reset, with each aircraft's latest callsign and velocity carried from call
+    to call; read the last decode's packets with flightgear_bytes() / flightgear_bytes_device() and send them with
+    flightgear.fg_sender (DESIGN.md §8 "FlightGear multiplayer feed")."""
 
     def __init__(self, my_location=None, device: int = 0, local_cpr: int = 0, track: int = 0, commb: int = 0,
                  opstatus: int = 0, track_ext: int = 0, sbs1=False, sbs1_tz: int = 0, coverage=False,
-                 reports=False, beast=False, avr: int = 0):
+                 reports=False, beast=False, avr: int = 0, flightgear=False):
         values = dict(local_cpr=local_cpr, track=track, commb=commb, opstatus=opstatus, track_ext=track_ext, sbs1=sbs1,
-                      sbs1_tz=sbs1_tz, coverage=coverage, reports=reports, beast=beast, avr=avr)
+                      sbs1_tz=sbs1_tz, coverage=coverage, reports=reports, beast=beast, avr=avr, flightgear=flightgear)
         settings = {name: check_option(name, values[name]) for name in OPTIONS}
         self._lib = _lib.load()
         h = C.c_void_p()
@@ -513,6 +519,23 @@ class batch_decoder:
         """avr_text() into out_dev, a CUDA uint8 tensor; returns the byte count. Only the count crosses PCIe. Raises
         RuntimeError (with the size needed) when out_dev is too small."""
         return self._text_device(self._lib.amb_decoder_avr_device, "avr_text_device", out_dev)
+
+    def set_flightgear(self, on):
+        """Option flightgear on (True) or off (False); applies from the next decode."""
+        self._set_option("flightgear", on)
+
+    def get_flightgear(self) -> bool:
+        return bool(self._options["flightgear"])
+
+    def flightgear_bytes(self) -> bytes:
+        """The FlightGear position packets of the last decode, concatenated (232 bytes each). Needs the option
+        flightgear on."""
+        return self._text(self._lib.amb_decoder_flightgear)
+
+    def flightgear_bytes_device(self, out_dev) -> int:
+        """flightgear_bytes() into out_dev, a CUDA uint8 tensor; returns the byte count. Only the count crosses PCIe.
+        Raises RuntimeError (with the size needed) when out_dev is too small."""
+        return self._text_device(self._lib.amb_decoder_flightgear_device, "flightgear_bytes_device", out_dev)
 
     def set_coverage(self, on):
         """Option coverage on (True) or off (False); applies from the next decode. The grid is kept while it is off."""

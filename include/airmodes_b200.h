@@ -687,6 +687,45 @@ typedef struct amb_aircraft_ext {
  * Per frame of capacity, 4 + 44 bytes (Beast) and 4 + 43 bytes (AVR) plus 12 bytes per 128 frames each, allocated at
  * the first decode with the option on. A decode launches three kernels more per option that is on; with both off
  * nothing changes. */
+
+/* FlightGear multiplayer feed (amb_decoder_set_option(d, "flightgear", 1)): every decode also writes the position
+ * packets that the reference's output_flightgear (python/flightgear.py, modes_rx -m HOST:PORT) would send by UDP for
+ * its records, in record order, continuing across calls since the last amb_decoder_reset. t = secs + frac of the
+ * record's frame.
+ *   1 published  a record counts when its frame was queued, its status lacks AMB_FS_NO_HANDLER, its df is 17 and its
+ *                bds is 0x05, 0x06, 0x08 or 0x09 (the type17_dl messages, flightgear.py:28); icao is the address.
+ *   2 callsign   BDS0,8 sets the address's (ident, model): ident = the record's 8 characters; model = modelmap
+ *                (flightgear.py:116-132) of categories[ftc - 1][cat] (parse.py:270-275), the santa model where modelmap
+ *                has no entry (RESERVED, PARACHUTE, the OBSTRUCTIONs). A cat beyond its ftc row (ftc 2, cat 7: the
+ *                reference raises IndexError) changes nothing.
+ *   3 velocity   BDS0,9 subtype 0 sets (heading, velocity, turn rate) = (val[1], val[0], val[3]); subtype 1 sets
+ *                (val[1], val[0], 0); subtype 3 changes nothing.
+ *   4 packet     BDS0,5 with AMB_FS_HAS_POS gives (lat, lon, altitude), BDS0,6 with it (lat, lon, 0); a local fix
+ *                (option "local_cpr") counts. When the address has had a callsign and a velocity since the reset (in
+ *                this call or an earlier one), the record writes one packet with the latest of each. Callsign and
+ *                velocity records write none. No packet either where the reference raises TypeError: the half angle
+ *                of the orientation has sin < 1e-12 (e.g. lat -90, lon 0, heading 0 or 360).
+ *   5 bytes      232, big-endian: "FGFS", 0x00010001, msgid 7, msglen 232, 0, 0, ident (8 bytes); the model path
+ *                NUL-padded to 96 bytes; t and 0.0 as doubles (the reference's time.time() replaced by the frame's
+ *                stamp); llh2ecef(lat, lon, alt * 0.3048) (mlat.py:75-86) as three doubles; the orientation as three
+ *                floats; (float)(velocity * 0.514444444), 0, 0; 0, 0, (float)(turn rate * (pi / 180.)); six zero
+ *                floats and a zero uint32.
+ *   orientation  angle * axis of Quat([lat, lon]) * Quat([heading, 0, 0]) (Quaternion.py), each IEEE double operation
+ *                in the reference's order, then rounded to float. With P = pi / 180.:
+ *                  a = (-S zd * S yd, C zd * S yd, S zd * C yd, C zd * C yd), zd = 0.5 * (lon * P),
+ *                      yd = -0.25 * pi - 0.5 * (lat * P), S = sin, C = cos (_latlontoquat);
+ *                  ra = heading * (pi / 180.0), dec = roll = 0.0 * (pi / 180.0); T = the matrix of
+ *                      _equatorial2transform with its products as written (T00 = ca * cd, T10 = -ca * sd * sr - sa * cr,
+ *                      ...); den = (1 + T00 - T11 - T22, 1 - T00 + T11 - T22, 1 - T00 - T11 + T22, 1 + T00 + T11 + T22);
+ *                      m = the first index of the largest den; b[m] = 0.5 * sqrt(den[m]), the other three from the
+ *                      off-diagonal sums over 4 b[m] (_transform2quat);
+ *                  q = a * b (the product of Quaternion.py:393-415, left to right), then q = -q unless q[3] > 0;
+ *                  norm = sqrt(((q0^2 + q1^2) + q2^2) + q3^2), rnorm = 1 / norm, angle = acos(clamp(rnorm * q3, -1, 1)),
+ *                      s = sin(angle); orientation_i = (float)((2 * angle) * ((rnorm / s) * q_i)).
+ * The latest callsign and velocity of every address live in a direct-mapped table in device memory (2^24 x 32 B =
+ * 512 MiB), allocated at the first decode with the option on and cleared by amb_decoder_reset; per frame of capacity
+ * 32 + 4 + 232 bytes plus 12 bytes per 128 frames. A decode with the option on launches nine kernels more; with it off
+ * nothing changes. */
 typedef struct amb_decoder amb_decoder;
 /* cpr_decoder(my_location) (cpr.py:184-190) + the parser; have_location = 0 is my_location = None. */
 AMB_API int amb_decoder_create(int device, int have_location, double lat, double lon, amb_decoder** out);
@@ -716,6 +755,8 @@ AMB_API int amb_decoder_create(int device, int have_location, double lat, double
  * "beast": 0 (default, off) or 1, the Beast binary feed (see amb_decoder_beast); applies from the next call.
  * "avr": 0 (default, off), 1 ("*" lines) or 2 ("@" lines with the timestamp), the AVR raw feed (see amb_decoder_avr);
  * applies from the next call.
+ * "flightgear": 0 (default, off) or 1, the FlightGear multiplayer feed (see amb_decoder_flightgear); applies from the
+ * next call.
  * Unknown names and out-of-range values return AMB_ERR_INVALID. */
 AMB_API int amb_decoder_set_option(amb_decoder* d, const char* name, int value);
 /* Snapshot of the per-aircraft table at time `now`: every row with seen <= now and now - seen <= S, in ascending
@@ -752,6 +793,12 @@ AMB_API int amb_decoder_beast(amb_decoder* d, char* out, size_t cap, size_t* n_b
 AMB_API int amb_decoder_beast_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes);
 AMB_API int amb_decoder_avr(amb_decoder* d, char* out, size_t cap, size_t* n_bytes);
 AMB_API int amb_decoder_avr_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes);
+/* The FlightGear position packets of the last decode (232 bytes each, one UDP datagram apiece), concatenated, into out
+ * (cap bytes); *n_bytes = their length. AMB_ERR_STATE when the option "flightgear" is off; a buffer of fewer than
+ * *n_bytes bytes returns AMB_ERR_OVERFLOW with nothing written (out may then be NULL with cap 0). One 8-byte copy to
+ * the host, then the bytes; _device copies them to device memory instead, so only the byte count crosses PCIe. */
+AMB_API int amb_decoder_flightgear(amb_decoder* d, char* out, size_t cap, size_t* n_bytes);
+AMB_API int amb_decoder_flightgear_device(amb_decoder* d, char* out_dev, size_t cap, size_t* n_bytes);
 /* The coverage grid, AMB_COVERAGE_ROWS x AMB_COVERAGE_BANDS doubles, row-major (bearing row first, band second), into
  * out (host memory); _device copies it to device memory. All zeros before the first decode with the option on.
  * amb_decoder_coverage_reset clears the grid and nothing else (az_map_model.reset, az_map.py:77-82). All three return
@@ -763,7 +810,8 @@ AMB_API void amb_decoder_destroy(amb_decoder* d);
 AMB_API int amb_decoder_set_location(amb_decoder* d, int have_location, double lat, double lon);   /* cpr.py:192-193 */
 AMB_API int amb_decoder_reset(amb_decoder* d);                      /* forget every stored report, reference position,
                                                                        velocity, op status, aircraft and extension
-                                                                       group, and clear the coverage grid */
+                                                                       group, SBS-1 id and FlightGear callsign and
+                                                                       velocity, and clear the coverage grid */
 /* Decode n frames (host or device array, stream order = non-decreasing time). out: n records in host memory.
  * Frames with passed == 0 get AMB_FS_NOT_QUEUED and do not touch the CPR state. */
 AMB_API int amb_decode_frames(amb_decoder* d, const amb_frame* frames, int n, int mem_kind, amb_fields* out);

@@ -16,8 +16,10 @@ GPU by the decoder (option coverage) and written to PATH as JSON after every chu
 served as the Beast binary feed of dump1090 and readsb (default port 30005, what mlat-client and the other consumers of
 a receiver's raw frames read), with --avr [PORT] as the AVR raw feed (default port 30002; --avr-mlat for the "@" lines
 with the timestamp): the bytes are formed on the GPU by the decoder (options beast and avr) from the receive chain's own
-frames, stamps and levels, and sent by gr_air_modes_b200.sbs1's server. KML and FlightGear outputs are the reference's
-own pure-Python consumers of the dl_data feed and are not re-implemented.
+frames, stamps and levels, and sent by gr_air_modes_b200.sbs1's server. With -m HOST:PORT (--multiplayer, as
+apps/modes_rx -m) every aircraft heard with a callsign, a velocity and a position is sent to a FlightGear multiplayer
+server or instance at HOST:PORT, one UDP position packet per position message: the packets are formed on the GPU by the
+decoder (option flightgear) and sent by gr_air_modes_b200.flightgear, stamped with the message's time.
 
 With --input beast the frames come from another receiver instead of the IQ chain: -s FILE replays a recorded Beast
 binary byte stream, -s HOST:PORT connects over TCP to a Beast server (dump1090 or readsb on port 30005, or this tool's
@@ -37,6 +39,7 @@ chain (-d, -r, -T, --ec, --ec-any, --ap-filter, --resample) are errors with --in
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -l 37.4,-122.1 -P 30003
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -l 37.4,-122.1 --coverage coverage.json
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -n --beast 30005 --avr 30002 --avr-mlat
+    python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -l 37.4,-122.1 -m 127.0.0.1:5000
     python tools/modes_rx_b200.py --input beast -s 192.168.1.20:30005 --reports
     python tools/modes_rx_b200.py --input beast -s feed.bin -l 37.4,-122.1 -P 30003
 
@@ -159,24 +162,26 @@ class report_queue:
     the lines on the device (option reports: gr_air_modes_b200.report's lines). out=None decodes without printing;
     aircraft=PATH writes the decoder's aircraft table (option track) to PATH after every batch, with the extension of
     every row when track_ext is on; sbs1=server (gr_air_modes_b200.sbs1.sbs1_server) sends the batch's SBS-1 lines to
-    it, with the date and time shifted by sbs1_tz minutes; coverage=PATH writes the decoder's coverage map (option
+    it, with the date and time shifted by sbs1_tz minutes; flightgear=sender (gr_air_modes_b200.flightgear.fg_sender)
+    sends the batch's FlightGear position packets to it; coverage=PATH writes the decoder's coverage map (option
     coverage) to PATH after every batch (decode.coverage_to_dict). A decoder given as `decoder` is used as it is, except
     that option reports is turned on when out is not None."""
 
     def __init__(self, location, device, out=sys.stdout, local_cpr=0, track=0, aircraft=None, decoder=None, commb=0,
-                 opstatus=0, track_ext=0, sbs1=None, sbs1_tz=0, coverage=None):
+                 opstatus=0, track_ext=0, sbs1=None, sbs1_tz=0, coverage=None, flightgear=None):
         from gr_air_modes_b200 import decode
         self._dec = decoder if decoder is not None else \
             decode.batch_decoder(location, device, local_cpr=local_cpr, track=track, commb=commb,
                                  opstatus=opstatus, track_ext=track_ext, sbs1=sbs1 is not None,
                                  sbs1_tz=sbs1_tz, coverage=coverage is not None,
-                                 reports=out is not None)   # = cpr_decoder(my_position), apps/modes_rx:68
+                                 flightgear=flightgear is not None, reports=out is not None)   # = cpr_decoder(my_position), apps/modes_rx:68
         if decoder is not None and out is not None:
             decoder.set_reports(True)                   # flush() prints the decoder's text reports
         self._out, self._texts, self.count, self._aircraft = out, [], 0, aircraft
         self._coverage, self._location = coverage, location
         self._ext = track_ext > 0
         self._sbs1 = sbs1
+        self._fg = flightgear
 
     def handle(self, msg):
         text = msg.to_string()
@@ -190,6 +195,8 @@ class report_queue:
             self._dec.decode_messages(self._texts)
             if self._sbs1 is not None:
                 self._sbs1.send(self._dec.sbs1_text())
+            if self._fg is not None:
+                self._fg.send(self._dec.flightgear_bytes())
             if self._out is not None:
                 text = self._dec.report_text()
                 self._out.write(text.decode("latin-1"))
@@ -209,6 +216,8 @@ class report_queue:
         self._dec.close()
         if self._sbs1 is not None:
             self._sbs1.close()
+        if self._fg is not None:
+            self._fg.close()
 
 
 class raw_feed:
@@ -364,6 +373,8 @@ def parse_args(argv=None):
     ap.add_argument("--sbs1-wait", type=float, default=0.0, metavar="S",
                     help="with -P: wait up to S seconds for the first SBS-1 client before reading the source (for "
                          "replaying a recording); 0 = start at once, as modes_rx")
+    ap.add_argument("-m", "--multiplayer", type=str, default=None, metavar="HOST:PORT",
+                    help="FlightGear multiplayer feed: UDP position packets to HOST:PORT")                      # apps/modes_rx:50-51
     ap.add_argument("--coverage", type=str, default=None, metavar="PATH",
                     help="after every chunk, write the receiver coverage map to PATH as JSON: the greatest range "
                          "(statute miles) heard per 5-degree bearing sector and altitude band, as modes_gui's azimuth "
@@ -404,6 +415,11 @@ def parse_args(argv=None):
         ap.error("--feed-wait: 0 .. 3600 seconds")
     if args.feed_wait and args.beast is None and args.avr is None:
         ap.error("--feed-wait needs --beast or --avr")
+    if args.multiplayer is not None:
+        m = re.fullmatch(r"(.+):(\d{1,5})", args.multiplayer)                                                    # apps/modes_rx:80-82
+        if not m or not 0 < int(m.group(2)) < 65536:
+            ap.error("--multiplayer: HOST:PORT with a UDP port 1 .. 65535")
+        args.multiplayer = (m.group(1), int(m.group(2)))
     if not 0 <= args.track <= 3600:
         ap.error("--track: 0 (off) .. 3600 seconds")
     if args.aircraft and args.track <= 0:
@@ -520,6 +536,9 @@ def make_outputs(args):
     feed = {"sbs1": server, "sbs1_tz": local_utc_offset_minutes()} if server is not None else {}
     if args.coverage:
         feed["coverage"] = args.coverage
+    if args.multiplayer is not None:
+        from gr_air_modes_b200.flightgear import fg_sender
+        feed["flightgear"] = fg_sender(*args.multiplayer)                                                         # apps/modes_rx:80-82
     if not args.no_print:
         if args.reports or args.location is not None:
             reporter = report_queue(my_position, args.device, local_cpr=args.local_cpr, track=args.track, commb=args.commb,
@@ -528,7 +547,7 @@ def make_outputs(args):
         else:
             printer = print_queue()
             sinks.append(printer)
-    if (args.aircraft or server is not None or args.coverage) and reporter is None:   # no printed reports
+    if (args.aircraft or server is not None or args.coverage or args.multiplayer) and reporter is None:   # no printed reports
         reporter = report_queue(my_position, args.device, out=None, local_cpr=args.local_cpr, track=args.track,
                                 aircraft=args.aircraft, **({"commb": args.commb, "opstatus": args.opstatus,
                                                             "track_ext": args.track_ext} if args.track_ext else {}),
