@@ -11,8 +11,8 @@ reference's names for the path (python/__init__.py:34,44 exports the swig blocks
 Importing the package does not need a GPU; constructing a block does (no CPU fallback).
 """
 from .blocks import (preamble, slicer, rx_path, modes_check_crc, modes_crc, msg_queue, message,
-                     message_from_string, format_message, query_geometry)
+                     message_from_string, format_message, query_geometry, MODEAC_DTYPE)
 from ._lib import Frame, Stats
 
 __all__ = ["preamble", "slicer", "rx_path", "modes_check_crc", "modes_crc", "msg_queue", "message",
-           "message_from_string", "format_message", "query_geometry", "Frame", "Stats"]
+           "message_from_string", "format_message", "query_geometry", "MODEAC_DTYPE", "Frame", "Stats"]

@@ -203,6 +203,12 @@ assert C.sizeof(MlatFix) == 112
 assert C.sizeof(MlatCounts) == 80
 assert C.sizeof(BeastCounts) == 72
 
+
+class ModeacStats(C.Structure):
+    _fields_ = [("candidates", C.c_uint64), ("replies", C.c_uint64), ("overlap_drops", C.c_uint64), ("with_altitude", C.c_uint64)]
+
+assert C.sizeof(ModeacStats) == 32
+
 # every symbol include/airmodes_b200.h declares: (name, restype, argtypes)
 _vp, _f32p, _u64p = C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_uint64)
 SYMBOLS = [
@@ -238,6 +244,10 @@ SYMBOLS = [
     ("amb_join", C.c_int, [_vp]),
     ("amb_debug_candidates", C.c_int, [_vp, _u64p, C.POINTER(C.c_uint32), C.c_int]),
     ("amb_set_option", C.c_int, [_vp, C.c_char_p, C.c_int]),
+    ("amb_poll_modeac", C.c_int, [_vp, _vp, C.c_int]),
+    ("amb_pending_modeac", C.c_int, [_vp]),
+    ("amb_drain_modeac_device", C.c_int, [_vp, _vp, C.c_int]),
+    ("amb_get_modeac_stats", C.c_int, [_vp, C.POINTER(ModeacStats)]),
     ("amb_dump_stage", C.c_int, [_vp, C.c_int, _f32p, C.c_size_t, _f32p]),
     ("amb_seek", C.c_int, [_vp, C.c_uint64, C.c_uint64, C.POINTER(WalkState)]),
     ("amb_resolve", C.c_int, [_vp, C.POINTER(WalkState)]),

@@ -18,7 +18,13 @@ import threading
 import numpy as np
 
 from . import _lib
-from ._lib import Frame, Geometry, Stats, WalkState, WalkSummary, check
+from ._lib import Frame, Geometry, ModeacStats, Stats, WalkState, WalkSummary, check
+
+# amb_modeac (include/airmodes_b200.h, option "modeac"): one Mode A/C reply, 48 bytes
+MODEAC_DTYPE = np.dtype([("sample_index", "<u8"), ("secs", "<u8"), ("frac", "<f8"), ("peak", "<f4"), ("floor", "<f4"),
+                         ("altitude", "<i4"), ("code", "<u2"), ("squawk", "<u2"), ("spi", "u1"), ("pad_", "u1", (7,))])
+assert MODEAC_DTYPE.itemsize == 48
+NO_ALTITUDE = -(1 << 31)    # AMB_NO_ALTITUDE
 
 
 # ---------------------------------------------------------------------------------------------
@@ -346,10 +352,15 @@ class rx_path:
     last S seconds of the stream (counted in samples, S * int(rate)); DF11 replies whose parity carries a non-zero
     interrogator code (syndrome 1..0x7F) are accepted when their address is known that way. Frames record the outcome in
     .ap. reset() / set_rate() forget the confirmed addresses and keep the option. Not available with seek() /
+    defer_resolve().
+
+    modeac=True (extension, default off): also find Mode A/C replies (F1, 13 code pulses, F2 at 20.3 us, SPI) in the same
+    front end, by the rules of include/airmodes_b200.h; modeac() / modeac_device() return them in stream order. Set
+    before the first process() of a stream (set_modeac); kept across reset() / set_rate(). Not available with seek() /
     defer_resolve()."""
 
     def __init__(self, rate, threshold, queue, use_pmf=False, use_dcblock=False, device: int = 0, ec: int = 0,
-                 ec_any: int = 0, ap_filter: int = 0):
+                 ec_any: int = 0, ap_filter: int = 0, modeac: bool = False):
         self._rate = int(rate)                      # rx_path.py:32
         self._threshold = threshold
         self._queue = queue
@@ -359,6 +370,9 @@ class rx_path:
         self._slicer = slicer(queue, device, _ctx=self._ctx, ec=ec, ec_any=ec_any)
         if ap_filter:
             self.set_ap_filter(ap_filter)
+        self._modeac = False
+        if modeac:
+            self.set_modeac(True)
         self.frames = []                            # every detection of the last process() call
         self._keep = []                             # device inputs still being read
 
@@ -406,6 +420,44 @@ class rx_path:
 
     def get_ap_filter(self) -> int:
         return self._ctx.ap_filter
+
+    # -- extension: Mode A/C replies (see the class docstring)
+    def set_modeac(self, on: bool):
+        """Find Mode A/C replies from the next stream on: only before the first process() after construction, reset()
+        or set_rate()."""
+        self._ctx.call("amb_set_option", b"modeac", int(bool(on)))
+        self._modeac = bool(on)
+
+    def get_modeac(self) -> bool:
+        return self._modeac
+
+    def modeac(self) -> np.ndarray:
+        """Every reply not handed out yet, in stream order and stamped: a numpy array of MODEAC_DTYPE (waits for the
+        work given so far)."""
+        n = self._ctx.call("amb_pending_modeac")
+        out = np.zeros(n, MODEAC_DTYPE)
+        got = self._ctx.call("amb_poll_modeac", out.ctypes.data_as(C.c_void_p), n) if n else 0
+        return out[:got]
+
+    def modeac_device(self, out=None):
+        """The device-side modeac(): a torch CUDA uint8 tensor of n * 48 bytes (amb_modeac records in stream order,
+        stamped) that never crosses to the host. Replies modeac() already fetched are not included."""
+        import torch
+        n = self._ctx.call("amb_drain_modeac_device", None, 0)
+        dev = torch.device("cuda", self._ctx.device)
+        if out is None:
+            out = torch.empty(n * 48, dtype=torch.uint8, device=dev)
+        elif out.numel() < n * 48:
+            raise ValueError("modeac_device: out holds %d bytes, %d needed" % (out.numel(), n * 48))
+        torch.cuda.current_stream(dev).synchronize()
+        got = self._ctx.call("amb_drain_modeac_device", C.c_void_p(out.data_ptr()), int(out.numel() // 48)) if n else 0
+        return out[:got * 48]
+
+    def modeac_stats(self) -> ModeacStats:
+        """Counts since the stream began: candidates (rules 1-2), replies, overlap drops (rule 7), with altitude."""
+        st = ModeacStats()
+        self._ctx.call("amb_get_modeac_stats", C.byref(st))
+        return st
 
     # -- data path
     def process(self, iq, flush: bool = False, collect: bool = True) -> int:
@@ -477,13 +529,15 @@ class rx_path:
 
     def set_option(self, name: str, value: int):
         """Library options: "coalesce", "ingest_chunk", "copy_threads", "resolver", "overlap", "keep_chips", "exact_dense",
-        "scan_ctas", "order_tile", "ec", "ec_any", "ap_filter"."""
+        "scan_ctas", "order_tile", "ec", "ec_any", "ap_filter", "modeac"."""
         if name == "ec":
             return self.set_ec(value)
         if name == "ec_any":
             return self.set_ec_any(value)
         if name == "ap_filter":
             return self.set_ap_filter(value)
+        if name == "modeac":
+            return self.set_modeac(value)
         self._ctx.call("amb_set_option", name.encode(), int(value))
 
     def reset(self):

@@ -101,6 +101,9 @@ struct amb_ctx {
     int ec_any = 0;                      // option "ec_any": DF17 correction over up to M (1, 2) bits anywhere (0 = off)
     int ap_filter = 0;                   // option "ap_filter": address/parity check against the last S seconds (0 = off)
     bool seeked = false;                 // positioned by amb_seek since the last reset (no "ap_filter" there)
+    int modeac = 0;                      // option "modeac": Mode A/C replies (set before a stream's first amb_process)
+    bool started = false;                // amb_process called since create / reset / set_rate
+    std::vector<amb_modeac> mac_pending; // replies read out of the device queue, stamped, not handed out yet
     // time-sharded operation (amb_seek / amb_resolve): a call whose walk + slice stages are still to run
     int defer = 0;                       // option "defer_resolve"
     int def_kind = 0;                    // 0 nothing pending, 1 full (walk + slice), 2 sequential walk only, 3 state only
@@ -201,8 +204,11 @@ static int reset_stream(amb_ctx* ctx)
     ctx->snap_tail = ctx->snap_head; ctx->polled = 0;
     ctx->time_tags.clear();
     ctx->seeked = false;
+    ctx->started = false;
+    ctx->mac_pending.clear();
     AmbChainErr er;
     if (amb_chain_reset(&ctx->bufs, ctx->stream_b, &er) < 0) return chain_fail(ctx, er);
+    if (ctx->modeac && amb_chain_modeac_reset(&ctx->bufs, ctx->stream_b, &er) < 0) return chain_fail(ctx, er);
     return AMB_OK;
 }
 
@@ -388,6 +394,18 @@ int amb_set_option(amb_ctx* ctx, const char* name, int value)
             return fail(ctx, AMB_ERR_STATE, "ap_filter needs the whole stream: not available in time-sharded operation");
         ctx->ap_filter = value; return AMB_OK;
     }
+    if (!strcmp(name, "modeac")) {
+        if (value < 0 || value > 1) return AMB_ERR_INVALID;
+        if (ctx->started) return fail(ctx, AMB_ERR_STATE, "modeac can only be set before the first amb_process of a stream");
+        if (value && (ctx->defer || ctx->seeked))
+            return fail(ctx, AMB_ERR_STATE, "modeac is not available in time-sharded operation");
+        if (value && !ctx->modeac) {
+            CK(ctx, cudaSetDevice(ctx->device));
+            AmbChainErr er;
+            if (amb_chain_modeac_reset(&ctx->bufs, ctx->stream_b, &er) < 0) return chain_fail(ctx, er);
+        }
+        ctx->modeac = value; return AMB_OK;
+    }
     if (!strcmp(name, "keep_chips")) { ctx->keep_chips = value != 0; return AMB_OK; }
     if (!strcmp(name, "overlap")) { ctx->overlap = value != 0; return AMB_OK; }
     if (!strcmp(name, "coalesce")) {                       // samples of small host calls gathered before a dispatch
@@ -415,6 +433,7 @@ int amb_set_option(amb_ctx* ctx, const char* name, int value)
     if (!strcmp(name, "defer_resolve")) {
         if (ctx->def_kind && !ctx->def_resolved) return fail(ctx, AMB_ERR_STATE, "amb_resolve pending");
         if (value && ctx->ap_filter) return fail(ctx, AMB_ERR_STATE, "defer_resolve is not available with ap_filter on");
+        if (value && ctx->modeac) return fail(ctx, AMB_ERR_STATE, "defer_resolve is not available with modeac on");
         ctx->def_kind = 0; ctx->def_resolved = false;
         ctx->defer = value != 0; return AMB_OK;
     }
@@ -539,6 +558,11 @@ static int process_core(amb_ctx* ctx, const float* iq, size_t n_complex, int mem
         const int k = amb_chain_launch(a, call, &ctx->bufs, opts, ctx->defer != 0, sb, &ctx->def, &er);
         if (k < 0) return chain_fail(ctx, er);
         ctx->stats.kernel_launches += (uint64_t)k;
+        if (ctx->modeac) {
+            const int km = amb_chain_modeac(a, org, &ctx->bufs, sb, [ctx] { return sync_all(ctx); }, &er);
+            if (km < 0) return chain_fail(ctx, er);
+            ctx->stats.kernel_launches += (uint64_t)km;
+        }
         if (ctx->defer) { ctx->def_kind = 1; ctx->def_resolved = false; ctx->def_set = set; }
         ctx->ev_valid = ctx->timing;
     } else {
@@ -808,7 +832,10 @@ int amb_process(amb_ctx* ctx, const float* iq, size_t n_complex, int mem_kind, i
     if (ctx->flushed) return fail(ctx, AMB_ERR_STATE, "stream already flushed; amb_reset first");
     if (ctx->def_kind && !ctx->def_resolved)
         return fail(ctx, AMB_ERR_STATE, "amb_resolve pending (deferred mode allows one call per span)");
+    if (ctx->modeac && (!ctx->use_pmf || ctx->P.spc_i < 2))
+        return fail(ctx, AMB_ERR_UNSUPPORTED, "modeac needs the PMF and a rate of at least 4 Msps");
     CK(ctx, cudaSetDevice(ctx->device));
+    ctx->started = true;
     if (ctx->defer) {     // time-sharded span: one pass, input stays where it is (or goes through the one-piece staging buffer)
         if (mem_kind != AMB_MEM_HOST && mem_kind != AMB_MEM_DEVICE)
             return fail(ctx, AMB_ERR_UNSUPPORTED, "16-bit input is not available in deferred (time-sharded) mode");
@@ -844,6 +871,7 @@ int amb_seek(amb_ctx* ctx, uint64_t first_sample, uint64_t first_decision, const
     }
     if (first_sample > (1ull << 62) || first_decision > (1ull << 62)) return fail(ctx, AMB_ERR_INVALID, "index out of range");
     if (ctx->ap_filter) return fail(ctx, AMB_ERR_STATE, "amb_seek is not available with ap_filter on (it needs the whole stream)");
+    if (ctx->modeac) return fail(ctx, AMB_ERR_STATE, "amb_seek is not available with modeac on (it needs the whole stream)");
     int rc = reset_stream(ctx);
     if (rc != AMB_OK) return rc;
     ctx->n_in = first_sample;
@@ -1131,6 +1159,123 @@ int amb_drain_device(amb_ctx* ctx, amb_frame* out_dev, int cap)
     return (int)n;
 }
 
+/* ---- Mode A/C replies (option "modeac") ---------------------------------------------------------------------- */
+// Device drain: out[i] = queue[i] stamped as stamp() stamps it (the expressions of amb_order_gather_kernel).
+__global__ void __launch_bounds__(128) amb_modeac_stamp_kernel(const amb_modeac* __restrict__ q, unsigned n, amb_modeac* __restrict__ out,
+                                                               unsigned long long rate, unsigned long long t0_secs, double t0_frac,
+                                                               const AmbTagDev* __restrict__ tags, int ntags)
+{
+    const unsigned i = blockIdx.x * 128u + threadIdx.x;
+    if (i >= n) return;
+    amb_modeac m = q[i];
+    unsigned long long off = 0, t_secs = t0_secs; double t_frac = t0_frac;
+    for (int k = ntags; k-- > 0;)
+        if (tags[k].offset <= m.sample_index) { off = tags[k].offset; t_secs = tags[k].secs; t_frac = tags[k].frac; break; }
+    const unsigned long long cnt = m.sample_index - off;
+    m.secs = t_secs + cnt / rate;
+    m.frac = t_frac + (double)(cnt % rate) / (double)rate;
+    if (m.frac > 1.0f) { m.frac -= 1.0f; m.secs += 1; }
+    out[i] = m;
+}
+
+// A reply is stamped as a frame at its sample index.
+static void stamp_modeac(const amb_ctx* ctx, amb_modeac* m)
+{
+    amb_frame f{};
+    f.sample_index = m->sample_index;
+    stamp(ctx, &f);
+    m->secs = f.secs; m->frac = f.frac;
+}
+
+// Everything enqueued is through; *n = replies in the device queue (0 with the option off).
+static int modeac_sync(amb_ctx* ctx, unsigned* n)
+{
+    CK(ctx, cudaSetDevice(ctx->device));
+    if (ctx->pend_n) { int rc = ingest_dispatch_pending(ctx, 0); if (rc) return rc; }
+    CK(ctx, sync_all(ctx));
+    *n = 0;
+    if (ctx->bufs.mac_state) CK(ctx, cudaMemcpy(n, ctx->bufs.mac_state + 6, sizeof(unsigned), cudaMemcpyDeviceToHost));
+    return AMB_OK;
+}
+
+static int modeac_consumed(amb_ctx* ctx, unsigned n)
+{
+    if (n) CK(ctx, cudaMemset(ctx->bufs.mac_state + 6, 0, sizeof(unsigned long long)));
+    ctx->bufs.mac_ub = 0;
+    return AMB_OK;
+}
+
+static int modeac_collect(amb_ctx* ctx)
+{
+    unsigned n = 0;
+    { int rc = modeac_sync(ctx, &n); if (rc) return rc; }
+    if (!n) return AMB_OK;
+    const size_t base = ctx->mac_pending.size();
+    ctx->mac_pending.resize(base + n);
+    CK(ctx, cudaMemcpy(ctx->mac_pending.data() + base, ctx->bufs.mac_queue, (size_t)n * sizeof(amb_modeac), cudaMemcpyDeviceToHost));
+    for (size_t k = base; k < ctx->mac_pending.size(); k++) stamp_modeac(ctx, &ctx->mac_pending[k]);
+    return modeac_consumed(ctx, n);
+}
+
+int amb_pending_modeac(amb_ctx* ctx)
+{
+    if (!ctx) return AMB_ERR_INVALID;
+    int rc = modeac_collect(ctx);
+    if (rc != AMB_OK) return rc;
+    return (int)ctx->mac_pending.size();
+}
+
+int amb_poll_modeac(amb_ctx* ctx, amb_modeac* out, int max)
+{
+    if (!ctx || (!out && max > 0)) return AMB_ERR_INVALID;
+    int rc = modeac_collect(ctx);
+    if (rc != AMB_OK) return rc;
+    const int n = (int)std::min<size_t>(ctx->mac_pending.size(), (size_t)std::max(max, 0));
+    if (n) memcpy(out, ctx->mac_pending.data(), (size_t)n * sizeof(amb_modeac));
+    ctx->mac_pending.erase(ctx->mac_pending.begin(), ctx->mac_pending.begin() + n);
+    return n;
+}
+
+int amb_drain_modeac_device(amb_ctx* ctx, amb_modeac* out_dev, int cap)
+{
+    if (!ctx || cap < 0) return AMB_ERR_INVALID;
+    unsigned n = 0;
+    { int rc = modeac_sync(ctx, &n); if (rc) return rc; }
+    if (!out_dev) return (int)n;
+    if ((unsigned)cap < n) return fail(ctx, AMB_ERR_OVERFLOW, "amb_drain_modeac_device: output buffer too small");
+    if (n) {
+        const int ntags = (int)ctx->time_tags.size();
+        if (ntags) {
+            if (ctx->tags_dev_cap < ntags) {
+                cudaFree(ctx->tags_dev); ctx->tags_dev = nullptr; ctx->tags_dev_cap = 0;
+                CK(ctx, cudaMalloc(&ctx->tags_dev, (size_t)ntags * 2 * sizeof(AmbTagDev)));
+                ctx->tags_dev_cap = ntags * 2;
+            }
+            std::vector<AmbTagDev> t((size_t)ntags);
+            for (int k = 0; k < ntags; k++) t[(size_t)k] = {ctx->time_tags[(size_t)k].offset, ctx->time_tags[(size_t)k].secs, ctx->time_tags[(size_t)k].frac};
+            CK(ctx, cudaMemcpy(ctx->tags_dev, t.data(), (size_t)ntags * sizeof(AmbTagDev), cudaMemcpyHostToDevice));
+        }
+        AMB_LAUNCH((amb_modeac_stamp_kernel), (n + 127) / 128, 128, 0, ctx->stream_b, ctx->bufs.mac_queue, n, out_dev,
+                   (unsigned long long)ctx->P.rate_int, ctx->t0_secs, ctx->t0_frac, ctx->tags_dev, ntags);
+        CK(ctx, cudaGetLastError());
+        ctx->stats.kernel_launches += 1;
+        CK(ctx, cudaStreamSynchronize(ctx->stream_b));
+    }
+    { int rc = modeac_consumed(ctx, n); if (rc) return rc; }
+    return (int)n;
+}
+
+int amb_get_modeac_stats(amb_ctx* ctx, amb_modeac_stats* out)
+{
+    if (!ctx || !out) return AMB_ERR_INVALID;
+    unsigned n = 0;
+    { int rc = modeac_sync(ctx, &n); if (rc) return rc; }
+    unsigned long long w[4] = {0, 0, 0, 0};
+    if (ctx->bufs.mac_state) CK(ctx, cudaMemcpy(w, ctx->bufs.mac_state + 2, sizeof w, cudaMemcpyDeviceToHost));
+    out->candidates = w[0]; out->replies = w[1]; out->overlap_drops = w[2]; out->with_altitude = w[3];
+    return AMB_OK;
+}
+
 int amb_add_time_tag(amb_ctx* ctx, uint64_t offset, uint64_t secs, double frac)
 {
     if (!ctx) return AMB_ERR_INVALID;
@@ -1380,6 +1525,7 @@ int amb_preamble_process(amb_ctx* ctx, const float* in0, const float* in1, size_
 {
     if (!ctx || (n && (!in0 || !in1)) || max_det < 0 || (max_det && (!chips_out || !index_out))) return AMB_ERR_INVALID;
     if (n > 0x40000000ull) return fail(ctx, AMB_ERR_INVALID, "at most 2^30 items per call");
+    if (ctx->modeac) return fail(ctx, AMB_ERR_STATE, "the split-form preamble block does not find Mode A/C replies (option modeac)");
     CK(ctx, cudaSetDevice(ctx->device));
     CK(ctx, sync_all(ctx));
     const AmbParams& P = ctx->P;

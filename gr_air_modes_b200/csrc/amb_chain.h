@@ -2,8 +2,9 @@
 // (tests/simt/kernels_emul.cc): the geometry of a call (carry and guard, segments, scan rows and spans, candidate and
 // frame bounds), the one owner of the per-call buffers (AmbChainBufs with amb_chain_prepare / _reset / _free) and the
 // one sparse launch sequence, compact -> exact -> [walk -> slice -> ec -> ap], which returns how many kernels it
-// launched. Host code only, with memory handled through cudaMalloc / cudaMemsetAsync / cudaMemcpy / cudaFree, so that
-// tests/simt/simt_cudart.h can stand in for the runtime.
+// launched, and beside it the Mode A/C sequence of option "modeac" (amb_chain_modeac). Host code only, with memory
+// handled through cudaMalloc / cudaMemsetAsync / cudaMemcpy / cudaFree, so that tests/simt/simt_cudart.h can stand in
+// for the runtime.
 #pragma once
 #include "amb_internal.h"
 
@@ -84,6 +85,12 @@ struct AmbChainBufs {
     unsigned frames_ub = 0;              // bound on the frames queued since they were last read out
     float* chips = nullptr;
     AmbApState ap{};                     // allocated at the first call with option "ap_filter" on
+    // option "modeac": per-call tile slots and counts, the queue of replies not read out yet, and the state
+    // {last_prev, last_cur, candidates, replies, overlap drops, with altitude, queue count} (amb_modeac.cuh)
+    amb_modeac* mac_rec = nullptr; unsigned* mac_tile_count = nullptr; size_t mac_rec_cap = 0; int mac_tiles_cap = 0;
+    amb_modeac* mac_queue = nullptr; unsigned mac_queue_cap = 0;
+    unsigned mac_ub = 0;                 // bound on the replies queued since they were last read out
+    unsigned long long* mac_state = nullptr;
 };
 
 // What failed: the call's text and its error.
@@ -204,12 +211,79 @@ static int amb_chain_reset(AmbChainBufs* b, cudaStream_t s, AmbChainErr* err)
     return 0;
 }
 
+// ---- Mode A/C replies (option "modeac") ---------------------------------------------------------------------------
+#define AMB_MODEAC_STATE_WORDS 7
+static inline int amb_modeac_off(double t_us, int rate_int) { return (int)floor(t_us * (double)rate_int / 1e6 + 0.5); }
+static inline AmbModeacGeom amb_chain_modeac_geom(int rate_int)
+{
+    AmbModeacGeom G;
+    for (int k = 0; k < 15; k++) G.slot[k] = amb_modeac_off(1.45 * k, rate_int);
+    for (int g = 0; g < 14; g++) G.gap[g] = amb_modeac_off(1.45 * g + 0.725, rate_int);
+    G.spi = amb_modeac_off(24.65, rate_int);
+    G.back = amb_modeac_off(25.1, rate_int);
+    return G;
+}
+
+// The state on s for a new stream (allocated at the first use), and nothing queued.
+static int amb_chain_modeac_reset(AmbChainBufs* b, cudaStream_t s, AmbChainErr* err)
+{
+    if (!b->mac_state) AMB_CHAIN_TRY(cudaMalloc(&b->mac_state, AMB_MODEAC_STATE_WORDS * sizeof(unsigned long long)));
+    AMB_CHAIN_TRY(cudaMemsetAsync(b->mac_state, 0, AMB_MODEAC_STATE_WORDS * sizeof(unsigned long long), s));
+    b->mac_ub = 0;
+    return 0;
+}
+
+// A call's Mode A/C pass on s over the starts [a.j_lo, a.j_hi) of the scan a (org: reported index of j = 0): buffers
+// grown (sync() once before the first growth; queued replies are copied over), then the tile and emit kernels. Returns
+// the kernels launched, or -1 with *err set.
+template <class Sync>
+static int amb_chain_modeac(const AmbScanArgs& a, long long org, AmbChainBufs* b, cudaStream_t s, Sync sync, AmbChainErr* err)
+{
+    AmbModeacArgs m{};
+    m.P = a.P; m.S = a.S; m.G = amb_chain_modeac_geom(a.P.rate_int);
+    m.j_lo = a.j_lo; m.j_hi = a.j_hi; m.org = org;
+    m.na_cap = AMB_MODEAC_TILE + m.G.back + a.P.L;
+    m.nb_cap = m.na_cap + m.G.spi + 2;
+    m.cap_tile = AMB_MODEAC_TILE / (m.G.back + 1) + 1;
+    const int n_tiles = (a.j_hi - a.j_lo + AMB_MODEAC_TILE - 1) / AMB_MODEAC_TILE;
+    const size_t rec_need = (size_t)n_tiles * m.cap_tile;
+    const unsigned ub = (unsigned)std::min<size_t>(rec_need, (size_t)(a.j_hi - a.j_lo) / (m.G.back + 1) + 1);
+    bool synced = false;
+    auto grow = [&]() -> cudaError_t { if (synced) return cudaSuccess; synced = true; return sync(); };
+    if (b->mac_rec_cap < rec_need || b->mac_tiles_cap < n_tiles) {
+        AMB_CHAIN_TRY(grow());
+        cudaFree(b->mac_rec); cudaFree(b->mac_tile_count); b->mac_rec = nullptr; b->mac_tile_count = nullptr;
+        AMB_CHAIN_TRY(cudaMalloc(&b->mac_rec, (rec_need + rec_need / 8) * sizeof(amb_modeac)));
+        AMB_CHAIN_TRY(cudaMalloc(&b->mac_tile_count, (size_t)(n_tiles + n_tiles / 8 + 1) * sizeof(unsigned)));
+        b->mac_rec_cap = rec_need + rec_need / 8; b->mac_tiles_cap = n_tiles + n_tiles / 8 + 1;
+    }
+    if (b->mac_queue_cap < b->mac_ub + ub) {
+        AMB_CHAIN_TRY(grow());
+        const unsigned ncap = (b->mac_ub + ub) * 2 + 1024;
+        amb_modeac* nq = nullptr;
+        AMB_CHAIN_TRY(cudaMalloc(&nq, (size_t)ncap * sizeof(amb_modeac)));
+        if (b->mac_queue && b->mac_ub)
+            AMB_CHAIN_TRY(cudaMemcpy(nq, b->mac_queue, (size_t)std::min(b->mac_ub, b->mac_queue_cap) * sizeof(amb_modeac), cudaMemcpyDeviceToDevice));
+        cudaFree(b->mac_queue);
+        b->mac_queue = nq; b->mac_queue_cap = ncap;
+    }
+    b->mac_ub += ub;
+    m.rec = b->mac_rec; m.tile_count = b->mac_tile_count;
+    m.last_prev = b->mac_state; m.last_cur = b->mac_state + 1; m.stats = b->mac_state + 2;
+    m.queue = b->mac_queue; m.q_count = reinterpret_cast<unsigned*>(b->mac_state + 6);
+    cudaError_t e = cudaSuccess;
+    const int k = amb_launch_modeac(m, s, &e);
+    AMB_CHAIN_TRY(e);
+    return k;
+}
+
 // Free everything and leave the buffers as new ones (the caller has synchronised with their last use).
 static void amb_chain_free(AmbChainBufs* b)
 {
     void* const all[] = {b->coarse[0], b->coarse[1], b->fine[0], b->fine[1], b->span_count[0], b->span_count[1],
                          b->cand_j, b->cand_info, b->cand_avg, b->det_list, b->walk_scratch, b->frames, b->chips,
-                         b->ap.last, b->ap.count, b->ap.off, b->ap.cursor, b->ap.ent};
+                         b->ap.last, b->ap.count, b->ap.off, b->ap.cursor, b->ap.ent,
+                         b->mac_rec, b->mac_tile_count, b->mac_queue, b->mac_state};
     for (void* p : all) cudaFree(p);
     *b = AmbChainBufs();
 }

@@ -157,4 +157,22 @@ cudaError_t amb_launch_dcblock(const float2* rawcarry, int nc, const float2* fre
 cudaError_t amb_launch_prologue(float2* tail, int tail_cap, const float2* src_rem, int n_rem,
                                 uint32_t* group_count, int n_groups, cudaStream_t s);
 size_t amb_scan_smem_bytes(int spc_i);
+// Mode A/C replies (option "modeac", amb_modeac.cuh). Offsets in samples of o(t) = floor(t * rate_int / 1e6 + 0.5):
+// slot k = o(1.45 k), gap g = o(1.45 g + 0.725), spi = o(24.65), back = o(25.1).
+#define AMB_MODEAC_TILE 2048     // starts per CTA of the tile kernel
+struct AmbModeacGeom { int slot[15]; int gap[14]; int spi; int back; };
+struct AmbModeacArgs {
+    AmbParams P; AmbSegs S; AmbModeacGeom G;
+    int j_lo, j_hi;                  // starts decided by this call (the scan's range)
+    long long org;                   // reported index of j = 0
+    int na_cap, nb_cap;              // per-tile shared-memory spans (amb_modeac_smem_bytes)
+    int cap_tile;                    // record slots per tile: replies lie more than G.back apart
+    amb_modeac* rec; unsigned* tile_count;                 // per-call slots
+    unsigned long long* last_prev;   // 1 + reported index of the last start passing rules 1-5 before this call (0: none)
+    unsigned long long* last_cur;    // ... in this call (atomicMax, folded into last_prev by the emit kernel)
+    unsigned long long* stats;       // candidates, replies, overlap drops, with altitude
+    amb_modeac* queue; unsigned* q_count;                  // replies not read out yet, in stream order
+};
+size_t amb_modeac_smem_bytes(const AmbModeacArgs& a);
+int amb_launch_modeac(const AmbModeacArgs& a, cudaStream_t s, cudaError_t* err);   // returns the kernels launched
 cudaError_t amb_launch_widen_sc16(const void* in_sc16, float2* out, long long n, int sm_count, cudaStream_t s);

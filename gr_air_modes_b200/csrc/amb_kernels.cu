@@ -2433,3 +2433,8 @@ cudaError_t amb_upload_tables(const int*)
     }
     return cudaMemcpyToSymbol(c_crc_rem, rem, sizeof(rem));
 }
+
+// ------------------------------------------------------------------------------------------------
+// Mode A/C replies (option "modeac")
+// ------------------------------------------------------------------------------------------------
+#include "amb_modeac.cuh"

@@ -492,3 +492,78 @@ def make_mlat_scenes(rate: float, n: int, stations, aircraft, n_tx: int, seed: i
             bursts.append(b)
         scenes.append(Scene(rate, n, iq.reshape(2 * n), bursts))
     return scenes, truth
+
+
+# ---------------------------------------------------------------------------------------------------------
+# Mode A/C replies (option "modeac"): F1, the 13 code pulses C1 A1 C2 A2 C4 A4 X B1 D1 B2 D2 B4 D4 at 1.45 us steps,
+# F2 at 20.3 us and the optional SPI pulse at 24.65 us, each 0.45 us long. New functions with random streams of their own.
+# ---------------------------------------------------------------------------------------------------------
+MODEAC_PULSE_US = 0.45
+
+
+def modeac_waveform(code: int, spi: bool, start: float, amplitude: float, phase: float, spc: float):
+    """(first_sample, complex64 samples) of one reply whose F1 leading edge is at fractional sample `start`: box-car
+    integrated rectangular pulses, as burst_waveform. `code` is the 13-bit C1..D4 word (bit 12 = C1); X (bit 6) is
+    never sent."""
+    spu = 2.0 * spc                                   # samples per microsecond
+    t = [0.0] + [1.45 * k for k in range(1, 14) if k != 7 and (code >> (13 - k)) & 1] + [20.3]
+    if spi:
+        t.append(24.65)
+    n0 = int(np.floor(start))
+    n1 = int(np.ceil(start + (24.65 + MODEAC_PULSE_US) * spu)) + 1
+    lo = np.arange(n0, n1, dtype=np.float64) - start
+    cover = np.zeros(lo.size)
+    for p in t:                                       # overlap of [lo, lo + 1) with [p, p + width) in samples
+        a, b = p * spu, (p + MODEAC_PULSE_US) * spu
+        cover += np.clip(np.minimum(lo + 1, b) - np.maximum(lo, a), 0.0, None)
+    return n0, (amplitude * cover * np.exp(1j * phase)).astype(np.complex64)
+
+
+@dataclasses.dataclass
+class ModeacReply:
+    start: float          # fractional sample index of the F1 leading edge
+    code: int
+    spi: bool
+    amplitude: float
+    phase: float
+
+
+def make_modeac_scene(rate: float, n: int, n_replies: int, seed: int, *, noise_sigma: float = 0.01,
+                      snr_db=(15.0, 30.0), n_bursts: int = 0, codes=None, spis=None, gap_us: float = 30.0):
+    """Complex Gaussian noise + `n_replies` Mode A/C replies + `n_bursts` Mode S bursts, none overlapping another: each
+    goes into its own slot of a jittered grid (a reply's slot is 26 us + gap, a burst's 120 us + gap, in random order).
+    codes / spis: the replies' codes and SPI flags (default random, X = 0). Returns (Scene, [ModeacReply]) with the
+    replies in start order; Scene.bursts holds the Mode S bursts."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    spc = rate / 2e6
+    spu = 2.0 * spc
+    iq = (rng.standard_normal((n, 2), dtype=np.float32) * np.float32(noise_sigma))
+    c = iq.view(np.complex64).reshape(n)
+    kinds = np.array([0] * n_replies + [1] * n_bursts)
+    rng.shuffle(kinds)
+    lens = np.where(kinds == 0, 26.0, 120.0) * spu + gap_us * spu
+    if lens.sum() > n - 64 * spu:
+        raise ValueError("make_modeac_scene: %d replies and %d bursts do not fit in %d samples" % (n_replies, n_bursts, n))
+    slack = (n - 64 * spu - lens.sum()) / max(kinds.size, 1)
+    if codes is None:
+        codes = rng.integers(0, 1 << 13, n_replies) & ~0x40
+    if spis is None:
+        spis = rng.random(n_replies) < 0.5
+    pos = 32 * spu
+    replies, bursts, r = [], [], 0
+    for k, kind in enumerate(kinds):
+        s = pos + rng.uniform(0, slack)
+        amp = float(np.sqrt(2.0 * noise_sigma ** 2 * 10 ** (rng.uniform(*snr_db) / 10)))
+        ph = float(rng.uniform(0, 2 * np.pi))
+        if kind == 0:
+            rep = ModeacReply(float(s), int(codes[r]) & ~0x40, bool(spis[r]), amp, ph)
+            n0, w = modeac_waveform(rep.code, rep.spi, rep.start, amp, ph, spc)
+            replies.append(rep)
+            r += 1
+        else:
+            b = Burst(float(s), make_frame(int(rng.choice((11, 17))), rng), amp, ph)
+            n0, w = burst_waveform(b, spc)
+            bursts.append(b)
+        c[n0:n0 + w.size] += w[:max(0, min(w.size, n - n0))]
+        pos += lens[k] + slack
+    return Scene(rate, n, iq.reshape(2 * n), bursts), replies

@@ -327,6 +327,63 @@ AMB_API int amb_resolve_device(amb_ctx* ctx, const int64_t* entry_dev, void* aft
 /* cuda_stream / after_stream: the caller's stream the exchange runs on (NULL: the caller-visible stream). Running the
  * collective on a side stream (amb_join_stream) keeps the scan stream free for the next pass. */
 AMB_API int amb_join_stream(amb_ctx* ctx, void* cuda_stream);
+
+/* ---- Mode A/C replies (option "modeac", no reference equivalent) ---------------------------------------------
+ * Secondary-radar replies: a framing pulse F1, 13 code pulses 1.45 us apart, F2 at 20.3 us and an optional SPI pulse
+ * at 24.65 us. With amb_set_option(ctx, "modeac", 1) every call also finds them in the same canonical front end the
+ * preamble block reads. Notation, on the stream since amb_create / amb_reset / amb_set_rate (not on its cut into calls):
+ *   in[n]   the canonical bb (PMF output, or |x|^2 without the PMF; after the DC blocker when that is on), zeros
+ *           before sample 0 and after the end at flush
+ *   avg[n]  the canonical 48*spc noise floor; thr = the preamble threshold (amb_geometry.threshold)
+ *   o(t)    (int)floor(t * rate_int / 1e6 + 0.5), the sample offset of t us, evaluated in double
+ *   slot k  o(1.45 k), k = 0..14: F1, C1 A1 C2 A2 C4 A4 X B1 D1 B2 D2 B4 D4, F2; gap g = o(1.45 g + 0.725), g = 0..13;
+ *           SPI = o(24.65)
+ * A start i is a reply when
+ *   1  in[i] > avg[i]*thr, in[i-1] < in[i] and !(in[i+1] > in[i])     (rising-edge peak, preamble_impl.cc:173-175)
+ *   2  !(in[i+o(20.3)] < avg[i]*thr)                                  (F2)
+ *   3  avgpeak = (in[i] + in[i+o(20.3)]) / 2.0f, space = avg[i] + (avgpeak - avg[i]) / thr   (float, as :198-203)
+ *   4  in[i] and in[i+o(20.3)] both > space and > (avg[i]*thr)*thr, and !(in[i+o(10.15)] > space)
+ *                                                                     (framing pulses clear of the floor, X quiet)
+ *   5  !(in[i+gap g] > space) for all 14 gaps                         (what keeps Mode S data blocks out)
+ *   6  code bit 12-(k-1) = in[i+slot k] > space (k = 1..13; bit 6 = X = 0); spi = in[i+o(24.65)] > space
+ *   7  no j with i - o(25.1) <= j < i satisfies 1-5, whether or not j was dropped itself (a reply's own code pulses)
+ * and becomes a record: sample_index = the reported index frames use (sample + history()-1), stamped as a frame at that
+ * index (tag_to_timestamp), code and spi, peak = avgpeak and floor = avg[i] (raw floats, no dB), squawk =
+ * decode_id(code) (parse.py:233-254), altitude = decode_alt(code, True) (altitude.py) when D1 = 0 and C1 C2 C4 is one of
+ * 001, 011, 010, 110, 100, else AMB_NO_ALTITUDE. Records come in ascending sample_index, whatever the cut into calls.
+ * The option needs the PMF and at least 4 Msps (2 samples per 0.5 us chip; amb_process returns AMB_ERR_UNSUPPORTED
+ * otherwise): without them a 0.45 us pulse is sampled too coarsely for the fixed offsets. It is accepted only before
+ * the first amb_process after amb_create / amb_reset / amb_set_rate (AMB_ERR_STATE otherwise) and persists across them. It is not available in time-sharded operation or with the split-form
+ * amb_preamble_process (AMB_ERR_STATE). With it off nothing is launched and nothing changes. */
+typedef struct amb_modeac {
+    uint64_t sample_index;   /* reported index of F1 (the same numbering as amb_frame.sample_index) */
+    uint64_t secs;           /* tag_to_timestamp, as a frame at sample_index */
+    double frac;
+    float peak;              /* avgpeak of rule 3 */
+    float floor;             /* avg[i] */
+    int32_t altitude;        /* feet, or AMB_NO_ALTITUDE */
+    uint16_t code;           /* 13 bits C1 A1 C2 A2 C4 A4 X B1 D1 B2 D2 B4 D4, MSB first (the Mode S ID13 / AC13 layout) */
+    uint16_t squawk;         /* decode_id(code): four octal digits read as a decimal number (7700 = 0x1E14) */
+    uint8_t spi;             /* 1 when the SPI pulse is present */
+    uint8_t pad_[7];
+} amb_modeac;                /* 48 bytes */
+#ifdef __cplusplus
+static_assert(sizeof(amb_modeac) == 48, "amb_modeac is 48 bytes");
+#else
+_Static_assert(sizeof(amb_modeac) == 48, "amb_modeac is 48 bytes");
+#endif
+/* Counts since amb_create / amb_reset / amb_set_rate: starts passing rules 1-2, replies, starts that pass 1-6 but are
+ * dropped by rule 7, and replies with an altitude. */
+typedef struct amb_modeac_stats { uint64_t candidates, replies, overlap_drops, with_altitude; } amb_modeac_stats;
+/* Wait for enqueued work and copy out up to `max` replies in stream order, stamped; returns the count. */
+AMB_API int amb_poll_modeac(amb_ctx* ctx, amb_modeac* out, int max);
+AMB_API int amb_pending_modeac(amb_ctx* ctx);
+/* The device-side amb_poll_modeac: every reply not handed out yet, in stream order and stamped, written to DEVICE
+ * memory. out_dev == NULL: report the count, consume nothing. AMB_ERR_OVERFLOW (nothing consumed) if cap is too small.
+ * Replies already moved to the host by amb_poll_modeac / amb_pending_modeac stay there. */
+AMB_API int amb_drain_modeac_device(amb_ctx* ctx, amb_modeac* out_dev, int cap);
+AMB_API int amb_get_modeac_stats(amb_ctx* ctx, amb_modeac_stats* out);   /* synchronises */
+
 /* ---- batch field decode of queued frames (SURVEY.md 8 row f4) ---------------------------------------
  * What the reference does per message in Python after the slicer: modes_reply field extraction
  * (python/parse.py:27-231), decode_alt (python/altitude.py:28-108), decode_id (parse.py:233-254), the BDS0,5 / 0,6 /

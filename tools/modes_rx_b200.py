@@ -27,7 +27,10 @@ own --beast) and ends when the server closes. The bytes are parsed on the GPU (g
 chunk's frames go where the receive chain's go: their message lines to stdout, -t, --reports / -l, -P, --track /
 --aircraft and --coverage, and the frames themselves to --beast / --avr. The stamps are the feed's 48-bit 12 MHz
 counter, not wall-clock time: SBS-1 dates on Beast input follow that counter. Options that only configure the receive
-chain (-d, -r, -T, --ec, --ec-any, --ap-filter, --resample) are errors with --input beast.
+chain (-d, -r, -T, --ec, --ec-any, --ap-filter, --resample, --modeac) are errors with --input beast.
+
+With --modeac the receive chain also finds Mode A/C replies (squawk, altitude, SPI) on the GPU and prints one line per
+reply after each chunk's messages (the format is in the option's help).
 
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 [-T 7.0] [-d] [-t 5556] [-n] [--reports | -l 37.4,-122.1]
     python tools/modes_rx_b200.py -s 127.0.0.1:12345 -r 4e6 --udp-idle 2.0
@@ -40,6 +43,7 @@ chain (-d, -r, -T, --ec, --ec-any, --ap-filter, --resample) are errors with --in
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -l 37.4,-122.1 --coverage coverage.json
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -n --beast 30005 --avr 30002 --avr-mlat
     python tools/modes_rx_b200.py -s capture.cfile -r 4e6 -l 37.4,-122.1 -m 127.0.0.1:5000
+    python tools/modes_rx_b200.py -s capture.cfile -r 4e6 --modeac
     python tools/modes_rx_b200.py --input beast -s 192.168.1.20:30005 --reports
     python tools/modes_rx_b200.py --input beast -s feed.bin -l 37.4,-122.1 -P 30003
 
@@ -345,6 +349,11 @@ def parse_args(argv=None):
                     help="correct DF11/DF17 frames over at most K (1..23) low-confidence bits; 0 = off, as the reference")
     ap.add_argument("--ec-any", type=int, default=0, metavar="M",
                     help="correct DF17 frames by at most M (1, 2) flipped bits anywhere, after --ec; 0 = off, as the reference")
+    ap.add_argument("--modeac", action="store_true", default=False,
+                    help="also find Mode A/C replies (needs the PMF and -r >= 4e6) and print one line per reply after "
+                         "each chunk's messages, in stream order: 'modeac SQUAWK ALT SPI PEAK FLOOR SECS FRAC' with SQUAWK "
+                         "the four octal digits, ALT the Gillham altitude in feet or '-', SPI 0 or 1, PEAK and FLOOR the "
+                         "reply's linear levels (%%.6e) and SECS FRAC its time stamp (%%d %%.9f)")
     ap.add_argument("--ap-filter", type=int, default=0, metavar="S",
                     help="drop address/parity replies from aircraft not confirmed by a clean DF11/DF17 in the last S "
                          "seconds, and accept DF11 replies with an II/SI code from confirmed ones; 0 = off, as the reference")
@@ -392,12 +401,14 @@ def parse_args(argv=None):
     if args.input == "beast":
         given = [name for name, on in (("-d", args.dcblock), ("-r", args.rate is not None), ("-T", args.threshold is not None),
                                         ("--ec", args.ec), ("--ec-any", args.ec_any), ("--ap-filter", args.ap_filter),
-                                        ("--resample", args.resample)) if on]
+                                        ("--resample", args.resample), ("--modeac", args.modeac)) if on]
         if given:
             ap.error("%s configure%s the receive chain, which --input beast does not run" %
                      (", ".join(given), "s" if len(given) == 1 else ""))
     args.rate = 4e6 if args.rate is None else args.rate
     args.threshold = 7.0 if args.threshold is None else args.threshold
+    if args.modeac and (not args.pmf or (int(args.rate) < 4e6 and not args.resample)):
+        ap.error("--modeac needs the PMF and a chain rate of at least 4 Msps")
     if args.coverage and args.location is None:
         ap.error("--coverage needs -l LAT,LON")
     if args.sbs1 is not None and not 0 < args.sbs1 < 65536:
@@ -440,6 +451,13 @@ def parse_args(argv=None):
     return args
 
 
+def format_modeac(r) -> str:
+    """One --modeac line: 'modeac SQUAWK ALT SPI PEAK FLOOR SECS FRAC' (see the option's help)."""
+    alt = "-" if int(r["altitude"]) == air_modes.blocks.NO_ALTITUDE else "%d" % int(r["altitude"])
+    return "modeac %04d %s %d %.6e %.6e %d %.9f" % (int(r["squawk"]), alt, int(r["spi"]), float(r["peak"]), float(r["floor"]),
+                                                   int(r["secs"]), float(r["frac"]))
+
+
 def main(argv=None):
     args = parse_args(argv)
 
@@ -462,7 +480,7 @@ def main(argv=None):
               "reproduced; --resample runs a stand-in); running the chain at the native rate" % rate, file=sys.stderr)
     sinks, printer, reporter, raw, pub = make_outputs(args)
     rx = air_modes.rx_path(rx_rate, args.threshold, tee_queue(sinks), args.pmf, args.dcblock, device=args.device,
-                           ec=args.ec, ec_any=args.ec_any, ap_filter=args.ap_filter)   # radio.py:55-56
+                           ec=args.ec, ec_any=args.ec_any, ap_filter=args.ap_filter, modeac=args.modeac)   # radio.py:55-56
 
     if ":" in args.source and not os.path.exists(args.source):
         m = re.search(r"(.*)\:(\d{1,5})$", args.source)                                                           # radio.py:223-226
@@ -486,6 +504,10 @@ def main(argv=None):
             reporter.flush()
         if raw:
             raw.flush(rx.frames)
+        if args.modeac:
+            for r in rx.modeac():
+                print(format_modeac(r))
+            sys.stdout.flush()
     st = rx.stats()
     print("# %d samples in, %d messages" % (st.samples_in, total), file=sys.stderr)
     close_outputs(reporter, raw, pub)
